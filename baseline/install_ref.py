@@ -13,7 +13,7 @@ result because baseline/_ref is git-ignored but NOT gpurun-ignored):
     from a scratch copy under /tmp (the source tree is read-only and setuptools writes egg-info in place).
     BUILD_NO_CUDA=1 is the reference's own switch (setup.py:40) for a Python-only install.
  2. compiles the reference's CUDA sources where they lie with the committed recipe oracle/build_ref.py
-    (--full: 3DGS + 3DGUT + adam + relocation + camera wrappers, channels 1,3,4,6,8,21,23,24,32,128 as in the reference's pytest.ini, sm_100a, the reference's release
+    (--full: 3DGS + 3DGUT + adam + relocation + camera wrappers, channels 1,3,4,6,8,21,23,24,32,128 as in the reference's pytest.ini, sm_90a, the reference's release
     flags; about 25 minutes from scratch on 8 cores, seconds when oracle/_ref/obj_full is warm) and places the result as the
     prebuilt module the package looks for first: ``gsplat/csrc.so`` (gsplat/cuda/_backend.py:30).
  3. copies what the reference's own hot-path tests need at run time: tests/ + the root conftest.py (the

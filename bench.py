@@ -47,7 +47,7 @@ def workload_config(n_gpus: int) -> dict:
         + (" + all-reduce (SUM) of the Gaussian grads over NVLink" if n_gpus > 1 else ""),
         "views_per_step": n_gpus,
         "parallelism": f"view-axis DP x{n_gpus} (replicated Gaussians)" if n_gpus > 1 else "single GPU",
-        "l2": "inputs (236 MB of Gaussian parameters + 25 MB target) exceed the 126 MB L2; no explicit flush",
+        "l2": "inputs (236 MB of Gaussian parameters + 25 MB target) exceed the H100's 50 MB L2; no explicit flush",
     }
 
 
@@ -111,7 +111,7 @@ def measured_peak_gbs() -> tuple[float, str]:
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data-sheet HBM3 bandwidth (not measured)"
 
 
 def build_scene():
@@ -196,7 +196,7 @@ def run_cpu_reference(steps: int, warmup: int, n_gpus: int, as_main_line: bool):
 def run_ref_cuda(params, vm, K, target, steps: int):
     """Extra information (not the contract's reference arm): the REAL reference's CUDA kernels
     (oracle/_ref/gsplat_ref.so, built by oracle/build_ref.py with the reference's release flags for
-    sm_100a) chained as its orchestrator chains them (csrc/Rendering.cpp:976-1447) on the same inputs,
+    sm_90a) chained as its orchestrator chains them (csrc/Rendering.cpp:976-1447) on the same inputs,
     forward ops + the matching *_bwd ops called by hand (no autograd / Python overhead -> a lower bound
     on the reference's train step).  Returns None when the library is absent."""
     import torch
@@ -242,7 +242,7 @@ def run_ref_cuda(params, vm, K, target, steps: int):
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / steps
         return {
-            "what": "HAND-CHAINED: reference gsplat v1.6.0 CUDA kernels (sm_100a, -use_fast_math), ops called one by one, "
+            "what": "HAND-CHAINED: reference gsplat v1.6.0 CUDA kernels (sm_90a, -use_fast_math), ops called one by one, "
             "no autograd overhead (not the reference's stock path: see ref_cuda_stock)",
             "ms_per_step": ms, "views_per_s": 1e3 / ms, "n_isects": int(out[3].numel()),
         }
@@ -358,6 +358,10 @@ def run_trainer_bench(steps: int):
     default and MCMC strategies (tools/trainer_bench.py, one subprocess per run).  Returns the `trainer` object."""
     import subprocess as sp
 
+    from oracle import refcuda
+
+    if not refcuda.package_available():
+        return None  # both arms drive the reference's trainer package
     tool = os.path.join(ROOT, "tools", "trainer_bench.py")
     out = {}
     arms = (("ref", ["--backend", "reference"]), ("ours", ["--backend", "b200"]),
@@ -399,6 +403,26 @@ def run_trainer_bench(steps: int):
     return out
 
 
+DUMP_GAUSSIAN_ROWS = 65536
+
+
+def dump_outputs(out_dir: str, last: dict, grads: dict) -> None:
+    """Writes what the timed path computed in its last step as float32 .npy files: the rendered colours and alphas, the
+    loss, and the gradients of the Gaussian parameters at a fixed, seeded sample of DUMP_GAUSSIAN_ROWS Gaussians (all of
+    them would be 240 MB; the sampled indices are written as gaussian_rows.npy)."""
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    n = grads["means"].shape[0]
+    rows = np.sort(np.random.RandomState(0).choice(n, min(DUMP_GAUSSIAN_ROWS, n), replace=False))
+    np.save(os.path.join(out_dir, "gaussian_rows.npy"), rows.astype(np.float64))
+    arrays = {k: v.detach() for k, v in last.items()}
+    idx = torch.from_numpy(rows).to(grads["means"].device)
+    arrays.update({f"v_{k}": g.detach().index_select(0, idx) for k, g in grads.items()})
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.float().cpu().numpy())
+
+
 # --------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -409,7 +433,10 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-trainer", action="store_true", help="skip the cfg5 trainer-loop runs (about 2 minutes)")
     ap.add_argument("--trainer-steps", type=int, default=700)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last step computed as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -513,6 +540,8 @@ def main():
         )
         loss = gsplat_b200.l1_loss(rc, tgt)  # == (rc - tgt).abs().mean(), fused (losses.py)
         loss.backward()
+        if args.dump_outputs:
+            last.update(render_colors=rc, render_alphas=ra, loss=loss)
         if world > 1:
             all_reduce_grads()  # the 59 floats / Gaussian (SURVEY.md section 8e), one launch, in place
         if e2e:
@@ -521,6 +550,7 @@ def main():
         return meta
 
     host_issue_ms = {}
+    last = {}  # with --dump-outputs: the outputs of the most recent step
 
     def timed(e2e: bool, steps: int) -> float:
         if world > 1:
@@ -571,6 +601,8 @@ def main():
     ms_dev = timed(False, args.steps)
     ms_e2e = timed(True, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last, {k: params[k].grad for k in grad_names})
 
     # ---- N > 1 diagnostics (outside the timed regions): where a DP step spends its time on every rank, and the
     # same job (world views / step over the same Gaussians, every gradient summed over all views) laid out the
@@ -744,13 +776,13 @@ def main():
         "required, pair throughput below is the meaningful figure",
         "raster_fwd": {"ms": ms_rfwd, "achieved": bytes_fwd / (ms_rfwd * 1e-3) / 1e9, "algorithmic_bytes": bytes_fwd},
         # compute-side figure (SURVEY.md section 8d): candidate (pixel, gaussian) pairs = 256 per (tile, gaussian)
-        # intersection; the kernels are instruction-issue bound (profiles/r02_v7_ncu.md: 77 % / 93 % issue-active)
+        # intersection; issue peak = SMs x 4 schedulers x the maximum SM clock nvidia-smi reports
         "pairs": {
             "candidate_pairs": 256 * S,
             "bwd_gpairs_per_s": 256 * S / (ms_rbwd * 1e-3) / 1e9,
             "fwd_gpairs_per_s": 256 * S / (ms_rfwd * 1e-3) / 1e9,
-            "issue_peak_ginst_per_s": 148 * 4 * 1.965,
-            "issue_evidence": "profiles/r02_v7_ncu.md (smsp__issue_active 77 % / 93 %, smsp__inst_executed: 418 M backward, 251 M forward)",
+            "issue_peak_ginst_per_s": (torch.cuda.get_device_properties(dev).multi_processor_count * 4 * clocks["sm_max_mhz"] / 1e3
+                                       if clocks and clocks.get("sm_max_mhz") else None),
         },
     }
 
@@ -782,7 +814,7 @@ def main():
                 "input": ("target image shipped as uint8 HWC from pinned memory and converted to float on the device inside "
                           "the timed region" if e2e_u8 else "target image shipped as float32 HWC from pinned memory"),
             },
-            # our own kernels per step (profiles/r02_v9_launches.csv): project_sh_fwd (+ tile counts + row records),
+            # our own kernels per step: project_sh_fwd (+ tile counts + row records),
             # publish_totals, depth_key_rows_bounded, isect_emit_coop, isect_offsets_tilekeys, pack_rows, tile_order,
             # raster_fwd, l1 partial/final/bwd, raster_bwd2, project_sh_bwd (= 13; the cub select / scan / radix-sort launches
             # made by the library are not counted); timed region = `steps` device-resident + `steps` e2e steps

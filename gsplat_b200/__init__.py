@@ -1,4 +1,4 @@
-"""gsplat_b200 -- B200-native (sm_100a) kernels behind gsplat's rasterization() operator surface.
+"""gsplat_b200 -- H100-native (sm_90a) kernels behind gsplat's rasterization() operator surface.
 
 Public names mirror /root/reference/gsplat/__init__.py:19-104 for the hot path:
 rasterization, fully_fused_projection, spherical_harmonics, isect_tiles, isect_offset_encode,

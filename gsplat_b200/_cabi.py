@@ -155,7 +155,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise GsplatB200Error(
                 f"{LIB_PATH} is missing: build it with `python -m gsplat_b200.build` "
-                "(nvcc, sm_100a). gsplat_b200 has no CPU / PyTorch fallback."
+                "(nvcc, sm_90a). gsplat_b200 has no CPU / PyTorch fallback."
             )
         L = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
@@ -198,7 +198,7 @@ def require_cuda(*tensors: Optional[torch.Tensor]) -> torch.device:
             continue
         if not t.is_cuda:
             raise GsplatB200Error(
-                "gsplat_b200 operators run only on CUDA tensors (sm_100a kernels; there is no CPU fallback)"
+                "gsplat_b200 operators run only on CUDA tensors (sm_90a kernels; there is no CPU fallback)"
             )
         if dev is None:
             dev = t.device

@@ -1,4 +1,4 @@
-"""Builds gsplat_b200/libgsplat_b200.so in-tree with nvcc for sm_100a (no torch headers involved).
+"""Builds gsplat_b200/libgsplat_b200.so in-tree with nvcc for sm_90a (no torch headers involved).
 
     python -m gsplat_b200.build [--force]
 
@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libgsplat_b200.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "--expt-extended-lambda"]
 UNITS = {
     # file: extra flags

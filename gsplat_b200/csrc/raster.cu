@@ -1,11 +1,11 @@
-// raster.cu -- rasterize_to_pixels forward / backward for sm_100a.
+// raster.cu -- rasterize_to_pixels forward / backward for sm_90a (H100).
 //
 // Replaces (behaviour, not code) the reference kernels
 //   csrc/RasterizeToPixels3DGSSerialBatchFwd.cu:41-297   (forward)
 //   csrc/RasterizeToPixels3DGSSerialBatchBwd.cu:41-320   (backward)
 //   csrc/RasterizeToPixels3DGSDevice.cuh:37-173          (per-pair math)
 //
-// B200 design (see DESIGN.md section "rasterize"):
+// Design:
 //  * a pack pass gathers the depth-sorted per-intersection records ONCE per view into three
 //    contiguous float4 streams (cull: mean + conservative half extents of the alpha>=1/255 ellipse,
 //    geom: conic + opacity, color), so that every tile's list is a contiguous byte range;
@@ -786,7 +786,7 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd_kernel(
 //     compile-time immediates) and the D colour sums in registers -- no cross-lane traffic; the moments are
 //     re-centred on the gaussian's mean once per gaussian, the two halves are combined with one shuffle per
 //     value, and the 12-float gradient record is added with three 128-bit REDs instead of nine scalar ones.
-// Per survivor: ~45 + ~16 instructions instead of 130 (DESIGN.md section 3).
+// Per survivor: ~45 + ~16 instructions instead of 130.
 constexpr int kBwdBatch = 64; // records per ring stage (smaller than the forward's: the per-warp buffers need the room)
 constexpr int kRound    = 16; // survivors per reduction round of a warp
 constexpr int kRowF2    = 33; // row stride of the round buffer in float2 units (odd: conflict-free in both phases)
@@ -1183,6 +1183,27 @@ static SideLane *side_lane()
     return &l;
 }
 
+// SMs of the current device, queried once per device.
+static unsigned sm_count()
+{
+    static int counts[64] = {}; // 0 = not queried yet
+    int dev = 0;
+    if(cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64)
+        return 132;
+    if(counts[dev] == 0)
+    {
+        int n = 0;
+        if(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+            n = 132; // H100 SXM
+        counts[dev] = n;
+    }
+    return (unsigned)counts[dev];
+}
+
+// The tile dispatch order (heaviest tiles first) matters once there are at least two waves of tiles per SM.  The pack,
+// the forward and the backward all decide with this one function, so the order stream is written whenever it is read.
+static bool use_tile_order(unsigned n_tiles) { return n_tiles >= 2 * sm_count(); }
+
 template<int CDIM>
 static int launch_pack(
     const float *means2d, const float *conics, const float *colors, const float *opacities, const int32_t *offsets,
@@ -1190,7 +1211,7 @@ static int launch_pack(
 )
 {
     RecordStreams r = carve_records(records, S, RecLayout<CDIM>::kColorVec4);
-    const bool want_order = S > 0 && n_tiles >= 2 * 148; // enough tiles for dispatch order to matter
+    const bool want_order = S > 0 && use_tile_order(n_tiles);
     std::unique_lock<std::mutex> side_lock(g_side_mu, std::defer_lock);
     if(want_order)
         side_lock.lock();
@@ -1240,7 +1261,7 @@ static int launch_fwd(
     if(int rc = launch_pack<CDIM>(means2d, conics, colors, opacities, offsets, flatten_ids, S, n_tiles, records, st, rows))
         return rc;
     RecordStreams r      = carve_records(records, S, RecLayout<CDIM>::kColorVec4);
-    const int32_t *order = (S > 0 && n_tiles >= 2 * 148) ? r.order : nullptr;
+    const int32_t *order = (S > 0 && use_tile_order(n_tiles)) ? r.order : nullptr;
     // default for CDIM <= 4: barrier-free ring (0.333 -> 0.304 ms incl. pack at cfg3); GSB200_FWD_PIPE=0 keeps the CTA barrier
     static const bool pipe = [] {
         const char *e = std::getenv("GSB200_FWD_PIPE");
@@ -1277,7 +1298,7 @@ static int launch_bwd(
         return GSB200_OK; // reference: no launch when there are no intersections (Bwd.cu:350-354)
     RecordStreams r    = carve_records(const_cast<void *>(records), S, RecLayout<CDIM>::kColorVec4);
     const unsigned n_tiles = (unsigned)(I * tw * th);
-    const int32_t *order   = (n_tiles >= 2 * 148) ? r.order : nullptr; // written by the forward
+    const int32_t *order   = use_tile_order(n_tiles) ? r.order : nullptr; // written by the forward
     const bool absg        = dst.abs != nullptr;
     // version 2 (transposed reduction) is the default; GSB200_BWD_ALGO=butterfly selects version 1 (measurements)
     static const bool use_v2 = [] {

@@ -1,7 +1,7 @@
 // sort.cu -- (isect_id, flatten_id) radix sort and library-level helpers.
 //
 // The sorts are cub::DeviceRadixSort::SortPairs (the library call the reference makes,
-// csrc/IntersectTile.cu:1078-1121; its onesweep kernels are compiled here for sm_100a), used twice:
+// csrc/IntersectTile.cu:1078-1121; its onesweep kernels are compiled here for sm_90a), used twice:
 // once over the N projected rows on (image, depth) and once over the S intersections on the (image, tile)
 // bits only -- see gsb200_isect_depth_order below.
 #include <cub/device/device_radix_sort.cuh>
@@ -18,7 +18,7 @@ static thread_local cudaError_t g_last_error = cudaSuccess;
 void set_last_cuda_error(cudaError_t e) { g_last_error = e; }
 } // namespace gsb
 
-extern "C" const char *gsb200_version(void) { return "gsplat_b200 0.1.0 (sm_100a)"; }
+extern "C" const char *gsb200_version(void) { return "gsplat_b200 0.1.0 (sm_90a)"; }
 
 extern "C" const char *gsb200_error_string(int code)
 {

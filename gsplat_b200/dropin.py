@@ -17,7 +17,7 @@ preserved; ``stats`` counts per name how many calls ran on the b200 kernels and 
 
 Nothing else of the package is touched: strategies, exporters, the Python reference implementations
 (``_rasterization``, ``_torch_impl``) keep running the package's own code -- which is what lets the reference's
-own tests compare the b200 kernels with the reference's Python twins (tests/test_reference_suite.py) and lets
+own tests compare the b200 kernels with the reference's Python twins and lets
 ``examples/simple_trainer.py`` run unchanged (it imports ``from gsplat.rendering import rasterization`` after
 this has been applied, e.g. from a ``sitecustomize`` / ``GSPLAT_BACKEND=b200`` hook).
 

@@ -8,7 +8,7 @@ Reference wrappers mirrored here (file:line in /root/reference/gsplat/cuda/_wrap
 and their autograd registrations (:559-716, :966-1191, :2010-2117).
 
 PyTorch is plumbing here (device memory, streams, autograd graph); every number is produced by the
-hand-written sm_100a kernels.
+hand-written sm_90a kernels.
 """
 from __future__ import annotations
 

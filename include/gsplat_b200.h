@@ -1,5 +1,5 @@
 /*
- * gsplat_b200.h -- C ABI of libgsplat_b200.so: the B200-native (sm_100a) replacement for the
+ * gsplat_b200.h -- C ABI of libgsplat_b200.so: the H100-native (sm_90a) replacement for the
  * CUDA operators behind gsplat.rasterization().
  *
  * This is the drop-in boundary.  Every entry point takes plain DEVICE pointers, sizes and a

@@ -7,8 +7,8 @@ this repository) with a recipe written here -- the reference's own build system 
 JIT via torch.utils.cpp_extension.load) is NOT run; its flag set for a "3DGS only" release build is
 restated: -std=c++20 -O3 -DNDEBUG -use_fast_math -DGSPLAT_BUILD_3DGS=1 (every other module then defaults
 to off, csrc/Config.h:28-60) and -DGSPLAT_NUM_CHANNELS=1,3,4 (Config.h:70-72) to keep compile time sane.
-Target: sm_100a.  Only runs where /root/reference exists (the build container); the resulting .so is
-git-ignored but travels to the GPU box, where tests/test_gpu_vs_reference_cuda.py and bench.py load it
+Target: sm_90a.  Only runs where the reference sources exist; the resulting .so is
+git-ignored; tests/golden/make_ref_cuda_golden.py (which records tests/golden/ref_cuda.npz) and bench.py load it
 with torch.ops.load_library and call torch.ops.gsplat.* directly.  The pybind module inside is named ``csrc``
 (TORCH_EXTENSION_NAME), so that baseline/install_ref.py can also place a copy as the prebuilt ``gsplat/csrc.so``
 the reference's Python package imports first (gsplat/cuda/_backend.py:30) -- one process must load only ONE of
@@ -57,7 +57,7 @@ def main():
            f"-DGSPLAT_NUM_CHANNELS={NUM_CHANNELS}"]
     nvcc = [
         "/usr/local/cuda/bin/nvcc", "-ccbin", "/usr/bin/g++", "-std=c++20", "-O3", "-use_fast_math", "--expt-relaxed-constexpr",
-        "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-diag-suppress", "3189,20012,186", "-w",
+        "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-diag-suppress", "3189,20012,186", "-w",
         "-DGSPLAT_NUM_CHANNELS=" + NUM_CHANNELS.replace(",", "\\,"),
         "-D__CUDA_NO_HALF_OPERATORS__", "-D__CUDA_NO_HALF_CONVERSIONS__", "-D__CUDA_NO_BFLOAT16_CONVERSIONS__",
         "-D__CUDA_NO_HALF2_OPERATORS__",
@@ -77,11 +77,15 @@ def main():
         sources.insert(0, os.path.join(REF, "csrc", "CameraWrappers.cu"))
         objdir = OBJ + "_full"
         os.makedirs(objdir, exist_ok=True)
+    # objects are reused only when they were compiled with the same flags (a changed -gencode rebuilds everything)
+    stamp = os.path.join(objdir, "flags.txt")
+    flags = "\n".join(" ".join(x) for x in (nvcc, cxx, defs, incf))
+    same_flags = os.path.exists(stamp) and open(stamp).read() == flags
     cmds, objs = [], []
     for s in sources:
         o = os.path.join(objdir, os.path.basename(s) + ".o")
         objs.append(o)
-        if os.path.exists(o) and os.path.getmtime(o) > os.path.getmtime(s):
+        if same_flags and os.path.exists(o) and os.path.getmtime(o) > os.path.getmtime(s):
             continue
         base = nvcc if s.endswith(".cu") else cxx
         cmds.append((s, base + defs + incf + ["-c", s, "-o", o]))
@@ -101,6 +105,8 @@ def main():
     if any(rcs):
         print("build_ref: compilation failed")
         return 1
+    with open(stamp, "w") as f:
+        f.write(flags)
     tlib = os.path.join(os.path.dirname(torch.__file__), "lib")
     out_lib = LIB
     link = ["/usr/bin/g++", "-shared", "-o", out_lib] + objs + [

@@ -5,7 +5,7 @@
  * reference algorithms (nerfstudio-project/gsplat v1.6.0, /root/reference/gsplat/cuda);
  * each function cites the file:line it follows.  Parity status: pinned against the
  * reference's own Python twins (_torch_impl.py / _math.py) through the committed
- * fixtures in tests/golden/ (generator: tests/golden/make_golden.py) -- see DESIGN.md.
+ * fixtures in tests/golden/ (generator: tests/golden/make_golden.py).
  *
  * Built by oracle/Makefile into oracle/libgs_oracle.so:
  *     gcc -O2 -fopenmp -ffp-contract=off -shared -fPIC gs_oracle.c -lm

@@ -36,7 +36,7 @@ def load_ops():
     if _loaded is None:
         so = PKG_SO if os.path.exists(PKG_SO) else BARE_SO
         if not os.path.exists(so):
-            raise FileNotFoundError("reference CUDA build missing: run python baseline/install_ref.py in the build container")
+            raise FileNotFoundError("reference CUDA build missing: run python oracle/build_ref.py where the reference sources are")
         torch.ops.load_library(so)
         _loaded = so
     return torch.ops.gsplat
@@ -46,7 +46,7 @@ def import_package():
     """``import gsplat`` = the unmodified reference package from baseline/_ref (stock path).  The nerfacc
     stand-in written by baseline/install_ref.py sits next to it."""
     if not package_available():
-        raise FileNotFoundError("baseline/_ref not installed: run python baseline/install_ref.py in the build container")
+        raise FileNotFoundError("reference package not installed in baseline/_ref (python baseline/install_ref.py, where the reference sources are)")
     load_ops()
     if PKG_DIR not in sys.path:
         sys.path.insert(0, PKG_DIR)

@@ -1,7 +1,7 @@
 """Deterministic scene builder shared by tests, bench.py and __graft_entry__.smoke().
 
 Restates the recipe of the reference's ``load_test_data`` (/root/reference/gsplat/_helper.py:51-102):
-the [-2,2]^3 crop of assets/test_garden.npz (committed as tests/golden/garden.npz), optionally
+the [-2,2]^3 crop of assets/test_garden.npz (committed as tests/golden/garden.npz + garden_means_tail.npz), optionally
 tiled ``scene_grid`` x ``scene_grid`` times, with random scales in [1e-4, 0.02], unit quaternions
 and opacities in [0,1).  Unlike the reference, the random attributes come from numpy's
 RandomState(seed) so that every machine (CPU container, GPU box) sees identical inputs.
@@ -18,8 +18,11 @@ SH_C0 = 0.28209479177387814
 
 
 def load_garden():
+    """The scene; its points are stored in two files of under 1 MB each (means rows split in halves)."""
     d = np.load(os.path.join(_GOLDEN, "garden.npz"))
-    return {k: d[k] for k in d.files}
+    out = {k: d[k] for k in d.files}
+    out["means"] = np.concatenate([out["means"], np.load(os.path.join(_GOLDEN, "garden_means_tail.npz"))["means"]])
+    return out
 
 
 def make_scene(scene_grid: int = 1, n_max: int | None = None, sh_degree: int = 3, seed: int = 42):

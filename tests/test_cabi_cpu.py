@@ -61,7 +61,7 @@ def test_host_only_entry_points():
     from gsplat_b200 import _cabi
 
     L = _cabi.lib()
-    assert b"sm_100a" in L.gsb200_version()
+    assert b"sm_90a" in L.gsb200_version()
 
 
 def test_shipped_binary_matches_the_sources():

@@ -1,6 +1,6 @@
 """GPU parity tests: every CUDA kernel, called through the C ABI / operator surface, against the CPU
 oracle (oracle/) on the same seeded inputs, and against the committed golden vectors produced by the
-reference's own Python twins (tests/golden/).  Run on the B200 box:  pytest -m gpu
+reference's own Python twins (tests/golden/).  Run on a GPU machine:  pytest -m gpu
 
 Tolerances (written here as the contract):
   * integer / index outputs (radii, tiles_per_gauss, isect_ids, flatten_ids, offsets): bit-exact
@@ -775,7 +775,10 @@ def test_full_size_properties_1080p(gs):
     v = torch.randn_like(rc)
     g1 = torch.autograd.grad((rc * v).sum(), t["sh"], retain_graph=True)[0]
     g2 = torch.autograd.grad((rc * (2 * v)).sum(), t["sh"], retain_graph=True)[0]
-    assert torch.allclose(g2, 2 * g1, rtol=1e-3, atol=1e-6)
+    # doubling the cotangent is exact, so only the order of the float atomics that add per-tile partial gradients
+    # separates g2 from 2 * g1: elementwise that is rounding noise (large relative to near-zero sums), in L2 it is tiny
+    rel = float((g2.double() - 2 * g1.double()).norm() / (2 * g1.double()).norm())
+    assert rel < 1e-5, f"backward not linear in the cotangent: rel L2 {rel:.3e}"
     # background only changes pixels by T * bg
     bg = torch.tensor([[0.2, 0.4, 0.6]], device=DEV)
     rc_bg, _, _ = gs.rasterization(*args, sh_degree=3, packed=False, backgrounds=bg)
@@ -904,7 +907,7 @@ def _torchrun2(script, port):
     import sys as _sys
 
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run under gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     root = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
     r = subprocess.run(
         [_sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",

@@ -3,7 +3,7 @@
 rasterization() + fused L1 + backward).  The step is GPU-bound only while the host can issue it faster than the GPU
 executes it; this prints the host's issue time per step next to the device time, and the top functions.
 
-    python tools/host_profile.py --steps 300 > gpurun_out/host_profile.txt
+    python tools/host_profile.py --steps 300 > out/host_profile.txt
 """
 import argparse
 import cProfile

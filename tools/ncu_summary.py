@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Summarises an .ncu-rep (read here with `ncu -i ... --page raw --csv`) into the markdown tables kept under
-profiles/, and prints the DRAM traffic of the compositing kernels for profiles/roofline_traffic.json.
+"""Summarises an .ncu-rep (read here with `ncu -i ... --page raw --csv`) into markdown tables, and prints
+the DRAM traffic of the compositing kernels (bench.py reads it from profiles/roofline_traffic.json when present).
 
-    python tools/ncu_summary.py gpurun_out/prof.ncu-rep profiles/r01_v6_ncu.md "title"
+    python tools/ncu_summary.py out/prof.ncu-rep out/ncu.md "title"
 """
 import csv
 import io

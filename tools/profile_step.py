@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """One bench.py-style train step of the BASELINE workload, for use under ncu:
 
-  ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv \
+  ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file out/launches.csv \
       python tools/profile_step.py --steps 2 --warmup 2
-  ncu --set full --clock-control none --import-source on -k regex:raster_bwd -s 2 -c 1 -o gpurun_out/prof_bwd \
+  ncu --set full --clock-control none --import-source on -k regex:raster_bwd -s 2 -c 1 -o out/prof_bwd \
       python tools/profile_step.py --steps 1 --warmup 2
 
 Numbers printed by a run under ncu are never bench values.  Also prints a CUDA-event breakdown per stage
@@ -99,6 +99,6 @@ if args.breakdown:
     ms_step, _ = t(step, 10)
     print("note: each stage below is timed by calling its operator back to back outside autograd (wide-key isect_tiles, per-intersection "
           "pack, no row records, host sync included): the stages do not add up to the step and are not what rasterization() runs since "
-          "round 2 -- use the ncu launch lists under profiles/ for shares of the real step")
+          "round 2 -- use an ncu launch list of the real step for its shares")
     print(f"BREAKDOWN ms: project_sh_fwd {ms_p:.3f} | isect(order+count+scan+sync+emit+sort) {ms_i:.3f} (unsorted {ms_in:.3f}) | offsets {ms_o:.3f} | "
           f"raster_fwd(pack+raster) {ms_r:.3f} | raster_bwd(+memset) {ms_rb:.3f} | project_sh_bwd {ms_pb:.3f} | full step {ms_step:.3f}")

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Per-kernel SASS mnemonic counts of the built objects (gsplat_b200/build/*.o) -- the evidence table for
-"what proves a Blackwell-native kernel" (B200_PROFILING.md): UBLKCP (1-D bulk TMA), SYNCS (mbarrier), REDG
+"""Per-kernel SASS mnemonic counts of the built objects (gsplat_b200/build/*.o) -- which Hopper
+features each kernel really uses: UBLKCP (1-D bulk TMA), SYNCS (mbarrier), REDG
 (incl. the 128-bit REDG.E.ADD.F32x4 of the version-2 backward), MUFU, SHFL, VOTE, LDGMC / multimem (NVLS), ...
 
-    python tools/sass_summary.py > profiles/r02_sass_summary.txt
+    python tools/sass_summary.py > out/sass_summary.txt
 """
 import collections
 import glob
@@ -17,7 +17,7 @@ KEYS = ["UBLKCP", "UTMALDG", "SYNCS", "REDG", "REDG.E.ADD.F32x4", "ATOMG", "ATOM
 
 
 def main():
-    print("# SASS mnemonic counts per kernel (cuobjdump -sass of gsplat_b200/build/*.o, sm_100a); total = instructions")
+    print("# SASS mnemonic counts per kernel (cuobjdump -sass of gsplat_b200/build/*.o, sm_90a); total = instructions")
     print("# kernel".ljust(72) + " total " + " ".join(k.rjust(7) for k in ("UBLKCP", "SYNCS", "REDG", "REDG.x4", "MUFU", "SHFL", "VOTE", "LDGMC", "LDL+STL")))
     for obj in sorted(glob.glob(os.path.join(ROOT, "gsplat_b200", "build", "*.o"))):
         txt = subprocess.run(["cuobjdump", "-sass", obj], capture_output=True, text=True).stdout
