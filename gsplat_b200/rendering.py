@@ -282,6 +282,10 @@ def rasterization(
                 raise ValueError(f"SH colors must be [N, K, D], got {tuple(colors.shape)}")
             if (sh_degree + 1) ** 2 > colors.shape[-2]:
                 raise ValueError(f"sh_degree={sh_degree} needs K >= {(sh_degree + 1) ** 2}, got {colors.shape[-2]}")
+            if colors.dtype in (torch.float16, torch.bfloat16):
+                # half-precision SH storage: evaluated in fp32 on every path (as ops.spherical_harmonics does); the
+                # cast is differentiable, so the gradient comes back in the storage dtype
+                colors = colors.float()
 
     antialiased = rasterize_mode == "antialiased"
 

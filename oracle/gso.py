@@ -323,53 +323,129 @@ def rasterize_to_pixels_bwd(
 
 
 # --------------------------------------------------------------------------
+RENDER_MODES = ("RGB", "D", "ED", "RGB+D", "RGB+ED")
+
+
 def rasterization_fwd_bwd(
     means, quats, scales, opacities, sh_coeffs, viewmats, Ks, width, height, sh_degree, v_render_colors,
     v_render_alphas, near_plane=0.01, far_plane=1e10, radius_clip=0.0, eps2d=0.3, tile_size=16, backgrounds=None,
+    *, covars=None, rasterize_mode="classic", render_mode="RGB", camera_model="pinhole", viewmats_requires_grad=False,
 ):
-    """The whole hot path on the CPU (dense, pinhole, RGB, SH colours, C cameras, B=1):
-    projection -> SH (+0.5, clamp at 0) -> isect -> offsets -> raster fwd -> raster bwd -> SH bwd ->
-    projection bwd.  Orchestration follows rendering._rasterization
-    (/root/reference/gsplat/rendering.py:722-1106).  Returns (fwd dict, grads dict)."""
+    """The whole hot path on the CPU, dense layout: projection -> colours -> isect -> offsets -> raster fwd ->
+    raster bwd -> colour bwd -> projection bwd.  Orchestration follows rendering._rasterization
+    (/root/reference/gsplat/rendering.py:722-1106) and gsplat_b200.rendering.rasterization.
+
+    means [..., N, 3] with optional leading batch dimensions, viewmats / Ks [..., C, 4, 4] / [..., C, 3, 3].
+    ``sh_coeffs`` is the SH table [N, K, 3] when ``sh_degree`` is set, else post-activation colours [..., N, D] or
+    [..., C, N, D]; None for ``render_mode`` "D" / "ED".  ``covars`` [..., N, 6] (triu) replaces quats / scales.
+    ``rasterize_mode="antialiased"`` composites ``opacities * compensations``; the depth modes append the depth channel
+    after the colours (background 0); "ED" / "RGB+ED" divide it by max(alpha, 1e-10).  ``v_render_colors`` is the
+    cotangent of the returned render (so of the normalised depth in the ED modes).  Returns (fwd dict, grads dict)."""
+    if render_mode not in RENDER_MODES:
+        raise ValueError(f"render_mode {render_mode!r}")
     dt = means.dtype
-    C, N = viewmats.shape[0], means.shape[0]
-    radii, means2d, depths, conics, _ = fully_fused_projection(
-        means, None, quats, scales, viewmats, Ks, width, height, eps2d, near_plane, far_plane, radius_clip,
-        False, "pinhole", opacities,
+    batch = means.shape[:-2]
+    C, N = viewmats.shape[-3], means.shape[-2]
+    I = int(np.prod(batch)) * C
+    has_color = render_mode in ("RGB", "RGB+D", "RGB+ED")
+    has_depth = render_mode != "RGB"
+    expected = render_mode in ("ED", "RGB+ED")
+    antialiased = rasterize_mode == "antialiased"
+    radii, means2d, depths, conics, comps = fully_fused_projection(
+        means, covars, quats, scales, viewmats, Ks, width, height, eps2d, near_plane, far_plane, radius_clip,
+        antialiased, camera_model, opacities,
     )
-    op_cn = np.ascontiguousarray(np.broadcast_to(opacities[None, :], (C, N)))
+    op_in = np.ascontiguousarray(np.broadcast_to(opacities[..., None, :], batch + (C, N)))
+    op_cn = op_in * comps if antialiased else op_in
     tw, th = math.ceil(width / tile_size), math.ceil(height / tile_size)
     tpg, isect_ids, flatten_ids = isect_tiles(
         means2d, radii, depths, tile_size, tw, th, True, conics, op_cn
     )
-    offsets = isect_offset_encode(isect_ids, C, tw, th)
+    offsets = isect_offset_encode(isect_ids, I, tw, th).reshape(batch + (C, th, tw))
     valid = (radii > 0).all(-1)
-    raw = spherical_harmonics(sh_degree, means, viewmats, sh_coeffs, valid)
-    colors = np.maximum(raw + dt.type(0.5), dt.type(0.0))
-    rc, ra, li, mg = rasterize_to_pixels(
-        means2d, conics, colors, op_cn, width, height, tile_size, offsets, flatten_ids, backgrounds, None, True
+    raw = None
+    if not has_color:
+        colors = depths[..., None]
+    elif sh_degree is not None:
+        raw = spherical_harmonics(sh_degree, means, viewmats, sh_coeffs, valid)
+        colors = np.maximum(raw + dt.type(0.5), dt.type(0.0))
+    else:
+        per_gauss = sh_coeffs.ndim == means.ndim  # [..., N, D] shared by the cameras, else [..., C, N, D]
+        colors = np.broadcast_to(sh_coeffs[..., None, :, :] if per_gauss else sh_coeffs, batch + (C, N, sh_coeffs.shape[-1]))
+    if has_color and has_depth:
+        colors = np.concatenate([colors, depths[..., None]], -1)
+    bg = backgrounds
+    if backgrounds is not None and has_depth:
+        bg = np.zeros(batch + (C, 1), dt)
+        if has_color:
+            bg = np.concatenate([backgrounds, bg], -1)
+    acc, ra, li, mg = rasterize_to_pixels(
+        means2d, conics, colors, op_cn, width, height, tile_size, offsets, flatten_ids, bg, None, True
     )
+    rc = acc
+    if expected:
+        rc = np.concatenate([acc[..., :-1], acc[..., -1:] / np.maximum(ra, 1e-10)], -1)
     fwd = dict(
         radii=radii, means2d=means2d, depths=depths, conics=conics, colors=colors, tiles_per_gauss=tpg,
         isect_ids=isect_ids, flatten_ids=flatten_ids, isect_offsets=offsets, render_colors=rc, render_alphas=ra,
-        last_ids=li, margins=mg, sh_raw=raw,
+        last_ids=li, margins=mg, sh_raw=raw, compensations=comps, opacities=op_cn,
     )
     if v_render_colors is None:
         return fwd, None
+    v_acc, v_ra = v_render_colors, v_render_alphas
+    if expected:
+        # d = acc / max(alpha, 1e-10): v_acc = v_d / max(alpha, 1e-10), v_alpha += -v_d acc / alpha^2 where alpha > 1e-10
+        v_d = v_render_colors[..., -1:]
+        live = ra > 1e-10
+        v_acc = np.concatenate([v_render_colors[..., :-1], v_d / np.maximum(ra, 1e-10)], -1)
+        v_ra = v_render_alphas - np.where(live, v_d * acc[..., -1:] / np.where(live, ra, 1.0) ** 2, 0.0)
     g = rasterize_to_pixels_bwd(
-        means2d, conics, colors, op_cn, width, height, tile_size, offsets, flatten_ids, ra, li, v_render_colors,
-        v_render_alphas, backgrounds,
+        means2d, conics, colors, op_cn, width, height, tile_size, offsets, flatten_ids, ra, li, v_acc,
+        v_ra, bg,
     )
-    v_colors = (g["v_colors"] * ((raw + dt.type(0.5)) > 0)).astype(dt)
-    v_coeffs, v_means_sh = spherical_harmonics_bwd(sh_degree, means, viewmats, sh_coeffs, valid, v_colors)
-    v_means, _, v_quats, v_scales, _ = fully_fused_projection_bwd(
-        means, None, quats, scales, viewmats, Ks, width, height, eps2d, radii, conics, None,
-        g["v_means2d"].astype(dt), np.zeros_like(depths), g["v_conics"].astype(dt),
+    grads = dict(raster=g)
+    v_feat = g["v_colors"]
+    v_depths = np.zeros_like(depths)
+    if has_depth:
+        v_depths = v_feat[..., -1].astype(dt)
+        v_feat = v_feat[..., :-1]
+    v_means_sh = 0
+    if has_color and sh_degree is not None:
+        v_colors = (v_feat * ((raw + dt.type(0.5)) > 0)).astype(dt)
+        v_coeffs, v_means_sh = spherical_harmonics_bwd(sh_degree, means, viewmats, sh_coeffs, valid, v_colors)
+        grads["v_sh"] = v_coeffs
+    elif has_color:
+        grads["v_colors"] = (v_feat.sum(-3) if per_gauss else v_feat).astype(dt)
+    v_op = g["v_opacities"]
+    v_comps = None
+    if antialiased:
+        v_comps = (v_op * op_in).astype(dt)
+        v_op = v_op * comps
+    v_means, v_covars, v_quats, v_scales, v_vm = fully_fused_projection_bwd(
+        means, covars, quats, scales, viewmats, Ks, width, height, eps2d, radii, conics, comps,
+        g["v_means2d"].astype(dt), v_depths, g["v_conics"].astype(dt), v_comps, viewmats_requires_grad, camera_model,
     )
-    grads = dict(
-        v_means=v_means + v_means_sh, v_quats=v_quats, v_scales=v_scales,
-        v_opacities=g["v_opacities"].sum(0).astype(dt), v_sh=v_coeffs, raster=g,
+    if viewmats_requires_grad and has_color and sh_degree is not None and sh_degree > 0:
+        # SH view direction dir = mean + R^T t: dL/dR = t S^T, dL/dt = R S with S = sum_n dL/ddir_n per image
+        mb, vmb = means.reshape((-1, N, 3)), viewmats.reshape((-1, C, 4, 4))
+        vcb, vab = v_colors.reshape((-1, C, N, 3)), valid.reshape((-1, C, N))
+        v_vm = v_vm.reshape((-1, C, 4, 4))
+        for b in range(vmb.shape[0]):
+            for c in range(C):
+                _, v_dir = spherical_harmonics_bwd(
+                    sh_degree, mb[b], vmb[b, c : c + 1], sh_coeffs, vab[b, c : c + 1], vcb[b, c : c + 1]
+                )
+                S = v_dir.sum(0)
+                R, t = vmb[b, c, :3, :3], vmb[b, c, :3, 3]
+                v_vm[b, c, :3, :3] += t[:, None] * S[None, :]
+                v_vm[b, c, :3, 3] += R @ S
+        v_vm = v_vm.reshape(viewmats.shape)
+    grads.update(
+        v_means=v_means + v_means_sh, v_quats=v_quats, v_scales=v_scales, v_covars=v_covars, v_viewmats=v_vm,
+        v_opacities=v_op.sum(-2).astype(dt), v_compensations=v_comps,
     )
+    if backgrounds is not None and has_color:
+        grads["v_backgrounds"] = g["v_backgrounds"][..., : backgrounds.shape[-1]].astype(dt)
     return fwd, grads
 
 

@@ -623,46 +623,111 @@ def test_raster_masks_and_empty(gs):
     rc.sum().backward()  # backward with n_isects == 0 must be a clean no-op
 
 
-def _pipeline_case(gs, sc, W, H, Ks, C, sh_degree, packed=False, **kw):
+def _pipeline_case(
+    gs, sc, W, H, Ks, C, sh_degree, packed=False, *, colors=None, covars=False, batch=0, viewmats_grad=False,
+    backgrounds=False, render_mode="RGB", camera_model="pinhole", oracle_dtype=np.float64, render_tol=(1e-4, 1e-5),
+    **kw,
+):
+    """rasterization() fwd + bwd on the GPU against the float64 oracle chain (gso.rasterization_fwd_bwd).
+
+    ``sh_degree=None`` renders ``colors`` (post-activation [N, D] / [C, N, D]) or, for render_mode "D" / "ED", no
+    colours; ``covars`` feeds the [N, 3, 3] covariances of the scene's quats / scales instead of them; ``batch=2``
+    adds a leading batch dimension whose element 1 is element 0 with its means shifted; ``viewmats_grad`` asks for
+    pose gradients; ``backgrounds`` adds random backgrounds.  ``kw`` goes to both sides (rasterize_mode, near_plane,
+    radius_clip, eps2d, ...).  ``oracle_dtype=np.float32`` compares against the float32 oracle instead (the fisheye
+    projection is not bit-compatible with the float64 one)."""
     c32 = lambda k: sc[k].astype(np.float32)  # noqa: E731
     vm = sc["viewmats"][:C]
-    K = (sh_degree + 1) ** 2
-    sh = np.ascontiguousarray(sc["sh"][:, :K])
+    Kc = Ks[:C]
+    P = {k: c32(k) for k in ("means", "quats", "scales", "opacities")}
+    if covars:
+        P["covars"] = gso.quat_scale_to_covar_preci(P.pop("quats"), P.pop("scales"), True, False, True)[0]
+    if batch:
+        # element b: the scene shifted by 0.05 b along x, seen by the same cameras
+        P = {k: np.stack([v + (np.float32(0.05 * b) * np.array([1, 0, 0], np.float32) if k == "means" else 0)
+                          for b in range(batch)]).astype(np.float32) for k, v in P.items()}
+        vm, Kc = np.stack([vm] * batch), np.stack([Kc] * batch)
+    lead = vm.shape[:-2]  # batch + (C,)
+    has_color = render_mode in ("RGB", "RGB+D", "RGB+ED")
+    has_depth = render_mode != "RGB"
+    expected = render_mode in ("ED", "RGB+ED")
+    if not has_color:
+        col, n_col = None, 0
+    elif sh_degree is None:
+        col, n_col = np.ascontiguousarray(colors, np.float32), colors.shape[-1]
+    else:
+        col, n_col = np.ascontiguousarray(sc["sh"][:, : (sh_degree + 1) ** 2]), 3
     rng = np.random.RandomState(11)
-    v_rc = rng.standard_normal((C, H, W, 3)).astype(np.float32)
-    v_ra = rng.standard_normal((C, H, W, 1)).astype(np.float32)
-    f64 = lambda a: a.astype(np.float64)  # noqa: E731
-    fwd, grads = gso.rasterization_fwd_bwd(
-        f64(c32("means")), f64(c32("quats")), f64(c32("scales")), f64(c32("opacities")), f64(sh), f64(vm), f64(Ks[:C]),
-        W, H, sh_degree, f64(v_rc), f64(v_ra), **kw,
-    )
-    tens = {k: _t(c32(k), True) for k in ("means", "quats", "scales", "opacities")}
-    tsh = _t(sh, True)
+    v_rc = rng.standard_normal(lead + (H, W, n_col + has_depth)).astype(np.float32)
+    v_ra = rng.standard_normal(lead + (H, W, 1)).astype(np.float32)
+    bg = rng.random_sample(lead[-1:] + (n_col,)).astype(np.float32) if backgrounds else None
+    if batch and bg is not None:
+        bg = np.stack([bg] * batch)
+    cast = lambda a: None if a is None else a.astype(oracle_dtype)  # noqa: E731
+    okw = dict(kw, covars=cast(P.get("covars")), render_mode=render_mode, camera_model=camera_model,
+               viewmats_requires_grad=viewmats_grad)
+    oargs = (cast(P["means"]), cast(P.get("quats")), cast(P.get("scales")), cast(P["opacities"]), cast(col), cast(vm),
+             cast(Kc), W, H, sh_degree)
+    alive = None
+    if expected:
+        # d(acc / alpha) / d alpha = -acc / alpha^2 is unbounded as alpha -> 0: a float32 alpha within its rounding of
+        # 1e-4 carries an arbitrary depth gradient.  The depth cotangent goes on pixels whose alpha is above 1e-2 only.
+        f0, _ = gso.rasterization_fwd_bwd(*oargs, None, None, backgrounds=cast(bg), **okw)
+        alive = f0["render_alphas"] > 1e-2
+        v_rc[..., -1:] *= alive
+    fwd, grads = gso.rasterization_fwd_bwd(*oargs, cast(v_rc), cast(v_ra), backgrounds=cast(bg), **okw)
+    tens = {k: _t(v, True) for k, v in P.items()}
+    if covars:
+        c6 = P["covars"]
+        full = np.stack([c6[..., [0, 1, 2]], c6[..., [1, 3, 4]], c6[..., [2, 4, 5]]], -2)
+        tens["covars"] = _t(full, True)
+    tcol = _t(col, True) if col is not None else None
+    tvm = _t(vm, viewmats_grad)
+    tbg = _t(bg, True) if bg is not None else None
     rc, ra, meta = gs.rasterization(
-        tens["means"], tens["quats"], tens["scales"], tens["opacities"], tsh, _t(vm), _t(Ks[:C]), W, H,
-        sh_degree=sh_degree, packed=packed, **kw,
+        tens["means"], tens.get("quats"), tens.get("scales"), tens["opacities"], tcol, tvm, _t(Kc), W, H,
+        sh_degree=sh_degree, packed=packed, covars=tens.get("covars"), backgrounds=tbg, render_mode=render_mode,
+        camera_model=camera_model, **kw,
     )
     ok = fwd["margins"] > 1e-4
     # the float32 projection can move a gaussian across a tile / cull boundary relative to float64; such
     # (rare) pixels show up as mismatches and are bounded, not excused: <= 0.05 % of pixels
-    err = np.abs(_n(rc).astype(np.float64) - fwd["render_colors"]) - (1e-4 * np.abs(fwd["render_colors"]) + 1e-5)
+    ref_rc, got_rc = fwd["render_colors"], _n(rc).astype(np.float64)
+    if expected:  # the expected depth divides by alpha: compared where the depth cotangent is (alpha > 1e-2)
+        keep_ch = np.concatenate([np.ones(ref_rc.shape[:-1] + (n_col,), bool), alive], -1)
+        ref_rc, got_rc = np.where(keep_ch, ref_rc, 0.0), np.where(keep_ch, got_rc, 0.0)
+    rtol, atol = render_tol
+    err = np.abs(got_rc - ref_rc) - (rtol * np.abs(ref_rc) + atol)
     bad = (err.max(-1) > 0) & ok
-    assert bad.mean() < 5e-4, f"{bad.mean() * 100:.4f}% of non-marginal pixels exceed rtol 1e-4 / atol 1e-5"
-    assert np.abs(_n(rc) - fwd["render_colors"]).max() < 5e-2
+    assert bad.mean() < 5e-4, f"{bad.mean() * 100:.4f}% of non-marginal pixels exceed rtol {rtol} / atol {atol}"
+    assert np.abs(got_rc - ref_rc).max() < 5e-2
     loss = (rc * _t(v_rc)).sum() + (ra * _t(v_ra)).sum()
     meta["means2d"].retain_grad()
     loss.backward()
-    for k, ok_rel in (("means", 2e-3), ("quats", 2e-3), ("scales", 2e-3), ("opacities", 1e-3)):
+    checks = [("means", 2e-3), ("opacities", 1e-3)]
+    checks += [("covars", 1e-3)] if covars else [("quats", 2e-3), ("scales", 2e-3)]
+    for k, ok_rel in checks:
         a, ref = _n(tens[k].grad), grads["v_" + k]
+        if k == "covars":  # the [N, 3, 3] input is read through its upper triangle
+            a = a[..., [0, 0, 0, 1, 1, 2], [0, 1, 2, 1, 2, 2]]
         rel = np.linalg.norm(a - ref) / np.linalg.norm(ref)
         assert rel < ok_rel, f"v_{k}: relative L2 error vs float64 oracle {rel:.3e}"
-    # SH colours pass through max(x + 0.5, 0): gaussians whose pre-activation value sits on the kink
-    # (|x + 0.5| < 1e-5 in any view / channel -- e.g. pure black points at SH degree 0) legitimately get
-    # either sub-gradient depending on float32 rounding and are excluded, like marginal pixels
-    kink = (np.abs(fwd["sh_raw"] + 0.5) < 1e-5).any(axis=(0, 2))
-    a, ref = _n(tsh.grad)[~kink], grads["v_sh"][~kink]
-    rel = np.linalg.norm(a - ref) / np.linalg.norm(ref)
-    assert kink.mean() < 0.2 and rel < 1e-3, f"v_sh: relative L2 error {rel:.3e} (kink fraction {kink.mean():.3f})"
+    if has_color and sh_degree is not None:
+        # SH colours pass through max(x + 0.5, 0): gaussians whose pre-activation value sits on the kink
+        # (|x + 0.5| < 1e-5 in any view / channel -- e.g. pure black points at SH degree 0) legitimately get
+        # either sub-gradient depending on float32 rounding and are excluded, like marginal pixels
+        raw = fwd["sh_raw"]
+        kink = (np.abs(raw + 0.5) < 1e-5).any(axis=tuple(range(raw.ndim - 2)) + (raw.ndim - 1,))
+        a, ref = _n(tcol.grad)[~kink], grads["v_sh"][~kink]
+        rel = np.linalg.norm(a - ref) / np.linalg.norm(ref)
+        assert kink.mean() < 0.2 and rel < 1e-3, f"v_sh: relative L2 error {rel:.3e} (kink fraction {kink.mean():.3f})"
+    others = [(tcol, "v_colors")] if has_color and sh_degree is None else []
+    others += [(tvm, "v_viewmats")] if viewmats_grad else []
+    others += [(tbg, "v_backgrounds")] if bg is not None else []
+    for t, key in others:
+        a, ref = _n(t.grad), grads[key]
+        rel = np.linalg.norm(a - ref) / np.linalg.norm(ref)
+        assert rel < 1e-3, f"{key}: relative L2 error vs float64 oracle {rel:.3e}"
     assert meta["means2d"].grad is not None and meta["means2d"].grad.abs().sum() > 0
     return rc, ra, meta, fwd
 
