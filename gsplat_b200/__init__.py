@@ -2,19 +2,23 @@
 
 Public names mirror /root/reference/gsplat/__init__.py:19-104 for the hot path:
 rasterization, fully_fused_projection, spherical_harmonics, isect_tiles, isect_offset_encode,
-rasterize_to_pixels, quat_scale_to_covar_preci.  Importing the package does not need a GPU; calling an
+rasterize_to_pixels, quat_scale_to_covar_preci, and the sparse-pixel ops build_sparse_tile_layout,
+isect_tiles_sparse, rasterize_to_pixels_sparse.  Importing the package does not need a GPU; calling an
 operator does (and needs gsplat_b200/libgsplat_b200.so, built by ``python -m gsplat_b200.build``).
 """
 from .ops import (  # noqa: F401
     adam,
+    build_sparse_tile_layout,
     compute_relocation,
     mcmc_perturb_positions,
     fully_fused_projection,
     fused_project_sh,
     isect_offset_encode,
     isect_tiles,
+    isect_tiles_sparse,
     quat_scale_to_covar_preci,
     rasterize_to_pixels,
+    rasterize_to_pixels_sparse,
     spherical_harmonics,
 )
 from .losses import l1_loss, ssim_loss  # noqa: F401
@@ -65,6 +69,9 @@ __all__ = [
     "isect_tiles",
     "isect_offset_encode",
     "rasterize_to_pixels",
+    "build_sparse_tile_layout",
+    "isect_tiles_sparse",
+    "rasterize_to_pixels_sparse",
     "quat_scale_to_covar_preci",
     "compute_relocation",
     "mcmc_perturb_positions",

@@ -139,6 +139,28 @@ _SIGNATURES = {
         [c_i64, c_i64, c_int, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
          c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp],
     ),
+    "gsb200_sparse_layout_workspace_bytes": (c_sz, [c_i64, c_i64, c_u32, c_u32]),
+    "gsb200_sparse_layout_sort": (c_int, [c_i64, c_vp, c_vp, c_i64, c_u32, c_u32, c_u32, c_vp, c_sz, c_vp, c_vp]),
+    "gsb200_sparse_layout_finish": (c_int, [c_i64, c_i64, c_u32, c_u32, c_i64, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "gsb200_isect_sparse_count_workspace_bytes": (c_sz, [c_i64, c_i64]),
+    "gsb200_isect_sparse_count": (
+        c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp, c_sz, c_vp],
+    ),
+    "gsb200_isect_sparse_emit_workspace_bytes": (c_sz, [c_i64, c_i64, c_u32, c_u32]),
+    "gsb200_isect_sparse_emit": (
+        c_int,
+        [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp],
+    ),
+    "gsb200_raster_sparse_fwd": (
+        c_int,
+        [c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp,
+         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    ),
+    "gsb200_raster_sparse_bwd": (
+        c_int,
+        [c_i64, c_int, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
+         c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp],
+    ),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -1846,6 +1846,233 @@ extern "C" int gsb200_isect_emit(
     return check_launch();
 }
 
+// ---- tile intersection restricted to the tiles of a mask (isect_tiles_sparse).  Same enumeration as the dense AABB
+// path (tiles_of_gaussian without conics), in the depth order of gsb200_isect_depth_order; a tile whose tile_mask entry
+// is 0 is neither counted nor emitted.  Keys are dense tile ids image * th * tw + tile (32 bits).
+namespace gsb
+{
+__device__ __forceinline__ int64_t masked_row_image(int64_t i, int64_t N, const int64_t *__restrict__ image_ids)
+{
+    return image_ids ? image_ids[i] : i / N;
+}
+
+__global__ void __launch_bounds__(kThreads) isect_count_masked_kernel(
+    int64_t total, int64_t N, int64_t I, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
+    const int64_t *__restrict__ image_ids, const uint8_t *__restrict__ tile_mask, const int32_t *__restrict__ order,
+    uint32_t tile_size, uint32_t tw, uint32_t th, int32_t *__restrict__ counts_in_order
+)
+{
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(j >= total)
+        return;
+    const int64_t i = order[j];
+    const int2 r    = reinterpret_cast<const int2 *>(radii)[i];
+    int cnt         = 0;
+    const int64_t img = masked_row_image(i, N, image_ids);
+    if(r.x > 0 && r.y > 0 && img >= 0 && img < I)
+    {
+        const float2 m     = reinterpret_cast<const float2 *>(means2d)[i];
+        const uint8_t *tm  = tile_mask + img * (int64_t)tw * th;
+        tiles_of_gaussian(m.x, m.y, r.x, r.y, nullptr, nullptr, tile_size, tw, th, [&](int64_t t) { cnt += tm[t] != 0; });
+    }
+    counts_in_order[j] = cnt;
+}
+
+__global__ void __launch_bounds__(kThreads) isect_emit_masked_kernel(
+    int64_t total, int64_t N, int64_t I, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
+    const int64_t *__restrict__ image_ids, const uint8_t *__restrict__ tile_mask, const int32_t *__restrict__ order,
+    const int64_t *__restrict__ cum_tiles, uint32_t tile_size, uint32_t tw, uint32_t th, uint32_t *__restrict__ keys,
+    int32_t *__restrict__ flatten_ids
+)
+{
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(j >= total)
+        return;
+    int64_t cur       = j == 0 ? 0 : cum_tiles[j - 1];
+    const int64_t end = cum_tiles[j];
+    if(end == cur)
+        return;
+    const int64_t i   = order[j];
+    const int2 r      = reinterpret_cast<const int2 *>(radii)[i];
+    const float2 m    = reinterpret_cast<const float2 *>(means2d)[i];
+    const int64_t img = masked_row_image(i, N, image_ids);
+    const uint8_t *tm = tile_mask + img * (int64_t)tw * th;
+    const uint32_t base = (uint32_t)(img * (int64_t)tw * th);
+    tiles_of_gaussian(m.x, m.y, r.x, r.y, nullptr, nullptr, tile_size, tw, th, [&](int64_t t) {
+        if(tm[t] != 0 && cur < end)
+        {
+            keys[cur]        = base + (uint32_t)t;
+            flatten_ids[cur] = (int32_t)i;
+            ++cur;
+        }
+    });
+}
+
+// tile_offsets[a] = first sorted intersection of active tile a (lower bound of its id in the sorted keys), a < AT;
+// tile_offsets[AT] = n_isects
+__global__ void __launch_bounds__(kThreads) isect_offsets_sparse_kernel(
+    int64_t n_active, const int32_t *__restrict__ active_tiles, int64_t n_isects, const uint32_t *__restrict__ keys,
+    int32_t *__restrict__ tile_offsets
+)
+{
+    const int64_t a = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(a > n_active)
+        return;
+    if(a == n_active)
+    {
+        tile_offsets[a] = (int32_t)n_isects;
+        return;
+    }
+    const uint32_t t = (uint32_t)active_tiles[a];
+    int64_t lo = 0, hi = n_isects;
+    while(lo < hi)
+    {
+        const int64_t mid = (lo + hi) >> 1;
+        if(keys[mid] < t)
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    tile_offsets[a] = (int32_t)lo;
+}
+
+struct SparseCountLayout
+{
+    size_t depth, counts, scan, total;
+};
+static SparseCountLayout sparse_count_layout(int64_t I, int64_t total)
+{
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    SparseCountLayout L;
+    size_t scan = 0;
+    cub::DeviceScan::InclusiveSum((void *)nullptr, scan, (const int32_t *)nullptr, (int64_t *)nullptr, total);
+    L.depth  = 0;
+    L.counts = L.depth + al(gsb200_isect_depth_order_workspace_bytes(I, total));
+    L.scan   = L.counts + al(sizeof(int32_t) * (size_t)total);
+    L.total  = L.scan + al(scan) + 256;
+    return L;
+}
+
+struct SparseEmitLayout
+{
+    size_t keys_in, vals_in, keys_out, sort, total;
+};
+static SparseEmitLayout sparse_emit_layout(int64_t n_isects, int end_bit)
+{
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    SparseEmitLayout L;
+    L.keys_in  = 0;
+    L.vals_in  = L.keys_in + al(sizeof(uint32_t) * (size_t)n_isects);
+    L.keys_out = L.vals_in + al(sizeof(int32_t) * (size_t)n_isects);
+    L.sort     = L.keys_out + al(sizeof(uint32_t) * (size_t)n_isects);
+    L.total    = L.sort + al(gsb200_sort_tile_pairs_workspace_bytes(n_isects, 4, end_bit)) + 256;
+    return L;
+}
+
+static int sparse_isect_args(int64_t I, int64_t N, const int64_t *image_ids, uint32_t tile_size, uint32_t tw, uint32_t th, int64_t &total)
+{
+    if(I < 0 || N < 0 || tile_size == 0)
+        return GSB200_E_INVALID;
+    total = image_ids ? N : I * N; // packed: N rows, image_ids[i] in [0, I)
+    if(total > 0x7fffffffLL)
+        return GSB200_E_INVALID;
+    if(bits_for_count(I) + bits_for_count((int64_t)tw * th) > 32)
+        return GSB200_E_KEYBITS;
+    return GSB200_OK;
+}
+} // namespace gsb
+
+extern "C" size_t gsb200_isect_sparse_count_workspace_bytes(int64_t I, int64_t total_rows)
+{
+    if(I <= 0 || total_rows <= 0)
+        return 0;
+    return gsb::sparse_count_layout(I, total_rows).total;
+}
+
+extern "C" int gsb200_isect_sparse_count(
+    int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const int64_t *image_ids,
+    const uint8_t *tile_mask, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *order,
+    int64_t *cum_tiles, void *workspace, size_t workspace_bytes, void *stream
+)
+{
+    int64_t total = 0;
+    if(int rc = gsb::sparse_isect_args(I, N, image_ids, tile_size, tile_width, tile_height, total))
+        return rc;
+    if(total == 0)
+        return GSB200_OK;
+    if(!means2d || !radii || !depths || !tile_mask || !order || !cum_tiles || !workspace)
+        return GSB200_E_INVALID;
+    const auto L = gsb::sparse_count_layout(I, total);
+    if(L.total > workspace_bytes)
+        return GSB200_E_WORKSPACE;
+    char *ws        = static_cast<char *>(workspace);
+    cudaStream_t st = (cudaStream_t)stream;
+    // 1. rows in (image, depth) order
+    if(int rc = gsb200_isect_depth_order(I, N, radii, depths, image_ids, order, ws + L.depth, L.counts - L.depth, stream))
+        return rc;
+    // 2. masked tile counts in that order; 3. inclusive scan
+    int32_t *counts = reinterpret_cast<int32_t *>(ws + L.counts);
+    gsb::isect_count_masked_kernel<<<gsb::grid_for(total, gsb::kThreads), gsb::kThreads, 0, st>>>(
+        total, N, I, means2d, radii, image_ids, tile_mask, order, tile_size, tile_width, tile_height, counts
+    );
+    if(int rc = gsb::check_launch())
+        return rc;
+    size_t scan_bytes = L.total - L.scan;
+    GSB_CUDA_TRY(cub::DeviceScan::InclusiveSum(ws + L.scan, scan_bytes, counts, cum_tiles, total, st));
+    return GSB200_OK;
+}
+
+extern "C" size_t gsb200_isect_sparse_emit_workspace_bytes(int64_t I, int64_t n_isects, uint32_t tile_width, uint32_t tile_height)
+{
+    if(I <= 0 || n_isects <= 0)
+        return 0;
+    const int end_bit = (int)gsb::bits_for_count(I * (int64_t)tile_width * tile_height);
+    return gsb::sparse_emit_layout(n_isects, end_bit > 0 ? end_bit : 1).total;
+}
+
+extern "C" int gsb200_isect_sparse_emit(
+    int64_t I, int64_t N, const float *means2d, const int32_t *radii, const int64_t *image_ids, const uint8_t *tile_mask,
+    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *order, const int64_t *cum_tiles,
+    int64_t n_isects, int64_t n_active, const int32_t *active_tiles, int32_t *tile_offsets, int32_t *flatten_ids,
+    void *workspace, size_t workspace_bytes, void *stream
+)
+{
+    int64_t total = 0;
+    if(int rc = gsb::sparse_isect_args(I, N, image_ids, tile_size, tile_width, tile_height, total))
+        return rc;
+    if(n_isects < 0 || n_isects > 0x7fffffffLL || n_active < 0 || !tile_offsets || (n_active > 0 && !active_tiles))
+        return GSB200_E_INVALID;
+    cudaStream_t st = (cudaStream_t)stream;
+    const uint32_t *sorted = nullptr;
+    if(n_isects > 0)
+    {
+        if(total == 0 || !means2d || !radii || !tile_mask || !order || !cum_tiles || !flatten_ids || !workspace)
+            return GSB200_E_INVALID;
+        int end_bit  = (int)gsb::bits_for_count(I * (int64_t)tile_width * tile_height);
+        end_bit      = end_bit > 0 ? end_bit : 1;
+        const auto L = gsb::sparse_emit_layout(n_isects, end_bit);
+        if(L.total > workspace_bytes)
+            return GSB200_E_WORKSPACE;
+        char *ws          = static_cast<char *>(workspace);
+        uint32_t *keys_in = reinterpret_cast<uint32_t *>(ws + L.keys_in), *keys_out = reinterpret_cast<uint32_t *>(ws + L.keys_out);
+        int32_t *vals_in  = reinterpret_cast<int32_t *>(ws + L.vals_in);
+        // 4. emission in depth order; 5. stable sort on the (image, tile) bits
+        gsb::isect_emit_masked_kernel<<<gsb::grid_for(total, gsb::kThreads), gsb::kThreads, 0, st>>>(
+            total, N, I, means2d, radii, image_ids, tile_mask, order, cum_tiles, tile_size, tile_width, tile_height, keys_in, vals_in
+        );
+        if(int rc = gsb::check_launch())
+            return rc;
+        if(int rc = gsb200_sort_tile_pairs(n_isects, 4, end_bit, keys_in, vals_in, keys_out, flatten_ids, ws + L.sort, L.total - L.sort, stream))
+            return rc;
+        sorted = keys_out;
+    }
+    // 6. per-active-tile offsets from the sorted keys
+    gsb::isect_offsets_sparse_kernel<<<gsb::grid_for(n_active + 1, gsb::kThreads), gsb::kThreads, 0, st>>>(
+        n_active, active_tiles, n_isects, sorted, tile_offsets
+    );
+    return gsb::check_launch();
+}
+
 extern "C" int gsb200_isect_count_totals(
     int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *conics, const float *opacities,
     uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *tiles_per_gauss, int64_t *totals, void *stream

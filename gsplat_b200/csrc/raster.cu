@@ -186,9 +186,8 @@ struct TileGeom
     int image_id, tile_id, tile_x, tile_y;
 };
 
-__device__ __forceinline__ TileGeom decode_tile(const int32_t *__restrict__ order, uint32_t tw, uint32_t th)
+__device__ __forceinline__ TileGeom decode_block(const uint32_t block, uint32_t tw, uint32_t th)
 {
-    const uint32_t block = order ? (uint32_t)order[blockIdx.x] : blockIdx.x;
     TileGeom t;
     const uint32_t per = tw * th;
     t.image_id         = block / per;
@@ -196,6 +195,65 @@ __device__ __forceinline__ TileGeom decode_tile(const int32_t *__restrict__ orde
     t.tile_x           = t.tile_id % tw;
     t.tile_y           = t.tile_id / tw;
     return t;
+}
+
+__device__ __forceinline__ TileGeom decode_tile(const int32_t *__restrict__ order, uint32_t tw, uint32_t th)
+{
+    return decode_block(order ? (uint32_t)order[blockIdx.x] : blockIdx.x, tw, th);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Pixel addressing of the compositing kernels, a compile-time policy.
+//  DensePixels: one CTA per tile of the [I, th, tw] grid; offsets [I * th * tw] (the last range ends at n_isects); the
+//    pixel (x, y) of image i is live when it lies inside the W x H image and is stored at (i * H + y) * W + x.
+//  SparsePixels: one CTA per ACTIVE tile ord (rasterize_to_pixels_sparse); the tile is active_tiles[ord], its list is
+//    offsets[ord] .. offsets[ord + 1], and a pixel is live when its bit in the tile's raster-order mask is set.  Its
+//    output slot is pixel_map[start + rank], start = the live pixels of the tiles before (inclusive cumsum[ord - 1])
+//    and rank = the live pixels before it in the tile.  Live margin pixels of a partial tile are rendered too.
+struct DensePixels
+{
+    static constexpr bool kSparse = false;
+};
+
+struct SparsePixels
+{
+    static constexpr bool kSparse = true;
+    const int32_t *active_tiles;      // [AT] dense tile ids image * th * tw + ty * tw + tx, ascending
+    const uint64_t *tile_pixel_mask;  // [AT, 4] bit (y % 16) * 16 + x % 16 of word >> 6
+    const int64_t *tile_pixel_cumsum; // [AT] inclusive prefix sum of the live pixels per tile
+    const int64_t *pixel_map;         // [P] (tile, in-tile) order -> output row
+
+    // output row of in-tile position `pos` of active tile `ord`; live = false (and row 0) if the pixel was not requested
+    __device__ __forceinline__ int64_t slot(const uint32_t ord, const int pos, bool &live) const
+    {
+        const uint64_t *words = tile_pixel_mask + (size_t)ord * 4;
+        const int w = pos >> 6, bit = pos & 63;
+        const uint64_t mw = words[w];
+        live = ((mw >> bit) & 1ull) != 0ull;
+        if(!live)
+            return 0;
+        int rank = __popcll(mw & ((1ull << bit) - 1ull));
+        for(int q = 0; q < w; ++q)
+            rank += __popcll(words[q]);
+        const int64_t start = ord == 0 ? 0 : tile_pixel_cumsum[ord - 1];
+        return pixel_map[start + rank];
+    }
+};
+
+// tile of this CTA; ord = its position in the launch's tile list (the block index after the tile order)
+template<class Pix>
+__device__ __forceinline__ TileGeom block_tile(const int32_t *__restrict__ order, uint32_t tw, uint32_t th, const Pix &pm, uint32_t &ord)
+{
+    if constexpr(Pix::kSparse)
+    {
+        ord = order ? (uint32_t)order[blockIdx.x] : blockIdx.x;
+        return decode_block((uint32_t)pm.active_tiles[ord], tw, th);
+    }
+    else
+    {
+        ord = 0;
+        return decode_tile(order, tw, th);
+    }
 }
 
 // the axis stream lies between the cull and geom streams, equally sized: midpoint of the two pointers
@@ -270,13 +328,13 @@ __device__ __forceinline__ bool block_may_touch(const float4 q, const float4 ax,
 // early exit of the barrier version).
 constexpr int kPipeStages = 3;
 
-template<int CDIM, bool PIPE = false>
+template<int CDIM, bool PIPE = false, class Pix = DensePixels>
 __global__ void __launch_bounds__(kWarps * 32) raster_fwd_kernel(
     const uint32_t I, const int64_t n_isects, const float4 *__restrict__ gcull, const float4 *__restrict__ ggeom,
     const float4 *__restrict__ gcolor, const int32_t *__restrict__ order, const float *__restrict__ backgrounds,
     const uint8_t *__restrict__ masks, const uint32_t W, const uint32_t H, const uint32_t tw, const uint32_t th,
     const int32_t *__restrict__ offsets, float *__restrict__ render_colors, float *__restrict__ render_alphas,
-    int32_t *__restrict__ last_ids
+    int32_t *__restrict__ last_ids, const Pix pixmap = Pix{}
 )
 {
     constexpr int CV = RecLayout<CDIM>::kColorVec4;
@@ -289,7 +347,8 @@ __global__ void __launch_bounds__(kWarps * 32) raster_fwd_kernel(
     __shared__ int32_t s_cnt[kPipeStages]; // PIPE: warps that are through with the stage's current batch
     __shared__ int32_t s_alive;            // PIPE: warps with an unsaturated pixel
     __shared__ int32_t s_stop;             // PIPE: first batch that will not be fetched (read and written with atomics only)
-    const TileGeom tg   = decode_tile(order, tw, th);
+    uint32_t ord;
+    const TileGeom tg   = block_tile(order, tw, th, pixmap, ord);
     const unsigned tid  = threadIdx.x;
     const unsigned warp = tid >> 5, lane = tid & 31;
     int32_t *surv       = s_surv[warp];
@@ -299,8 +358,15 @@ __global__ void __launch_bounds__(kWarps * 32) raster_fwd_kernel(
     const int by0 = tg.tile_y * kTile + (warp >> 1) * 4;
     const int px_i = bx0 + (lane & 7), py_i = by0 + (lane >> 3);
     const float px = (float)px_i + 0.5f, py = (float)py_i + 0.5f;
-    const bool inside = (px_i < (int)W) && (py_i < (int)H);
-    const int64_t pix = ((int64_t)tg.image_id * H + py_i) * W + px_i;
+    bool inside;
+    int64_t pix;
+    if constexpr(Pix::kSparse)
+        pix = pixmap.slot(ord, (int)(((warp >> 1) * 4 + (lane >> 3)) * kTile + (warp & 1) * 8 + (lane & 7)), inside);
+    else
+    {
+        inside = (px_i < (int)W) && (py_i < (int)H);
+        pix    = ((int64_t)tg.image_id * H + py_i) * W + px_i;
+    }
     const float *bg   = backgrounds ? backgrounds + (size_t)tg.image_id * CDIM : nullptr;
 
     const int64_t tile_lin = (int64_t)tg.image_id * tw * th + tg.tile_id;
@@ -317,8 +383,17 @@ __global__ void __launch_bounds__(kWarps * 32) raster_fwd_kernel(
         return;
     }
 
-    const int32_t range_start = offsets[tile_lin];
-    const int32_t range_end   = (tile_lin == (int64_t)I * tw * th - 1) ? (int32_t)n_isects : offsets[tile_lin + 1];
+    int32_t range_start, range_end;
+    if constexpr(Pix::kSparse)
+    {
+        range_start = offsets[ord];
+        range_end   = offsets[ord + 1];
+    }
+    else
+    {
+        range_start = offsets[tile_lin];
+        range_end   = (tile_lin == (int64_t)I * tw * th - 1) ? (int32_t)n_isects : offsets[tile_lin + 1];
+    }
     const int num_batches     = (range_end - range_start + kBatch - 1) / kBatch;
 
     if(tid == 0)
@@ -815,14 +890,14 @@ __device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float 
 // the bulk copies of the batch three ahead.  Warps of a tile differ a lot in survivors per 64-record batch, and with
 // two CTA barriers per batch every warp ran at the pace of the slowest one.  The gaussian ids are read from global
 // memory when a survivor's data is materialised (no per-batch staging, hence no barrier for it either).
-template<int CDIM, bool ABS, int MINB, bool PIPE = false>
+template<int CDIM, bool ABS, int MINB, bool PIPE = false, class Pix = DensePixels>
 __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
     const uint32_t I, const int64_t n_isects, const float4 *__restrict__ gcull, const float4 *__restrict__ ggeom,
     const float4 *__restrict__ gcolor, const int32_t *__restrict__ order, const int32_t *__restrict__ flatten_ids,
     const float *__restrict__ backgrounds, const uint8_t *__restrict__ masks, const uint32_t W, const uint32_t H,
     const uint32_t tw, const uint32_t th, const int32_t *__restrict__ offsets, const float *__restrict__ render_alphas,
     const int32_t *__restrict__ last_ids, const float *__restrict__ v_render_colors,
-    const float *__restrict__ v_render_alphas, const GradDst dst, const uint32_t packed_stride
+    const float *__restrict__ v_render_alphas, const GradDst dst, const uint32_t packed_stride, const Pix pixmap = Pix{}
 )
 {
     constexpr int CV  = RecLayout<CDIM>::kColorVec4;
@@ -836,14 +911,24 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
     __shared__ int32_t s_tile_bin;
     __shared__ int32_t s_done[kPipeStages]; // PIPE: warps that have finished with the stage's current batch
 
-    const TileGeom tg      = decode_tile(order, tw, th);
+    uint32_t ord;
+    const TileGeom tg      = block_tile(order, tw, th, pixmap, ord);
     const unsigned tid     = threadIdx.x;
     const unsigned warp    = tid >> 5, lane = tid & 31;
     const int64_t tile_lin = (int64_t)tg.image_id * tw * th + tg.tile_id;
     if(masks != nullptr && !masks[tile_lin])
         return;
-    const int32_t range_start = offsets[tile_lin];
-    const int32_t range_end0  = (tile_lin == (int64_t)I * tw * th - 1) ? (int32_t)n_isects : offsets[tile_lin + 1];
+    int32_t range_start, range_end0;
+    if constexpr(Pix::kSparse)
+    {
+        range_start = offsets[ord];
+        range_end0  = offsets[ord + 1];
+    }
+    else
+    {
+        range_start = offsets[tile_lin];
+        range_end0  = (tile_lin == (int64_t)I * tw * th - 1) ? (int32_t)n_isects : offsets[tile_lin + 1];
+    }
     if(range_end0 <= range_start)
         return;
 
@@ -851,8 +936,15 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
     const int by0 = tg.tile_y * kTile + (warp >> 1) * 4;
     const int px_i = bx0 + (lane & 7), py_i = by0 + (lane >> 3);
     const float px = (float)px_i + 0.5f, py = (float)py_i + 0.5f;
-    const bool inside = (px_i < (int)W) && (py_i < (int)H);
-    const int64_t pix = inside ? ((int64_t)tg.image_id * H + py_i) * W + px_i : 0;
+    bool inside;
+    int64_t pix;
+    if constexpr(Pix::kSparse)
+        pix = pixmap.slot(ord, (int)(((warp >> 1) * 4 + (lane >> 3)) * kTile + (warp & 1) * 8 + (lane & 7)), inside);
+    else
+    {
+        inside = (px_i < (int)W) && (py_i < (int)H);
+        pix    = inside ? ((int64_t)tg.image_id * H + py_i) * W + px_i : 0;
+    }
     const float *bg   = backgrounds ? backgrounds + (size_t)tg.image_id * CDIM : nullptr;
 
     const float T_final = inside ? 1.0f - render_alphas[pix] : 1.f;
@@ -1286,6 +1378,20 @@ static int launch_fwd(
     return check_launch();
 }
 
+// Are the five gradient destinations one packed, 16-byte aligned record [v_xy 2 | v_conic 3 | v_opacity 1 | v_rgb D | abs 2]
+// per gaussian?  Its stride in floats if so (raster_bwd2_kernel then adds with 128-bit REDs), else 0.
+template<int CDIM>
+static uint32_t packed_grad_stride(const GradDst &dst)
+{
+    const bool absg = dst.abs != nullptr;
+    const int64_t P = dst.s_means2d;
+    if(P > 0 && (P % 4) == 0 && P >= 6 + CDIM + (absg ? 2 : 0) && dst.s_conics == P && dst.s_colors == P && dst.s_opacities == P
+       && dst.conics == dst.means2d + 2 && dst.opacities == dst.means2d + 5 && dst.colors == dst.means2d + 6
+       && (!absg || (dst.s_abs == P && dst.abs == dst.means2d + 6 + CDIM)) && (reinterpret_cast<uintptr_t>(dst.means2d) & 15) == 0)
+        return (uint32_t)P;
+    return 0;
+}
+
 template<int CDIM>
 static int launch_bwd(
     int64_t I, const float *backgrounds, const uint8_t *masks, uint32_t W, uint32_t H, uint32_t tw, uint32_t th,
@@ -1307,13 +1413,7 @@ static int launch_bwd(
     }();
     if(use_v2)
     {
-        // are the five destinations one packed, 16-byte aligned record [v_xy 2 | v_conic 3 | v_opacity 1 | v_rgb D | abs 2]?
-        const int64_t P  = dst.s_means2d;
-        uint32_t packed  = 0;
-        if(P > 0 && (P % 4) == 0 && P >= 6 + CDIM + (absg ? 2 : 0) && dst.s_conics == P && dst.s_colors == P && dst.s_opacities == P
-           && dst.conics == dst.means2d + 2 && dst.opacities == dst.means2d + 5 && dst.colors == dst.means2d + 6
-           && (!absg || (dst.s_abs == P && dst.abs == dst.means2d + 6 + CDIM)) && (reinterpret_cast<uintptr_t>(dst.means2d) & 15) == 0)
-            packed = (uint32_t)P;
+        const uint32_t packed = packed_grad_stride<CDIM>(dst);
         // GSB200_BWD_PIPE=0 keeps the two CTA barriers per batch (measurements); default: barrier-free ring
         static const bool pipe = [] {
             const char *e = std::getenv("GSB200_BWD_PIPE");
@@ -1405,6 +1505,60 @@ static int launch_bwd(
     }
 #undef GSB_BWD_LAUNCH
     return check_launch();
+}
+
+// ---------------------------------------------------------------------------------------------
+// sparse pixels (rasterize_to_pixels_sparse): the same pack pass, tile order and kernels as the dense path, one CTA per
+// active tile, with the default kernel variants (barrier-free ring for CDIM <= 4).
+template<int CDIM>
+static int launch_sparse_fwd(
+    const float *means2d, const float *conics, const float *colors, const float *opacities, const float *backgrounds,
+    const uint8_t *masks, uint32_t W, uint32_t H, uint32_t tw, uint32_t th, unsigned n_active, const int32_t *tile_offsets,
+    const int32_t *flatten_ids, int64_t S, const SparsePixels &pm, void *records, float *render_colors, float *render_alphas,
+    int32_t *last_ids, cudaStream_t st
+)
+{
+    if(int rc = launch_pack<CDIM>(means2d, conics, colors, opacities, tile_offsets, flatten_ids, S, n_active, records, st))
+        return rc;
+    RecordStreams r      = carve_records(records, S, RecLayout<CDIM>::kColorVec4);
+    const int32_t *order = (S > 0 && use_tile_order(n_active)) ? r.order : nullptr;
+    constexpr bool pipe  = CDIM <= 4;
+    const size_t smem    = ring_smem_bytes<CDIM, kBatch, pipe ? kPipeStages : kStages>();
+    GSB_CUDA_TRY(cudaFuncSetAttribute(raster_fwd_kernel<CDIM, pipe, SparsePixels>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    raster_fwd_kernel<CDIM, pipe, SparsePixels><<<n_active, kWarps * 32, smem, st>>>(
+        1u, S, r.cull, r.geom, r.color, order, backgrounds, masks, W, H, tw, th, tile_offsets, render_colors, render_alphas,
+        last_ids, pm
+    );
+    return check_launch();
+}
+
+template<int CDIM>
+static int launch_sparse_bwd(
+    const float *backgrounds, const uint8_t *masks, uint32_t W, uint32_t H, uint32_t tw, uint32_t th, unsigned n_active,
+    const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t S, const SparsePixels &pm, const void *records,
+    const float *render_alphas, const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas,
+    const GradDst &dst, cudaStream_t st
+)
+{
+    if(S == 0)
+        return GSB200_OK;
+    RecordStreams r       = carve_records(const_cast<void *>(records), S, RecLayout<CDIM>::kColorVec4);
+    const int32_t *order  = use_tile_order(n_active) ? r.order : nullptr; // written by the forward
+    const uint32_t packed = packed_grad_stride<CDIM>(dst);
+    constexpr bool pipe   = CDIM <= 4;
+    constexpr int minb    = CDIM <= 4 ? 4 : 1;
+    const size_t smem     = Bwd2Smem<CDIM, pipe>::total;
+    auto launch           = [&](auto kernel) -> int {
+        GSB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kernel<<<n_active, kWarps * 32, smem, st>>>(
+            1u, S, r.cull, r.geom, r.color, order, flatten_ids, backgrounds, masks, W, H, tw, th, tile_offsets, render_alphas,
+            last_ids, v_render_colors, v_render_alphas, dst, packed, pm
+        );
+        return check_launch();
+    };
+    if(dst.abs != nullptr)
+        return launch(raster_bwd2_kernel<CDIM, true, minb, pipe, SparsePixels>);
+    return launch(raster_bwd2_kernel<CDIM, false, minb, pipe, SparsePixels>);
 }
 } // namespace gsb
 
@@ -1566,6 +1720,108 @@ extern "C" int gsb200_raster_bwd(
         return gsb::launch_bwd<n>(                                                                                 \
             I, backgrounds, masks, image_width, image_height, tile_width, tile_height, offsets, flatten_ids,       \
             n_isects, records, render_alphas, last_ids, v_render_colors, v_render_alphas, dst, st                  \
+        );
+        GSB_FOR_CHANNELS(X)
+#undef X
+    default:
+        return GSB200_E_UNSUPPORTED;
+    }
+}
+
+// ---- sparse pixels: one CTA per active tile of the layout of gsb200_sparse_layout_*, outputs [P, D] / [P] in the original
+// pixel order.  `records` is caller scratch of gsb200_raster_records_bytes(n_isects, D, n_active).
+static int sparse_args_ok(
+    int64_t n_active, const int32_t *active_tiles, const int32_t *tile_offsets, const uint64_t *tile_pixel_mask,
+    const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, uint32_t W, uint32_t H, uint32_t tw, uint32_t th
+)
+{
+    if(n_active < 0 || n_active > 0x7fffffffLL)
+        return GSB200_E_INVALID;
+    if(n_active > 0 && (!active_tiles || !tile_offsets || !tile_pixel_mask || !tile_pixel_cumsum || !pixel_map))
+        return GSB200_E_INVALID;
+    if((uint64_t)tw * gsb::kTile < W || (uint64_t)th * gsb::kTile < H)
+        return GSB200_E_INVALID;
+    return GSB200_OK;
+}
+
+extern "C" int gsb200_raster_sparse_fwd(
+    int D, const float *means2d, const float *conics, const float *colors, const float *opacities, const float *backgrounds,
+    const uint8_t *masks, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
+    uint32_t tile_height, int64_t n_active, const int32_t *active_tiles, const int32_t *tile_offsets,
+    const int32_t *flatten_ids, int64_t n_isects, const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum,
+    const int64_t *pixel_map, void *records, float *render_colors, float *render_alphas, int32_t *last_ids, void *stream
+)
+{
+    if(tile_size != (uint32_t)gsb::kTile)
+        return GSB200_E_UNSUPPORTED;
+    if(n_isects < 0)
+        return GSB200_E_INVALID;
+    if(int rc = sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_width, tile_height))
+        return rc;
+    if(n_active == 0)
+        return GSB200_OK;
+    if(!render_colors || !render_alphas || !last_ids || !records)
+        return GSB200_E_INVALID;
+    if(n_isects > 0 && (!means2d || !conics || !colors || !opacities || !flatten_ids))
+        return GSB200_E_INVALID;
+    const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
+    cudaStream_t st = (cudaStream_t)stream;
+    switch(D)
+    {
+#define X(n)                                                                                                         \
+    case n:                                                                                                          \
+        return gsb::launch_sparse_fwd<n>(                                                                            \
+            means2d, conics, colors, opacities, backgrounds, masks, image_width, image_height, tile_width, tile_height, \
+            (unsigned)n_active, tile_offsets, flatten_ids, n_isects, pm, records, render_colors, render_alphas, last_ids, st \
+        );
+        GSB_FOR_CHANNELS(X)
+#undef X
+    default:
+        return GSB200_E_UNSUPPORTED;
+    }
+}
+
+extern "C" int gsb200_raster_sparse_bwd(
+    int64_t n_rows, int D, const float *backgrounds, const uint8_t *masks, uint32_t image_width, uint32_t image_height,
+    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t n_active, const int32_t *active_tiles,
+    const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t n_isects, const uint64_t *tile_pixel_mask,
+    const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, const void *records, const float *render_alphas,
+    const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, float *v_means2d,
+    int64_t v_means2d_stride, float *v_conics, int64_t v_conics_stride, float *v_colors, int64_t v_colors_stride,
+    float *v_opacities, int64_t v_opacities_stride, float *v_means2d_abs, int64_t v_means2d_abs_stride, void *stream
+)
+{
+    if(tile_size != (uint32_t)gsb::kTile)
+        return GSB200_E_UNSUPPORTED;
+    if(n_rows < 0 || n_isects < 0)
+        return GSB200_E_INVALID;
+    if(int rc = sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_width, tile_height))
+        return rc;
+    if(n_isects == 0 || n_active == 0)
+        return GSB200_OK;
+    if(!flatten_ids || !records || !render_alphas || !last_ids || !v_render_colors || !v_means2d || !v_conics || !v_colors
+       || !v_opacities)
+        return GSB200_E_INVALID;
+    {   // the kernels address gradient rows with 32-bit element offsets
+        const int64_t smax = std::max(std::max(v_means2d_stride, v_conics_stride), std::max(std::max(v_colors_stride, v_opacities_stride), v_means2d_abs ? v_means2d_abs_stride : (int64_t)0));
+        if(smax < 0 || (double)n_rows * (double)smax >= 4294967296.0)
+            return GSB200_E_UNSUPPORTED;
+    }
+    gsb::GradDst dst;
+    dst.means2d = v_means2d, dst.s_means2d = v_means2d_stride;
+    dst.conics = v_conics, dst.s_conics = v_conics_stride;
+    dst.colors = v_colors, dst.s_colors = v_colors_stride;
+    dst.opacities = v_opacities, dst.s_opacities = v_opacities_stride;
+    dst.abs = v_means2d_abs, dst.s_abs = v_means2d_abs_stride;
+    const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
+    cudaStream_t st = (cudaStream_t)stream;
+    switch(D)
+    {
+#define X(n)                                                                                                       \
+    case n:                                                                                                        \
+        return gsb::launch_sparse_bwd<n>(                                                                          \
+            backgrounds, masks, image_width, image_height, tile_width, tile_height, (unsigned)n_active, tile_offsets, \
+            flatten_ids, n_isects, pm, records, render_alphas, last_ids, v_render_colors, v_render_alphas, dst, st \
         );
         GSB_FOR_CHANNELS(X)
 #undef X

@@ -4,6 +4,8 @@ executable form).  ``apply()`` rebinds, in place, the names the reference's call
   gsplat.rasterization / gsplat.rendering.rasterization                      (rendering.py:234)
   gsplat.cuda._wrapper.{quat_scale_to_covar_preci, fully_fused_projection, spherical_harmonics, isect_tiles,
                         isect_offset_encode, rasterize_to_pixels, adam}        (_wrapper.py:419,436,657,819,1196,1328,1497)
+  gsplat.cuda._wrapper.{build_sparse_tile_layout, isect_tiles_sparse,
+                        rasterize_to_pixels_sparse}                          (_wrapper.py:1433,1352,1566)
   gsplat.<the same re-exports>                                               (__init__.py:23-62)
   gsplat.relocation.compute_relocation (+ its import in gsplat.strategy.ops) (relocation.py:25, strategy/ops.py:26)
   gsplat.strategy.ops._cuda_fused_mcmc_perturb                               (strategy/ops.py:405)
@@ -36,6 +38,9 @@ _OPS = (
     "isect_tiles",
     "isect_offset_encode",
     "rasterize_to_pixels",
+    "build_sparse_tile_layout",
+    "isect_tiles_sparse",
+    "rasterize_to_pixels_sparse",
 )
 
 _saved: List[Tuple[object, str, object]] = []

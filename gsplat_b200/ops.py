@@ -1211,6 +1211,313 @@ def rasterize_to_pixels_rows(
 
 
 # --------------------------------------------------------------------------------------------
+# sparse pixels: build_sparse_tile_layout / isect_tiles_sparse / rasterize_to_pixels_sparse
+# (reference wrappers /root/reference/gsplat/cuda/_wrapper.py:1352, :1433, :1566).  At every requested pixel the result
+# is the dense rendering's; only the active tiles are intersected and composited, and only the requested pixels written.
+
+_TILE_WORDS = 4  # uint64 words of a 16 x 16 tile's pixel mask
+
+
+@torch.no_grad()
+def build_sparse_tile_layout(
+    pixels: Tensor,  # [P, 2] int, (row, col)
+    image_ids: Tensor,  # [P] int
+    n_images: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """Tile / pixel bookkeeping of a set of requested pixels ``pixels[p] = (row, col)`` of image ``image_ids[p]``.
+    Returns (active_tiles int32 [AT] ascending dense tile ids ``image * th * tw + (row // 16) * tw + col // 16``,
+    active_tile_mask bool [n_images, th, tw], tile_pixel_mask uint64 [AT, 4] raster-order in-tile bits,
+    tile_pixel_cumsum int64 [AT] inclusive (length 1, zero, when P == 0), pixel_map int64 [P]: the pixel indices in
+    (tile, in-tile) order).  Pixels must not repeat.  Reads the number of active tiles back to the host once."""
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    if pixels.dim() != 2 or pixels.shape[1] != 2:
+        raise ValueError(f"pixels must be [P, 2], got {tuple(pixels.shape)}")
+    P = pixels.shape[0]
+    if tuple(image_ids.shape) != (P,):
+        raise ValueError(f"image_ids must be [{P}], got {tuple(image_ids.shape)}")
+    if pixels.is_floating_point() or image_ids.is_floating_point():
+        raise TypeError("pixels and image_ids must be integer tensors")
+    n_images, tile_width, tile_height = int(n_images), int(tile_width), int(tile_height)
+    if n_images < 0 or tile_width <= 0 or tile_height <= 0:
+        raise ValueError(f"bad layout n_images={n_images} tile_width={tile_width} tile_height={tile_height}")
+    if n_images * tile_width * tile_height >= 1 << 31:
+        raise ValueError(f"build_sparse_tile_layout: n_images * n_tiles ({n_images * tile_width * tile_height}) must be < 2^31.")
+    if P > 0:
+        # range checks on whatever device the inputs live on, before anything is launched here
+        rows, cols = pixels[:, 0], pixels[:, 1]
+        bad_px = (rows < 0) | (rows >= tile_height * tile_size) | (cols < 0) | (cols >= tile_width * tile_size)
+        bad_id = (image_ids < 0) | (image_ids >= n_images)
+        n_bad_px, n_bad_id = (int(v) for v in torch.stack([bad_px.sum(), bad_id.sum()]).tolist())
+        if n_bad_px:
+            raise ValueError(
+                f"build_sparse_tile_layout: {n_bad_px} pixel(s) outside the {tile_height * tile_size} x {tile_width * tile_size} "
+                "tile grid (pixels are (row, col))"
+            )
+        if n_bad_id:
+            raise ValueError(f"build_sparse_tile_layout: {n_bad_id} image id(s) outside [0, {n_images})")
+    dev = require_cuda(pixels, image_ids)
+    i32 = dict(device=dev, dtype=torch.int32)
+    i64 = dict(device=dev, dtype=torch.int64)
+    mask8 = torch.empty((n_images, tile_height, tile_width), device=dev, dtype=torch.uint8)
+    L = lib()
+    with _Ctx(dev) as st:
+        if P == 0:
+            check(L.gsb200_sparse_layout_finish(0, n_images, tile_width, tile_height, 0, None, 0, None, ptr(mask8), None, None, None, st), "build_sparse_tile_layout")
+            return (
+                torch.empty(0, **i32), mask8.view(torch.bool), torch.empty((0, _TILE_WORDS), **i64).view(torch.uint64),
+                torch.zeros(1, **i64), torch.empty(0, **i64),
+            )
+        px = pixels.to(torch.int32).contiguous()
+        ids = image_ids.to(torch.int32).contiguous()
+        ws = _scratch_buffer(dev, "sparse_layout", L.gsb200_sparse_layout_workspace_bytes(P, n_images, tile_width, tile_height))
+        n_active = torch.empty(1, **i64)
+        check(
+            L.gsb200_sparse_layout_sort(P, ptr(px), ptr(ids), n_images, tile_size, tile_width, tile_height, ptr(ws), ws.numel(), ptr(n_active), st),
+            "build_sparse_tile_layout (sort)",
+        )
+        AT = int(n_active.item())  # the one host sync of the layout (the reference's builder synchronises too)
+        active_tiles = torch.empty(AT, **i32)
+        tile_pixel_mask = torch.empty((AT, _TILE_WORDS), **i64)
+        cumsum, pixel_map = torch.empty(AT, **i64), torch.empty(P, **i64)
+        check(
+            L.gsb200_sparse_layout_finish(
+                P, n_images, tile_width, tile_height, AT, ptr(ws), ws.numel(), ptr(active_tiles), ptr(mask8), ptr(tile_pixel_mask),
+                ptr(cumsum), ptr(pixel_map), st,
+            ),
+            "build_sparse_tile_layout (finish)",
+        )
+    return active_tiles, mask8.view(torch.bool), tile_pixel_mask.view(torch.uint64), cumsum, pixel_map
+
+
+@torch.no_grad()
+def isect_tiles_sparse(
+    means2d: Tensor,  # [I, N, 2] or [nnz, 2]
+    radii: Tensor,  # [I, N, 2] or [nnz, 2]
+    depths: Tensor,  # [I, N] or [nnz]
+    tile_mask: Tensor,  # [n_images, tile_height, tile_width] bool
+    active_tiles: Tensor,  # [AT] int32
+    n_images: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+    image_ids: Optional[Tensor] = None,  # [nnz], packed only
+) -> Tuple[Tensor, Tensor]:
+    """The intersections of ``isect_tiles(..., conics=None)`` that fall in tiles flagged by ``tile_mask`` (the
+    ``active_tile_mask`` of build_sparse_tile_layout), in the same (image, tile, depth) order, with per-active-tile
+    offsets.  Returns (tile_offsets int32 [AT + 1], ``tile_offsets[AT] == n_isects``; flatten_ids int32 [n_isects])."""
+    packed = means2d.dim() == 2
+    n_images = int(n_images)
+    if packed:
+        nnz = means2d.shape[0]
+        if tuple(means2d.shape) != (nnz, 2) or tuple(radii.shape) != (nnz, 2) or tuple(depths.shape) != (nnz,):
+            raise ValueError(f"packed inputs must be means2d [nnz, 2], radii [nnz, 2], depths [nnz]; got "
+                             f"{tuple(means2d.shape)}, {tuple(radii.shape)}, {tuple(depths.shape)}")
+        if image_ids is None or tuple(image_ids.shape) != (nnz,):
+            raise ValueError("image_ids [nnz] is required when means2d is packed ([nnz, 2]).")
+        I, N = n_images, nnz
+    else:
+        if means2d.dim() != 3:
+            raise ValueError(f"means2d must be [I, N, 2] or [nnz, 2], got {tuple(means2d.shape)}")
+        I, N = means2d.shape[0], means2d.shape[1]
+        if tuple(means2d.shape) != (I, N, 2) or tuple(radii.shape) != (I, N, 2) or tuple(depths.shape) != (I, N):
+            raise ValueError(f"dense inputs must be means2d [I, N, 2], radii [I, N, 2], depths [I, N]; got "
+                             f"{tuple(means2d.shape)}, {tuple(radii.shape)}, {tuple(depths.shape)}")
+        if I != n_images:
+            raise ValueError(f"means2d has {I} images, n_images is {n_images}")
+    if tuple(tile_mask.shape) != (n_images, tile_height, tile_width) or tile_mask.dtype != torch.bool:
+        raise ValueError(f"tile_mask must be bool [{n_images}, {tile_height}, {tile_width}], got {tile_mask.dtype} {tuple(tile_mask.shape)}")
+    if active_tiles.dim() != 1 or active_tiles.dtype != torch.int32:
+        raise ValueError(f"active_tiles must be int32 [AT], got {active_tiles.dtype} {tuple(active_tiles.shape)}")
+    if radii.dtype != torch.int32:
+        raise TypeError("radii must be int32")
+    image_bits, tile_bits = _cabi.bits_for_count(n_images), _cabi.bits_for_count(tile_width * tile_height)
+    if image_bits + tile_bits > 32:
+        raise RuntimeError(
+            f"intersect_tile: (image, tile) id packing needs {image_bits + tile_bits} bits but only 32 are "
+            f"available (I={n_images}, n_tiles={tile_width * tile_height})."
+        )
+    dev = require_cuda(means2d, radii, depths, tile_mask, active_tiles, image_ids)
+    means2d, depths = f32c(means2d, "means2d"), f32c(depths, "depths")
+    radii, tm = radii.contiguous(), tile_mask.contiguous().view(torch.uint8)
+    active = active_tiles.contiguous()
+    img = image_ids.to(torch.int64).contiguous() if packed else None
+    AT, total = active.shape[0], N if packed else I * N
+    L = lib()
+    tile_offsets = torch.empty(AT + 1, device=dev, dtype=torch.int32)
+    with _Ctx(dev) as st:
+        n_isects = 0
+        order = torch.empty(total, device=dev, dtype=torch.int32)
+        cum = torch.empty(total, device=dev, dtype=torch.int64)
+        if total > 0:
+            ws = _scratch_buffer(dev, "sparse_count", L.gsb200_isect_sparse_count_workspace_bytes(I, total))
+            check(
+                L.gsb200_isect_sparse_count(
+                    I, N, ptr(means2d), ptr(radii), ptr(depths), ptr(img), ptr(tm), tile_size, tile_width, tile_height, ptr(order),
+                    ptr(cum), ptr(ws), ws.numel(), st,
+                ),
+                "intersect_tile_sparse (count)",
+            )
+            n_isects = int(cum[-1].item())  # the one host sync (as in isect_tiles)
+        flatten_ids = torch.empty(n_isects, device=dev, dtype=torch.int32)
+        ws = _scratch_buffer(dev, "sparse_emit", L.gsb200_isect_sparse_emit_workspace_bytes(I, n_isects, tile_width, tile_height))
+        check(
+            L.gsb200_isect_sparse_emit(
+                I, N, ptr(means2d), ptr(radii), ptr(img), ptr(tm), tile_size, tile_width, tile_height, ptr(order), ptr(cum),
+                n_isects, AT, ptr(active), ptr(tile_offsets), ptr(flatten_ids), ptr(ws), ws.numel(), st,
+            ),
+            "intersect_tile_sparse (emit)",
+        )
+    return tile_offsets, flatten_ids
+
+
+class _RasterizeToPixelsSparse(torch.autograd.Function):
+    @staticmethod
+    def forward(
+        ctx, means2d, conics, colors, opacities, backgrounds, masks, image_ids, active_tiles, tile_offsets, flatten_ids,
+        tile_pixel_mask, tile_pixel_cumsum, pixel_map, width, height, tile_width, tile_height, absgrad_holder,
+    ):
+        dev = require_cuda(means2d, conics, colors, opacities, active_tiles, tile_offsets, flatten_ids, pixel_map)
+        means2d, conics, colors, opacities = f32c(means2d, "means2d"), f32c(conics, "conics"), f32c(colors, "colors"), f32c(opacities, "opacities")
+        backgrounds = f32c(backgrounds, "backgrounds")
+        row_dims = tuple(means2d.shape[:-1])
+        R, D, P = _prod(row_dims), colors.shape[-1], pixel_map.shape[0]
+        m8 = None
+        if masks is not None:
+            m8 = masks.contiguous().view(torch.uint8) if masks.dtype == torch.bool else masks.to(torch.uint8).contiguous()
+        active, offsets, fl = active_tiles.contiguous(), tile_offsets.contiguous(), flatten_ids.contiguous()
+        words = tile_pixel_mask.contiguous()
+        cumsum, pmap = tile_pixel_cumsum.contiguous(), pixel_map.contiguous()
+        AT, S = active.shape[0], fl.shape[0]
+        L = lib()
+        records = torch.empty(max(L.gsb200_raster_records_bytes(S, D, AT), 16), device=dev, dtype=torch.uint8)
+        o = dict(device=dev, dtype=torch.float32)
+        render_colors, render_alphas = torch.empty((P, D), **o), torch.empty((P, 1), **o)
+        last_ids = torch.empty(P, device=dev, dtype=torch.int32)
+        with _Ctx(dev) as st:
+            check(
+                L.gsb200_raster_sparse_fwd(
+                    D, ptr(means2d), ptr(conics), ptr(colors), ptr(opacities), ptr(backgrounds), ptr(m8), width, height, 16,
+                    tile_width, tile_height, AT, ptr(active), ptr(offsets), ptr(fl), S, ptr(words), ptr(cumsum), ptr(pmap),
+                    ptr(records), ptr(render_colors), ptr(render_alphas), ptr(last_ids), st,
+                ),
+                "rasterize_to_pixels_sparse",
+            )
+        ctx.save_for_backward(backgrounds, m8, image_ids, active, offsets, fl, words, cumsum, pmap, records, render_alphas, last_ids)
+        ctx.set_materialize_grads(False)
+        ctx.absgrad_holder = absgrad_holder  # filled in place by backward; deliberately not a saved tensor
+        ctx.meta = (row_dims, R, D, width, height, tile_width, tile_height)
+        return render_colors, render_alphas
+
+    @staticmethod
+    def backward(ctx, v_render_colors, v_render_alphas):
+        backgrounds, m8, image_ids, active, offsets, fl, words, cumsum, pmap, records, render_alphas, last_ids = ctx.saved_tensors
+        absgrad_holder = ctx.absgrad_holder
+        row_dims, R, D, width, height, tw, th = ctx.meta
+        dev = render_alphas.device
+        if v_render_colors is None:
+            v_render_colors = torch.zeros(render_alphas.shape[:-1] + (D,), device=dev, dtype=torch.float32)
+        v_render_colors = v_render_colors.contiguous()
+        v_render_alphas = v_render_alphas.contiguous() if v_render_alphas is not None else None
+        absgrad = absgrad_holder is not None
+        Pw = _grad_record_width(D, absgrad)
+        # one packed gradient record per gaussian: [v_xy 2 | v_conic 3 | v_opacity 1 | v_rgb D | (abs 2) | pad]
+        rec = torch.zeros((R, Pw), device=dev, dtype=torch.float32)
+        base = rec.data_ptr()
+        with _Ctx(dev) as st:
+            check(
+                lib().gsb200_raster_sparse_bwd(
+                    R, D, ptr(backgrounds), ptr(m8), width, height, 16, tw, th, active.shape[0], ptr(active), ptr(offsets), ptr(fl),
+                    fl.shape[0], ptr(words), ptr(cumsum), ptr(pmap), ptr(records), ptr(render_alphas), ptr(last_ids),
+                    ptr(v_render_colors), ptr(v_render_alphas), base, Pw, base + 8, Pw, base + 24, Pw, base + 20, Pw,
+                    (base + 4 * (6 + D)) if absgrad else None, Pw, st,
+                ),
+                "rasterize_to_pixels_sparse_bwd",
+            )
+        rec = rec.view(row_dims + (Pw,))
+        v_means2d, v_conics, v_opacities, v_colors = rec[..., 0:2], rec[..., 2:5], rec[..., 5], rec[..., 6 : 6 + D]
+        if absgrad:
+            absgrad_holder.copy_(rec[..., 6 + D : 8 + D])
+        v_backgrounds = None
+        if backgrounds is not None and ctx.needs_input_grad[4]:
+            v_backgrounds = torch.zeros_like(backgrounds).index_add_(0, image_ids.long(), v_render_colors * (1.0 - render_alphas))
+        return (v_means2d, v_conics, v_colors, v_opacities, v_backgrounds) + (None,) * 13
+
+
+def rasterize_to_pixels_sparse(
+    means2d: Tensor,  # [..., N, 2] or [nnz, 2]
+    conics: Tensor,  # [..., N, 3] or [nnz, 3]
+    colors: Tensor,  # [..., N, channels] or [nnz, channels]
+    opacities: Tensor,  # [..., N] or [nnz]
+    image_ids: Tensor,  # [P]
+    active_tiles: Tensor,  # [AT]
+    tile_offsets: Tensor,  # [AT + 1]
+    flatten_ids: Tensor,  # [n_isects]
+    tile_pixel_mask: Tensor,  # [AT, 4]
+    tile_pixel_cumsum: Tensor,  # [AT]
+    pixel_map: Tensor,  # [P]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+    backgrounds: Optional[Tensor] = None,  # [n_images, channels]
+    masks: Optional[Tensor] = None,  # [n_images, tile_height, tile_width]
+    packed: bool = False,
+    absgrad: bool = False,
+) -> Tuple[Tensor, Tensor]:
+    """rasterize_to_pixels at the pixels of a build_sparse_tile_layout layout only, with the lists of
+    isect_tiles_sparse.  Returns (render_colors [P, channels], render_alphas [P, 1]) in the original pixel order; each
+    value is the dense rendering's at that pixel (requested pixels in the margin of a partial tile included).  With
+    ``absgrad`` the backward fills ``means2d.absgrad``."""
+    if packed != (means2d.dim() == 2):
+        raise ValueError(f"packed={packed} but means2d has shape {tuple(means2d.shape)}")
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    D = colors.shape[-1]
+    if D > 32:
+        raise ValueError(
+            f"Unsupported number of color channels: {D}. gsplat_b200 rasterizes up to 32 channels per pass "
+            "(rasterization() chunks wider features with channel_chunk=32)."
+        )
+    AT, P = active_tiles.shape[0] if active_tiles.dim() == 1 else -1, pixel_map.shape[0] if pixel_map.dim() == 1 else -1
+    if AT < 0 or P < 0 or active_tiles.dtype != torch.int32:
+        raise ValueError("active_tiles must be int32 [AT] and pixel_map [P]")
+    if tuple(tile_offsets.shape) != (AT + 1,) or tile_offsets.dtype != torch.int32 or flatten_ids.dtype != torch.int32:
+        raise ValueError(f"tile_offsets must be int32 [{AT + 1}] and flatten_ids int32 (isect_tiles_sparse)")
+    if tuple(tile_pixel_mask.shape) != (AT, _TILE_WORDS) or tile_pixel_mask.element_size() != 8:
+        raise ValueError(f"tile_pixel_mask must be 64-bit [{AT}, {_TILE_WORDS}], got {tile_pixel_mask.dtype} {tuple(tile_pixel_mask.shape)}")
+    n_cum = tile_pixel_cumsum.shape[0] if tile_pixel_cumsum.dim() == 1 else -1
+    if n_cum not in ((AT,) if AT > 0 else (0, 1)) or tile_pixel_cumsum.dtype != torch.int64 or pixel_map.dtype != torch.int64:
+        raise ValueError("tile_pixel_cumsum must be int64 [AT] and pixel_map int64 [P] (build_sparse_tile_layout)")
+    if tuple(image_ids.shape) != (P,):
+        raise ValueError(f"image_ids must be [{P}], got {tuple(image_ids.shape)}")
+    if tile_width * 16 < image_width or tile_height * 16 < image_height:
+        raise ValueError(f"a {tile_width} x {tile_height} tile grid does not cover {image_width} x {image_height} pixels")
+    pad = 0
+    if D not in _SUPPORTED_CHANNELS:
+        target = next(c for c in _SUPPORTED_CHANNELS if c >= D)
+        pad = target - D
+        colors = torch.nn.functional.pad(colors, (0, pad))
+        if backgrounds is not None:
+            backgrounds = torch.nn.functional.pad(backgrounds, (0, pad))
+    holder = torch.zeros_like(means2d) if absgrad else None
+    render_colors, render_alphas = _RasterizeToPixelsSparse.apply(
+        means2d, conics, colors, opacities, backgrounds, masks, image_ids, active_tiles, tile_offsets, flatten_ids,
+        tile_pixel_mask, tile_pixel_cumsum, pixel_map, int(image_width), int(image_height), int(tile_width), int(tile_height),
+        holder,
+    )
+    if absgrad:
+        means2d.absgrad = holder
+    if pad:
+        render_colors = render_colors[..., :D]
+    return render_colors, render_alphas
+
+
+# --------------------------------------------------------------------------------------------
 # MCMC strategy ops ("next" row, SURVEY.md section 8f.3)
 
 

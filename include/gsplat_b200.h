@@ -348,6 +348,67 @@ extern "C"
         void *stream
     );
 
+    /* ---- sparse pixels: build_sparse_tile_layout, isect_tiles_sparse, rasterize_to_pixels_sparse
+     * (_wrapper.py:1352-1665).  tile_size must be 16.
+     * Layout: pixels int32 [P, 2] (row, col) inside the tile grid, image_ids int32 [P] in [0, n_images) (the caller
+     * checks both).  gsb200_sparse_layout_sort sorts one key (dense tile id << 8 | in-tile position) per pixel and
+     * writes the number of active tiles to n_active (device int64); the caller reads it, then
+     * gsb200_sparse_layout_finish (same workspace) writes active_tiles int32 [AT] ascending, active_tile_mask bool
+     * bytes [n_images, th, tw], tile_pixel_mask uint64 [AT, 4] (raster-order in-tile bits), tile_pixel_cumsum int64
+     * [AT] (inclusive) and pixel_map int64 [P] (pixel index in (tile, in-tile) order). */
+    size_t gsb200_sparse_layout_workspace_bytes(int64_t P, int64_t n_images, uint32_t tile_width, uint32_t tile_height);
+    int gsb200_sparse_layout_sort(
+        int64_t P, const int32_t *pixels, const int32_t *image_ids, int64_t n_images, uint32_t tile_size,
+        uint32_t tile_width, uint32_t tile_height, void *workspace, size_t workspace_bytes, int64_t *n_active, void *stream
+    );
+    int gsb200_sparse_layout_finish(
+        int64_t P, int64_t n_images, uint32_t tile_width, uint32_t tile_height, int64_t n_active, const void *workspace,
+        size_t workspace_bytes, int32_t *active_tiles, uint8_t *active_tile_mask, uint64_t *tile_pixel_mask,
+        int64_t *tile_pixel_cumsum, int64_t *pixel_map, void *stream
+    );
+    /* Tile intersection restricted to the tiles whose tile_mask [I, th, tw] byte is set (radius AABB test).  Dense rows
+     * [I, N] (image_ids NULL) or packed rows [N] with int64 image_ids.  gsb200_isect_sparse_count orders the rows by
+     * (image, depth) into order int32 [rows] and writes the inclusive scan of their masked tile counts to cum_tiles
+     * int64 [rows]; the caller reads n_isects = cum_tiles[rows - 1], then gsb200_isect_sparse_emit emits, stably sorts
+     * by (image, tile) into flatten_ids int32 [n_isects] and writes tile_offsets int32 [n_active + 1] (the start of
+     * each active tile's range, and n_isects). */
+    size_t gsb200_isect_sparse_count_workspace_bytes(int64_t I, int64_t total_rows);
+    int gsb200_isect_sparse_count(
+        int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const int64_t *image_ids,
+        const uint8_t *tile_mask, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *order,
+        int64_t *cum_tiles, void *workspace, size_t workspace_bytes, void *stream
+    );
+    size_t gsb200_isect_sparse_emit_workspace_bytes(int64_t I, int64_t n_isects, uint32_t tile_width, uint32_t tile_height);
+    int gsb200_isect_sparse_emit(
+        int64_t I, int64_t N, const float *means2d, const int32_t *radii, const int64_t *image_ids, const uint8_t *tile_mask,
+        uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *order, const int64_t *cum_tiles,
+        int64_t n_isects, int64_t n_active, const int32_t *active_tiles, int32_t *tile_offsets, int32_t *flatten_ids,
+        void *workspace, size_t workspace_bytes, void *stream
+    );
+    /* Compositing of the requested pixels only: one CTA per active tile, tile_offsets [n_active + 1] and flatten_ids
+     * from gsb200_isect_sparse_emit, the layout tensors from gsb200_sparse_layout_finish.  Gaussian rows and
+     * backgrounds [n_images, D] / masks [n_images, th, tw] as in gsb200_raster_fwd; `records` of
+     * gsb200_raster_records_bytes(n_isects, D, n_active).  Outputs in the original pixel order: render_colors [P, D],
+     * render_alphas [P], last_ids int32 [P].  The backward accumulates into gradient rows g in [0, n_rows) like
+     * gsb200_raster_bwd; v_render_colors [P, D], v_render_alphas [P] or NULL. */
+    int gsb200_raster_sparse_fwd(
+        int D, const float *means2d, const float *conics, const float *colors, const float *opacities,
+        const float *backgrounds, const uint8_t *masks, uint32_t image_width, uint32_t image_height, uint32_t tile_size,
+        uint32_t tile_width, uint32_t tile_height, int64_t n_active, const int32_t *active_tiles,
+        const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t n_isects, const uint64_t *tile_pixel_mask,
+        const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, void *records, float *render_colors,
+        float *render_alphas, int32_t *last_ids, void *stream
+    );
+    int gsb200_raster_sparse_bwd(
+        int64_t n_rows, int D, const float *backgrounds, const uint8_t *masks, uint32_t image_width, uint32_t image_height,
+        uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t n_active, const int32_t *active_tiles,
+        const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t n_isects, const uint64_t *tile_pixel_mask,
+        const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, const void *records, const float *render_alphas,
+        const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, float *v_means2d,
+        int64_t v_means2d_stride, float *v_conics, int64_t v_conics_stride, float *v_colors, int64_t v_colors_stride,
+        float *v_opacities, int64_t v_opacities_stride, float *v_means2d_abs, int64_t v_means2d_abs_stride, void *stream
+    );
+
     /* ---- MCMC strategy ops ("next" row): relocation (ext.cpp `relocation`, gsplat/relocation.py:64,
      * csrc/RelocationCUDA.cu:36-80) and in-place position perturbation (csrc/MCMCPerturbCUDA.cu:28-60,
      * gsplat/strategy/ops.py).  ratios int32 [N] already clamped to [1, n_max]; binoms [n_max, n_max]. */

@@ -1,0 +1,112 @@
+"""Checks that a change leaves the existing kernels' machine code alone.
+
+    python tools/sass_compare.py [--base REV] [--units raster.cu sort.cu pergauss.cu]
+
+Compiles each unit twice for sm_90a with the flags of gsplat_b200/build.py -- once from the sources at git revision
+``--base`` (default HEAD), once from the working tree -- disassembles both objects with ``cuobjdump -sass`` and compares
+every kernel of the base object with the kernel of the same name in the new one.  Names are compared demangled, with
+the pixel-addressing policy of the compositing kernels (``gsb::DensePixels``) removed, so that a kernel that only gained
+that template argument is matched with its old self.  Instructions and their encodings must be identical;
+address and line-info comments are ignored.  Kernels that only the new object has are listed as new.  Exit status 1
+on any difference.  Needs nvcc / cuobjdump / cu++filt (no GPU).
+"""
+from __future__ import annotations
+
+import argparse
+import os
+import re
+import subprocess
+import sys
+import tempfile
+
+ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
+sys.path.insert(0, ROOT)
+
+from gsplat_b200 import build as B  # noqa: E402
+
+CUDA_BIN = os.path.dirname(B._nvcc()) if os.path.isabs(B._nvcc()) else "/usr/local/cuda/bin"
+# cu++filt prints the policy parameter of a kernel as `T<k>`: dropped together with the policy template argument
+POLICY_PARAM = re.compile(r",\s*T\d+\)$")
+
+
+def _tree_at(rev: str, dst: str) -> None:
+    """gsplat_b200/csrc and include/ as of `rev`, written under dst."""
+    files = subprocess.check_output(["git", "-C", ROOT, "ls-tree", "-r", "--name-only", rev, "gsplat_b200/csrc", "include"], text=True)
+    for rel in files.split():
+        out = os.path.join(dst, rel)
+        os.makedirs(os.path.dirname(out), exist_ok=True)
+        with open(out, "wb") as f:
+            f.write(subprocess.check_output(["git", "-C", ROOT, "show", f"{rev}:{rel}"]))
+
+
+def _compile(src_root: str, unit: str, obj: str) -> None:
+    cmd = [B._nvcc(), *B.ARCH, *B.COMMON, *B.UNITS[unit], "-c", os.path.join(src_root, "gsplat_b200", "csrc", unit), "-o", obj]
+    subprocess.check_call(cmd, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+
+
+def _demangle(names):
+    out = subprocess.run([os.path.join(CUDA_BIN, "cu++filt")], input="\n".join(names), capture_output=True, text=True, check=True)
+    return out.stdout.splitlines()
+
+
+def kernels(obj: str):
+    """{normalised demangled name: [instruction lines]}"""
+    text = subprocess.check_output([os.path.join(CUDA_BIN, "cuobjdump"), "-sass", obj], text=True)
+    raw, cur = {}, None
+    for line in text.splitlines():
+        m = re.match(r"\s*Function : (\S+)", line)
+        if m:
+            cur = m.group(1)
+            raw[cur] = []
+            continue
+        if cur is None:
+            continue
+        s = line.strip()
+        if not s or s.startswith("//") or s.startswith("."):
+            continue
+        s = re.sub(r"^/\*[0-9a-f]{4,}\*/\s*", "", s)  # instruction address
+        if s:
+            raw[cur].append(re.sub(r"\s+", " ", s))
+    names = list(raw)
+    out = {}
+    for n, d in zip(names, _demangle(names)):
+        if "DensePixels" in n or "SparsePixels" in n:
+            d = POLICY_PARAM.sub(")", d).replace(", gsb::DensePixels>", ">")
+        out[d] = raw[n]
+    return out
+
+
+def main() -> int:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--base", default="HEAD")
+    ap.add_argument("--units", nargs="+", default=["raster.cu", "sort.cu", "pergauss.cu"])
+    args = ap.parse_args()
+    bad = 0
+    with tempfile.TemporaryDirectory() as tmp:
+        base_root = os.path.join(tmp, "base")
+        _tree_at(args.base, base_root)
+        for unit in args.units:
+            o_base, o_new = os.path.join(tmp, "base_" + unit + ".o"), os.path.join(tmp, "new_" + unit + ".o")
+            _compile(base_root, unit, o_base)
+            _compile(ROOT, unit, o_new)
+            kb, kn = kernels(o_base), kernels(o_new)
+            same = [k for k in kb if k in kn and kb[k] == kn[k]]
+            missing = [k for k in kb if k not in kn]
+            changed = [k for k in kb if k in kn and kb[k] != kn[k]]
+            new = [k for k in kn if k not in kb]
+            n_instr = sum(len(kb[k]) for k in same)
+            print(f"{unit}: {len(kb)} kernels at {args.base}: {len(same)} identical ({n_instr} instructions), "
+                  f"{len(changed)} changed, {len(missing)} missing; {len(new)} new")
+            for k in changed:
+                print(f"  CHANGED {k} ({len(kb[k])} -> {len(kn[k])} instructions)")
+            for k in missing:
+                print(f"  MISSING {k}")
+            for k in new:
+                print(f"  new     {k}")
+            bad += len(changed) + len(missing)
+    print("dense kernels unchanged" if bad == 0 else f"{bad} kernels differ")
+    return 1 if bad else 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -1,0 +1,135 @@
+"""Sparse-pixel rendering against the dense pipeline on bench.py's scene (1M Gaussians, one 1920x1080 view, seed 42).
+
+    python tools/sparse_bench.py [--steps 20] [--warmup 5] [--out FILE]
+
+One step of each pipeline, timed on the host around a device synchronise (both pipelines read one count back to the
+host, so a step is not asynchronous anyway):
+  sparse: build_sparse_tile_layout + isect_tiles_sparse + rasterize_to_pixels_sparse forward + backward;
+  dense:  isect_tiles(conics=None) + isect_offset_encode + rasterize_to_pixels forward + backward over the whole image
+          (the same radius-AABB tile lists), the loss on the requested pixels only.
+Workloads: (a) 4096 random pixels, (b) sixteen 64x64 patches, (c) every pixel.  The projection runs once, outside the
+timed steps.  Prints one JSON line per workload with the median step times, and the device name and power limit.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
+sys.path.insert(0, ROOT)
+
+import gsplat_b200 as gs  # noqa: E402
+from tests import scene  # noqa: E402
+
+W, H, SCENE_GRID = 1920, 1080, 3
+TW, TH = (W + 15) // 16, (H + 15) // 16
+
+
+def device_info() -> dict:
+    info = {"device": torch.cuda.get_device_name(0)}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                             capture_output=True, text=True, timeout=30)
+        info["nvidia_smi"] = out.stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        info["nvidia_smi"] = f"unavailable: {e}"
+    return info
+
+
+def workloads(rng):
+    out = {}
+    flat = rng.choice(W * H, 4096, replace=False)
+    out["a_4096_random"] = np.stack([flat // W, flat % W], -1)
+    ys, xs = rng.randint(0, H - 64, 16), rng.randint(0, W - 64, 16)
+    yy, xx = np.meshgrid(np.arange(64), np.arange(64), indexing="ij")
+    p = np.concatenate([np.stack([y + yy.ravel(), x + xx.ravel()], -1) for y, x in zip(ys, xs)])
+    out["b_16_patches_64"] = np.unique(p, axis=0)  # overlapping patches: each pixel once
+    yy, xx = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
+    out["c_every_pixel"] = np.stack([yy.ravel(), xx.ravel()], -1)
+    return out
+
+
+def main() -> int:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--out", help="also append the JSON lines to this file")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("sparse_bench needs a GPU")
+    dev = "cuda:0"
+    sc = scene.make_scene(scene_grid=SCENE_GRID, sh_degree=0)
+    Ks = scene.rescale_K(sc["Ks"], sc["width"], sc["height"], W, H)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)  # noqa: E731
+    N = sc["means"].shape[0]
+    with torch.no_grad():
+        radii, m2, depths, conics, _ = gs.fully_fused_projection(
+            t(sc["means"]), None, t(sc["quats"]), t(sc["scales"]), t(sc["viewmats"][:1]), t(Ks[:1]), W, H
+        )
+    colors = t(sc["colors"])[None].contiguous()
+    opac = t(sc["opacities"])[None].contiguous()
+    params = [x.detach().clone().requires_grad_(True) for x in (m2, conics, colors, opac)]
+    info = device_info()
+    lines = []
+
+    def timed(fn):
+        for _ in range(args.warmup):
+            fn()
+        torch.cuda.synchronize()
+        ts = []
+        for _ in range(args.steps):
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            ts.append(time.perf_counter() - t0)
+        return statistics.median(ts) * 1e3, min(ts) * 1e3
+
+    for name, pix in workloads(np.random.RandomState(42)).items():
+        pixels = t(pix.astype(np.int32))
+        image_ids = torch.zeros(pixels.shape[0], device=dev, dtype=torch.int32)
+        P = pixels.shape[0]
+        v = torch.randn((P, 3), device=dev, generator=torch.Generator(device=dev).manual_seed(0))
+        v_img = torch.zeros((1, H, W, 3), device=dev)
+        v_img[0, pixels[:, 0].long(), pixels[:, 1].long()] = v
+        stats = {}
+
+        def sparse_step():
+            active, amask, words, cum, pmap = gs.build_sparse_tile_layout(pixels, image_ids, 1, 16, TW, TH)
+            toff, fl = gs.isect_tiles_sparse(m2, radii, depths, amask, active, 1, 16, TW, TH)
+            rc, _ = gs.rasterize_to_pixels_sparse(*params, image_ids, active, toff, fl, words, cum, pmap, W, H, 16, TW, TH)
+            (rc * v).sum().backward()
+            stats.update(n_active=int(active.shape[0]), n_isects=int(fl.shape[0]))
+
+        def dense_step():
+            _, ids, fl = gs.isect_tiles(m2, radii, depths, 16, TW, TH)
+            off = gs.isect_offset_encode(ids, 1, TW, TH)
+            rc, _ = gs.rasterize_to_pixels(*params, W, H, 16, off, fl)
+            (rc * v_img).sum().backward()
+            stats.update(dense_isects=int(fl.shape[0]))
+
+        sparse_ms, sparse_min = timed(sparse_step)
+        dense_ms, dense_min = timed(dense_step)
+        rec = dict(
+            workload=name, pixels=P, n_gaussians=N, image=f"{W}x{H}", steps=args.steps, sparse_ms=round(sparse_ms, 3),
+            sparse_min_ms=round(sparse_min, 3), dense_ms=round(dense_ms, 3), dense_min_ms=round(dense_min, 3),
+            sparse_over_dense=round(sparse_ms / dense_ms, 3), **stats, **info,
+        )
+        line = json.dumps(rec)
+        print(line, flush=True)
+        lines.append(line)
+    if args.out:
+        with open(args.out, "a") as f:
+            f.write("\n".join(lines) + "\n")
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
