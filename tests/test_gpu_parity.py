@@ -487,14 +487,16 @@ def test_isect_sorted_equals_stable_sort_of_unsorted(gs):
     assert e[1].numel() == 0
 
 
-def _raster_case(gs, m2, con, col, op, W, H, off, fl, bg=None, absgrad=False, seed=0, strict_frac=0.995):
-    """Runs fwd+bwd on the GPU and in the oracle (f64) and applies the module's tolerance contract."""
+def _raster_case(gs, m2, con, col, op, W, H, off, fl, bg=None, absgrad=False, seed=0, strict_frac=0.995, masks=None):
+    """Runs fwd+bwd on the GPU and in the oracle (f64) and applies the module's tolerance contract.  ``masks``
+    [..., th, tw] switches tiles off on both sides, forward and backward."""
     D = col.shape[-1]
     tm2, tcon, tcol, top = _t(m2, True), _t(con, True), _t(col, True), _t(op, True)
     tbg = _t(bg, True) if bg is not None else None
-    rc, ra = gs.rasterize_to_pixels(tm2, tcon, tcol, top, W, H, 16, _t(off), _t(fl), backgrounds=tbg, absgrad=absgrad)
+    tmask = _t(masks) if masks is not None else None
+    rc, ra = gs.rasterize_to_pixels(tm2, tcon, tcol, top, W, H, 16, _t(off), _t(fl), backgrounds=tbg, masks=tmask, absgrad=absgrad)
     d = lambda a: None if a is None else a.astype(np.float64)  # noqa: E731
-    orc, ora, oli, omg = gso.rasterize_to_pixels(d(m2), d(con), d(col), d(op), W, H, 16, off, fl, d(bg), None, True)
+    orc, ora, oli, omg = gso.rasterize_to_pixels(d(m2), d(con), d(col), d(op), W, H, 16, off, fl, d(bg), masks, True)
     ok = omg > 1e-4
     assert ok.mean() > strict_frac, f"too many marginal pixels: {1 - ok.mean():.4f}"
     _close(_n(rc)[ok], orc[ok], 1e-4, 1e-5, "render_colors")
@@ -505,7 +507,7 @@ def _raster_case(gs, m2, con, col, op, W, H, off, fl, bg=None, absgrad=False, se
     v_ra = rng.standard_normal(ora.shape).astype(np.float32)
     ins = [tm2, tcon, tcol, top] + ([tbg] if tbg is not None else [])
     grads = torch.autograd.grad((rc * _t(v_rc)).sum() + (ra * _t(v_ra)).sum(), ins)
-    og = gso.rasterize_to_pixels_bwd(d(m2), d(con), d(col), d(op), W, H, 16, off, fl, ora, oli, d(v_rc), d(v_ra), d(bg), None, absgrad)
+    og = gso.rasterize_to_pixels_bwd(d(m2), d(con), d(col), d(op), W, H, 16, off, fl, ora, oli, d(v_rc), d(v_ra), d(bg), masks, absgrad)
     # gaussians that touch a marginal pixel are excluded from the strict check
     th, tw = off.shape[-2:]
     I = int(np.prod(off.shape[:-2]))
