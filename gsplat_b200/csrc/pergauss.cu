@@ -188,10 +188,12 @@ __global__ void __launch_bounds__(kThreads) projection_bwd_kernel(
 #pragma unroll
     for(int k = 0; k < 9; ++k)
         v_cov.m[k] = 0.f;
+    bool seen = false; // some camera sees the gaussian: only then does it get a (quat, scale) gradient
     for(int64_t c = 0; c < C; ++c)
     {
         const int64_t idx = (b * C + c) * N + n;
         const bool vis    = active && radii[idx * 2] > 0 && radii[idx * 2 + 1] > 0;
+        seen |= vis;
         float vm_part[12];
 #pragma unroll
         for(int k = 0; k < 12; ++k)
@@ -265,8 +267,11 @@ __global__ void __launch_bounds__(kThreads) projection_bwd_kernel(
     }
     else
     {
+        // a gaussian no camera sees gets zero, as in the reference (its quaternion may be zero, and the VJP of the
+        // normalisation would turn the zero gradient into NaN)
         float vq[4] = {0.f, 0.f, 0.f, 0.f}, vs[3] = {0.f, 0.f, 0.f};
-        quat_scale_sym_vjp<false>(q, s, v_cov, vq, vs);
+        if(seen)
+            quat_scale_sym_vjp<false>(q, s, v_cov, vq, vs);
 #pragma unroll
         for(int k = 0; k < 4; ++k)
             v_quats[bn * 4 + k] = vq[k];

@@ -18,6 +18,20 @@
 
 /* -------- small dense helpers (row-major 3x3) -------- */
 
+/* float -> int32 with the GPU's conversion (cvt.rzi.s32: truncate toward zero, saturate at the int32 range, NaN -> 0).
+ * A plain C cast is undefined outside the int32 range (x86 returns INT32_MIN, which would turn a huge radius into a
+ * culled row and a far tile bound into the wrong end of the grid). */
+static inline int32_t FN(f2i)(REAL v)
+{
+    if(v != v)
+        return 0;
+    if(v >= (REAL)2147483647.0)
+        return INT32_MAX;
+    if(v <= (REAL)-2147483648.0)
+        return INT32_MIN;
+    return (int32_t)v;
+}
+
 static inline void FN(mat3_mul)(const REAL *A, const REAL *B, REAL *C_)
 {
     for(int i = 0; i < 3; ++i)
@@ -463,8 +477,8 @@ static inline int FN(project_one)(
         return 0;
     if(m2x + rx <= (REAL)0 || m2x - rx >= (REAL)W || m2y + ry <= (REAL)0 || m2y - ry >= (REAL)H)
         return 0;
-    radii[0]  = (int32_t)rx;
-    radii[1]  = (int32_t)ry;
+    radii[0]  = FN(f2i)(rx); /* rx >= 2^31 saturates to INT32_MAX like the kernels' conversion */
+    radii[1]  = FN(f2i)(ry);
     mean2d[0] = m2x;
     mean2d[1] = m2y;
     *depth    = pc[2];
@@ -900,8 +914,8 @@ static int FN(tiles_of_gaussian)(
         REAL BxC = B_ * xe / C_, ByA = B_ * ye / A_;
         /* argmin.x = y where x is minimal ; argmin.y = x where y is minimal */
         REAL argminx = my + BxC, argminy = mx + ByA, argmaxx = my - BxC, argmaxy = mx - ByA;
-        int rminx = FN(clampi)((int)(bminx / ts), 0, (int)tw), rminy = FN(clampi)((int)(bminy / ts), 0, (int)th);
-        int rmaxx = FN(clampi)((int)(bmaxx / ts + (REAL)1), 0, (int)tw), rmaxy = FN(clampi)((int)(bmaxy / ts + (REAL)1), 0, (int)th);
+        int rminx = FN(clampi)(FN(f2i)(bminx / ts), 0, (int)tw), rminy = FN(clampi)(FN(f2i)(bminy / ts), 0, (int)th);
+        int rmaxx = FN(clampi)(FN(f2i)(bmaxx / ts + (REAL)1), 0, (int)tw), rmaxy = FN(clampi)(FN(f2i)(bmaxy / ts + (REAL)1), 0, (int)th);
         int ys = rmaxy - rminy, xs = rmaxx - rminx;
         if(ys * xs == 0)
             return 0;
@@ -936,7 +950,7 @@ static int FN(tiles_of_gaussian)(
                 emax = bmaxv;
             else
                 emax = minhi > maxhi ? minhi : maxhi;
-            int e0 = (int)(emin / ts), e1 = (int)(emax / ts + (REAL)1);
+            int e0 = FN(f2i)(emin / ts), e1 = FN(f2i)(emax / ts + (REAL)1);
             int v0 = e0 < rv1 ? e0 : rv1; /* max(rv0, min(rv1, e0)) */
             v0     = v0 > rv0 ? v0 : rv0;
             int v1 = e1 > rv0 ? e1 : rv0; /* min(rv1, max(rv0, e1)) */
@@ -955,7 +969,7 @@ static int FN(tiles_of_gaussian)(
     else
     { /* AABB from radii: IntersectTile.cu:374-463 */
         REAL trx = (REAL)rx / ts, try_ = (REAL)ry / ts, tx = mx / ts, ty = my / ts;
-        int x0 = (int)R_FLOOR(tx - trx), y0 = (int)R_FLOOR(ty - try_), x1 = (int)R_CEIL(tx + trx), y1 = (int)R_CEIL(ty + try_);
+        int x0 = FN(f2i)(R_FLOOR(tx - trx)), y0 = FN(f2i)(R_FLOOR(ty - try_)), x1 = FN(f2i)(R_CEIL(tx + trx)), y1 = FN(f2i)(R_CEIL(ty + try_));
         x0 = FN(clampi)(x0, 0, (int)tw); y0 = FN(clampi)(y0, 0, (int)th);
         x1 = FN(clampi)(x1, 0, (int)tw); y1 = FN(clampi)(y1, 0, (int)th);
         for(int i = y0; i < y1; ++i)
