@@ -1834,20 +1834,10 @@ extern "C" int gsb200_isect_emit(
     const uint32_t tile_bits = bits_for_count((int64_t)tile_width * tile_height);
     if(bits_for_count(I) + tile_bits > 32)
         return GSB200_E_KEYBITS;
-    static const bool coop = [] {
-        const char *e = std::getenv("GSB200_EMIT");
-        return !(e && e[0] == 's'); // GSB200_EMIT=serial selects the one-thread-per-gaussian kernel (measurements)
-    }();
-    if(coop)
-        isect_emit_coop_kernel<int64_t><<<grid_for(total, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
-            total, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width, tile_height,
-            tile_bits, isect_ids, flatten_ids
-        );
-    else
-        isect_emit_kernel<int64_t><<<grid_for(total, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
-            total, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width, tile_height,
-            tile_bits, isect_ids, flatten_ids
-        );
+    isect_emit_coop_kernel<int64_t><<<grid_for(total, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
+        total, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width, tile_height,
+        tile_bits, isect_ids, flatten_ids
+    );
     return check_launch();
 }
 
@@ -2226,57 +2216,6 @@ extern "C" int gsb200_isect_emit_ordered(
         I, N, n_order, max_tiles_hint, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width,
         tile_height, isect_ids, flatten_ids, stream
     );
-}
-
-// Narrow-key variant: writes the dense tile id image * n_tiles + tile as a key_bytes-wide (2 or 4) unsigned integer.
-extern "C" int gsb200_isect_emit_tilekeys(
-    int64_t I, int64_t N, int64_t n_order, int64_t max_tiles_hint, const float *means2d, const int32_t *radii, const float *depths,
-    const float *conics, const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, const int32_t *order,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int key_bytes, void *tile_keys, int32_t *flatten_ids, void *stream
-)
-{
-    if(key_bytes == 2)
-        return gsb::emit_ordered<uint16_t>(
-            I, N, n_order, max_tiles_hint, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size,
-            tile_width, tile_height, static_cast<uint16_t *>(tile_keys), flatten_ids, stream
-        );
-    if(key_bytes == 4)
-        return gsb::emit_ordered<uint32_t>(
-            I, N, n_order, max_tiles_hint, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size,
-            tile_width, tile_height, static_cast<uint32_t *>(tile_keys), flatten_ids, stream
-        );
-    return GSB200_E_INVALID;
-}
-
-extern "C" int gsb200_isect_offsets_tilekeys(
-    int64_t n_isects, int key_bytes, const void *tile_keys, int64_t I, uint32_t tile_width, uint32_t tile_height, int32_t *offsets,
-    void *stream
-)
-{
-    if(n_isects < 0 || I < 0 || (key_bytes != 2 && key_bytes != 4))
-        return GSB200_E_INVALID;
-    const int64_t total = I * (int64_t)tile_width * tile_height;
-    if(total == 0)
-        return GSB200_OK;
-    if(!offsets)
-        return GSB200_E_INVALID;
-    cudaStream_t st = (cudaStream_t)stream;
-    if(n_isects == 0)
-    {
-        GSB_CUDA_TRY(cudaMemsetAsync(offsets, 0, sizeof(int32_t) * (size_t)total, st));
-        return GSB200_OK;
-    }
-    if(!tile_keys)
-        return GSB200_E_INVALID;
-    if(key_bytes == 2)
-        isect_offsets_tilekeys_kernel<uint16_t><<<grid_for(n_isects, kThreads), kThreads, 0, st>>>(
-            n_isects, static_cast<const uint16_t *>(tile_keys), total, offsets
-        );
-    else
-        isect_offsets_tilekeys_kernel<uint32_t><<<grid_for(n_isects, kThreads), kThreads, 0, st>>>(
-            n_isects, static_cast<const uint32_t *>(tile_keys), total, offsets
-        );
-    return check_launch();
 }
 
 extern "C" int gsb200_isect_ids_from_tilekeys(

@@ -1,7 +1,7 @@
-"""CPU model of the butterfly ("transpose") warp reduction used by the backward rasterizer
+"""CPU model of the butterfly ("transpose") warp reduction used by the projection backward and the SH backward
 (gsplat_b200/csrc/common.cuh: Butterfly<M,16> + butterfly_slot<M>).  The recursion is restated in numpy
 with an explicit shfl_xor so that slot ownership and sums can be checked for every M the kernels use
-(M = 6 + channels [+ 2 for absgrad], and 12 for the pose gradient)."""
+(M = 12 for the pose gradient, 3 for the SH backward's per-image view-direction sum), and for other widths."""
 import numpy as np
 import pytest
 
@@ -43,7 +43,7 @@ def slot_of(lane, M):
     return slot if (mr >= 1 and primary) else -1
 
 
-@pytest.mark.parametrize("M", [7, 8, 9, 10, 11, 12, 13, 14, 16, 22, 24, 38, 40])
+@pytest.mark.parametrize("M", [3, 7, 8, 9, 10, 11, 12, 13, 14, 16, 22, 24, 38, 40])
 def test_every_slot_owned_once_with_the_right_sum(M):
     rng = np.random.RandomState(M)
     vals = rng.standard_normal((32, M))

@@ -443,16 +443,21 @@ def test_fused_projection_row_side_outputs(gs):
         assert rel < 1e-5, (name, rel)  # same pairs, same arithmetic; only the order of the atomic adds differs
 
 
+def isect_sorted_equals_stable_sort(gs, m2, radii, dep, tw, th, **kw):
+    """isect_tiles(sort=True) equals one stable sort of isect_tiles(sort=False); returns the sorted result"""
+    a = gs.isect_tiles(_t(m2), _t(radii), _t(dep), 16, tw, th, **kw)
+    u = gs.isect_tiles(_t(m2), _t(radii), _t(dep), 16, tw, th, sort=False, **kw)
+    ids, perm = torch.sort(u[1], stable=True)
+    assert torch.equal(a[0], u[0]) and torch.equal(a[1], ids) and torch.equal(a[2], u[2][perm])
+    return a
+
+
 def test_isect_sorted_equals_stable_sort_of_unsorted(gs):
     """The two-level sort (rows by depth, then intersections by (image, tile) bits only) must give exactly what
     one stable sort of the reference's unsorted emission gives (csrc/Intersect.cpp:283-326)."""
 
     def check(m2, radii, dep, tw, th, **kw):
-        a = gs.isect_tiles(_t(m2), _t(radii), _t(dep), 16, tw, th, **kw)
-        u = gs.isect_tiles(_t(m2), _t(radii), _t(dep), 16, tw, th, sort=False, **kw)
-        ids, perm = torch.sort(u[1], stable=True)
-        assert torch.equal(a[0], u[0]) and torch.equal(a[1], ids) and torch.equal(a[2], u[2][perm])
-        return a
+        return isect_sorted_equals_stable_sort(gs, m2, radii, dep, tw, th, **kw)
 
     sc = scene.make_scene(n_max=80000)
     W, H = 800, 450

@@ -13,14 +13,9 @@
 * Tile intersection on the GPU's own projected rows and on a 2D adversarial set: accu and AABB, sorted and unsorted,
   equal the float32 oracle bit for bit; isect_tiles_sorted and the fused row side outputs equal isect_tiles;
   isect_tiles_sparse equals the masked subset of the AABB list; every decided pixel of alpha >= 1/255 is listed; and
-  the serial emit (GSB200_EMIT=serial, read once per process, so run in a subprocess) lists the same intersections as
-  the warp-cooperative one.
+  the one-thread-per-row emit lists the same intersections as the warp-cooperative one.
 """
 import math
-import os
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -28,11 +23,9 @@ import torch
 
 from oracle import gso
 from tests import projection_edges as pe
-from tests.test_gpu_parity import _n, _t, gs  # noqa: F401  (gs: fixture)
+from tests.test_gpu_parity import _n, _t, gs, isect_sorted_equals_stable_sort  # noqa: F401  (gs: fixture)
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -283,34 +276,19 @@ def test_isect_vs_oracle_and_coverage(gs, sweep):
         assert np.array_equal(np.diff(_n(offs)), lens)
 
 
-_SERIAL = r"""
-import sys, numpy as np, torch
-sys.path.insert(0, sys.argv[1])
-import gsplat_b200 as gs
-d = np.load(sys.argv[2])
-out = {}
-for k in range(int(d["n"])):
-    t = lambda a: torch.from_numpy(d[f"{a}{k}"]).to("cuda:0")
-    tw, th = (int(v) for v in d[f"grid{k}"])
-    tpg, ids, fl = gs.isect_tiles(t("m2"), t("radii"), t("dep"), 16, tw, th, conics=t("con"), opacities=t("op"))
-    out[f"ids{k}"], out[f"fl{k}"] = ids.cpu().numpy(), fl.cpu().numpy()
-np.savez(sys.argv[3], **out)
-"""
-
-
 def test_serial_emit_equals_cooperative(gs, sweep):
-    sets = _isect_sets(gs, sweep)
-    with tempfile.TemporaryDirectory() as tmp:
-        inp, outp = os.path.join(tmp, "in.npz"), os.path.join(tmp, "out.npz")
-        d = {"n": np.array(len(sets))}
-        for k, (_, m2, radii, dep, con, op, W2, H2) in enumerate(sets):
-            d.update({f"m2{k}": m2, f"radii{k}": radii, f"dep{k}": dep, f"con{k}": con, f"op{k}": op,
-                      f"grid{k}": np.array([math.ceil(W2 / 16), math.ceil(H2 / 16)])})
-        np.savez(inp, **d)
-        env = dict(os.environ, GSB200_EMIT="serial")
-        subprocess.run([sys.executable, "-c", _SERIAL, ROOT, inp, outp], check=True, env=env, timeout=600)
-        ser = np.load(outp)
-        for k, (name, m2, radii, dep, con, op, W2, H2) in enumerate(sets):
-            _, ids, fl = gs.isect_tiles(_t(m2), _t(radii), _t(dep), 16, math.ceil(W2 / 16), math.ceil(H2 / 16),
-                                        conics=_t(con), opacities=_t(op))
-            assert np.array_equal(ser[f"ids{k}"], _n(ids)) and np.array_equal(ser[f"fl{k}"], _n(fl)), name
+    """Sorted dense isect_tiles picks its emit kernel from the largest tile count of a row: one thread per row up to 96
+    tiles, warp-cooperative above; the unsorted path always emits cooperatively.  With the rows of more than 96 tiles
+    culled (radius 0), the sorted lists come from the one-thread-per-row kernel and must equal a stable sort of the
+    cooperative emission; on the full sets both sides are cooperative."""
+    for name, m2, radii, dep, con, op, W2, H2 in _isect_sets(gs, sweep):
+        tw, th = math.ceil(W2 / 16), math.ceil(H2 / 16)
+        kw = dict(conics=_t(con), opacities=_t(op))
+        tpg = _n(gs.isect_tiles(_t(m2), _t(radii), _t(dep), 16, tw, th, **kw)[0])
+        few = radii.copy()
+        few[tpg > 96] = 0
+        for rows, r in (("rows of <= 96 tiles", few), ("all rows", radii)):
+            a = isect_sorted_equals_stable_sort(gs, m2, r, dep, tw, th, **kw)
+            t = _n(a[0])
+            assert a[2].numel() > 1000, f"{name}, {rows}"
+            assert (t.max() <= 96) == (r is few), f"{name}, {rows}: largest row lists {t.max()} tiles"
