@@ -77,13 +77,9 @@ _SIGNATURES = {
         [c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_int, c_vp, c_vp, c_vp, c_vp,
          c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     ),
-    "gsb200_isect_depth_order_workspace_bytes": (c_sz, [c_i64, c_i64]),
-    "gsb200_isect_depth_order": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),
     "gsb200_isect_scan_workspace_bytes": (c_sz, [c_i64]),
-    "gsb200_isect_count": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp, c_sz, c_vp]),
-    "gsb200_isect_emit": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp]),
-    "gsb200_sort_workspace_bytes": (c_sz, [c_i64, c_int, c_int]),
-    "gsb200_sort_pairs": (c_int, [c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),
+    "gsb200_isect_count": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp, c_sz, c_vp]),
+    "gsb200_isect_emit": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp]),
     "gsb200_l1_loss_workspace_bytes": (c_sz, []),
     "gsb200_l1_loss_fwd": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "gsb200_l1_loss_bwd": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
@@ -95,11 +91,6 @@ _SIGNATURES = {
     "gsb200_p2p_allreduce_f32": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp]),
     "gsb200_rows_allreduce_f32": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp, c_vp]),
     "gsb200_isect_count_totals": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp]),
-    "gsb200_isect_order_visible_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64]),
-    "gsb200_isect_order_visible": (c_int, [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),
-    "gsb200_isect_emit_ordered": (
-        c_int, [c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp],
-    ),
     "gsb200_project_sh_fwd_rows": (
         c_int,
         [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32, c_f32, c_u32,
@@ -113,8 +104,8 @@ _SIGNATURES = {
     "gsb200_isect_sorted_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_i64, c_int, c_u32, c_u32]),
     "gsb200_isect_sorted": (
         c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp,
-         c_vp, c_sz, c_vp],
+        [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_vp,
+         c_vp, c_vp, c_sz, c_vp],
     ),
     "gsb200_sort_tile_pairs_workspace_bytes": (c_sz, [c_i64, c_int, c_int]),
     "gsb200_sort_tile_pairs": (c_int, [c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),

@@ -1048,18 +1048,15 @@ __device__ __forceinline__ int tiles_of_gaussian(
     return count;
 }
 
-// `order` (optional): thread j handles row order[j] (the depth order of gsb200_isect_depth_order) and also
-// writes its count to counts_in_order[j], the array the scan runs over.
+// row-order tile count of every row (the unsorted intersection's first pass)
 __global__ void __launch_bounds__(kThreads) isect_count_kernel(
     int64_t total, const float *__restrict__ means2d, const int32_t *__restrict__ radii, const float *__restrict__ conics,
-    const float *__restrict__ opacities, const int32_t *__restrict__ order, uint32_t tile_size, uint32_t tw, uint32_t th,
-    int32_t *__restrict__ tiles_per_gauss, int32_t *__restrict__ counts_in_order
+    const float *__restrict__ opacities, uint32_t tile_size, uint32_t tw, uint32_t th, int32_t *__restrict__ tiles_per_gauss
 )
 {
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(j >= total)
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(i >= total)
         return;
-    const int64_t i = order ? (int64_t)order[j] : j;
     const int2 r    = reinterpret_cast<const int2 *>(radii)[i];
     int cnt         = 0;
     if(r.x > 0 && r.y > 0)
@@ -1072,8 +1069,6 @@ __global__ void __launch_bounds__(kThreads) isect_count_kernel(
         cnt = tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [](int64_t) {});
     }
     tiles_per_gauss[i] = cnt;
-    if(order)
-        counts_in_order[j] = cnt;
 }
 
 // row-order count + the totals the host reads once: [0] = number of intersections, [1] = rows with tiles,
@@ -1783,13 +1778,13 @@ extern "C" size_t gsb200_isect_scan_workspace_bytes(int64_t n_elements)
     if(n_elements <= 0)
         return 0;
     cub::DeviceScan::InclusiveSum((void *)nullptr, bytes, (const int32_t *)nullptr, (int64_t *)nullptr, n_elements);
-    return ((bytes + 255) & ~(size_t)255) + sizeof(int32_t) * (size_t)n_elements + 256; // + counts in depth order
+    return bytes + 256;
 }
 
 extern "C" int gsb200_isect_count(
     int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *conics, const float *opacities,
-    const int32_t *order, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *tiles_per_gauss,
-    int64_t *cum_tiles, void *workspace, size_t workspace_bytes, void *stream
+    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *tiles_per_gauss, int64_t *cum_tiles,
+    void *workspace, size_t workspace_bytes, void *stream
 )
 {
     if(I < 0 || N < 0 || tile_size == 0)
@@ -1804,23 +1799,21 @@ extern "C" int gsb200_isect_count(
     cudaStream_t st = (cudaStream_t)stream;
     size_t need     = 0;
     cub::DeviceScan::InclusiveSum((void *)nullptr, need, tiles_per_gauss, cum_tiles, total, st);
-    const size_t scan_bytes = (need + 255) & ~(size_t)255;
-    if(scan_bytes + (order ? sizeof(int32_t) * (size_t)total : 0) > workspace_bytes)
+    if(need > workspace_bytes)
         return GSB200_E_WORKSPACE;
-    int32_t *counts_in_order = order ? reinterpret_cast<int32_t *>(static_cast<char *>(workspace) + scan_bytes) : nullptr;
     isect_count_kernel<<<grid_for(total, kThreads), kThreads, 0, st>>>(
-        total, means2d, radii, conics, opacities, order, tile_size, tile_width, tile_height, tiles_per_gauss, counts_in_order
+        total, means2d, radii, conics, opacities, tile_size, tile_width, tile_height, tiles_per_gauss
     );
     if(int rc = check_launch())
         return rc;
-    GSB_CUDA_TRY(cub::DeviceScan::InclusiveSum(workspace, need, order ? counts_in_order : tiles_per_gauss, cum_tiles, total, st));
+    GSB_CUDA_TRY(cub::DeviceScan::InclusiveSum(workspace, need, tiles_per_gauss, cum_tiles, total, st));
     return GSB200_OK;
 }
 
 extern "C" int gsb200_isect_emit(
     int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const float *conics,
-    const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, const int32_t *order, uint32_t tile_size,
-    uint32_t tile_width, uint32_t tile_height, int64_t *isect_ids, int32_t *flatten_ids, void *stream
+    const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, uint32_t tile_size, uint32_t tile_width,
+    uint32_t tile_height, int64_t *isect_ids, int32_t *flatten_ids, void *stream
 )
 {
     if(I < 0 || N < 0 || tile_size == 0)
@@ -1835,14 +1828,14 @@ extern "C" int gsb200_isect_emit(
     if(bits_for_count(I) + tile_bits > 32)
         return GSB200_E_KEYBITS;
     isect_emit_coop_kernel<int64_t><<<grid_for(total, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
-        total, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width, tile_height,
+        total, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, nullptr, tile_size, tile_width, tile_height,
         tile_bits, isect_ids, flatten_ids
     );
     return check_launch();
 }
 
 // ---- tile intersection restricted to the tiles of a mask (isect_tiles_sparse).  Same enumeration as the dense AABB
-// path (tiles_of_gaussian without conics), in the depth order of gsb200_isect_depth_order; a tile whose tile_mask entry
+// path (tiles_of_gaussian without conics), in the depth order of gsb::depth_order (sort.cu); a tile whose tile_mask entry
 // is 0 is neither counted nor emitted.  Keys are dense tile ids image * th * tw + tile (32 bits).
 namespace gsb
 {
@@ -1942,7 +1935,7 @@ static SparseCountLayout sparse_count_layout(int64_t I, int64_t total)
     size_t scan = 0;
     cub::DeviceScan::InclusiveSum((void *)nullptr, scan, (const int32_t *)nullptr, (int64_t *)nullptr, total);
     L.depth  = 0;
-    L.counts = L.depth + al(gsb200_isect_depth_order_workspace_bytes(I, total));
+    L.counts = L.depth + al(depth_order_workspace_bytes(I, total));
     L.scan   = L.counts + al(sizeof(int32_t) * (size_t)total);
     L.total  = L.scan + al(scan) + 256;
     return L;
@@ -2003,7 +1996,7 @@ extern "C" int gsb200_isect_sparse_count(
     char *ws        = static_cast<char *>(workspace);
     cudaStream_t st = (cudaStream_t)stream;
     // 1. rows in (image, depth) order
-    if(int rc = gsb200_isect_depth_order(I, N, radii, depths, image_ids, order, ws + L.depth, L.counts - L.depth, stream))
+    if(int rc = gsb::depth_order(I, N, radii, depths, image_ids, order, ws + L.depth, L.counts - L.depth, st))
         return rc;
     // 2. masked tile counts in that order; 3. inclusive scan
     int32_t *counts = reinterpret_cast<int32_t *>(ws + L.counts);
@@ -2093,58 +2086,38 @@ extern "C" int gsb200_isect_count_totals(
 
 namespace gsb
 {
-template<class KeyT>
-static int emit_ordered(
-    int64_t I, int64_t N, int64_t n_order, int64_t max_tiles_hint, const float *means2d, const int32_t *radii, const float *depths,
+// stage of gsb200_isect_sorted (sort.cu), which checked the arguments: emission of the cap_vis depth-ordered row slots
+// into capacity-sized outputs, real counts in `totals` (device)
+int emit_tilekeys_bounded(
+    int64_t N, int64_t cap_vis, int64_t max_tiles_hint, const float *means2d, const int32_t *radii, const float *depths,
     const float *conics, const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, const int32_t *order,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, KeyT *keys, int32_t *flatten_ids, void *stream,
-    const int64_t *totals = nullptr, int64_t cap_isects = 0
+    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int key_bytes, void *keys, int32_t *flatten_ids,
+    const int64_t *totals, int64_t cap_isects, cudaStream_t st
 )
 {
-    if(I < 0 || N < 0 || n_order < 0 || tile_size == 0)
-        return GSB200_E_INVALID;
-    if(n_order == 0)
-        return GSB200_OK;
-    if(!means2d || !radii || !depths || !cum_tiles || !order || !keys || !flatten_ids)
-        return GSB200_E_INVALID;
     const uint32_t tile_bits = bits_for_count((int64_t)tile_width * tile_height);
-    if(bits_for_count(I) + tile_bits > 32)
-        return GSB200_E_KEYBITS;
-    if(sizeof(KeyT) < 8 && bits_for_count(I * (int64_t)tile_width * tile_height) > 8 * sizeof(KeyT))
-        return GSB200_E_KEYBITS;
     // the cooperative kernel pays off when SOME gaussian covers many tiles (one lane looping over thousands of tiles is the
     // tail of the whole launch); when even the largest row has few, the plain one-thread-per-gaussian kernel is leaner
     // (38 vs 45 us at cfg3)
-    if(max_tiles_hint > 0 && max_tiles_hint <= 96)
-        isect_emit_kernel<KeyT><<<grid_for(n_order, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
-            n_order, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width, tile_height,
-            tile_bits, keys, flatten_ids, totals, cap_isects
-        );
-    else
-        isect_emit_coop_kernel<KeyT><<<grid_for(n_order, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
-            n_order, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width, tile_height,
-            tile_bits, keys, flatten_ids, totals, cap_isects
-        );
-    return check_launch();
-}
-
-// stage of gsb200_isect_sorted (sort.cu): emission into capacity-sized outputs, real counts in `totals` (device)
-int emit_tilekeys_bounded(
-    int64_t I, int64_t N, int64_t cap_vis, int64_t max_tiles_hint, const float *means2d, const int32_t *radii, const float *depths,
-    const float *conics, const float *opacities, const int64_t *cum_tiles, const int32_t *order, uint32_t tile_size,
-    uint32_t tile_width, uint32_t tile_height, int key_bytes, void *keys, int32_t *flatten_ids, const int64_t *totals,
-    int64_t cap_isects, cudaStream_t st
-)
-{
+    const bool serial = max_tiles_hint > 0 && max_tiles_hint <= 96;
+    auto launch = [&](auto *k) {
+        using KeyT = std::remove_pointer_t<decltype(k)>;
+        if(serial)
+            isect_emit_kernel<KeyT><<<grid_for(cap_vis, kThreads), kThreads, 0, st>>>(
+                cap_vis, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width,
+                tile_height, tile_bits, k, flatten_ids, totals, cap_isects
+            );
+        else
+            isect_emit_coop_kernel<KeyT><<<grid_for(cap_vis, kThreads), kThreads, 0, st>>>(
+                cap_vis, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width,
+                tile_height, tile_bits, k, flatten_ids, totals, cap_isects
+            );
+    };
     if(key_bytes == 2)
-        return emit_ordered<uint16_t>(
-            I, N, cap_vis, max_tiles_hint, means2d, radii, depths, conics, opacities, cum_tiles, nullptr, order, tile_size, tile_width,
-            tile_height, static_cast<uint16_t *>(keys), flatten_ids, st, totals, cap_isects
-        );
-    return emit_ordered<uint32_t>(
-        I, N, cap_vis, max_tiles_hint, means2d, radii, depths, conics, opacities, cum_tiles, nullptr, order, tile_size, tile_width,
-        tile_height, static_cast<uint32_t *>(keys), flatten_ids, st, totals, cap_isects
-    );
+        launch(static_cast<uint16_t *>(keys));
+    else
+        launch(static_cast<uint32_t *>(keys));
+    return check_launch();
 }
 
 // offsets[(image, tile)] from sorted dense tile ids (narrow keys): same contract as isect_offsets_kernel
@@ -2205,18 +2178,6 @@ __global__ void __launch_bounds__(kThreads) isect_ids_from_tilekeys_kernel(
     isect_ids[s] = (((image << tile_n_bits) | tile) << 32) | (int64_t)__float_as_uint(depths[flatten_ids[s]]);
 }
 } // namespace gsb
-
-extern "C" int gsb200_isect_emit_ordered(
-    int64_t I, int64_t N, int64_t n_order, int64_t max_tiles_hint, const float *means2d, const int32_t *radii, const float *depths,
-    const float *conics, const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, const int32_t *order,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t *isect_ids, int32_t *flatten_ids, void *stream
-)
-{
-    return gsb::emit_ordered<int64_t>(
-        I, N, n_order, max_tiles_hint, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width,
-        tile_height, isect_ids, flatten_ids, stream
-    );
-}
 
 extern "C" int gsb200_isect_ids_from_tilekeys(
     int64_t n_isects, int key_bytes, const void *tile_keys, const int32_t *flatten_ids, const float *depths, int64_t I,

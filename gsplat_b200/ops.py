@@ -738,66 +738,21 @@ def isect_tiles(
     tiles_per_gauss = torch.empty(image_dims + (N,), device=dev, dtype=torch.int32)
     if total == 0:
         return (tiles_per_gauss, torch.empty(0, device=dev, dtype=torch.int64), torch.empty(0, device=dev, dtype=torch.int32))
+    if sort:
+        hits = isect_tiles_sorted(
+            means2d, radii, depths, tile_size, tile_width, tile_height, conics=conics, opacities=opacities,
+            n_images=I if packed else None, image_ids=img_ids, _exact=True,
+        )
+        return hits.tiles_per_gauss, hits.isect_ids(), hits.flatten_ids
+    # unsorted (the reference's sort=False output): row-order count, scan, emission
     accu = conics is not None and opacities is not None
-    if sort and not packed:
-        # dense, sorted (the rasterization() path): count first, read both totals with ONE host sync, then order and
-        # scan only the rows that have tiles (a third of the rows at BASELINE configs[2]: the culled ones never enter
-        # the four radix passes of the depth order)
-        totals = torch.empty(3, device=dev, dtype=torch.int64)
-        with _Ctx(dev) as st:
-            check(
-                L.gsb200_isect_count_totals(
-                    I, N, ptr(means2d), ptr(radii), ptr(conics) if accu else None, ptr(opacities) if accu else None, tile_size,
-                    tile_width, tile_height, ptr(tiles_per_gauss), ptr(totals), st,
-                ),
-                "intersect_tile (count)",
-            )
-            n_isects, n_vis, max_tiles = (int(v) for v in totals.tolist())  # the one host sync of the forward (reference: csrc/Intersect.cpp:259)
-            isect_ids = torch.empty(n_isects, device=dev, dtype=torch.int64)
-            flatten_ids = torch.empty(n_isects, device=dev, dtype=torch.int32)
-            if n_isects == 0:
-                return tiles_per_gauss, isect_ids, flatten_ids
-            order = torch.empty(n_vis, device=dev, dtype=torch.int32)
-            cum = torch.empty(n_vis, device=dev, dtype=torch.int64)
-            ws = _scratch_buffer(dev, "vorder", L.gsb200_isect_order_visible_workspace_bytes(I, total, n_vis))
-            check(
-                L.gsb200_isect_order_visible(I, N, n_vis, ptr(tiles_per_gauss), ptr(depths), None, ptr(order), ptr(cum), ptr(ws), ws.numel(), st),
-                "intersect_tile (order)",
-            )
-            check(
-                L.gsb200_isect_emit_ordered(
-                    I, N, n_vis, max_tiles, ptr(means2d), ptr(radii), ptr(depths), ptr(conics) if accu else None,
-                    ptr(opacities) if accu else None, ptr(cum), None, ptr(order), tile_size, tile_width, tile_height,
-                    ptr(isect_ids), ptr(flatten_ids), st,
-                ),
-                "intersect_tile (emit)",
-            )
-            begin_bit, end_bit = 32, 32 + tile_bits + image_bits
-            keys_out, vals_out = torch.empty_like(isect_ids), torch.empty_like(flatten_ids)
-            ws = _scratch_buffer(dev, "sort", L.gsb200_sort_workspace_bytes(n_isects, begin_bit, end_bit))
-            check(
-                L.gsb200_sort_pairs(
-                    n_isects, begin_bit, end_bit, ptr(isect_ids), ptr(flatten_ids), ptr(keys_out), ptr(vals_out), ptr(ws), ws.numel(), st,
-                ),
-                "intersect_tile (sort)",
-            )
-        return tiles_per_gauss, keys_out, vals_out
     cum = torch.empty(total, device=dev, dtype=torch.int64)
     with _Ctx(dev) as st:
-        order = None
-        if sort:
-            # pass 0: rows in (image, depth) order, so that the S-sized sort below only has the (image, tile) bits left
-            order = torch.empty(total, device=dev, dtype=torch.int32)
-            ws = _scratch_buffer(dev, "dorder", L.gsb200_isect_depth_order_workspace_bytes(I, total))
-            check(
-                L.gsb200_isect_depth_order(I, N, ptr(radii), ptr(depths), ptr(img_ids), ptr(order), ptr(ws), ws.numel(), st),
-                "intersect_tile (depth order)",
-            )
         ws = _scratch_buffer(dev, "scan", L.gsb200_isect_scan_workspace_bytes(total))
         check(
             L.gsb200_isect_count(
                 I_count, N, ptr(means2d), ptr(radii), ptr(conics) if accu else None, ptr(opacities) if accu else None,
-                ptr(order), tile_size, tile_width, tile_height, ptr(tiles_per_gauss), ptr(cum), ptr(ws), ws.numel(), st,
+                tile_size, tile_width, tile_height, ptr(tiles_per_gauss), ptr(cum), ptr(ws), ws.numel(), st,
             ),
             "intersect_tile (count)",
         )
@@ -809,29 +764,18 @@ def isect_tiles(
         check(
             L.gsb200_isect_emit(
                 I, N, ptr(means2d), ptr(radii), ptr(depths), ptr(conics) if accu else None,
-                ptr(opacities) if accu else None, ptr(cum), ptr(img_ids), ptr(order), tile_size, tile_width, tile_height,
+                ptr(opacities) if accu else None, ptr(cum), ptr(img_ids), tile_size, tile_width, tile_height,
                 ptr(isect_ids), ptr(flatten_ids), st,
             ),
             "intersect_tile (emit)",
         )
-        if sort:
-            begin_bit, end_bit = 32, 32 + tile_bits + image_bits
-            keys_out, vals_out = torch.empty_like(isect_ids), torch.empty_like(flatten_ids)
-            ws = _scratch_buffer(dev, "sort", L.gsb200_sort_workspace_bytes(n_isects, begin_bit, end_bit))
-            check(
-                L.gsb200_sort_pairs(
-                    n_isects, begin_bit, end_bit, ptr(isect_ids), ptr(flatten_ids), ptr(keys_out), ptr(vals_out), ptr(ws),
-                    ws.numel(), st,
-                ),
-                "intersect_tile (sort)",
-            )
-            isect_ids, flatten_ids = keys_out, vals_out
     return tiles_per_gauss, isect_ids, flatten_ids
 
 
 class _IsectPredictor:
-    """Capacities for gsb200_isect_sorted from the totals of the last calls on the same (device, image count, tile grid),
-    and the asynchronous host read of the current totals (a kernel stores them into pinned memory, the host polls)."""
+    """Capacities for gsb200_isect_sorted from the totals of the last calls on the same (device, image count, tile grid,
+    row layout), and the asynchronous host read of the current totals (a kernel stores them into pinned memory, the host
+    polls)."""
 
     def __init__(self, dev: torch.device):
         self.hist = []  # (n_isects, n_vis, max_tiles) of the last 8 calls
@@ -891,8 +835,8 @@ class _IsectPredictor:
 _predictors = {}
 
 
-def _isect_predictor(dev: torch.device, I: int, tile_width: int, tile_height: int) -> _IsectPredictor:
-    key = (dev.index, I, tile_width, tile_height, stream(dev.index))
+def _isect_predictor(dev: torch.device, I: int, tile_width: int, tile_height: int, packed: bool = False) -> _IsectPredictor:
+    key = (dev.index, I, tile_width, tile_height, packed, stream(dev.index))
     p = _predictors.get(key)
     if p is None:
         p = _predictors[key] = _IsectPredictor(dev)
@@ -931,18 +875,27 @@ class SortedIntersections:
 def isect_tiles_sorted(
     means2d: Tensor, radii: Tensor, depths: Tensor, tile_size: int, tile_width: int, tile_height: int,
     conics: Optional[Tensor] = None, opacities: Optional[Tensor] = None, precounted: Optional[RowSideOutputs] = None,
+    n_images: Optional[int] = None, image_ids: Optional[Tensor] = None, _exact: bool = False,
 ) -> SortedIntersections:
-    """Dense-layout tile intersection + offsets for rasterization(): same intersections in the same order as
-    ``isect_tiles(sort=True)`` + ``isect_offset_encode`` (reference: csrc/Intersect.cpp:203-326, 330-382), with the
-    S-sized sort done on 2- or 4-byte dense tile ids instead of the 8-byte (image | tile | depth) ids."""
+    """Sorted tile intersection + offsets, the reference's sorted ``isect_tiles`` + ``isect_offset_encode``
+    (csrc/Intersect.cpp:203-326, 330-382), with the S-sized sort done on 2- or 4-byte dense tile ids instead of the
+    8-byte (image | tile | depth) ids.  Rows are dense ([..., N, 2] means2d), or packed ([nnz, 2] means2d with
+    ``n_images`` and the image of each row in ``image_ids``).  The stage is launched on capacities predicted from the
+    earlier calls of the same shape.  ``_exact`` (isect_tiles) reads the totals first and sizes the stage exactly, and
+    leaves that history alone: the call's own largest row then picks the emit kernel."""
     dev = require_cuda(means2d, radii, depths)
     means2d, depths = f32c(means2d, "means2d"), f32c(depths, "depths")
     conics, opacities = f32c(conics, "conics"), f32c(opacities, "opacities")
     if radii.dtype != torch.int32:
         raise TypeError("radii must be int32")
     radii = radii.contiguous()
-    image_dims = tuple(means2d.shape[:-2])
-    I, N = _prod(image_dims), means2d.shape[-2]
+    packed = image_ids is not None
+    if packed:
+        image_dims, I, N = (), int(n_images), means2d.shape[0]
+        image_ids = image_ids.to(torch.int64).contiguous()
+    else:
+        image_dims = tuple(means2d.shape[:-2])
+        I, N = _prod(image_dims), means2d.shape[-2]
     L = lib()
     n_tiles = tile_width * tile_height
     image_bits, tile_bits = _cabi.bits_for_count(I), _cabi.bits_for_count(n_tiles)
@@ -954,9 +907,10 @@ def isect_tiles_sorted(
     key_bits = _cabi.bits_for_count(I * n_tiles)
     key_bytes = 2 if key_bits <= 16 else 4
     key_dtype = torch.int16 if key_bytes == 2 else torch.int32  # raw storage; the kernels read them unsigned
-    total = I * N
+    I_count = 1 if packed else I  # the count sees packed rows as one flat list of N rows
+    total = I_count * N
     have_counts = (
-        precounted is not None and precounted.totals is not None and total > 0
+        not packed and precounted is not None and precounted.totals is not None and total > 0
         and (precounted.tile_size, precounted.tile_width, precounted.tile_height) == (tile_size, tile_width, tile_height)
         and precounted.tiles_per_gauss.numel() == total and conics is not None and opacities is not None
     )
@@ -978,12 +932,12 @@ def isect_tiles_sorted(
     if total == 0:
         return empty()
     totals = precounted.totals if have_counts else torch.empty(3, device=dev, dtype=torch.int64)
-    pred = _isect_predictor(dev, I, tile_width, tile_height)
+    pred = None if _exact else _isect_predictor(dev, I, tile_width, tile_height, packed)
     with _Ctx(dev) as st:
         if not have_counts:
             check(
                 L.gsb200_isect_count_totals(
-                    I, N, ptr(means2d), ptr(radii), ptr(conics) if accu else None, ptr(opacities) if accu else None, tile_size,
+                    I_count, N, ptr(means2d), ptr(radii), ptr(conics) if accu else None, ptr(opacities) if accu else None, tile_size,
                     tile_width, tile_height, ptr(tiles_per_gauss), ptr(totals), st,
                 ),
                 "intersect_tile (count)",
@@ -993,18 +947,18 @@ def isect_tiles_sorted(
             # compaction, depth order, scan, emission, tile sort, offsets: one call, every launch sized by the capacities
             keys_out = torch.empty(cap_isects, device=dev, dtype=key_dtype)
             vals_out = torch.empty(cap_isects, device=dev, dtype=torch.int32)
-            ws = _scratch_buffer(dev, "isect", L.gsb200_isect_sorted_workspace_bytes(I, N, cap_vis, cap_isects, key_bytes, tile_width, tile_height))
+            ws = _scratch_buffer(dev, "isect", L.gsb200_isect_sorted_workspace_bytes(I, total, cap_vis, cap_isects, key_bytes, tile_width, tile_height))
             check(
                 L.gsb200_isect_sorted(
                     I, N, ptr(means2d), ptr(radii), ptr(depths), ptr(conics) if accu else None, ptr(opacities) if accu else None,
-                    tile_size, tile_width, tile_height, ptr(tiles_per_gauss), ptr(totals), cap_vis, cap_isects, max_tiles, key_bytes,
+                    ptr(image_ids), tile_size, tile_width, tile_height, ptr(tiles_per_gauss), ptr(totals), cap_vis, cap_isects, max_tiles, key_bytes,
                     ptr(keys_out), ptr(vals_out), ptr(offsets), ptr(ws), ws.numel(), st,
                 ),
                 "intersect_tile (sorted)",
             )
             return keys_out, vals_out
 
-        caps = pred.capacities(total)
+        caps = pred.capacities(total) if pred is not None else None
         if caps is not None:
             # Launch on PREDICTED capacities, then read the totals: the host read (the reference's one sync of the forward,
             # csrc/Intersect.cpp:259) overlaps the queued stage instead of idling the GPU.  A miss (a count above its
@@ -1022,8 +976,9 @@ def isect_tiles_sorted(
                 pred.hits += 1
                 keys_out, vals_out = keys_out[:n_isects], vals_out[:n_isects]
         else:
-            n_isects, n_vis, max_tiles = (int(v) for v in totals.tolist())  # first call of a shape: exact sizes
-            pred.observe(n_isects, n_vis, max_tiles)
+            n_isects, n_vis, max_tiles = (int(v) for v in totals.tolist())  # exact sizes (first call of a shape)
+            if pred is not None:
+                pred.observe(n_isects, n_vis, max_tiles)
             if n_isects == 0:
                 return empty()
             keys_out, vals_out = run(n_vis, n_isects, max_tiles)

@@ -22,8 +22,6 @@ from .ops import (
     RowSideOutputs,
     fully_fused_projection,
     fused_project_sh,
-    isect_offset_encode,
-    isect_tiles,
     isect_tiles_sorted,
     rasterize_to_pixels,
     rasterize_to_pixels_rows,
@@ -377,21 +375,16 @@ def rasterization(
     # ---- tile intersection (AccuTile) + offsets
     tile_width = math.ceil(width / float(tile_size))
     tile_height = math.ceil(height / float(tile_size))
-    # packed rows, reference-shaped op sequence: depth order, count, emit, radix sort on the (image, tile) bits, offsets
-    if packed:
-        tiles_per_gauss, isect_ids, flatten_ids = isect_tiles(
-            means2d, radii, depths, tile_size, tile_width, tile_height, sort=True, segmented=segmented, packed=True,
-            n_images=I, image_ids=batch_ids * C + camera_ids, gaussian_ids=gaussian_ids, conics=conics, opacities=opac,
-        )
-        isect_offsets = isect_offset_encode(isect_ids, I, tile_width, tile_height)
-    else:
-        # dense rows: the S-sized sort runs on 2- / 4-byte tile ids; meta["isect_ids"] (the reference's 64-bit ids) is
-        # rebuilt from them on first access
-        hits = isect_tiles_sorted(
-            means2d, radii, depths, tile_size, tile_width, tile_height, conics=conics, opacities=opac, precounted=rows_out,
-        )
-        tiles_per_gauss, flatten_ids, isect_offsets = hits.tiles_per_gauss, hits.flatten_ids, hits.isect_offsets
-        isect_ids = _Lazy(hits.isect_ids)
+    # the S-sized sort runs on 2- / 4-byte tile ids; meta["isect_ids"] (the reference's 64-bit ids) is rebuilt from them
+    # on first access
+    if packed and segmented:
+        raise ValueError("segmented sort is not supported for packed inputs")
+    hits = isect_tiles_sorted(
+        means2d, radii, depths, tile_size, tile_width, tile_height, conics=conics, opacities=opac, precounted=rows_out,
+        n_images=I if packed else None, image_ids=batch_ids * C + camera_ids if packed else None,
+    )
+    tiles_per_gauss, flatten_ids, isect_offsets = hits.tiles_per_gauss, hits.flatten_ids, hits.isect_offsets
+    isect_ids = _Lazy(hits.isect_ids)
     isect_offsets = isect_offsets.reshape(batch_dims + (C, tile_height, tile_width))
 
     # ---- assemble channels: [colour | depth]

@@ -190,56 +190,32 @@ extern "C"
     );
 
     /* ---- intersect_tile : ext.cpp:1022-1026, _wrapper.py:1196-1266, host csrc/Intersect.cpp:170-329 ----
-     * Pass 0 (sorted output only): order int32 [rows] = the projected rows in ascending (image, depth bits,
-     * row) order, culled rows (radii <= 0) last.  Emitting the intersections in this order leaves only the
-     * (image, tile) key bits for the S-sized sort -- same final order as the reference's one stable sort on
-     * (image, tile, depth).  rows = I*N, or N when image_ids (packed layout) is given. */
-    size_t gsb200_isect_depth_order_workspace_bytes(int64_t I, int64_t total_rows);
-    int gsb200_isect_depth_order(
-        int64_t I, int64_t N, const int32_t *radii, const float *depths, const int64_t *image_ids, int32_t *order,
-        void *workspace, size_t workspace_bytes, void *stream
-    );
-    /* Pass 1: tiles_per_gauss int32 [I*N] (row order) and the inclusive scan cum_tiles int64 [I*N] of the
-     * counts taken in `order` (NULL = row order).  conics + opacities given -> AccuTile/SNUGBOX ellipse test,
-     * else AABB from radii.  The caller reads cum_tiles[I*N-1] (= n_isects) to size the pass-2 outputs. */
+     * Unsorted output (the reference's sort=False), in row order.
+     * Pass 1: tiles_per_gauss int32 [I*N] and their inclusive scan cum_tiles int64 [I*N].  conics + opacities
+     * given -> AccuTile/SNUGBOX ellipse test, else AABB from radii.  The caller reads cum_tiles[I*N-1]
+     * (= n_isects) to size the pass-2 outputs. */
     size_t gsb200_isect_scan_workspace_bytes(int64_t n_elements);
     int gsb200_isect_count(
         int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *conics,
-        const float *opacities, const int32_t *order, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const float *opacities, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
         int32_t *tiles_per_gauss, int64_t *cum_tiles, void *workspace, size_t workspace_bytes, void *stream
     );
-    /* Pass 2: isect_ids int64 [n_isects], flatten_ids int32 [n_isects], emitted in `order` (NULL = row order,
-     * the reference's unsorted output).  Packed layout (reference packed=True): pass image_ids int64 [N]
-     * (the image of each of the N rows); pass 1 is then called with I = 1. */
+    /* Pass 2: isect_ids int64 [n_isects], flatten_ids int32 [n_isects], emitted in row order.  Packed layout
+     * (reference packed=True): pass image_ids int64 [N] (the image of each of the N rows); pass 1 is then
+     * called with I = 1. */
     int gsb200_isect_emit(
         int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const float *conics,
-        const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, const int32_t *order,
-        uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t *isect_ids, int32_t *flatten_ids,
-        void *stream
+        const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, uint32_t tile_size,
+        uint32_t tile_width, uint32_t tile_height, int64_t *isect_ids, int32_t *flatten_ids, void *stream
     );
-    /* Faster pass 0 / 1 for the sorted dense layout (round 2): count first, in row order, and hand the host BOTH totals
-     * -- totals[0] = n_isects, totals[1] = rows that have tiles, totals[2] = largest tile count of a row -- in one read; then order ONLY those rows:
-     * gsb200_isect_order_visible compacts them (stable), sorts them by (image, depth) and scans their counts in that
-     * order (order int32 [n_vis], cum_tiles int64 [n_vis]); gsb200_isect_emit_ordered emits from the n_vis ordered rows
-     * (max_tiles_hint = totals[2], the largest tile count of a row, or 0: picks the one-thread-per-gaussian or the
-     * warp-cooperative kernel).  totals is int64 [3].
-     * Same intersections in the same final order as gsb200_isect_depth_order + gsb200_isect_count + gsb200_isect_emit. */
+    /* Sorted output, first pass: the row-order count, and the totals the host reads -- totals[0] = n_isects,
+     * totals[1] = rows that have tiles, totals[2] = largest tile count of a row (max_tiles_hint of gsb200_isect_sorted:
+     * picks the one-thread-per-gaussian or the warp-cooperative emit kernel).  totals is int64 [3].  Packed layout:
+     * call with I = 1, N = the number of rows. */
     int gsb200_isect_count_totals(
         int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *conics, const float *opacities,
         uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *tiles_per_gauss, int64_t *totals,
         void *stream
-    );
-    size_t gsb200_isect_order_visible_workspace_bytes(int64_t I, int64_t total_rows, int64_t n_vis);
-    int gsb200_isect_order_visible(
-        int64_t I, int64_t N, int64_t n_vis, const int32_t *tiles_per_gauss, const float *depths,
-        const int64_t *image_ids, int32_t *order, int64_t *cum_tiles, void *workspace, size_t workspace_bytes,
-        void *stream
-    );
-    int gsb200_isect_emit_ordered(
-        int64_t I, int64_t N, int64_t n_order, int64_t max_tiles_hint, const float *means2d, const int32_t *radii, const float *depths,
-        const float *conics, const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids,
-        const int32_t *order, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t *isect_ids,
-        int32_t *flatten_ids, void *stream
     );
     /* Narrow keys (round 2): the rows are emitted in depth order, so the S-sized sort only needs the dense tile id
      * image * n_tiles + tile, as a key_bytes-wide (2 when I * n_tiles <= 65536, else 4) unsigned integer.
@@ -255,10 +231,12 @@ extern "C"
         int64_t n_isects, int key_bytes, const void *tile_keys, const int32_t *flatten_ids, const float *depths, int64_t I,
         uint32_t tile_width, uint32_t tile_height, int64_t *isect_ids, void *stream
     );
-    /* The sorted dense intersection stage in ONE call, sized by capacities (round 2): rows-with-tiles compaction, depth
+    /* The sorted intersection stage in ONE call, sized by capacities (round 2): rows-with-tiles compaction, depth
      * order, scan, emission of (dense tile id, row) pairs, stable sort on the tile id, offsets.  Inputs: the per-row tile
-     * counts and `totals` (int64 [3], DEVICE memory) of gsb200_isect_count_totals / gsb200_project_sh_fwd_rows.  Every
-     * launch is sized by cap_vis (<= I * N) and cap_isects; the real counts are read on the device: entries past
+     * counts and `totals` (int64 [3], DEVICE memory) of gsb200_isect_count_totals / gsb200_project_sh_fwd_rows.
+     * rows = I*N, or N when image_ids int64 [N] (packed layout, the image of each row) is given; I is always the number
+     * of images (tile ids, offsets) and total_rows of the workspace size is that row count.  Every
+     * launch is sized by cap_vis (<= rows) and cap_isects; the real counts are read on the device: entries past
      * totals[0] in tile_keys / flatten_ids ([cap_isects] each) are padding, nothing is written past a capacity, and
      * offsets int32 [I, th, tw] is exact whenever totals[1] <= cap_vis and totals[0] <= cap_isects.  A caller may
      * therefore launch with PREDICTED capacities before it has read the totals (the host read then overlaps this work
@@ -266,11 +244,12 @@ extern "C"
      * totals[0] entries if both counts fit, and otherwise call again with capacities = totals.  key_bytes: 2 when
      * I * th * tw <= 65536, else 4. */
     size_t gsb200_isect_sorted_workspace_bytes(
-        int64_t I, int64_t N, int64_t cap_vis, int64_t cap_isects, int key_bytes, uint32_t tile_width, uint32_t tile_height
+        int64_t I, int64_t total_rows, int64_t cap_vis, int64_t cap_isects, int key_bytes, uint32_t tile_width,
+        uint32_t tile_height
     );
     int gsb200_isect_sorted(
         int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const float *conics,
-        const float *opacities, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const float *opacities, const int64_t *image_ids, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
         const int32_t *tiles_per_gauss, const int64_t *totals, int64_t cap_vis, int64_t cap_isects, int64_t max_tiles_hint,
         int key_bytes, void *tile_keys, int32_t *flatten_ids, int32_t *offsets, void *workspace, size_t workspace_bytes,
         void *stream
@@ -279,13 +258,6 @@ extern "C"
      * stores from a one-warp kernel, then writes seq into host_mapped[3]: the host polls that word instead of waiting for
      * a copy (which takes a copy engine and queues behind PCIe uploads). */
     int gsb200_publish_totals(const int64_t *totals, int64_t *host_mapped, int64_t seq, void *stream);
-    /* Stable radix sort of (isect_ids, flatten_ids) on key bits [begin_bit, end_bit)
-     * (cub::DeviceRadixSort::SortPairs, csrc/IntersectTile.cu:1078-1121); begin_bit = 32 after pass 0. */
-    size_t gsb200_sort_workspace_bytes(int64_t n_isects, int begin_bit, int end_bit);
-    int gsb200_sort_pairs(
-        int64_t n_isects, int begin_bit, int end_bit, const int64_t *keys_in, const int32_t *vals_in,
-        int64_t *keys_out, int32_t *vals_out, void *workspace, size_t workspace_bytes, void *stream
-    );
     /* ---- intersect_offset : ext.cpp:1027, _wrapper.py:1328-1347 ---- offsets int32 [I, th, tw]. */
     int gsb200_isect_offsets(
         int64_t n_isects, const int64_t *isect_ids, int64_t I, uint32_t tile_width, uint32_t tile_height,

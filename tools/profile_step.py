@@ -97,8 +97,8 @@ if args.breakdown:
                                       g[2].data_ptr(), g[2].stride(-2), None, ptr(outs[0]), ptr(outs[1]), ptr(outs[2]), ptr(outs[3]), None, stream())
     ms_pb, _ = t(pb)
     ms_step, _ = t(step, 10)
-    print("note: each stage below is timed by calling its operator back to back outside autograd (wide-key isect_tiles, per-intersection "
-          "pack, no row records, host sync included): the stages do not add up to the step and are not what rasterization() runs since "
+    print("note: each stage below is timed by calling its operator back to back outside autograd (isect_tiles with its int64 ids rebuilt, "
+          "per-intersection pack, no row records, host sync included): the stages do not add up to the step and are not what rasterization() runs since "
           "round 2 -- use an ncu launch list of the real step for its shares")
-    print(f"BREAKDOWN ms: project_sh_fwd {ms_p:.3f} | isect(order+count+scan+sync+emit+sort) {ms_i:.3f} (unsorted {ms_in:.3f}) | offsets {ms_o:.3f} | "
+    print(f"BREAKDOWN ms: project_sh_fwd {ms_p:.3f} | isect(count+sync+order+scan+emit+sort+offsets+ids) {ms_i:.3f} (unsorted {ms_in:.3f}) | offsets {ms_o:.3f} | "
           f"raster_fwd(pack+raster) {ms_r:.3f} | raster_bwd(+memset) {ms_rb:.3f} | project_sh_bwd {ms_pb:.3f} | full step {ms_step:.3f}")
