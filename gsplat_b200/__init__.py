@@ -2,8 +2,9 @@
 
 Public names mirror /root/reference/gsplat/__init__.py:19-104 for the hot path:
 rasterization, fully_fused_projection, spherical_harmonics, isect_tiles, isect_offset_encode,
-rasterize_to_pixels, quat_scale_to_covar_preci, and the sparse-pixel ops build_sparse_tile_layout,
-isect_tiles_sparse, rasterize_to_pixels_sparse.  Importing the package does not need a GPU; calling an
+rasterize_to_pixels, quat_scale_to_covar_preci, the sparse-pixel ops build_sparse_tile_layout,
+isect_tiles_sparse, rasterize_to_pixels_sparse, and 2DGS: rasterization_2dgs, fully_fused_projection_2dgs,
+rasterize_to_pixels_2dgs (dense layout).  Importing the package does not need a GPU; calling an
 operator does (and needs gsplat_b200/libgsplat_b200.so, built by ``python -m gsplat_b200.build``).
 """
 from .ops import (  # noqa: F401
@@ -12,18 +13,20 @@ from .ops import (  # noqa: F401
     compute_relocation,
     mcmc_perturb_positions,
     fully_fused_projection,
+    fully_fused_projection_2dgs,
     fused_project_sh,
     isect_offset_encode,
     isect_tiles,
     isect_tiles_sparse,
     quat_scale_to_covar_preci,
     rasterize_to_pixels,
+    rasterize_to_pixels_2dgs,
     rasterize_to_pixels_sparse,
     spherical_harmonics,
 )
 from .losses import l1_loss, ssim_loss  # noqa: F401
 from .optimizers import SelectiveAdam  # noqa: F401
-from .rendering import rasterization  # noqa: F401
+from .rendering import rasterization, rasterization_2dgs  # noqa: F401
 
 __version__ = "0.1.0"
 
@@ -45,7 +48,8 @@ def has_reloc() -> bool:
 
 
 def has_2dgs() -> bool:
-    return False
+    """Reference: _wrapper.py:274 -- 2DGS (surfel) projection and compositing are built (dense layout)."""
+    return True
 
 
 def has_3dgut() -> bool:
@@ -72,6 +76,9 @@ __all__ = [
     "build_sparse_tile_layout",
     "isect_tiles_sparse",
     "rasterize_to_pixels_sparse",
+    "rasterization_2dgs",
+    "fully_fused_projection_2dgs",
+    "rasterize_to_pixels_2dgs",
     "quat_scale_to_covar_preci",
     "compute_relocation",
     "mcmc_perturb_positions",

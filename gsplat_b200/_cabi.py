@@ -147,6 +147,24 @@ _SIGNATURES = {
         [c_i64, c_int, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
          c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp],
     ),
+    "gsb200_surfel_projection_fwd": (
+        c_int,
+        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    ),
+    "gsb200_surfel_projection_bwd": (
+        c_int,
+        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    ),
+    "gsb200_surfel_raster_fwd": (
+        c_int,
+        [c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64,
+         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    ),
+    "gsb200_surfel_raster_bwd": (
+        c_int,
+        [c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64,
+         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    ),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

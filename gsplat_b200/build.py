@@ -26,6 +26,7 @@ UNITS = {
     "sort.cu": [],
     "nvls.cu": [],
     "loss.cu": [],
+    "surfel.cu": ["-fmad=false"],
 }
 HEADERS = ["common.cuh", "gaussmath.cuh", "rowrec.cuh", os.path.join("..", "..", "include", "gsplat_b200.h")]
 

@@ -6,6 +6,8 @@ executable form).  ``apply()`` rebinds, in place, the names the reference's call
                         isect_offset_encode, rasterize_to_pixels, adam}        (_wrapper.py:419,436,657,819,1196,1328,1497)
   gsplat.cuda._wrapper.{build_sparse_tile_layout, isect_tiles_sparse,
                         rasterize_to_pixels_sparse}                          (_wrapper.py:1433,1352,1566)
+  gsplat.rasterization_2dgs / gsplat.rendering.rasterization_2dgs            (rendering.py:1358)
+  gsplat.cuda._wrapper.{fully_fused_projection_2dgs, rasterize_to_pixels_2dgs} (_wrapper.py:2633,2918)
   gsplat.<the same re-exports>                                               (__init__.py:23-62)
   gsplat.relocation.compute_relocation (+ its import in gsplat.strategy.ops) (relocation.py:25, strategy/ops.py:26)
   gsplat.strategy.ops._cuda_fused_mcmc_perturb                               (strategy/ops.py:405)
@@ -42,6 +44,8 @@ _OPS = (
     "isect_tiles_sparse",
     "rasterize_to_pixels_sparse",
 )
+# rebound only where the package has them (its build may leave 2DGS out)
+_OPS_2DGS = ("fully_fused_projection_2dgs", "rasterize_to_pixels_2dgs")
 
 _saved: List[Tuple[object, str, object]] = []
 
@@ -95,13 +99,13 @@ def apply(losses: bool = True, ops: bool = True) -> Dict[str, object]:
         _apply_ops(B, G)
     if losses:
         _apply_losses(G)
-    return {"package": G.__file__, "ops": (list(_OPS) + ["adam", "rasterization", "compute_relocation"]) if ops else [], "losses": losses}
+    return {"package": G.__file__, "ops": (list(_OPS + _OPS_2DGS) + ["adam", "rasterization", "rasterization_2dgs", "compute_relocation"]) if ops else [], "losses": losses}
 
 
 def _apply_ops(B, G) -> None:
     W = importlib.import_module("gsplat.cuda._wrapper")
     R = importlib.import_module("gsplat.rendering")
-    for name in _OPS:
+    for name in _OPS + tuple(n for n in _OPS_2DGS if hasattr(W, n)):
         fn = _delegating(name, getattr(B, name), getattr(W, name))
         _set(W, name, fn)
         if hasattr(G, name):
@@ -110,6 +114,12 @@ def _apply_ops(B, G) -> None:
     rast = _delegating("rasterization", B.rasterization, R.rasterization)
     _set(R, "rasterization", rast)
     _set(G, "rasterization", rast)
+    # 2DGS: packed / sparse_grad calls raise NotImplementedError on the b200 path and run the package's own
+    if hasattr(R, "rasterization_2dgs"):
+        rast2 = _delegating("rasterization_2dgs", B.rasterization_2dgs, R.rasterization_2dgs)
+        _set(R, "rasterization_2dgs", rast2)
+        if hasattr(G, "rasterization_2dgs"):
+            _set(G, "rasterization_2dgs", rast2)
 
     rel = importlib.import_module("gsplat.relocation")
     reloc = _delegating("compute_relocation", B.compute_relocation, rel.compute_relocation)

@@ -1162,6 +1162,258 @@ def rasterize_to_pixels_rows(
 
 
 # --------------------------------------------------------------------------------------------
+# 2DGS (surfel splatting), dense rows: fully_fused_projection_2dgs / rasterize_to_pixels_2dgs
+# (reference wrappers gsplat/cuda/_wrapper.py:2633, :2918 and their autograd hooks :2730-2806, :3004-3150)
+
+
+def _check_shape(t: Tensor, shape: tuple, name: str) -> None:
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{name} must have shape {tuple(shape)}, got {tuple(t.shape)}")
+
+
+class _FullyFusedProjection2DGS(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, means, quats, scales, viewmats, Ks, width, height, near_plane, far_plane, radius_clip):
+        dev = require_cuda(means, quats, scales, viewmats, Ks)
+        means, quats, scales = f32c(means, "means"), f32c(quats, "quats"), f32c(scales, "scales")
+        viewmats, Ks = f32c(viewmats, "viewmats"), f32c(Ks, "Ks")
+        batch = tuple(means.shape[:-2])
+        B, N, C = _prod(batch), means.shape[-2], viewmats.shape[-3]
+        o = dict(device=dev, dtype=torch.float32)
+        radii = torch.empty(batch + (C, N, 2), device=dev, dtype=torch.int32)
+        means2d = torch.empty(batch + (C, N, 2), **o)
+        depths = torch.empty(batch + (C, N), **o)
+        ray_transforms = torch.empty(batch + (C, N, 3, 3), **o)
+        normals = torch.empty(batch + (C, N, 3), **o)
+        with _Ctx(dev) as st:
+            check(
+                lib().gsb200_surfel_projection_fwd(
+                    B, C, N, ptr(means), ptr(quats), ptr(scales), ptr(viewmats), ptr(Ks), width, height, near_plane, far_plane,
+                    radius_clip, ptr(radii), ptr(means2d), ptr(depths), ptr(ray_transforms), ptr(normals), st,
+                ),
+                "projection_2dgs_fused",
+            )
+        ctx.save_for_backward(means, quats, scales, viewmats, Ks, radii, ray_transforms)
+        ctx.mark_non_differentiable(radii)
+        return radii, means2d, depths, ray_transforms, normals
+
+    @staticmethod
+    def backward(ctx, v_radii, v_means2d, v_depths, v_ray_transforms, v_normals):
+        means, quats, scales, viewmats, Ks, radii, ray_transforms = ctx.saved_tensors
+        batch = tuple(means.shape[:-2])
+        B, N, C = _prod(batch), means.shape[-2], viewmats.shape[-3]
+        dev = means.device
+
+        def grad(g, shape):
+            return torch.zeros(batch + (C, N) + shape, device=dev, dtype=torch.float32) if g is None else g.float().contiguous()
+
+        v_means2d, v_depths = grad(v_means2d, (2,)), grad(v_depths, ())
+        v_ray_transforms, v_normals = grad(v_ray_transforms, (3, 3)), grad(v_normals, (3,))
+        v_means, v_quats, v_scales = torch.empty_like(means), torch.empty_like(quats), torch.empty_like(scales)
+        v_viewmats = torch.empty_like(viewmats) if ctx.needs_input_grad[3] else None
+        with _Ctx(dev) as st:
+            check(
+                lib().gsb200_surfel_projection_bwd(
+                    B, C, N, ptr(means), ptr(quats), ptr(scales), ptr(viewmats), ptr(Ks), ptr(radii), ptr(ray_transforms),
+                    ptr(v_means2d), ptr(v_depths), ptr(v_ray_transforms), ptr(v_normals), ptr(v_means), ptr(v_quats),
+                    ptr(v_scales), ptr(v_viewmats), st,
+                ),
+                "projection_2dgs_fused_bwd",
+            )
+        return (v_means, v_quats, v_scales, v_viewmats) + (None,) * 6
+
+
+def fully_fused_projection_2dgs(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    width: int,
+    height: int,
+    eps2d: float = 0.3,
+    near_plane: float = 0.01,
+    far_plane: float = 1e10,
+    radius_clip: float = 0.0,
+    packed: bool = False,
+    sparse_grad: bool = False,
+) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """Projects 2D Gaussians (surfels).  Returns (radii int32 [..., C, N, 2], means2d [..., C, N, 2], depths [..., C, N],
+    ray_transforms [..., C, N, 3, 3], normals [..., C, N, 3]).  ``radii == 0`` marks culled entries; their float outputs
+    are zero.  ``eps2d`` is accepted and unused, as in the reference.  Only the dense layout is built: ``packed=True`` and
+    ``sparse_grad=True`` raise NotImplementedError."""
+    if packed or sparse_grad:
+        raise NotImplementedError("fully_fused_projection_2dgs: only the dense layout (packed=False) is built")
+    if means.dim() < 2 or means.shape[-1] != 3:
+        raise ValueError(f"means must be [..., N, 3], got {tuple(means.shape)}")
+    batch, N = tuple(means.shape[:-2]), means.shape[-2]
+    _check_shape(quats, batch + (N, 4), "quats")
+    _check_shape(scales, batch + (N, 3), "scales")
+    if viewmats.dim() != len(batch) + 3:
+        raise ValueError(f"viewmats must be [..., C, 4, 4], got {tuple(viewmats.shape)}")
+    C = viewmats.shape[-3]
+    _check_shape(viewmats, batch + (C, 4, 4), "viewmats")
+    _check_shape(Ks, batch + (C, 3, 3), "Ks")
+    return _FullyFusedProjection2DGS.apply(
+        means, quats, scales, viewmats, Ks, int(width), int(height), float(near_plane), float(far_plane), float(radius_clip),
+    )
+
+
+class _RasterizeToPixels2DGS(torch.autograd.Function):
+    @staticmethod
+    def forward(
+        ctx, means2d, ray_transforms, colors, opacities, normals, densify, backgrounds, masks, width, height, isect_offsets,
+        flatten_ids, absgrad_holder,
+    ):
+        dev = require_cuda(means2d, ray_transforms, colors, opacities, normals)
+        means2d, ray_transforms = f32c(means2d, "means2d"), f32c(ray_transforms, "ray_transforms")
+        colors, opacities, normals = f32c(colors, "colors"), f32c(opacities, "opacities"), f32c(normals, "normals")
+        backgrounds = f32c(backgrounds, "backgrounds")
+        image_dims = tuple(isect_offsets.shape[:-2])
+        I, N, D = _prod(image_dims), means2d.shape[-2], colors.shape[-1]
+        th, tw = isect_offsets.shape[-2:]
+        m8 = None
+        if masks is not None:
+            m8 = masks.contiguous().view(torch.uint8) if masks.dtype == torch.bool else masks.to(torch.uint8).contiguous()
+        offsets, fl = isect_offsets.contiguous(), flatten_ids.contiguous()
+        S = fl.shape[0]
+        o = dict(device=dev, dtype=torch.float32)
+        pix = image_dims + (height, width)
+        if S == 0:
+            # nothing intersects a tile: the background alone, no kernel launch
+            if backgrounds is not None:
+                render_colors = torch.broadcast_to(backgrounds[..., None, None, :], pix + (D,)).contiguous()
+            else:
+                render_colors = torch.zeros(pix + (D,), **o)
+            render_alphas, render_distort, render_median = (torch.zeros(pix + (1,), **o) for _ in range(3))
+            render_normals = torch.zeros(pix + (3,), **o)
+            last_ids = median_ids = torch.zeros(pix, device=dev, dtype=torch.int32)
+        else:
+            render_colors = torch.empty(pix + (D,), **o)
+            render_alphas, render_distort, render_median = (torch.empty(pix + (1,), **o) for _ in range(3))
+            render_normals = torch.empty(pix + (3,), **o)
+            last_ids = torch.empty(pix, device=dev, dtype=torch.int32)
+            median_ids = torch.empty(pix, device=dev, dtype=torch.int32)
+            with _Ctx(dev) as st:
+                check(
+                    lib().gsb200_surfel_raster_fwd(
+                        I, N, D, ptr(means2d), ptr(ray_transforms), ptr(colors), ptr(opacities), ptr(normals), ptr(backgrounds),
+                        ptr(m8), width, height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_colors), ptr(render_alphas),
+                        ptr(render_normals), ptr(render_distort), ptr(render_median), ptr(last_ids), ptr(median_ids), st,
+                    ),
+                    "rasterize_to_pixels_2dgs",
+                )
+        ctx.save_for_backward(
+            means2d, ray_transforms, colors, opacities, normals, backgrounds, m8, offsets, fl, render_colors, render_alphas,
+            last_ids, median_ids,
+        )
+        ctx.set_materialize_grads(False)
+        ctx.absgrad_holder = absgrad_holder  # filled in place by backward; deliberately not a saved tensor
+        ctx.meta = (I, N, D, width, height, tw, th, S, tuple(densify.shape))
+        return render_colors, render_alphas, render_normals, render_distort, render_median
+
+    @staticmethod
+    def backward(ctx, v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median):
+        (means2d, ray_transforms, colors, opacities, normals, backgrounds, m8, offsets, fl, render_colors, render_alphas,
+         last_ids, median_ids) = ctx.saved_tensors
+        I, N, D, width, height, tw, th, S, densify_shape = ctx.meta
+        dev = render_alphas.device
+        if v_render_colors is None:
+            v_render_colors = torch.zeros_like(render_colors)
+        v_render_colors = v_render_colors.contiguous()
+        c = lambda g: None if g is None else g.contiguous()  # noqa: E731
+        v_render_alphas, v_render_normals = c(v_render_alphas), c(v_render_normals)
+        v_render_distort, v_render_median = c(v_render_distort), c(v_render_median)
+        v_means2d, v_ray_transforms = torch.zeros_like(means2d), torch.zeros_like(ray_transforms)
+        v_colors, v_opacities, v_normals = torch.zeros_like(colors), torch.zeros_like(opacities), torch.zeros_like(normals)
+        v_densify = torch.zeros(densify_shape, device=dev, dtype=torch.float32)
+        holder = ctx.absgrad_holder
+        v_abs = torch.zeros_like(means2d) if holder is not None else None
+        if S > 0:
+            with _Ctx(dev) as st:
+                check(
+                    lib().gsb200_surfel_raster_bwd(
+                        I, N, D, ptr(means2d), ptr(ray_transforms), ptr(colors), ptr(opacities), ptr(normals), ptr(backgrounds),
+                        ptr(m8), width, height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_colors), ptr(render_alphas),
+                        ptr(last_ids), ptr(median_ids), ptr(v_render_colors), ptr(v_render_alphas), ptr(v_render_normals),
+                        ptr(v_render_distort), ptr(v_render_median), ptr(v_means2d), ptr(v_ray_transforms), ptr(v_colors),
+                        ptr(v_opacities), ptr(v_normals), ptr(v_densify), ptr(v_abs), st,
+                    ),
+                    "rasterize_to_pixels_2dgs_bwd",
+                )
+        if holder is not None:
+            holder.copy_(v_abs)
+        v_backgrounds = None
+        if backgrounds is not None and ctx.needs_input_grad[6]:
+            v_backgrounds = (v_render_colors * (1.0 - render_alphas)).sum(dim=(-3, -2))
+        return (v_means2d, v_ray_transforms, v_colors, v_opacities, v_normals, v_densify, v_backgrounds) + (None,) * 6
+
+
+def rasterize_to_pixels_2dgs(
+    means2d: Tensor,  # [..., N, 2]
+    ray_transforms: Tensor,  # [..., N, 3, 3]
+    colors: Tensor,  # [..., N, channels]
+    opacities: Tensor,  # [..., N]
+    normals: Tensor,  # [..., N, 3]
+    densify: Tensor,  # [..., N, 2]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    isect_offsets: Tensor,  # [..., tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+    backgrounds: Optional[Tensor] = None,  # [..., channels]
+    masks: Optional[Tensor] = None,  # [..., tile_height, tile_width]
+    packed: bool = False,
+    absgrad: bool = False,
+    distloss: bool = False,
+) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """Front-to-back compositing of depth-sorted surfels per 16x16 tile.  Returns (render_colors [..., H, W, channels],
+    render_alphas [..., H, W, 1], render_normals [..., H, W, 3], render_distort [..., H, W, 1], render_median
+    [..., H, W, 1]).  The last colour channel is the depth that the distortion and the median depth are taken from; the
+    distortion is always computed (``distloss`` only matters to the caller that appends the depth channel, as in the
+    reference).  ``densify`` receives the densification gradient; with ``absgrad`` the backward fills ``means2d.absgrad``."""
+    if packed:
+        raise NotImplementedError("rasterize_to_pixels_2dgs: only the dense layout (packed=False) is built")
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    if isect_offsets.dim() < 2:
+        raise ValueError(f"isect_offsets must be [..., tile_height, tile_width], got {tuple(isect_offsets.shape)}")
+    image_dims, (th, tw) = tuple(isect_offsets.shape[:-2]), tuple(isect_offsets.shape[-2:])
+    if th * 16 < image_height or tw * 16 < image_width:
+        raise ValueError(f"isect_offsets tile grid {tw}x{th} does not cover a {image_width}x{image_height} image")
+    if means2d.dim() < 2 or tuple(means2d.shape[:-2]) != image_dims or means2d.shape[-1] != 2:
+        raise ValueError(f"means2d must be {image_dims + ('N', 2)}, got {tuple(means2d.shape)}")
+    N = means2d.shape[-2]
+    if colors.dim() != means2d.dim():
+        raise ValueError(f"colors must be [..., N, channels], got {tuple(colors.shape)}")
+    D = colors.shape[-1]
+    _check_shape(ray_transforms, image_dims + (N, 3, 3), "ray_transforms")
+    _check_shape(colors, image_dims + (N, D), "colors")
+    _check_shape(opacities, image_dims + (N,), "opacities")
+    _check_shape(normals, image_dims + (N, 3), "normals")
+    _check_shape(densify, image_dims + (N, 2), "densify")
+    if backgrounds is not None:
+        _check_shape(backgrounds, image_dims + (D,), "backgrounds")
+    if masks is not None:
+        _check_shape(masks, image_dims + (th, tw), "masks")
+    if isect_offsets.dtype != torch.int32 or flatten_ids.dtype != torch.int32 or flatten_ids.dim() != 1:
+        raise ValueError("isect_offsets and flatten_ids must be int32, flatten_ids one-dimensional")
+    if D not in _SUPPORTED_CHANNELS:
+        raise NotImplementedError(
+            f"rasterize_to_pixels_2dgs: {D} channels; the 2DGS kernels are built for {_SUPPORTED_CHANNELS} (the last channel "
+            "is the depth, so the channels cannot be padded)"
+        )
+    holder = torch.zeros_like(means2d) if absgrad else None
+    outs = _RasterizeToPixels2DGS.apply(
+        means2d, ray_transforms, colors, opacities, normals, densify, backgrounds, masks, int(image_width), int(image_height),
+        isect_offsets, flatten_ids, holder,
+    )
+    if absgrad:
+        means2d.absgrad = holder
+    return outs
+
+
+# --------------------------------------------------------------------------------------------
 # sparse pixels: build_sparse_tile_layout / isect_tiles_sparse / rasterize_to_pixels_sparse
 # (reference wrappers /root/reference/gsplat/cuda/_wrapper.py:1352, :1433, :1566).  At every requested pixel the result
 # is the dense rendering's; only the active tiles are intersected and composited, and only the requested pixels written.

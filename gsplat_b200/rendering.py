@@ -9,6 +9,10 @@ Scope: the 3DGS EWA path named by BASELINE.json (pinhole / orthographic / fishey
 backgrounds, masks, absgrad, SH or post-activation colours, ``distributed=True`` Gaussian sharding).
 3DGUT (with_ut / with_eval3d), lidar, distortion, rolling shutter, extra signals and normals are out of scope
 and raise NotImplementedError.
+
+rasterization_2dgs(): surfel splatting (2DGS) on the dense layout, following the reference's orchestrator
+(csrc/Rendering.cpp:1705-1958): ray-transform projection -> radius-box tile intersection -> compositing of colours,
+normals, distortion and median depth.
 """
 from __future__ import annotations
 
@@ -21,9 +25,11 @@ from torch import Tensor
 from .ops import (
     RowSideOutputs,
     fully_fused_projection,
+    fully_fused_projection_2dgs,
     fused_project_sh,
     isect_tiles_sorted,
     rasterize_to_pixels,
+    rasterize_to_pixels_2dgs,
     rasterize_to_pixels_rows,
     spherical_harmonics,
     spherical_harmonics_rows,
@@ -443,3 +449,171 @@ def rasterization(
         "n_cameras": C,
     })
     return render_colors, render_alphas, meta
+
+
+def _depth_to_normal(depths: Tensor, camtoworlds: Tensor, Ks: Tensor) -> Tensor:
+    """Surface normals of a z-depth map [..., H, W, 1] (reference csrc/Rendering.cpp:1659-1702 depth_to_points_2dgs /
+    depth_to_normal_2dgs): unproject every pixel with its unnormalised ray, take the cross product of the central
+    differences of the neighbouring points, normalise, and pad the one-pixel border with zeros.  Returns [..., H, W, 3]
+    in world space."""
+    H, W = depths.shape[-3], depths.shape[-2]
+    y, x = torch.meshgrid(
+        torch.arange(H, device=depths.device, dtype=depths.dtype), torch.arange(W, device=depths.device, dtype=depths.dtype),
+        indexing="ij",
+    )
+    fx, fy = Ks[..., 0, 0, None, None], Ks[..., 1, 1, None, None]
+    cx, cy = Ks[..., 0, 2, None, None], Ks[..., 1, 2, None, None]
+    dirs = torch.stack([(x - cx + 0.5) / fx, (y - cy + 0.5) / fy], dim=-1)
+    dirs = torch.nn.functional.pad(dirs, (0, 1), value=1.0)  # [..., H, W, 3]
+    dirs = torch.einsum("...ij,...hwj->...hwi", camtoworlds[..., :3, :3], dirs)
+    points = camtoworlds[..., None, None, :3, 3] + depths * dirs
+    dx = points[..., 2:, 1:-1, :] - points[..., :-2, 1:-1, :]
+    dy = points[..., 1:-1, 2:, :] - points[..., 1:-1, :-2, :]
+    normals = torch.linalg.cross(dx, dy, dim=-1)
+    # the reference's sqrt(sum of squares); vector_norm's backward is 0 (not NaN) where the cross product vanishes
+    normals = normals / torch.linalg.vector_norm(normals, dim=-1, keepdim=True).clamp_min(1e-12)
+    return torch.nn.functional.pad(normals, (0, 0, 1, 1, 1, 1), value=0.0)
+
+
+def rasterization_2dgs(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    opacities: Tensor,  # [..., N]
+    colors: Tensor,  # [..., (C,) N, D] post-activation colours, or [N, K, D] SH coefficients
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    width: int,
+    height: int,
+    near_plane: float = 0.01,
+    far_plane: float = 1e10,
+    radius_clip: float = 0.0,
+    eps2d: float = 0.3,
+    sh_degree: Optional[int] = None,
+    packed: bool = False,
+    tile_size: int = 16,
+    backgrounds: Optional[Tensor] = None,
+    render_mode: str = "RGB",
+    sparse_grad: bool = False,
+    absgrad: bool = False,
+    distloss: bool = False,
+    depth_mode: str = "expected",
+) -> Tuple[Tensor, Tensor, Tensor, Optional[Tensor], Tensor, Tensor, Dict]:
+    """Rasterize N 2D Gaussians (surfels) to C image planes, signature-compatible with the reference
+    (gsplat/rendering.py:1358, orchestration csrc/Rendering.cpp:1705-1958).  Returns (render_colors
+    [..., C, H, W, X], render_alphas [..., C, H, W, 1], render_normals [..., C, H, W, 3] in world space, surf_normals
+    (normals of the rendered depth, world space; None unless the mode renders both colour and depth), render_distort
+    [..., C, H, W, 1], render_median [..., C, H, W, 1], meta).  ``meta["gradient_2dgs"]`` is the tensor whose ``.grad``
+    is the densification signal; with ``absgrad`` the backward fills ``meta["means2d"].absgrad``.  Dense rows only:
+    ``packed=True`` and ``sparse_grad=True`` raise NotImplementedError."""
+    if packed or sparse_grad:
+        raise NotImplementedError("rasterization_2dgs: only the dense layout (packed=False) is built")
+    if render_mode not in _ALL_MODES:
+        raise ValueError(f"unknown render_mode {render_mode!r}")
+    if render_mode in _HIT_DISTANCE_MODES:
+        raise NotImplementedError(f"rasterization_2dgs(render_mode={render_mode!r}): hit-distance modes are not built")
+    if depth_mode not in ("expected", "median"):
+        raise ValueError(f"unknown depth_mode {depth_mode!r}")
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    has_color = render_mode in _COLOR_MODES
+    has_depth = render_mode in _DEPTH_MODES
+    if distloss and not has_depth:
+        raise ValueError("distloss requires a depth render mode")
+    if means.dim() < 2 or means.shape[-1] != 3:
+        raise ValueError(f"means must be [..., N, 3], got {tuple(means.shape)}")
+    batch_dims = tuple(means.shape[:-2])
+    nb = len(batch_dims)
+    N = means.shape[-2]
+    if viewmats.dim() != nb + 3:
+        raise ValueError(f"viewmats must be [..., C, 4, 4], got {tuple(viewmats.shape)}")
+    C = viewmats.shape[-3]
+    if tuple(opacities.shape) != batch_dims + (N,):
+        raise ValueError(f"opacities must be [..., N], got {tuple(opacities.shape)}")
+    if has_color:
+        if sh_degree is None:
+            ok = (colors.dim() == nb + 2 and tuple(colors.shape[:-1]) == batch_dims + (N,)) or (
+                colors.dim() == nb + 3 and tuple(colors.shape[:-1]) == batch_dims + (C, N)
+            )
+            if not ok:
+                raise ValueError(f"colors must be [..., N, D] or [..., C, N, D], got {tuple(colors.shape)}")
+        else:
+            if colors.dim() != 3 or colors.shape[0] != N:
+                raise ValueError(f"SH colors must be [N, K, D], got {tuple(colors.shape)}")
+            if (sh_degree + 1) ** 2 > colors.shape[-2]:
+                raise ValueError(f"sh_degree={sh_degree} needs K >= {(sh_degree + 1) ** 2}, got {colors.shape[-2]}")
+
+    # ---- projection (ray-splat transforms), reference Rendering.cpp:1802-1814
+    radii, means2d, depths, ray_transforms, normals = fully_fused_projection_2dgs(
+        means, quats, scales, viewmats, Ks, width, height, eps2d=eps2d, near_plane=near_plane, far_plane=far_plane,
+        radius_clip=radius_clip,
+    )
+    opac = torch.broadcast_to(opacities[..., None, :], batch_dims + (C, N))
+    # the densification signal: the compositing backward writes its gradient here
+    densify = torch.zeros_like(means2d, requires_grad=True)
+
+    # ---- tile intersection: the radius box (no conic / opacity test), sorted by depth per tile
+    tile_width = math.ceil(width / float(tile_size))
+    tile_height = math.ceil(height / float(tile_size))
+    hits = isect_tiles_sorted(means2d, radii, depths, tile_size, tile_width, tile_height)
+    tiles_per_gauss, flatten_ids = hits.tiles_per_gauss, hits.flatten_ids
+    isect_offsets = hits.isect_offsets.reshape(batch_dims + (C, tile_height, tile_width))
+
+    # ---- channels: [colour | depth]
+    feat = None
+    if has_color:
+        if sh_degree is None:
+            feat = colors
+            if feat.dim() == nb + 2:
+                feat = torch.broadcast_to(feat[..., None, :, :], batch_dims + (C, N, feat.shape[-1]))
+        else:
+            valid = (radii > 0).all(dim=-1)
+            feat = spherical_harmonics(sh_degree, means, viewmats, colors, masks=valid)
+            feat = torch.clamp_min(feat + 0.5, 0.0)
+    if has_depth:
+        if has_color:
+            feat = torch.cat((feat, depths[..., None]), dim=-1)
+            if backgrounds is not None:
+                backgrounds = torch.cat([backgrounds, torch.zeros_like(backgrounds[..., :1])], dim=-1)
+        else:
+            feat = depths[..., None]
+
+    render_colors, render_alphas, render_normals, render_distort, render_median = rasterize_to_pixels_2dgs(
+        means2d, ray_transforms, feat, opac, normals, densify, width, height, tile_size, isect_offsets, flatten_ids,
+        backgrounds=backgrounds, absgrad=absgrad, distloss=distloss,
+    )
+
+    if render_mode in _EXPECTED_MODES:  # ED / RGB+ED: normalise the accumulated depth
+        depth = render_colors[..., -1:] / render_alphas.clamp(min=1e-10)
+        render_colors = torch.cat([render_colors[..., :-1], depth], dim=-1)
+
+    camtoworlds = torch.linalg.inv(viewmats)
+    surf_normals = None
+    if has_depth and has_color:
+        depth_for_normal = render_median if depth_mode == "median" else render_colors[..., -1:]
+        surf_normals = _depth_to_normal(depth_for_normal, camtoworlds, Ks).squeeze(0)
+    render_normals = torch.einsum("...ij,...hwj->...hwi", camtoworlds[..., :3, :3], render_normals)
+
+    meta = _Meta({
+        "camera_ids": None,
+        "gaussian_ids": None,
+        "radii": radii,
+        "means2d": means2d,
+        "depths": depths,
+        "ray_transforms": ray_transforms,
+        "opacities": opac,
+        "normals": normals,
+        "tile_width": tile_width,
+        "tile_height": tile_height,
+        "tiles_per_gauss": tiles_per_gauss,
+        "isect_ids": _Lazy(hits.isect_ids),
+        "flatten_ids": flatten_ids,
+        "isect_offsets": isect_offsets,
+        "width": width,
+        "height": height,
+        "tile_size": tile_size,
+        "n_cameras": C,
+        "render_distort": render_distort,
+        "gradient_2dgs": densify,
+    })
+    return render_colors, render_alphas, render_normals, surf_normals, render_distort, render_median, meta

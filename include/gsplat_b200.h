@@ -370,6 +370,57 @@ extern "C"
         float *v_opacities, int64_t v_opacities_stride, float *v_means2d_abs, int64_t v_means2d_abs_stride, void *stream
     );
 
+    /* ---- 2DGS (surfel splatting), dense layout: projection_2dgs_fused / _bwd and rasterize_to_pixels_2dgs / _bwd
+     * (ext.cpp, _wrapper.py:2633-2727, 2918-3150; kernels csrc/Projection2DGSFused.cu,
+     * csrc/RasterizeToPixels2DGSSerialBatch{Fwd,Bwd}.cu).
+     * Projection: means [B,N,3], quats [B,N,4], scales [B,N,3] (scales[..., 2] unused), viewmats [B,C,4,4], Ks [B,C,3,3].
+     * Outputs [B,C,N,*]: radii int32 [.., 2], means2d [.., 2], depths, ray_transforms [.., 3, 3] (row-major
+     * K * [R rot(q) diag(s0, s1, 1) columns 0, 1 | camera-space mean]), normals [.., 3] (camera space, facing the camera).
+     * Culled rows (near / far, degenerate, radius_clip, off-screen) get radii = 0 and zero float outputs. */
+    int gsb200_surfel_projection_fwd(
+        int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales,
+        const float *viewmats, const float *Ks, uint32_t image_width, uint32_t image_height, float near_plane,
+        float far_plane, float radius_clip, int32_t *radii, float *means2d, float *depths, float *ray_transforms,
+        float *normals, void *stream
+    );
+    /* All v_* inputs contiguous [B,C,N,*].  v_means [B,N,3], v_quats [B,N,4], v_scales [B,N,3] (v_scales[..., 2] = 0) are
+     * fully written, summed over the cameras without atomics; v_viewmats [B,C,4,4] or NULL is zeroed here, then
+     * accumulated. */
+    int gsb200_surfel_projection_bwd(
+        int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales,
+        const float *viewmats, const float *Ks, const int32_t *radii, const float *ray_transforms, const float *v_means2d,
+        const float *v_depths, const float *v_ray_transforms, const float *v_normals, float *v_means, float *v_quats,
+        float *v_scales, float *v_viewmats, void *stream
+    );
+    /* Compositing, dense rows: means2d [I,N,2], ray_transforms [I,N,3,3], colors [I,N,D] (the last channel is the depth
+     * that distortion and median depth use), opacities [I,N], normals [I,N,3], backgrounds [I,D] or NULL, masks
+     * [I,th,tw] bool bytes or NULL, offsets [I,th,tw], flatten_ids [n_isects].  tile_size must be 16; D one of the
+     * channel counts of gsb200_raster_supports_channels.  Outputs: render_colors [I,H,W,D], render_alphas, render_distort,
+     * render_median [I,H,W,1], render_normals [I,H,W,3], last_ids and median_ids int32 [I,H,W] (indices into
+     * flatten_ids). */
+    int gsb200_surfel_raster_fwd(
+        int64_t I, int64_t N, int D, const float *means2d, const float *ray_transforms, const float *colors,
+        const float *opacities, const float *normals, const float *backgrounds, const uint8_t *masks,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, float *render_colors, float *render_alphas,
+        float *render_normals, float *render_distort, float *render_median, int32_t *last_ids, int32_t *median_ids,
+        void *stream
+    );
+    /* Gradient outputs are ACCUMULATED into contiguous rows (caller zero-initialises): v_means2d [I,N,2], v_ray_transforms
+     * [I,N,3,3], v_colors [I,N,D], v_opacities [I,N], v_normals [I,N,3], v_densify [I,N,2] (v_ray_transforms[.., 0:2, 2]
+     * * ray_transforms[.., 2, 2]), v_means2d_abs [I,N,2] or NULL.  v_render_alphas / _normals / _distort / _median may
+     * be NULL (no gradient flows into that output). */
+    int gsb200_surfel_raster_bwd(
+        int64_t I, int64_t N, int D, const float *means2d, const float *ray_transforms, const float *colors,
+        const float *opacities, const float *normals, const float *backgrounds, const uint8_t *masks,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, const float *render_colors,
+        const float *render_alphas, const int32_t *last_ids, const int32_t *median_ids, const float *v_render_colors,
+        const float *v_render_alphas, const float *v_render_normals, const float *v_render_distort,
+        const float *v_render_median, float *v_means2d, float *v_ray_transforms, float *v_colors, float *v_opacities,
+        float *v_normals, float *v_densify, float *v_means2d_abs, void *stream
+    );
+
     /* ---- MCMC strategy ops ("next" row): relocation (ext.cpp `relocation`, gsplat/relocation.py:64,
      * csrc/RelocationCUDA.cu:36-80) and in-place position perturbation (csrc/MCMCPerturbCUDA.cu:28-60,
      * gsplat/strategy/ops.py).  ratios int32 [N] already clamped to [1, n_max]; binoms [n_max, n_max]. */
