@@ -123,7 +123,7 @@ _SIGNATURES = {
     "gsb200_raster_bwd": (
         c_int,
         [c_i64, c_i64, c_int, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp],
+         c_vp, c_int, c_vp, c_vp],
     ),
     "gsb200_sparse_layout_workspace_bytes": (c_sz, [c_i64, c_i64, c_u32, c_u32]),
     "gsb200_sparse_layout_sort": (c_int, [c_i64, c_vp, c_vp, c_i64, c_u32, c_u32, c_u32, c_vp, c_sz, c_vp, c_vp]),
@@ -145,7 +145,7 @@ _SIGNATURES = {
     "gsb200_raster_sparse_bwd": (
         c_int,
         [c_i64, c_int, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp],
+         c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp],
     ),
     "gsb200_surfel_projection_fwd": (
         c_int,

@@ -16,8 +16,6 @@
 //    (exact: the skipped pairs are `continue`d by the reference too); finished warps drop out by ballot;
 //  * the backward walks the same ring back to front and reduces each gaussian's gradients over a warp's
 //    pixels in two phases, pixel-major then gaussian-major (raster_bwd2_kernel).
-#include <algorithm>
-
 #include <mutex>
 
 #include "common.cuh"
@@ -596,11 +594,6 @@ __global__ void __launch_bounds__(kWarps * 32) raster_fwd_kernel(
 
 // ---------------------------------------------------------------------------------------------
 // backward
-struct GradDst
-{
-    float *means2d, *conics, *colors, *opacities, *abs;
-    int64_t s_means2d, s_conics, s_colors, s_opacities, s_abs;
-};
 
 // Transposed reduction.
 //
@@ -656,7 +649,7 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
     const float *__restrict__ backgrounds, const uint8_t *__restrict__ masks, const uint32_t W, const uint32_t H,
     const uint32_t tw, const uint32_t th, const int32_t *__restrict__ offsets, const float *__restrict__ render_alphas,
     const int32_t *__restrict__ last_ids, const float *__restrict__ v_render_colors,
-    const float *__restrict__ v_render_alphas, const GradDst dst, const uint32_t packed_stride, const Pix pixmap = Pix{}
+    const float *__restrict__ v_render_alphas, float *__restrict__ v_grad_records, const Pix pixmap = Pix{}
 )
 {
     constexpr int CV  = RecLayout<CDIM>::kColorVec4;
@@ -852,33 +845,13 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
         for(int k = 0; k < NV; ++k)
             vals[k] += __shfl_xor_sync(0xffffffffu, vals[k], 16);
         if(gslot < nslots)
-        {
+        { // one 16-byte aligned record per gaussian: 128-bit REDs, alternating between the two halves
             const uint32_t gid = __float_as_uint(m1.z);
-            if(packed_stride != 0u)
-            { // one 16-byte aligned record per gaussian: 128-bit REDs, alternating between the two halves
-                float *rec = dst.means2d + (size_t)(gid * packed_stride);
+            float *rec         = v_grad_records + (size_t)(gid * (uint32_t)(NV4 * 4));
 #pragma unroll
-                for(int c = 0; c < NV4; ++c)
-                    if((c & 1) == half)
-                        red_add_v4(rec + 4 * c, vals[4 * c], vals[4 * c + 1], vals[4 * c + 2], vals[4 * c + 3]);
-            }
-            else if(half == 0)
-            {
-                atomicAdd(dst.means2d + (size_t)gid * dst.s_means2d, vals[0]);
-                atomicAdd(dst.means2d + (size_t)gid * dst.s_means2d + 1, vals[1]);
-                atomicAdd(dst.conics + (size_t)gid * dst.s_conics, vals[2]);
-                atomicAdd(dst.conics + (size_t)gid * dst.s_conics + 1, vals[3]);
-                atomicAdd(dst.conics + (size_t)gid * dst.s_conics + 2, vals[4]);
-                atomicAdd(dst.opacities + (size_t)gid * dst.s_opacities, vals[5]);
-#pragma unroll
-                for(int k = 0; k < CDIM; ++k)
-                    atomicAdd(dst.colors + (size_t)gid * dst.s_colors + k, vals[6 + k]);
-                if constexpr(ABS)
-                {
-                    atomicAdd(dst.abs + (size_t)gid * dst.s_abs, vals[6 + CDIM]);
-                    atomicAdd(dst.abs + (size_t)gid * dst.s_abs + 1, vals[7 + CDIM]);
-                }
-            }
+            for(int c = 0; c < NV4; ++c)
+                if((c & 1) == half)
+                    red_add_v4(rec + 4 * c, vals[4 * c], vals[4 * c + 1], vals[4 * c + 2], vals[4 * c + 3]);
         }
         __syncwarp();
     };
@@ -1125,45 +1098,30 @@ static int launch_fwd(
     return check_launch();
 }
 
-// Are the five gradient destinations one packed, 16-byte aligned record [v_xy 2 | v_conic 3 | v_opacity 1 | v_rgb D | abs 2]
-// per gaussian?  Its stride in floats if so (raster_bwd2_kernel then adds with 128-bit REDs), else 0.
-template<int CDIM>
-static uint32_t packed_grad_stride(const GradDst &dst)
-{
-    const bool absg = dst.abs != nullptr;
-    const int64_t P = dst.s_means2d;
-    if(P > 0 && (P % 4) == 0 && P >= 6 + CDIM + (absg ? 2 : 0) && dst.s_conics == P && dst.s_colors == P && dst.s_opacities == P
-       && dst.conics == dst.means2d + 2 && dst.opacities == dst.means2d + 5 && dst.colors == dst.means2d + 6
-       && (!absg || (dst.s_abs == P && dst.abs == dst.means2d + 6 + CDIM)) && (reinterpret_cast<uintptr_t>(dst.means2d) & 15) == 0)
-        return (uint32_t)P;
-    return 0;
-}
-
 template<int CDIM, class Pix>
 static int launch_bwd(
     unsigned n_tiles, uint32_t I, const float *backgrounds, const uint8_t *masks, uint32_t W, uint32_t H, uint32_t tw,
     uint32_t th, const int32_t *offsets, const int32_t *flatten_ids, int64_t S, const Pix &pm, const void *records,
     const float *render_alphas, const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas,
-    const GradDst &dst, cudaStream_t st
+    bool absgrad, float *v_grad_records, cudaStream_t st
 )
 {
     if(S == 0)
         return GSB200_OK; // reference: no launch when there are no intersections (Bwd.cu:350-354)
-    RecordStreams r       = carve_records(const_cast<void *>(records), S, RecLayout<CDIM>::kColorVec4);
-    const int32_t *order  = use_tile_order(n_tiles) ? r.order : nullptr; // written by the forward
-    const uint32_t packed = packed_grad_stride<CDIM>(dst);
-    constexpr bool pipe   = CDIM <= 4;
-    constexpr int minb    = pipe ? 4 : 1;
-    const size_t smem     = Bwd2Smem<CDIM, pipe>::total;
-    auto launch           = [&](auto kernel) -> int {
+    RecordStreams r      = carve_records(const_cast<void *>(records), S, RecLayout<CDIM>::kColorVec4);
+    const int32_t *order = use_tile_order(n_tiles) ? r.order : nullptr; // written by the forward
+    constexpr bool pipe  = CDIM <= 4;
+    constexpr int minb   = pipe ? 4 : 1;
+    const size_t smem    = Bwd2Smem<CDIM, pipe>::total;
+    auto launch          = [&](auto kernel) -> int {
         GSB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kernel<<<n_tiles, kWarps * 32, smem, st>>>(
             I, S, r.cull, r.geom, r.color, order, flatten_ids, backgrounds, masks, W, H, tw, th, offsets, render_alphas, last_ids,
-            v_render_colors, v_render_alphas, dst, packed, pm
+            v_render_colors, v_render_alphas, v_grad_records, pm
         );
         return check_launch();
     };
-    if(dst.abs != nullptr)
+    if(absgrad)
         return launch(raster_bwd2_kernel<CDIM, true, minb, pipe, Pix>);
     return launch(raster_bwd2_kernel<CDIM, false, minb, pipe, Pix>);
 }
@@ -1294,13 +1252,24 @@ extern "C" int gsb200_raster_fwd_rows(
     }
 }
 
+// The gradient records of the backward (include/gsplat_b200.h): a 16-byte aligned base, and rows * row width below 2^32
+// because the kernel addresses a row with a 32-bit element offset.
+static int grad_records_ok(double rows, int D, int absgrad, const float *v_grad_records)
+{
+    if(!v_grad_records || (reinterpret_cast<uintptr_t>(v_grad_records) & 15) != 0)
+        return GSB200_E_INVALID;
+    const int64_t width = (6 + (int64_t)D + (absgrad ? 2 : 0) + 3) / 4 * 4;
+    if(rows * (double)width >= 4294967296.0)
+        return GSB200_E_UNSUPPORTED;
+    return GSB200_OK;
+}
+
 extern "C" int gsb200_raster_bwd(
     int64_t I, int64_t N, int D, const float *backgrounds, const uint8_t *masks, uint32_t image_width,
     uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
     const int32_t *flatten_ids, int64_t n_isects, const void *records, const float *render_alphas,
-    const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, float *v_means2d,
-    int64_t v_means2d_stride, float *v_conics, int64_t v_conics_stride, float *v_colors, int64_t v_colors_stride,
-    float *v_opacities, int64_t v_opacities_stride, float *v_means2d_abs, int64_t v_means2d_abs_stride, void *stream
+    const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, int absgrad,
+    float *v_grad_records, void *stream
 )
 {
     if(I < 0 || N < 0 || n_isects < 0)
@@ -1309,20 +1278,10 @@ extern "C" int gsb200_raster_bwd(
         return GSB200_E_UNSUPPORTED;
     if(n_isects == 0 || I == 0)
         return GSB200_OK;
-    if(!offsets || !flatten_ids || !records || !render_alphas || !last_ids || !v_render_colors
-       || !v_means2d || !v_conics || !v_colors || !v_opacities)
+    if(!offsets || !flatten_ids || !records || !render_alphas || !last_ids || !v_render_colors)
         return GSB200_E_INVALID;
-    {   // the kernels address gradient rows with 32-bit element offsets
-        const int64_t smax = std::max(std::max(v_means2d_stride, v_conics_stride), std::max(std::max(v_colors_stride, v_opacities_stride), v_means2d_abs ? v_means2d_abs_stride : (int64_t)0));
-        if(smax < 0 || (double)I * (double)N * (double)smax >= 4294967296.0)
-            return GSB200_E_UNSUPPORTED;
-    }
-    gsb::GradDst dst;
-    dst.means2d = v_means2d, dst.s_means2d = v_means2d_stride;
-    dst.conics = v_conics, dst.s_conics = v_conics_stride;
-    dst.colors = v_colors, dst.s_colors = v_colors_stride;
-    dst.opacities = v_opacities, dst.s_opacities = v_opacities_stride;
-    dst.abs = v_means2d_abs, dst.s_abs = v_means2d_abs_stride;
+    if(int rc = grad_records_ok((double)I * (double)N, D, absgrad, v_grad_records))
+        return rc;
     const unsigned n_tiles = (unsigned)(I * tile_width * tile_height);
     cudaStream_t st        = (cudaStream_t)stream;
     switch(D)
@@ -1332,7 +1291,7 @@ extern "C" int gsb200_raster_bwd(
         return gsb::launch_bwd<n>(                                                                                 \
             n_tiles, (uint32_t)I, backgrounds, masks, image_width, image_height, tile_width, tile_height, offsets, \
             flatten_ids, n_isects, gsb::DensePixels{}, records, render_alphas, last_ids, v_render_colors,           \
-            v_render_alphas, dst, st                                                                               \
+            v_render_alphas, absgrad != 0, v_grad_records, st                                                      \
         );
         GSB_FOR_CHANNELS(X)
 #undef X
@@ -1400,9 +1359,8 @@ extern "C" int gsb200_raster_sparse_bwd(
     uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t n_active, const int32_t *active_tiles,
     const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t n_isects, const uint64_t *tile_pixel_mask,
     const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, const void *records, const float *render_alphas,
-    const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, float *v_means2d,
-    int64_t v_means2d_stride, float *v_conics, int64_t v_conics_stride, float *v_colors, int64_t v_colors_stride,
-    float *v_opacities, int64_t v_opacities_stride, float *v_means2d_abs, int64_t v_means2d_abs_stride, void *stream
+    const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, int absgrad, float *v_grad_records,
+    void *stream
 )
 {
     if(tile_size != (uint32_t)gsb::kTile)
@@ -1413,20 +1371,10 @@ extern "C" int gsb200_raster_sparse_bwd(
         return rc;
     if(n_isects == 0 || n_active == 0)
         return GSB200_OK;
-    if(!flatten_ids || !records || !render_alphas || !last_ids || !v_render_colors || !v_means2d || !v_conics || !v_colors
-       || !v_opacities)
+    if(!flatten_ids || !records || !render_alphas || !last_ids || !v_render_colors)
         return GSB200_E_INVALID;
-    {   // the kernels address gradient rows with 32-bit element offsets
-        const int64_t smax = std::max(std::max(v_means2d_stride, v_conics_stride), std::max(std::max(v_colors_stride, v_opacities_stride), v_means2d_abs ? v_means2d_abs_stride : (int64_t)0));
-        if(smax < 0 || (double)n_rows * (double)smax >= 4294967296.0)
-            return GSB200_E_UNSUPPORTED;
-    }
-    gsb::GradDst dst;
-    dst.means2d = v_means2d, dst.s_means2d = v_means2d_stride;
-    dst.conics = v_conics, dst.s_conics = v_conics_stride;
-    dst.colors = v_colors, dst.s_colors = v_colors_stride;
-    dst.opacities = v_opacities, dst.s_opacities = v_opacities_stride;
-    dst.abs = v_means2d_abs, dst.s_abs = v_means2d_abs_stride;
+    if(int rc = grad_records_ok((double)n_rows, D, absgrad, v_grad_records))
+        return rc;
     const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
     cudaStream_t st = (cudaStream_t)stream;
     switch(D)
@@ -1436,7 +1384,7 @@ extern "C" int gsb200_raster_sparse_bwd(
         return gsb::launch_bwd<n>(                                                                                 \
             (unsigned)n_active, 1u, backgrounds, masks, image_width, image_height, tile_width, tile_height,        \
             tile_offsets, flatten_ids, n_isects, pm, records, render_alphas, last_ids, v_render_colors,            \
-            v_render_alphas, dst, st                                                                               \
+            v_render_alphas, absgrad != 0, v_grad_records, st                                                      \
         );
         GSB_FOR_CHANNELS(X)
 #undef X

@@ -1011,6 +1011,47 @@ def _grad_record_width(D: int, absgrad: bool) -> int:
     return ((6 + D + (2 if absgrad else 0)) + 3) // 4 * 4
 
 
+def _grad_records(row_dims: tuple, D: int, absgrad: bool, device) -> Tensor:
+    """Zeroed gradient records of the compositing backward, one per Gaussian row (layout: gsb200_raster_bwd in
+    include/gsplat_b200.h)."""
+    return torch.zeros(tuple(row_dims) + (_grad_record_width(D, absgrad),), device=device, dtype=torch.float32)
+
+
+def _split_grad_records(rec: Tensor, D: int, absgrad: bool):
+    """Views (v_means2d, v_conics, v_colors, v_opacities, v_means2d_abs or None) into the records of _grad_records."""
+    return rec[..., 0:2], rec[..., 2:5], rec[..., 6 : 6 + D], rec[..., 5], (rec[..., 6 + D : 8 + D] if absgrad else None)
+
+
+def _rasterize_padded(means2d, colors, backgrounds, tile_size, packed, absgrad, composite):
+    """Shared by the compositing entry points: checks the arguments, pads colors / backgrounds with zero channels up to
+    the next count the kernels are built for, runs composite(colors, backgrounds, absgrad_holder, padded), sets
+    ``means2d.absgrad`` and cuts the padding off the rendered colours."""
+    if packed != (means2d.dim() == 2):
+        raise ValueError(f"packed={packed} but means2d has shape {tuple(means2d.shape)}")
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    D = colors.shape[-1]
+    if D > 32:
+        raise ValueError(
+            f"Unsupported number of color channels: {D}. gsplat_b200 rasterizes up to 32 channels per pass "
+            "(rasterization() chunks wider features with channel_chunk=32)."
+        )
+    pad = 0
+    if D not in _SUPPORTED_CHANNELS:
+        target = next(c for c in _SUPPORTED_CHANNELS if c >= D)
+        pad = target - D
+        colors = torch.nn.functional.pad(colors, (0, pad))
+        if backgrounds is not None:
+            backgrounds = torch.nn.functional.pad(backgrounds, (0, pad))
+    holder = torch.zeros_like(means2d) if absgrad else None
+    render_colors, render_alphas = composite(colors, backgrounds, holder, pad > 0)
+    if absgrad:
+        means2d.absgrad = holder
+    if pad:
+        render_colors = render_colors[..., :D]
+    return render_colors, render_alphas
+
+
 class _RasterizeToPixels(torch.autograd.Function):
     @staticmethod
     def forward(
@@ -1063,14 +1104,14 @@ class _RasterizeToPixels(torch.autograd.Function):
         ctx.save_for_backward(backgrounds, m8, offsets, fl, records, render_alphas, last_ids)
         ctx.set_materialize_grads(False)
         ctx.absgrad_holder = absgrad_holder  # filled in place by backward; deliberately not a saved tensor
-        ctx.meta = (row_dims, I, N, R, D, width, height, tile_size, tw, th, S)
+        ctx.meta = (row_dims, I, N, D, width, height, tile_size, tw, th, S)
         return render_colors, render_alphas
 
     @staticmethod
     def backward(ctx, v_render_colors, v_render_alphas):
         backgrounds, m8, offsets, fl, records, render_alphas, last_ids = ctx.saved_tensors
         absgrad_holder = ctx.absgrad_holder
-        row_dims, I, N, R, D, width, height, tile_size, tw, th, S = ctx.meta
+        row_dims, I, N, D, width, height, tile_size, tw, th, S = ctx.meta
         dev = render_alphas.device
         # set_materialize_grads(False): an output the loss does not use arrives as None instead of a zero-filled tensor
         # (render_alphas in a plain photometric loss: 8 MB of zeros per 1080p step); the kernel takes a null pointer for it
@@ -1079,23 +1120,19 @@ class _RasterizeToPixels(torch.autograd.Function):
         v_render_colors = v_render_colors.contiguous()
         v_render_alphas = v_render_alphas.contiguous() if v_render_alphas is not None else None
         absgrad = absgrad_holder is not None
-        P = _grad_record_width(D, absgrad)
-        # one packed gradient record per gaussian: [v_xy 2 | v_conic 3 | v_opacity 1 | v_rgb D | (abs 2) | pad]
-        rec = torch.zeros((R, P), device=dev, dtype=torch.float32)
-        base = rec.data_ptr()
+        rec = _grad_records(row_dims, D, absgrad, dev)
         with _Ctx(dev) as st:
             check(
                 lib().gsb200_raster_bwd(
                     I, N, D, ptr(backgrounds), ptr(m8), width, height, tile_size, tw, th, ptr(offsets), ptr(fl), S,
-                    ptr(records), ptr(render_alphas), ptr(last_ids), ptr(v_render_colors), ptr(v_render_alphas),
-                    base, P, base + 8, P, base + 24, P, base + 20, P, (base + 4 * (6 + D)) if absgrad else None, P, st,
+                    ptr(records), ptr(render_alphas), ptr(last_ids), ptr(v_render_colors), ptr(v_render_alphas), absgrad,
+                    ptr(rec), st,
                 ),
                 "rasterize_to_pixels_3dgs_bwd",
             )
-        rec = rec.view(row_dims + (P,))
-        v_means2d, v_conics, v_opacities, v_colors = rec[..., 0:2], rec[..., 2:5], rec[..., 5], rec[..., 6 : 6 + D]
+        v_means2d, v_conics, v_colors, v_opacities, v_abs = _split_grad_records(rec, D, absgrad)
         if absgrad:
-            absgrad_holder.copy_(rec[..., 6 + D : 8 + D])
+            absgrad_holder.copy_(v_abs)
         v_backgrounds = None
         if backgrounds is not None and ctx.needs_input_grad[4]:
             v_backgrounds = (v_render_colors * (1.0 - render_alphas)).sum(dim=(-3, -2))
@@ -1132,33 +1169,14 @@ def rasterize_to_pixels_rows(
 ) -> Tuple[Tensor, Tensor]:
     """rasterize_to_pixels with the optional ``RowSideOutputs.rows`` of the fused projection that produced the inputs
     (rasterization() passes them; the forward's pack pass then only gathers)."""
-    if packed != (means2d.dim() == 2):
-        raise ValueError(f"packed={packed} but means2d has shape {tuple(means2d.shape)}")
-    if tile_size != 16:
-        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
-    D = colors.shape[-1]
-    if D > 32:
-        raise ValueError(
-            f"Unsupported number of color channels: {D}. gsplat_b200 rasterizes up to 32 channels per pass "
-            "(rasterization() chunks wider features with channel_chunk=32)."
+
+    def composite(colors, backgrounds, holder, padded):
+        return _RasterizeToPixels.apply(
+            means2d, conics, colors, opacities, backgrounds, masks, int(image_width), int(image_height), int(tile_size),
+            isect_offsets, flatten_ids, holder, None if padded else _row_records,
         )
-    pad = 0
-    if D not in _SUPPORTED_CHANNELS:
-        target = next(c for c in _SUPPORTED_CHANNELS if c >= D)
-        pad = target - D
-        colors = torch.nn.functional.pad(colors, (0, pad))
-        if backgrounds is not None:
-            backgrounds = torch.nn.functional.pad(backgrounds, (0, pad))
-    holder = torch.zeros_like(means2d) if absgrad else None
-    render_colors, render_alphas = _RasterizeToPixels.apply(
-        means2d, conics, colors, opacities, backgrounds, masks, int(image_width), int(image_height), int(tile_size),
-        isect_offsets, flatten_ids, holder, _row_records if pad == 0 else None,
-    )
-    if absgrad:
-        means2d.absgrad = holder
-    if pad:
-        render_colors = render_colors[..., :D]
-    return render_colors, render_alphas
+
+    return _rasterize_padded(means2d, colors, backgrounds, tile_size, packed, absgrad, composite)
 
 
 # --------------------------------------------------------------------------------------------
@@ -1626,24 +1644,19 @@ class _RasterizeToPixelsSparse(torch.autograd.Function):
         v_render_colors = v_render_colors.contiguous()
         v_render_alphas = v_render_alphas.contiguous() if v_render_alphas is not None else None
         absgrad = absgrad_holder is not None
-        Pw = _grad_record_width(D, absgrad)
-        # one packed gradient record per gaussian: [v_xy 2 | v_conic 3 | v_opacity 1 | v_rgb D | (abs 2) | pad]
-        rec = torch.zeros((R, Pw), device=dev, dtype=torch.float32)
-        base = rec.data_ptr()
+        rec = _grad_records(row_dims, D, absgrad, dev)
         with _Ctx(dev) as st:
             check(
                 lib().gsb200_raster_sparse_bwd(
                     R, D, ptr(backgrounds), ptr(m8), width, height, 16, tw, th, active.shape[0], ptr(active), ptr(offsets), ptr(fl),
                     fl.shape[0], ptr(words), ptr(cumsum), ptr(pmap), ptr(records), ptr(render_alphas), ptr(last_ids),
-                    ptr(v_render_colors), ptr(v_render_alphas), base, Pw, base + 8, Pw, base + 24, Pw, base + 20, Pw,
-                    (base + 4 * (6 + D)) if absgrad else None, Pw, st,
+                    ptr(v_render_colors), ptr(v_render_alphas), absgrad, ptr(rec), st,
                 ),
                 "rasterize_to_pixels_sparse_bwd",
             )
-        rec = rec.view(row_dims + (Pw,))
-        v_means2d, v_conics, v_opacities, v_colors = rec[..., 0:2], rec[..., 2:5], rec[..., 5], rec[..., 6 : 6 + D]
+        v_means2d, v_conics, v_colors, v_opacities, v_abs = _split_grad_records(rec, D, absgrad)
         if absgrad:
-            absgrad_holder.copy_(rec[..., 6 + D : 8 + D])
+            absgrad_holder.copy_(v_abs)
         v_backgrounds = None
         if backgrounds is not None and ctx.needs_input_grad[4]:
             v_backgrounds = torch.zeros_like(backgrounds).index_add_(0, image_ids.long(), v_render_colors * (1.0 - render_alphas))
@@ -1676,16 +1689,6 @@ def rasterize_to_pixels_sparse(
     isect_tiles_sparse.  Returns (render_colors [P, channels], render_alphas [P, 1]) in the original pixel order; each
     value is the dense rendering's at that pixel (requested pixels in the margin of a partial tile included).  With
     ``absgrad`` the backward fills ``means2d.absgrad``."""
-    if packed != (means2d.dim() == 2):
-        raise ValueError(f"packed={packed} but means2d has shape {tuple(means2d.shape)}")
-    if tile_size != 16:
-        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
-    D = colors.shape[-1]
-    if D > 32:
-        raise ValueError(
-            f"Unsupported number of color channels: {D}. gsplat_b200 rasterizes up to 32 channels per pass "
-            "(rasterization() chunks wider features with channel_chunk=32)."
-        )
     AT, P = active_tiles.shape[0] if active_tiles.dim() == 1 else -1, pixel_map.shape[0] if pixel_map.dim() == 1 else -1
     if AT < 0 or P < 0 or active_tiles.dtype != torch.int32:
         raise ValueError("active_tiles must be int32 [AT] and pixel_map [P]")
@@ -1700,24 +1703,15 @@ def rasterize_to_pixels_sparse(
         raise ValueError(f"image_ids must be [{P}], got {tuple(image_ids.shape)}")
     if tile_width * 16 < image_width or tile_height * 16 < image_height:
         raise ValueError(f"a {tile_width} x {tile_height} tile grid does not cover {image_width} x {image_height} pixels")
-    pad = 0
-    if D not in _SUPPORTED_CHANNELS:
-        target = next(c for c in _SUPPORTED_CHANNELS if c >= D)
-        pad = target - D
-        colors = torch.nn.functional.pad(colors, (0, pad))
-        if backgrounds is not None:
-            backgrounds = torch.nn.functional.pad(backgrounds, (0, pad))
-    holder = torch.zeros_like(means2d) if absgrad else None
-    render_colors, render_alphas = _RasterizeToPixelsSparse.apply(
-        means2d, conics, colors, opacities, backgrounds, masks, image_ids, active_tiles, tile_offsets, flatten_ids,
-        tile_pixel_mask, tile_pixel_cumsum, pixel_map, int(image_width), int(image_height), int(tile_width), int(tile_height),
-        holder,
-    )
-    if absgrad:
-        means2d.absgrad = holder
-    if pad:
-        render_colors = render_colors[..., :D]
-    return render_colors, render_alphas
+
+    def composite(colors, backgrounds, holder, padded):
+        return _RasterizeToPixelsSparse.apply(
+            means2d, conics, colors, opacities, backgrounds, masks, image_ids, active_tiles, tile_offsets, flatten_ids,
+            tile_pixel_mask, tile_pixel_cumsum, pixel_map, int(image_width), int(image_height), int(tile_width),
+            int(tile_height), holder,
+        )
+
+    return _rasterize_padded(means2d, colors, backgrounds, tile_size, packed, absgrad, composite)
 
 
 # --------------------------------------------------------------------------------------------

@@ -19,6 +19,7 @@ import torch
 from ._cabi import stream as _raw_stream
 
 from ._cabi import check, lib, ptr
+from .ops import _grad_records, _split_grad_records
 
 _libs = []
 
@@ -74,8 +75,7 @@ def rasterize_to_pixels_3dgs_bwd(means2d, conics, colors, opacities, backgrounds
     N = (R + max(I, 1) - 1) // max(I, 1)
     means2d, conics, colors, opacities = means2d.contiguous(), conics.contiguous(), colors.contiguous(), opacities.contiguous()
     offsets, fl = tile_offsets.contiguous(), flatten_ids.contiguous()
-    P = (6 + D + (2 if absgrad else 0) + 3) // 4 * 4
-    g = torch.zeros(rows + (P,), device=dev)
+    g = _grad_records(rows, D, absgrad, dev)
     m8 = None if masks is None else masks.contiguous().view(torch.uint8)
     with torch.cuda.device(dev):
         rec = torch.empty(max(L.gsb200_raster_records_bytes(S, D, I * th * tw), 16), dtype=torch.uint8, device=dev)
@@ -83,21 +83,20 @@ def rasterize_to_pixels_3dgs_bwd(means2d, conics, colors, opacities, backgrounds
             L.gsb200_raster_pack(I, D, ptr(means2d), ptr(conics), ptr(colors), ptr(opacities), tw, th, ptr(offsets), ptr(fl), S, ptr(rec), _stream()),
             "raster_pack",
         )
-        b = g.data_ptr()
         check(
             L.gsb200_raster_bwd(
                 I, N, D, ptr(backgrounds), ptr(m8), image_width, image_height, tile_size, tw, th, ptr(offsets), ptr(fl), S,
                 ptr(rec), ptr(render_alphas.contiguous()), ptr(last_ids.contiguous()), ptr(v_render_colors.contiguous()),
-                ptr(v_render_alphas.contiguous()), b, P, b + 8, P, b + 24, P, b + 20, P, (b + 4 * (6 + D)) if absgrad else None, P,
-                _stream(),
+                ptr(v_render_alphas.contiguous()), absgrad, ptr(g), _stream(),
             ),
             "rasterize_to_pixels_3dgs_bwd",
         )
     v_bg = None
     if compute_v_backgrounds and backgrounds is not None:
         v_bg = (v_render_colors * (1.0 - render_alphas)).sum(dim=(-3, -2))
-    v_abs = g[..., 6 + D : 8 + D].contiguous() if absgrad else None
-    return v_abs, g[..., 0:2].contiguous(), g[..., 2:5].contiguous(), g[..., 6 : 6 + D].contiguous(), g[..., 5].contiguous(), v_bg
+    v_m2, v_con, v_col, v_op, v_abs = _split_grad_records(g, D, absgrad)
+    v_abs = v_abs.contiguous() if absgrad else None
+    return v_abs, v_m2.contiguous(), v_con.contiguous(), v_col.contiguous(), v_op.contiguous(), v_bg
 
 
 def register(namespace: str = "gsplat") -> None:

@@ -296,17 +296,18 @@ extern "C"
         const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, void *records, float *render_colors,
         float *render_alphas, int32_t *last_ids, void *stream
     );
-    /* Gradient outputs are ACCUMULATED into (caller zero-initialises): each is addressed as
-     * ptr[g * stride + k], g in [0, I*N), so they may be views into one packed record per gaussian.
-     * v_means2d_abs may be NULL (absgrad off); v_render_alphas may be NULL (no gradient flows into render_alphas). */
+    /* The gradients are ACCUMULATED into v_grad_records, one record per gaussian row g in [0, I*N): a row of
+     * round_up4(6 + D + 2*absgrad) floats laid out
+     *     [v_means2d 2 | v_conics 3 | v_opacities 1 | v_colors D | v_means2d_abs 2 if absgrad | zero pad].
+     * The caller zero-fills the records; their base must be 16-byte aligned (GSB200_E_INVALID otherwise) and
+     * rows * row width must stay below 2^32 (GSB200_E_UNSUPPORTED otherwise).
+     * v_render_alphas may be NULL (no gradient flows into render_alphas). */
     int gsb200_raster_bwd(
         int64_t I, int64_t N, int D, const float *backgrounds, const uint8_t *masks, uint32_t image_width,
         uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
         const int32_t *flatten_ids, int64_t n_isects, const void *records, const float *render_alphas,
-        const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, float *v_means2d,
-        int64_t v_means2d_stride, float *v_conics, int64_t v_conics_stride, float *v_colors, int64_t v_colors_stride,
-        float *v_opacities, int64_t v_opacities_stride, float *v_means2d_abs, int64_t v_means2d_abs_stride,
-        void *stream
+        const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, int absgrad,
+        float *v_grad_records, void *stream
     );
 
     /* ---- sparse pixels: build_sparse_tile_layout, isect_tiles_sparse, rasterize_to_pixels_sparse
@@ -350,8 +351,8 @@ extern "C"
      * from gsb200_isect_sparse_emit, the layout tensors from gsb200_sparse_layout_finish.  Gaussian rows and
      * backgrounds [n_images, D] / masks [n_images, th, tw] as in gsb200_raster_fwd; `records` of
      * gsb200_raster_records_bytes(n_isects, D, n_active).  Outputs in the original pixel order: render_colors [P, D],
-     * render_alphas [P], last_ids int32 [P].  The backward accumulates into gradient rows g in [0, n_rows) like
-     * gsb200_raster_bwd; v_render_colors [P, D], v_render_alphas [P] or NULL. */
+     * render_alphas [P], last_ids int32 [P].  The backward accumulates into the gradient records of gsb200_raster_bwd,
+     * one per gaussian row g in [0, n_rows); v_render_colors [P, D], v_render_alphas [P] or NULL. */
     int gsb200_raster_sparse_fwd(
         int D, const float *means2d, const float *conics, const float *colors, const float *opacities,
         const float *backgrounds, const uint8_t *masks, uint32_t image_width, uint32_t image_height, uint32_t tile_size,
@@ -365,9 +366,8 @@ extern "C"
         uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t n_active, const int32_t *active_tiles,
         const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t n_isects, const uint64_t *tile_pixel_mask,
         const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, const void *records, const float *render_alphas,
-        const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, float *v_means2d,
-        int64_t v_means2d_stride, float *v_conics, int64_t v_conics_stride, float *v_colors, int64_t v_colors_stride,
-        float *v_opacities, int64_t v_opacities_stride, float *v_means2d_abs, int64_t v_means2d_abs_stride, void *stream
+        const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, int absgrad,
+        float *v_grad_records, void *stream
     );
 
     /* ---- 2DGS (surfel splatting), dense layout: projection_2dgs_fused / _bwd and rasterize_to_pixels_2dgs / _bwd

@@ -79,6 +79,33 @@ def test_shipped_binary_matches_the_sources():
     assert L.gsb200_error_string(-5).startswith(b"intersect_tile")
 
 
+def test_raster_bwd_checks_gradient_records():
+    """Both compositing backwards check the gradient records before anything is launched: a null or non-16-byte-aligned
+    base is GSB200_E_INVALID, rows * row width of 2^32 floats or more is GSB200_E_UNSUPPORTED (the kernel addresses a
+    row with a 32-bit element offset)."""
+    from gsplat_b200 import _cabi
+
+    L = _cabi.lib()
+    fake = 1 << 20  # never dereferenced: every call below returns before the kernel is launched
+
+    def dense(N, rec, absgrad=0):
+        return L.gsb200_raster_bwd(
+            1, N, 3, None, None, 16, 16, 16, 1, 1, fake, fake, 1, fake, fake, fake, fake, None, absgrad, rec, None
+        )
+
+    def sparse(n_rows, rec, absgrad=0):
+        return L.gsb200_raster_sparse_bwd(
+            n_rows, 3, None, None, 16, 16, 16, 1, 1, 1, fake, fake, fake, 1, fake, fake, fake, fake, fake, fake, fake, None,
+            absgrad, rec, None,
+        )
+
+    too_many = (1 << 32) // 12 + 1  # D = 3 with absgrad: 12-float rows
+    for call in (dense, sparse):
+        assert call(4, None) == -1
+        assert call(4, fake + 4) == -1
+        assert call(too_many, fake, absgrad=1) == -2
+
+
 def test_no_cpu_fallback():
     import gsplat_b200
     from gsplat_b200._cabi import GsplatB200Error
