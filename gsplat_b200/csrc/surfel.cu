@@ -97,7 +97,13 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_project_fwd_kernel(
                 const float fr_y = ceilf(kGaussianExtend * sqrtf(fmaxf(1e-4f, ey)));
                 const bool clipped = fr_x <= radius_clip && fr_y <= radius_clip;
                 const bool off     = m2x + fr_x <= 0.f || m2x - fr_x >= (float)W || m2y + fr_y <= 0.f || m2y - fr_y >= (float)H;
-                if(!clipped && !off)
+                // finite inputs can overflow here (fx * scale beyond FLT_MAX): a NaN screen mean passes every off-screen
+                // test and composites at alpha 0.99 wherever it is listed, so such a row is culled
+                bool finite = isfinite(m2x) && isfinite(m2y) && isfinite(z);
+#pragma unroll
+                for(int k = 0; k < 3; ++k)
+                    finite = finite && isfinite(T0[k]) && isfinite(T1[k]) && isfinite(T2[k]);
+                if(!clipped && !off && finite)
                 {
                     rx = (int)fr_x, ry = (int)fr_y;
                     mx = m2x, my = m2y, depth = z;

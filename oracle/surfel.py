@@ -1,5 +1,6 @@
 """Float64 PyTorch-on-CPU restatement of the 2DGS (surfel) kernels of gsplat_b200/csrc/surfel.cu, the truth the GPU tests
-compare against.  Same culls (near / far, degenerate ray transform, radius_clip, off-screen), ``ceil`` radii, alpha
+compare against.  Same culls (near / far, degenerate ray transform, radius_clip, off-screen; float32 overflow only
+approximately, see project), ``ceil`` radii, alpha
 threshold, exclusive transmittance stop, median rule and L1 distortion; every gradient comes from autograd.
 
   project(...)       -> radii, means2d, depths, ray_transforms, normals     (differentiable)
@@ -64,6 +65,12 @@ def project(means, quats, scales, viewmats, Ks, width, height, near_plane=0.01, 
     md = m2.detach()
     off = (md[..., 0] + r[..., 0] <= 0) | (md[..., 0] - r[..., 0] >= width) | (md[..., 1] + r[..., 1] <= 0) | (md[..., 1] - r[..., 1] >= height)
     ok = ok & ~off
+    # the kernel culls a row whose float32 ray transform, screen mean or depth is not finite.  This restates that only
+    # for final values beyond float32's range: a row whose float32 intermediates overflow (the products in the screen
+    # mean) while these values fit is culled by the kernel and kept here
+    f32max = float(np.finfo(np.float32).max)
+    fits = (M.detach().abs() <= f32max).all(-1).all(-1) & (md.abs() <= f32max).all(-1) & (z.detach().abs() <= f32max)
+    ok = ok & fits
     radii = torch.where(ok[..., None], r, torch.zeros_like(r)).to(torch.int32)
     nrm = RS_c[..., 2]
     cosv = -(nrm * mc).sum(-1, keepdim=True)
