@@ -107,8 +107,6 @@ _SIGNATURES = {
         [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_vp,
          c_vp, c_vp, c_sz, c_vp],
     ),
-    "gsb200_sort_tile_pairs_workspace_bytes": (c_sz, [c_i64, c_int, c_int]),
-    "gsb200_sort_tile_pairs": (c_int, [c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),
     "gsb200_isect_ids_from_tilekeys": (c_int, [c_i64, c_int, c_vp, c_vp, c_vp, c_i64, c_u32, c_u32, c_vp, c_vp]),
     "gsb200_isect_offsets": (c_int, [c_i64, c_vp, c_i64, c_u32, c_u32, c_vp, c_vp]),
     "gsb200_relocation": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_f32, c_vp, c_vp, c_vp]),

@@ -23,12 +23,13 @@ UNITS = {
     # file: extra flags
     "raster.cu": [],
     "pergauss.cu": ["-fmad=false"],
+    "isect.cu": ["-fmad=false"],
     "sort.cu": [],
     "nvls.cu": [],
     "loss.cu": [],
     "surfel.cu": ["-fmad=false"],
 }
-HEADERS = ["common.cuh", "gaussmath.cuh", "rowrec.cuh", os.path.join("..", "..", "include", "gsplat_b200.h")]
+HEADERS = ["common.cuh", "gaussmath.cuh", "isect.cuh", "rowrec.cuh", os.path.join("..", "..", "include", "gsplat_b200.h")]
 
 
 def _nvcc() -> str:

@@ -58,23 +58,6 @@ inline uint32_t bits_for_count(int64_t count)
 
 inline unsigned grid_for(int64_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
-// stages of gsb200_isect_sorted (sort.cu) that live with the tile-intersection kernels (pergauss.cu)
-int emit_tilekeys_bounded(
-    int64_t N, int64_t cap_vis, int64_t max_tiles_hint, const float *means2d, const int32_t *radii, const float *depths,
-    const float *conics, const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, const int32_t *order,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int key_bytes, void *keys, int32_t *flatten_ids,
-    const int64_t *totals, int64_t cap_isects, cudaStream_t st
-);
-// depth order of every projected row (sort.cu), the first stage of gsb200_isect_sparse_count (pergauss.cu)
-size_t depth_order_workspace_bytes(int64_t I, int64_t total_rows);
-int depth_order(
-    int64_t I, int64_t N, const int32_t *radii, const float *depths, const int64_t *image_ids, int32_t *order,
-    void *workspace, size_t workspace_bytes, cudaStream_t st
-);
-int offsets_tilekeys_bounded(
-    int64_t cap_isects, int key_bytes, const void *keys, int64_t total_tiles, int32_t *offsets, const int64_t *totals, cudaStream_t st
-);
-
 #ifdef __CUDACC__
 // ---- mbarrier / bulk-copy (TMA 1-D, SASS UBLKCP) wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -1,13 +1,14 @@
 // pergauss.cu -- the per-gaussian (HBM-bound) kernels: quat/scale -> covariance, EWA projection,
-// spherical harmonics, the fused projection + conic + SH->RGB pass, tile counting / emission and
-// the tile-offset encoder.  Compiled with -fmad=false (see gaussmath.cuh).
+// spherical harmonics, the fused projection + conic + SH->RGB pass, and the MCMC / Adam updates.
+// Compiled with -fmad=false (see gaussmath.cuh).
 //
 // Reference kernels replaced: csrc/QuatScaleToCovarCUDA.cu:37,211;
 // csrc/ProjectionEWA3DGSFused.cu:38-219,376-638; csrc/SphericalHarmonicsCUDA.cu:443-569,785-890,
-// 1085-1250 (assemble_proj_features); csrc/IntersectTile.cu:83-464,925-988.
+// 1085-1250 (assemble_proj_features).
 #include <cub/device/device_scan.cuh>
 
 #include "gaussmath.cuh"
+#include "isect.cuh"
 #include "rowrec.cuh"
 
 namespace gsb
@@ -480,12 +481,6 @@ __global__ void __launch_bounds__(kThreads) sh_rows_bwd_kernel(
 // ------------------------------------------------------------------ fused projection + conic + SH -> RGB
 // One thread per (camera, gaussian).  SH coefficients of a visible gaussian are fetched with 128-bit
 // loads (48 floats = 12 x float4 when K = 16); culled gaussians never touch them.
-template<class F>
-__device__ __forceinline__ int tiles_of_gaussian(
-    float mx, float my, int rx, int ry, const float *conic, const float *opacity, uint32_t tile_size, uint32_t tw,
-    uint32_t th, F &&f
-); // defined with the tile intersection kernels below
-
 // ROWS: the epilogue also produces what the next two stages would otherwise recompute per row / per intersection --
 // the row's tile count and the three totals of gsb200_isect_count_totals (same device function as the emit pass, so the
 // counts agree bit for bit), and the 64-byte compositing row record {cull | axis | geom | rgb0} of rowrec.cuh, which
@@ -502,13 +497,9 @@ __global__ void __launch_bounds__(kThreads, 4) project_sh_fwd_kernel(
     int32_t *__restrict__ tiles_per_gauss, unsigned long long *__restrict__ totals
 )
 {
-    __shared__ unsigned long long s_tot[3];
+    unsigned long long *s_tot = nullptr;
     if constexpr(ROWS)
-    {
-        if(threadIdx.x < 3)
-            s_tot[threadIdx.x] = 0ull;
-        __syncthreads();
-    }
+        s_tot = block_tile_totals_begin();
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int cnt           = 0;
     if(idx < C * N)
@@ -587,22 +578,7 @@ __global__ void __launch_bounds__(kThreads, 4) project_sh_fwd_kernel(
     }
     }
     if constexpr(ROWS)
-    { // the three totals, as isect_count_totals_kernel forms them
-        const int wsum         = __reduce_add_sync(0xffffffffu, cnt);
-        const int wmax         = __reduce_max_sync(0xffffffffu, cnt);
-        const unsigned nonzero = __ballot_sync(0xffffffffu, cnt > 0);
-        if((threadIdx.x & 31) == 0 && nonzero != 0u)
-        {
-            atomicAdd(&s_tot[0], (unsigned long long)wsum);
-            atomicAdd(&s_tot[1], (unsigned long long)__popc(nonzero));
-            atomicMax(&s_tot[2], (unsigned long long)wmax);
-        }
-        __syncthreads();
-        if(threadIdx.x < 2 && s_tot[threadIdx.x] != 0ull)
-            atomicAdd(&totals[threadIdx.x], s_tot[threadIdx.x]);
-        if(threadIdx.x == 2 && s_tot[2] != 0ull)
-            atomicMax(&totals[2], s_tot[2]);
-    }
+        block_tile_totals(cnt, s_tot, totals);
 }
 
 // One thread per gaussian, looping over cameras: v_means / v_quats / v_scales / v_sh written once.
@@ -964,477 +940,6 @@ __global__ void __launch_bounds__(kThreads) projection_packed_bwd_kernel(
     }
 }
 
-// ------------------------------------------------------------------ tile intersection
-// Enumerates the tiles of one gaussian in the reference's emit order, calling f(tile_id).
-// AccuTile / SNUGBOX (csrc/IntersectTile.cu:83-207, 288-373) or the radius AABB (:374-463).
-template<class F>
-__device__ __forceinline__ int tiles_of_gaussian(
-    float mx, float my, int rx, int ry, const float *conic, const float *opacity, uint32_t tile_size, uint32_t tw,
-    uint32_t th, F &&f
-)
-{
-    if(rx <= 0 || ry <= 0)
-        return 0;
-    int count      = 0;
-    const float ts = (float)tile_size;
-    auto clampi    = [](int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); };
-    if(conic != nullptr && opacity != nullptr)
-    {
-        const float A = conic[0], Bc = conic[1], Cc = conic[2];
-        const float disc = Bc * Bc - A * Cc;
-        float t          = 2.f * exact_log(*opacity / kAlphaThreshold);
-        const float cap  = kGaussianExtend * kGaussianExtend;
-        t                = t < cap ? t : cap;
-        const float ntd  = -t / disc;
-        const float xe = sqrtf(ntd * Cc), ye = sqrtf(ntd * A);
-        const float bminx = mx - xe, bminy = my - ye, bmaxx = mx + xe, bmaxy = my + ye;
-        const float BxC = Bc * xe / Cc, ByA = Bc * ye / A;
-        const float argminx = my + BxC, argminy = mx + ByA, argmaxx = my - BxC, argmaxy = mx - ByA;
-        const int rminx = clampi((int)(bminx / ts), 0, (int)tw), rminy = clampi((int)(bminy / ts), 0, (int)th);
-        const int rmaxx = clampi((int)(bmaxx / ts + 1.f), 0, (int)tw), rmaxy = clampi((int)(bmaxy / ts + 1.f), 0, (int)th);
-        const int ys = rmaxy - rminy, xs = rmaxx - rminx;
-        if(ys * xs == 0)
-            return 0;
-        const bool isY = ys < xs;
-        const int ru0 = isY ? rminy : rminx, ru1 = isY ? rmaxy : rmaxx, rv0 = isY ? rminx : rminy, rv1 = isY ? rmaxx : rmaxy;
-        const float bminu = isY ? bminy : bminx, bmaxu = isY ? bmaxy : bmaxx;
-        const float bminv = isY ? bminx : bminy, bmaxv = isY ? bmaxx : bmaxy;
-        const float amin_v = isY ? argminx : argminy, amax_v = isY ? argmaxx : argmaxy;
-        const float pu = isY ? my : mx, pv = isY ? mx : my, coeff = isY ? A : Cc;
-        auto line = [&](float coord, float &lo, float &hi) {
-            const float h  = coord - pu;
-            const float sq = sqrtf(disc * h * h + t * coeff);
-            lo             = (-Bc * h - sq) / coeff + pv;
-            hi             = (-Bc * h + sq) / coeff + pv;
-        };
-        float maxlo = bmaxv, maxhi = bminv, minlo, minhi;
-        float min_line = (float)ru0 * ts;
-        if(bminu <= min_line)
-            line(min_line, minlo, minhi);
-        else
-            minlo = maxlo, minhi = maxhi;
-        for(int u = ru0; u < ru1; ++u)
-        {
-            const float max_line = min_line + ts;
-            if(max_line <= bmaxu)
-                line(max_line, maxlo, maxhi);
-            const float emin = (min_line <= amin_v && amin_v < max_line) ? bminv : (minlo < maxlo ? minlo : maxlo);
-            const float emax = (min_line <= amax_v && amax_v < max_line) ? bmaxv : (minhi > maxhi ? minhi : maxhi);
-            const int e0 = (int)(emin / ts), e1 = (int)(emax / ts + 1.f);
-            int v0 = e0 < rv1 ? e0 : rv1;
-            v0     = v0 > rv0 ? v0 : rv0;
-            int v1 = e1 > rv0 ? e1 : rv0;
-            v1     = v1 < rv1 ? v1 : rv1;
-            for(int v = v0; v < v1; ++v)
-            {
-                ++count;
-                f(isY ? (int64_t)u * tw + v : (int64_t)v * tw + u);
-            }
-            minlo = maxlo, minhi = maxhi, min_line = max_line;
-        }
-    }
-    else
-    {
-        const float trx = (float)rx / ts, try_ = (float)ry / ts, tx = mx / ts, ty = my / ts;
-        const int x0 = clampi((int)floorf(tx - trx), 0, (int)tw), y0 = clampi((int)floorf(ty - try_), 0, (int)th);
-        const int x1 = clampi((int)ceilf(tx + trx), 0, (int)tw), y1 = clampi((int)ceilf(ty + try_), 0, (int)th);
-        for(int i = y0; i < y1; ++i)
-            for(int j = x0; j < x1; ++j)
-            {
-                ++count;
-                f((int64_t)i * tw + j);
-            }
-    }
-    return count;
-}
-
-// row-order tile count of every row (the unsorted intersection's first pass)
-__global__ void __launch_bounds__(kThreads) isect_count_kernel(
-    int64_t total, const float *__restrict__ means2d, const int32_t *__restrict__ radii, const float *__restrict__ conics,
-    const float *__restrict__ opacities, uint32_t tile_size, uint32_t tw, uint32_t th, int32_t *__restrict__ tiles_per_gauss
-)
-{
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(i >= total)
-        return;
-    const int2 r    = reinterpret_cast<const int2 *>(radii)[i];
-    int cnt         = 0;
-    if(r.x > 0 && r.y > 0)
-    {
-        const float2 m = reinterpret_cast<const float2 *>(means2d)[i];
-        float cn[3] = {0.f, 0.f, 0.f}, op = 0.f;
-        const bool accu = conics != nullptr && opacities != nullptr;
-        if(accu)
-            cn[0] = conics[i * 3], cn[1] = conics[i * 3 + 1], cn[2] = conics[i * 3 + 2], op = opacities[i];
-        cnt = tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [](int64_t) {});
-    }
-    tiles_per_gauss[i] = cnt;
-}
-
-// row-order count + the totals the host reads once: [0] = number of intersections, [1] = rows with tiles,
-// [2] = the largest tile count of a row (picks the emit kernel)
-__global__ void __launch_bounds__(kThreads) isect_count_totals_kernel(
-    int64_t total, const float *__restrict__ means2d, const int32_t *__restrict__ radii, const float *__restrict__ conics,
-    const float *__restrict__ opacities, uint32_t tile_size, uint32_t tw, uint32_t th, int32_t *__restrict__ tiles_per_gauss,
-    unsigned long long *__restrict__ totals
-)
-{
-    __shared__ unsigned long long s_tot[3];
-    if(threadIdx.x < 3)
-        s_tot[threadIdx.x] = 0ull;
-    __syncthreads();
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int cnt         = 0;
-    if(i < total)
-    {
-        const int2 r = reinterpret_cast<const int2 *>(radii)[i];
-        if(r.x > 0 && r.y > 0)
-        {
-            const float2 m = reinterpret_cast<const float2 *>(means2d)[i];
-            float cn[3] = {0.f, 0.f, 0.f}, op = 0.f;
-            const bool accu = conics != nullptr && opacities != nullptr;
-            if(accu)
-                cn[0] = conics[i * 3], cn[1] = conics[i * 3 + 1], cn[2] = conics[i * 3 + 2], op = opacities[i];
-            cnt = tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [](int64_t) {});
-        }
-        tiles_per_gauss[i] = cnt;
-    }
-    const int wsum         = __reduce_add_sync(0xffffffffu, cnt);
-    const int wmax         = __reduce_max_sync(0xffffffffu, cnt);
-    const unsigned nonzero = __ballot_sync(0xffffffffu, cnt > 0);
-    if((threadIdx.x & 31) == 0 && nonzero != 0u)
-    {
-        atomicAdd(&s_tot[0], (unsigned long long)wsum);
-        atomicAdd(&s_tot[1], (unsigned long long)__popc(nonzero));
-        atomicMax(&s_tot[2], (unsigned long long)wmax);
-    }
-    __syncthreads();
-    if(threadIdx.x < 2 && s_tot[threadIdx.x] != 0ull)
-        atomicAdd(&totals[threadIdx.x], s_tot[threadIdx.x]);
-    if(threadIdx.x == 2 && s_tot[2] != 0ull)
-        atomicMax(&totals[2], s_tot[2]);
-}
-
-// Key of one (gaussian, tile) intersection.  int64_t: the reference's isect id, (image | tile) << 32 | depth bits
-// (csrc/IntersectTile.cu:925-988).  uint16_t / uint32_t: the dense tile id image * n_tiles + tile alone -- the rows are
-// emitted in depth order already, so the S-sized sort only needs those bits, and moving 2 + 4 instead of 8 + 4 bytes per
-// intersection and pass halves its traffic (the 64-bit ids are rebuilt on demand: isect_ids_from_tilekeys_kernel).
-template<class KeyT>
-struct IsectKey
-{
-    uint32_t base;
-    __device__ __forceinline__ IsectKey(int64_t image, uint32_t, uint32_t, int64_t n_tiles) : base((uint32_t)(image * n_tiles)) {}
-    __device__ __forceinline__ KeyT operator()(int64_t tile) const { return (KeyT)(base + (uint32_t)tile); }
-};
-template<>
-struct IsectKey<int64_t>
-{
-    int64_t hi_db;
-    __device__ __forceinline__ IsectKey(int64_t image, uint32_t dbits, uint32_t tile_n_bits, int64_t)
-        : hi_db((image << (32 + tile_n_bits)) | (int64_t)dbits)
-    {
-    }
-    __device__ __forceinline__ int64_t operator()(int64_t tile) const { return hi_db | (tile << 32); }
-};
-
-// Capacity-bounded emission (gsb200_isect_sorted): the launch covers `total` = capacity row slots and writes into
-// capacity-sized outputs, while the real counts sit in device memory (totals[0] intersections, totals[1] rows with
-// tiles).  Returns the number of real row slots; the slots between the real intersections and the capacity get padding
-// pairs (largest key: the stable sort leaves them behind every real pair; row 0: any valid row).
-template<class KeyT>
-__device__ __forceinline__ int64_t emit_bounded_rows(
-    int64_t j, int64_t n_threads, int64_t total, const int64_t *__restrict__ totals, int64_t cap_isects,
-    KeyT *__restrict__ isect_ids, int32_t *__restrict__ flatten_ids
-)
-{
-    const int64_t n_real = totals[0] < cap_isects ? totals[0] : cap_isects;
-    for(int64_t s = n_real + j; s < cap_isects; s += n_threads)
-    {
-        isect_ids[s]   = (KeyT)~(KeyT)0;
-        flatten_ids[s] = 0;
-    }
-    return totals[1] < total ? totals[1] : total;
-}
-
-template<class KeyT>
-__global__ void __launch_bounds__(kThreads) isect_emit_kernel(
-    int64_t total, int64_t N, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
-    const float *__restrict__ depths, const float *__restrict__ conics, const float *__restrict__ opacities,
-    const int64_t *__restrict__ cum_tiles, const int64_t *__restrict__ image_ids, const int32_t *__restrict__ order,
-    uint32_t tile_size, uint32_t tw, uint32_t th, uint32_t tile_n_bits, KeyT *__restrict__ isect_ids,
-    int32_t *__restrict__ flatten_ids, const int64_t *__restrict__ totals = nullptr, int64_t cap_isects = 0
-)
-{
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(totals != nullptr)
-        total = emit_bounded_rows<KeyT>(j, (int64_t)gridDim.x * blockDim.x, total, totals, cap_isects, isect_ids, flatten_ids);
-    if(j >= total)
-        return;
-    if(totals != nullptr && cum_tiles[j] > cap_isects)
-        return; // beyond the speculative capacity: the host sees totals[0] > capacity and redoes the stage
-    const int64_t i = order ? (int64_t)order[j] : j;
-    const int2 r    = reinterpret_cast<const int2 *>(radii)[i];
-    if(r.x <= 0 || r.y <= 0)
-        return;
-    const float2 m = reinterpret_cast<const float2 *>(means2d)[i];
-    float cn[3] = {0.f, 0.f, 0.f}, op = 0.f;
-    const bool accu = conics != nullptr && opacities != nullptr;
-    if(accu)
-        cn[0] = conics[i * 3], cn[1] = conics[i * 3 + 1], cn[2] = conics[i * 3 + 2], op = opacities[i];
-    int64_t cur         = (j == 0) ? 0 : cum_tiles[j - 1];
-    // packed rows carry their image id
-    const IsectKey<KeyT> key(image_ids ? image_ids[i] : (i / N), __float_as_uint(depths[i]), tile_n_bits, (int64_t)tw * th);
-    tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [&](int64_t tile) {
-        isect_ids[cur]   = key(tile);
-        flatten_ids[cur] = (int32_t)i;
-        ++cur;
-    });
-}
-
-// ---- warp-cooperative emit.  One thread per gaussian with a loop over ITS tiles (isect_emit_kernel) leaves a warp
-// waiting for its largest gaussian and writes 8 + 4 byte records at lane-dependent strides: at S = 20 M (large
-// screen-space gaussians) it took 444 us for 240 MB of output.  Here a gaussian with more than kSmallTiles tiles is
-// handed to its whole warp: the tile interval of every tile row is a closed form of the row index (the incremental
-// scheme of tiles_of_gaussian only carries the previous row's far line over as the next row's near line), so lane r
-// computes row ru0 + r, a warp scan places the rows, and the lanes then write the tiles round-robin -- consecutive
-// lanes, consecutive addresses -- in the same order as the sequential enumeration.
-constexpr int kSmallTiles = 64; // measured: below ~2 warps' worth of tiles the per-gaussian warp hand-over costs more than it saves
-
-struct AccuGauss
-{
-    float mx, my, A, Bc, Cc, disc, t, ts;
-    float bminu, bmaxu, bminv, bmaxv, amin_v, amax_v, pu, pv, coeff;
-    int ru0, ru1, rv0, rv1;
-    bool isY, accu, empty;
-    int x0, x1; // AABB path
-};
-
-__device__ __forceinline__ AccuGauss accu_setup(
-    float mx, float my, int rx, int ry, bool accu, float A, float Bc, float Cc, float opacity, uint32_t tile_size,
-    uint32_t tw, uint32_t th
-)
-{
-    AccuGauss g;
-    g.mx = mx, g.my = my, g.A = A, g.Bc = Bc, g.Cc = Cc, g.accu = accu, g.ts = (float)tile_size;
-    g.empty     = rx <= 0 || ry <= 0;
-    g.ru0 = g.ru1 = g.rv0 = g.rv1 = g.x0 = g.x1 = 0;
-    g.isY                                        = false;
-    auto clampi = [](int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); };
-    if(g.empty)
-        return g;
-    const float ts = g.ts;
-    if(accu)
-    {
-        g.disc          = Bc * Bc - A * Cc;
-        float t         = 2.f * exact_log(opacity / kAlphaThreshold);
-        const float cap = kGaussianExtend * kGaussianExtend;
-        g.t             = t < cap ? t : cap;
-        const float ntd = -g.t / g.disc;
-        const float xe = sqrtf(ntd * Cc), ye = sqrtf(ntd * A);
-        const float bminx = mx - xe, bminy = my - ye, bmaxx = mx + xe, bmaxy = my + ye;
-        const float BxC = Bc * xe / Cc, ByA = Bc * ye / A;
-        const float argminx = my + BxC, argminy = mx + ByA, argmaxx = my - BxC, argmaxy = mx - ByA;
-        const int rminx = clampi((int)(bminx / ts), 0, (int)tw), rminy = clampi((int)(bminy / ts), 0, (int)th);
-        const int rmaxx = clampi((int)(bmaxx / ts + 1.f), 0, (int)tw), rmaxy = clampi((int)(bmaxy / ts + 1.f), 0, (int)th);
-        const int ys = rmaxy - rminy, xs = rmaxx - rminx;
-        if(ys * xs == 0)
-        {
-            g.empty = true;
-            return g;
-        }
-        g.isY = ys < xs;
-        g.ru0 = g.isY ? rminy : rminx, g.ru1 = g.isY ? rmaxy : rmaxx, g.rv0 = g.isY ? rminx : rminy, g.rv1 = g.isY ? rmaxx : rmaxy;
-        g.bminu = g.isY ? bminy : bminx, g.bmaxu = g.isY ? bmaxy : bmaxx;
-        g.bminv = g.isY ? bminx : bminy, g.bmaxv = g.isY ? bmaxx : bmaxy;
-        g.amin_v = g.isY ? argminx : argminy, g.amax_v = g.isY ? argmaxx : argmaxy;
-        g.pu = g.isY ? my : mx, g.pv = g.isY ? mx : my, g.coeff = g.isY ? A : Cc;
-    }
-    else
-    {
-        const float trx = (float)rx / ts, try_ = (float)ry / ts, tx = mx / ts, ty = my / ts;
-        g.x0 = clampi((int)floorf(tx - trx), 0, (int)tw), g.ru0 = clampi((int)floorf(ty - try_), 0, (int)th);
-        g.x1 = clampi((int)ceilf(tx + trx), 0, (int)tw), g.ru1 = clampi((int)ceilf(ty + try_), 0, (int)th);
-        g.isY = true; // rows are tile rows
-        if(g.ru1 <= g.ru0 || g.x1 <= g.x0)
-            g.empty = true;
-    }
-    return g;
-}
-
-// tile interval [v0, v1) of row u (ru0 <= u < ru1); identical, bit for bit, to what tiles_of_gaussian enumerates
-__device__ __forceinline__ void accu_row(const AccuGauss &g, int u, int &v0, int &v1)
-{
-    if(!g.accu)
-    {
-        v0 = g.x0, v1 = g.x1;
-        return;
-    }
-    const float ts = g.ts;
-    auto line = [&](float coord, float &lo, float &hi) {
-        const float h  = coord - g.pu;
-        const float sq = sqrtf(g.disc * h * h + g.t * g.coeff);
-        lo             = (-g.Bc * h - sq) / g.coeff + g.pv;
-        hi             = (-g.Bc * h + sq) / g.coeff + g.pv;
-    };
-    const float min_line = (float)u * ts, max_line = min_line + ts;
-    float minlo = g.bmaxv, minhi = g.bminv; // the sequential scheme's initial values
-    if(u > g.ru0 || g.bminu <= min_line)
-        line(min_line, minlo, minhi);
-    float maxlo, maxhi;
-    if(max_line <= g.bmaxu)
-        line(max_line, maxlo, maxhi);
-    else if(u > g.ru0)
-        maxlo = minlo, maxhi = minhi; // the far line was not computed: the previous one is kept
-    else
-        maxlo = g.bmaxv, maxhi = g.bminv;
-    const float emin = (min_line <= g.amin_v && g.amin_v < max_line) ? g.bminv : (minlo < maxlo ? minlo : maxlo);
-    const float emax = (min_line <= g.amax_v && g.amax_v < max_line) ? g.bmaxv : (minhi > maxhi ? minhi : maxhi);
-    const int e0 = (int)(emin / ts), e1 = (int)(emax / ts + 1.f);
-    v0 = e0 < g.rv1 ? e0 : g.rv1;
-    v0 = v0 > g.rv0 ? v0 : g.rv0;
-    v1 = e1 > g.rv0 ? e1 : g.rv0;
-    v1 = v1 < g.rv1 ? v1 : g.rv1;
-    if(v1 < v0)
-        v1 = v0;
-}
-
-template<class KeyT>
-__global__ void __launch_bounds__(kThreads) isect_emit_coop_kernel(
-    int64_t total, int64_t N, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
-    const float *__restrict__ depths, const float *__restrict__ conics, const float *__restrict__ opacities,
-    const int64_t *__restrict__ cum_tiles, const int64_t *__restrict__ image_ids, const int32_t *__restrict__ order,
-    uint32_t tile_size, uint32_t tw, uint32_t th, uint32_t tile_n_bits, KeyT *__restrict__ isect_ids,
-    int32_t *__restrict__ flatten_ids, const int64_t *__restrict__ totals = nullptr, int64_t cap_isects = 0
-)
-{
-    const int64_t j     = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned lane = threadIdx.x & 31;
-    if(totals != nullptr)
-        total = emit_bounded_rows<KeyT>(j, (int64_t)gridDim.x * blockDim.x, total, totals, cap_isects, isect_ids, flatten_ids);
-    const bool active   = j < total && !(totals != nullptr && cum_tiles[j] > cap_isects);
-    const int64_t i     = active ? (order ? (int64_t)order[j] : j) : 0;
-    int2 r              = make_int2(0, 0);
-    float2 m            = make_float2(0.f, 0.f);
-    float cn0 = 0.f, cn1 = 0.f, cn2 = 0.f, op = 0.f;
-    const bool accu = conics != nullptr && opacities != nullptr;
-    int64_t cur = 0, img = 0;
-    uint32_t dbits = 0;
-    int cnt = 0;
-    if(active)
-    {
-        r = reinterpret_cast<const int2 *>(radii)[i];
-        if(r.x > 0 && r.y > 0)
-        {
-            m = reinterpret_cast<const float2 *>(means2d)[i];
-            if(accu)
-                cn0 = conics[i * 3], cn1 = conics[i * 3 + 1], cn2 = conics[i * 3 + 2], op = opacities[i];
-            cur   = (j == 0) ? 0 : cum_tiles[j - 1];
-            cnt   = (int)(cum_tiles[j] - cur);
-            img   = image_ids ? image_ids[i] : (i / N);
-            dbits = __float_as_uint(depths[i]);
-        }
-    }
-    // small gaussians: the owning lane writes its few tiles
-    if(cnt > 0 && cnt <= kSmallTiles)
-    {
-        float cn[3] = {cn0, cn1, cn2};
-        const IsectKey<KeyT> key(img, dbits, tile_n_bits, (int64_t)tw * th);
-        tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [&](int64_t tile) {
-            isect_ids[cur]   = key(tile);
-            flatten_ids[cur] = (int32_t)i;
-            ++cur;
-        });
-    }
-    // large gaussians: one at a time, the whole warp
-    uint32_t big = __ballot_sync(0xffffffffu, cnt > kSmallTiles);
-    while(big)
-    {
-        const int src = __ffs(big) - 1;
-        big &= big - 1;
-        const float bmx = __shfl_sync(0xffffffffu, m.x, src), bmy = __shfl_sync(0xffffffffu, m.y, src);
-        const int brx = __shfl_sync(0xffffffffu, r.x, src), bry = __shfl_sync(0xffffffffu, r.y, src);
-        const float b0 = __shfl_sync(0xffffffffu, cn0, src), b1 = __shfl_sync(0xffffffffu, cn1, src);
-        const float b2 = __shfl_sync(0xffffffffu, cn2, src), bop = __shfl_sync(0xffffffffu, op, src);
-        const int64_t bcur = __shfl_sync(0xffffffffu, cur, src), bimg = __shfl_sync(0xffffffffu, img, src);
-        const uint32_t bdb = __shfl_sync(0xffffffffu, dbits, src);
-        const IsectKey<KeyT> bkey(bimg, bdb, tile_n_bits, (int64_t)tw * th);
-        const int32_t bi  = (int32_t)__shfl_sync(0xffffffffu, i, src);
-        const AccuGauss g = accu_setup(bmx, bmy, brx, bry, accu, b0, b1, b2, bop, tile_size, tw, th);
-        if(g.empty)
-            continue;
-        int64_t base = bcur;
-        for(int u0 = g.ru0; u0 < g.ru1; u0 += 32)
-        {
-            const int u = u0 + (int)lane;
-            int v0 = 0, v1 = 0;
-            if(u < g.ru1)
-                accu_row(g, u, v0, v1);
-            const int len = v1 - v0;
-            int incl      = len;
-#pragma unroll
-            for(int o = 1; o < 32; o <<= 1)
-            {
-                const int up = __shfl_up_sync(0xffffffffu, incl, o);
-                if((int)lane >= o)
-                    incl += up;
-            }
-            const int excl  = incl - len;
-            const int chunk = __shfl_sync(0xffffffffu, incl, 31);
-            // tile k of this 32-row chunk: row = the last row with excl <= k (binary search over the lanes; the loop is
-            // warp-uniform so that every shuffle sees all 32 lanes, only the stores are predicated)
-            for(int k0 = 0; k0 < chunk; k0 += 32)
-            {
-                const int k = k0 + (int)lane;
-                int row     = 0;
-#pragma unroll
-                for(int step = 16; step > 0; step >>= 1)
-                {
-                    const int probe = row + step; // <= 31
-                    const int pe    = __shfl_sync(0xffffffffu, excl, probe);
-                    if(pe <= k)
-                        row = probe;
-                }
-                const int rex = __shfl_sync(0xffffffffu, excl, row);
-                const int rv0 = __shfl_sync(0xffffffffu, v0, row);
-                if(k < chunk)
-                {
-                    const int v        = rv0 + (k - rex);
-                    const int uu       = u0 + row;
-                    const int64_t tile = g.isY ? (int64_t)uu * tw + v : (int64_t)v * tw + uu;
-                    isect_ids[base + k]   = bkey(tile);
-                    flatten_ids[base + k] = bi;
-                }
-            }
-            base += chunk;
-        }
-    }
-}
-
-// offsets[(image, tile)] = first sorted index of that tile's run.  One thread per sorted
-// intersection; a thread that starts a new run also fills the empty tiles before it.
-__global__ void __launch_bounds__(kThreads) isect_offsets_kernel(
-    int64_t n_isects, const int64_t *__restrict__ isect_ids, int64_t total_tiles, int64_t n_tiles, uint32_t tile_n_bits,
-    int32_t *__restrict__ offsets
-)
-{
-    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(s >= n_isects)
-        return;
-    const int64_t mask = ((int64_t)1 << tile_n_bits) - 1;
-    const int64_t hi   = isect_ids[s] >> 32;
-    const int64_t id   = (hi >> tile_n_bits) * n_tiles + (hi & mask);
-    int64_t prev       = -1;
-    if(s > 0)
-    {
-        const int64_t hp = isect_ids[s - 1] >> 32;
-        prev             = (hp >> tile_n_bits) * n_tiles + (hp & mask);
-    }
-    for(int64_t k = prev + 1; k <= id; ++k)
-        offsets[k] = (int32_t)s;
-    if(s == n_isects - 1)
-        for(int64_t k = id + 1; k < total_tiles; ++k)
-            offsets[k] = (int32_t)n_isects;
-}
 // ------------------------------------------------------------------ MCMC strategy ops ("next" row, SURVEY 8f.3)
 // Relocation, Eq. 9 of "3D Gaussian Splatting as Markov Chain Monte Carlo" (reference:
 // csrc/RelocationCUDA.cu:36-80): new opacity 1 - (1 - o)^(1/n) clamped to [min_opacity, 1 - eps]; new scale
@@ -1768,465 +1273,6 @@ extern "C" int gsb200_project_sh_bwd(
     GSB_DEG_SWITCH(degrees_to_use, CALL)
 #undef CALL
 #undef CALL_ARGS
-    return check_launch();
-}
-
-// ---- isect
-extern "C" size_t gsb200_isect_scan_workspace_bytes(int64_t n_elements)
-{
-    size_t bytes = 0;
-    if(n_elements <= 0)
-        return 0;
-    cub::DeviceScan::InclusiveSum((void *)nullptr, bytes, (const int32_t *)nullptr, (int64_t *)nullptr, n_elements);
-    return bytes + 256;
-}
-
-extern "C" int gsb200_isect_count(
-    int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *conics, const float *opacities,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *tiles_per_gauss, int64_t *cum_tiles,
-    void *workspace, size_t workspace_bytes, void *stream
-)
-{
-    if(I < 0 || N < 0 || tile_size == 0)
-        return GSB200_E_INVALID;
-    const int64_t total = I * N;
-    if(total == 0)
-        return GSB200_OK;
-    if(!means2d || !radii || !tiles_per_gauss || !cum_tiles || !workspace || total > 0x7fffffffLL)
-        return GSB200_E_INVALID;
-    if(bits_for_count(I) + bits_for_count((int64_t)tile_width * tile_height) > 32)
-        return GSB200_E_KEYBITS;
-    cudaStream_t st = (cudaStream_t)stream;
-    size_t need     = 0;
-    cub::DeviceScan::InclusiveSum((void *)nullptr, need, tiles_per_gauss, cum_tiles, total, st);
-    if(need > workspace_bytes)
-        return GSB200_E_WORKSPACE;
-    isect_count_kernel<<<grid_for(total, kThreads), kThreads, 0, st>>>(
-        total, means2d, radii, conics, opacities, tile_size, tile_width, tile_height, tiles_per_gauss
-    );
-    if(int rc = check_launch())
-        return rc;
-    GSB_CUDA_TRY(cub::DeviceScan::InclusiveSum(workspace, need, tiles_per_gauss, cum_tiles, total, st));
-    return GSB200_OK;
-}
-
-extern "C" int gsb200_isect_emit(
-    int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const float *conics,
-    const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, uint32_t tile_size, uint32_t tile_width,
-    uint32_t tile_height, int64_t *isect_ids, int32_t *flatten_ids, void *stream
-)
-{
-    if(I < 0 || N < 0 || tile_size == 0)
-        return GSB200_E_INVALID;
-    // packed layout: N rows in total (image_ids given), I only sizes the key; dense: I * N rows
-    const int64_t total = image_ids ? N : I * N;
-    if(total == 0)
-        return GSB200_OK;
-    if(!means2d || !radii || !depths || !cum_tiles || !isect_ids || !flatten_ids)
-        return GSB200_E_INVALID;
-    const uint32_t tile_bits = bits_for_count((int64_t)tile_width * tile_height);
-    if(bits_for_count(I) + tile_bits > 32)
-        return GSB200_E_KEYBITS;
-    isect_emit_coop_kernel<int64_t><<<grid_for(total, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
-        total, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, nullptr, tile_size, tile_width, tile_height,
-        tile_bits, isect_ids, flatten_ids
-    );
-    return check_launch();
-}
-
-// ---- tile intersection restricted to the tiles of a mask (isect_tiles_sparse).  Same enumeration as the dense AABB
-// path (tiles_of_gaussian without conics), in the depth order of gsb::depth_order (sort.cu); a tile whose tile_mask entry
-// is 0 is neither counted nor emitted.  Keys are dense tile ids image * th * tw + tile (32 bits).
-namespace gsb
-{
-__device__ __forceinline__ int64_t masked_row_image(int64_t i, int64_t N, const int64_t *__restrict__ image_ids)
-{
-    return image_ids ? image_ids[i] : i / N;
-}
-
-__global__ void __launch_bounds__(kThreads) isect_count_masked_kernel(
-    int64_t total, int64_t N, int64_t I, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
-    const int64_t *__restrict__ image_ids, const uint8_t *__restrict__ tile_mask, const int32_t *__restrict__ order,
-    uint32_t tile_size, uint32_t tw, uint32_t th, int32_t *__restrict__ counts_in_order
-)
-{
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(j >= total)
-        return;
-    const int64_t i = order[j];
-    const int2 r    = reinterpret_cast<const int2 *>(radii)[i];
-    int cnt         = 0;
-    const int64_t img = masked_row_image(i, N, image_ids);
-    if(r.x > 0 && r.y > 0 && img >= 0 && img < I)
-    {
-        const float2 m     = reinterpret_cast<const float2 *>(means2d)[i];
-        const uint8_t *tm  = tile_mask + img * (int64_t)tw * th;
-        tiles_of_gaussian(m.x, m.y, r.x, r.y, nullptr, nullptr, tile_size, tw, th, [&](int64_t t) { cnt += tm[t] != 0; });
-    }
-    counts_in_order[j] = cnt;
-}
-
-__global__ void __launch_bounds__(kThreads) isect_emit_masked_kernel(
-    int64_t total, int64_t N, int64_t I, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
-    const int64_t *__restrict__ image_ids, const uint8_t *__restrict__ tile_mask, const int32_t *__restrict__ order,
-    const int64_t *__restrict__ cum_tiles, uint32_t tile_size, uint32_t tw, uint32_t th, uint32_t *__restrict__ keys,
-    int32_t *__restrict__ flatten_ids
-)
-{
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(j >= total)
-        return;
-    int64_t cur       = j == 0 ? 0 : cum_tiles[j - 1];
-    const int64_t end = cum_tiles[j];
-    if(end == cur)
-        return;
-    const int64_t i   = order[j];
-    const int2 r      = reinterpret_cast<const int2 *>(radii)[i];
-    const float2 m    = reinterpret_cast<const float2 *>(means2d)[i];
-    const int64_t img = masked_row_image(i, N, image_ids);
-    const uint8_t *tm = tile_mask + img * (int64_t)tw * th;
-    const uint32_t base = (uint32_t)(img * (int64_t)tw * th);
-    tiles_of_gaussian(m.x, m.y, r.x, r.y, nullptr, nullptr, tile_size, tw, th, [&](int64_t t) {
-        if(tm[t] != 0 && cur < end)
-        {
-            keys[cur]        = base + (uint32_t)t;
-            flatten_ids[cur] = (int32_t)i;
-            ++cur;
-        }
-    });
-}
-
-// tile_offsets[a] = first sorted intersection of active tile a (lower bound of its id in the sorted keys), a < AT;
-// tile_offsets[AT] = n_isects
-__global__ void __launch_bounds__(kThreads) isect_offsets_sparse_kernel(
-    int64_t n_active, const int32_t *__restrict__ active_tiles, int64_t n_isects, const uint32_t *__restrict__ keys,
-    int32_t *__restrict__ tile_offsets
-)
-{
-    const int64_t a = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(a > n_active)
-        return;
-    if(a == n_active)
-    {
-        tile_offsets[a] = (int32_t)n_isects;
-        return;
-    }
-    const uint32_t t = (uint32_t)active_tiles[a];
-    int64_t lo = 0, hi = n_isects;
-    while(lo < hi)
-    {
-        const int64_t mid = (lo + hi) >> 1;
-        if(keys[mid] < t)
-            lo = mid + 1;
-        else
-            hi = mid;
-    }
-    tile_offsets[a] = (int32_t)lo;
-}
-
-struct SparseCountLayout
-{
-    size_t depth, counts, scan, total;
-};
-static SparseCountLayout sparse_count_layout(int64_t I, int64_t total)
-{
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    SparseCountLayout L;
-    size_t scan = 0;
-    cub::DeviceScan::InclusiveSum((void *)nullptr, scan, (const int32_t *)nullptr, (int64_t *)nullptr, total);
-    L.depth  = 0;
-    L.counts = L.depth + al(depth_order_workspace_bytes(I, total));
-    L.scan   = L.counts + al(sizeof(int32_t) * (size_t)total);
-    L.total  = L.scan + al(scan) + 256;
-    return L;
-}
-
-struct SparseEmitLayout
-{
-    size_t keys_in, vals_in, keys_out, sort, total;
-};
-static SparseEmitLayout sparse_emit_layout(int64_t n_isects, int end_bit)
-{
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    SparseEmitLayout L;
-    L.keys_in  = 0;
-    L.vals_in  = L.keys_in + al(sizeof(uint32_t) * (size_t)n_isects);
-    L.keys_out = L.vals_in + al(sizeof(int32_t) * (size_t)n_isects);
-    L.sort     = L.keys_out + al(sizeof(uint32_t) * (size_t)n_isects);
-    L.total    = L.sort + al(gsb200_sort_tile_pairs_workspace_bytes(n_isects, 4, end_bit)) + 256;
-    return L;
-}
-
-static int sparse_isect_args(int64_t I, int64_t N, const int64_t *image_ids, uint32_t tile_size, uint32_t tw, uint32_t th, int64_t &total)
-{
-    if(I < 0 || N < 0 || tile_size == 0)
-        return GSB200_E_INVALID;
-    total = image_ids ? N : I * N; // packed: N rows, image_ids[i] in [0, I)
-    if(total > 0x7fffffffLL)
-        return GSB200_E_INVALID;
-    if(bits_for_count(I) + bits_for_count((int64_t)tw * th) > 32)
-        return GSB200_E_KEYBITS;
-    return GSB200_OK;
-}
-} // namespace gsb
-
-extern "C" size_t gsb200_isect_sparse_count_workspace_bytes(int64_t I, int64_t total_rows)
-{
-    if(I <= 0 || total_rows <= 0)
-        return 0;
-    return gsb::sparse_count_layout(I, total_rows).total;
-}
-
-extern "C" int gsb200_isect_sparse_count(
-    int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const int64_t *image_ids,
-    const uint8_t *tile_mask, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *order,
-    int64_t *cum_tiles, void *workspace, size_t workspace_bytes, void *stream
-)
-{
-    int64_t total = 0;
-    if(int rc = gsb::sparse_isect_args(I, N, image_ids, tile_size, tile_width, tile_height, total))
-        return rc;
-    if(total == 0)
-        return GSB200_OK;
-    if(!means2d || !radii || !depths || !tile_mask || !order || !cum_tiles || !workspace)
-        return GSB200_E_INVALID;
-    const auto L = gsb::sparse_count_layout(I, total);
-    if(L.total > workspace_bytes)
-        return GSB200_E_WORKSPACE;
-    char *ws        = static_cast<char *>(workspace);
-    cudaStream_t st = (cudaStream_t)stream;
-    // 1. rows in (image, depth) order
-    if(int rc = gsb::depth_order(I, N, radii, depths, image_ids, order, ws + L.depth, L.counts - L.depth, st))
-        return rc;
-    // 2. masked tile counts in that order; 3. inclusive scan
-    int32_t *counts = reinterpret_cast<int32_t *>(ws + L.counts);
-    gsb::isect_count_masked_kernel<<<gsb::grid_for(total, gsb::kThreads), gsb::kThreads, 0, st>>>(
-        total, N, I, means2d, radii, image_ids, tile_mask, order, tile_size, tile_width, tile_height, counts
-    );
-    if(int rc = gsb::check_launch())
-        return rc;
-    size_t scan_bytes = L.total - L.scan;
-    GSB_CUDA_TRY(cub::DeviceScan::InclusiveSum(ws + L.scan, scan_bytes, counts, cum_tiles, total, st));
-    return GSB200_OK;
-}
-
-extern "C" size_t gsb200_isect_sparse_emit_workspace_bytes(int64_t I, int64_t n_isects, uint32_t tile_width, uint32_t tile_height)
-{
-    if(I <= 0 || n_isects <= 0)
-        return 0;
-    const int end_bit = (int)gsb::bits_for_count(I * (int64_t)tile_width * tile_height);
-    return gsb::sparse_emit_layout(n_isects, end_bit > 0 ? end_bit : 1).total;
-}
-
-extern "C" int gsb200_isect_sparse_emit(
-    int64_t I, int64_t N, const float *means2d, const int32_t *radii, const int64_t *image_ids, const uint8_t *tile_mask,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *order, const int64_t *cum_tiles,
-    int64_t n_isects, int64_t n_active, const int32_t *active_tiles, int32_t *tile_offsets, int32_t *flatten_ids,
-    void *workspace, size_t workspace_bytes, void *stream
-)
-{
-    int64_t total = 0;
-    if(int rc = gsb::sparse_isect_args(I, N, image_ids, tile_size, tile_width, tile_height, total))
-        return rc;
-    if(n_isects < 0 || n_isects > 0x7fffffffLL || n_active < 0 || !tile_offsets || (n_active > 0 && !active_tiles))
-        return GSB200_E_INVALID;
-    cudaStream_t st = (cudaStream_t)stream;
-    const uint32_t *sorted = nullptr;
-    if(n_isects > 0)
-    {
-        if(total == 0 || !means2d || !radii || !tile_mask || !order || !cum_tiles || !flatten_ids || !workspace)
-            return GSB200_E_INVALID;
-        int end_bit  = (int)gsb::bits_for_count(I * (int64_t)tile_width * tile_height);
-        end_bit      = end_bit > 0 ? end_bit : 1;
-        const auto L = gsb::sparse_emit_layout(n_isects, end_bit);
-        if(L.total > workspace_bytes)
-            return GSB200_E_WORKSPACE;
-        char *ws          = static_cast<char *>(workspace);
-        uint32_t *keys_in = reinterpret_cast<uint32_t *>(ws + L.keys_in), *keys_out = reinterpret_cast<uint32_t *>(ws + L.keys_out);
-        int32_t *vals_in  = reinterpret_cast<int32_t *>(ws + L.vals_in);
-        // 4. emission in depth order; 5. stable sort on the (image, tile) bits
-        gsb::isect_emit_masked_kernel<<<gsb::grid_for(total, gsb::kThreads), gsb::kThreads, 0, st>>>(
-            total, N, I, means2d, radii, image_ids, tile_mask, order, cum_tiles, tile_size, tile_width, tile_height, keys_in, vals_in
-        );
-        if(int rc = gsb::check_launch())
-            return rc;
-        if(int rc = gsb200_sort_tile_pairs(n_isects, 4, end_bit, keys_in, vals_in, keys_out, flatten_ids, ws + L.sort, L.total - L.sort, stream))
-            return rc;
-        sorted = keys_out;
-    }
-    // 6. per-active-tile offsets from the sorted keys
-    gsb::isect_offsets_sparse_kernel<<<gsb::grid_for(n_active + 1, gsb::kThreads), gsb::kThreads, 0, st>>>(
-        n_active, active_tiles, n_isects, sorted, tile_offsets
-    );
-    return gsb::check_launch();
-}
-
-extern "C" int gsb200_isect_count_totals(
-    int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *conics, const float *opacities,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *tiles_per_gauss, int64_t *totals, void *stream
-)
-{
-    if(I < 0 || N < 0 || tile_size == 0 || !totals)
-        return GSB200_E_INVALID;
-    cudaStream_t st = (cudaStream_t)stream;
-    GSB_CUDA_TRY(cudaMemsetAsync(totals, 0, 3 * sizeof(int64_t), st));
-    const int64_t total = I * N;
-    if(total == 0)
-        return GSB200_OK;
-    if(!means2d || !radii || !tiles_per_gauss || total > 0x7fffffffLL)
-        return GSB200_E_INVALID;
-    if(bits_for_count(I) + bits_for_count((int64_t)tile_width * tile_height) > 32)
-        return GSB200_E_KEYBITS;
-    isect_count_totals_kernel<<<grid_for(total, kThreads), kThreads, 0, st>>>(
-        total, means2d, radii, conics, opacities, tile_size, tile_width, tile_height, tiles_per_gauss,
-        reinterpret_cast<unsigned long long *>(totals)
-    );
-    return check_launch();
-}
-
-namespace gsb
-{
-// stage of gsb200_isect_sorted (sort.cu), which checked the arguments: emission of the cap_vis depth-ordered row slots
-// into capacity-sized outputs, real counts in `totals` (device)
-int emit_tilekeys_bounded(
-    int64_t N, int64_t cap_vis, int64_t max_tiles_hint, const float *means2d, const int32_t *radii, const float *depths,
-    const float *conics, const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, const int32_t *order,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int key_bytes, void *keys, int32_t *flatten_ids,
-    const int64_t *totals, int64_t cap_isects, cudaStream_t st
-)
-{
-    const uint32_t tile_bits = bits_for_count((int64_t)tile_width * tile_height);
-    // the cooperative kernel pays off when SOME gaussian covers many tiles (one lane looping over thousands of tiles is the
-    // tail of the whole launch); when even the largest row has few, the plain one-thread-per-gaussian kernel is leaner
-    // (38 vs 45 us at cfg3)
-    const bool serial = max_tiles_hint > 0 && max_tiles_hint <= 96;
-    auto launch = [&](auto *k) {
-        using KeyT = std::remove_pointer_t<decltype(k)>;
-        if(serial)
-            isect_emit_kernel<KeyT><<<grid_for(cap_vis, kThreads), kThreads, 0, st>>>(
-                cap_vis, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width,
-                tile_height, tile_bits, k, flatten_ids, totals, cap_isects
-            );
-        else
-            isect_emit_coop_kernel<KeyT><<<grid_for(cap_vis, kThreads), kThreads, 0, st>>>(
-                cap_vis, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width,
-                tile_height, tile_bits, k, flatten_ids, totals, cap_isects
-            );
-    };
-    if(key_bytes == 2)
-        launch(static_cast<uint16_t *>(keys));
-    else
-        launch(static_cast<uint32_t *>(keys));
-    return check_launch();
-}
-
-// offsets[(image, tile)] from sorted dense tile ids (narrow keys): same contract as isect_offsets_kernel
-template<class KeyT>
-__global__ void __launch_bounds__(kThreads) isect_offsets_tilekeys_kernel(
-    int64_t n_isects, const KeyT *__restrict__ keys, int64_t total_tiles, int32_t *__restrict__ offsets,
-    const int64_t *__restrict__ totals = nullptr
-)
-{
-    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(totals != nullptr && totals[0] < n_isects)
-        n_isects = totals[0]; // capacity-sized launch: the pairs past the real count are padding
-    if(s >= n_isects)
-        return;
-    // Real keys are < total_tiles.  After a capacity miss (gsb200_isect_sorted with a count above its capacity) some
-    // slots hold uninitialised pairs: the result is discarded by the caller, but no write may leave the array.
-    int64_t id         = (int64_t)keys[s];
-    const int64_t prev = s > 0 ? (int64_t)keys[s - 1] : -1;
-    id                 = id < total_tiles ? id : total_tiles - 1;
-    for(int64_t k = prev + 1; k <= id; ++k)
-        offsets[k] = (int32_t)s;
-    if(s == n_isects - 1)
-        for(int64_t k = id + 1; k < total_tiles; ++k)
-            offsets[k] = (int32_t)n_isects;
-}
-
-int offsets_tilekeys_bounded(
-    int64_t cap_isects, int key_bytes, const void *keys, int64_t total_tiles, int32_t *offsets, const int64_t *totals, cudaStream_t st
-)
-{
-    // no thread writes anything when the real count is 0: start from zeros
-    GSB_CUDA_TRY(cudaMemsetAsync(offsets, 0, sizeof(int32_t) * (size_t)total_tiles, st));
-    if(cap_isects == 0)
-        return GSB200_OK;
-    if(key_bytes == 2)
-        isect_offsets_tilekeys_kernel<uint16_t><<<grid_for(cap_isects, kThreads), kThreads, 0, st>>>(
-            cap_isects, static_cast<const uint16_t *>(keys), total_tiles, offsets, totals
-        );
-    else
-        isect_offsets_tilekeys_kernel<uint32_t><<<grid_for(cap_isects, kThreads), kThreads, 0, st>>>(
-            cap_isects, static_cast<const uint32_t *>(keys), total_tiles, offsets, totals
-        );
-    return check_launch();
-}
-
-// the reference's 64-bit intersection ids, rebuilt from the sorted tile ids and the rows' depths
-template<class KeyT>
-__global__ void __launch_bounds__(kThreads) isect_ids_from_tilekeys_kernel(
-    int64_t n_isects, const KeyT *__restrict__ keys, const int32_t *__restrict__ flatten_ids, const float *__restrict__ depths,
-    int64_t n_tiles, uint32_t tile_n_bits, int64_t *__restrict__ isect_ids
-)
-{
-    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(s >= n_isects)
-        return;
-    const int64_t id = (int64_t)keys[s];
-    const int64_t image = id / n_tiles, tile = id - image * n_tiles;
-    isect_ids[s] = (((image << tile_n_bits) | tile) << 32) | (int64_t)__float_as_uint(depths[flatten_ids[s]]);
-}
-} // namespace gsb
-
-extern "C" int gsb200_isect_ids_from_tilekeys(
-    int64_t n_isects, int key_bytes, const void *tile_keys, const int32_t *flatten_ids, const float *depths, int64_t I,
-    uint32_t tile_width, uint32_t tile_height, int64_t *isect_ids, void *stream
-)
-{
-    if(n_isects < 0 || I < 0 || (key_bytes != 2 && key_bytes != 4))
-        return GSB200_E_INVALID;
-    if(n_isects == 0)
-        return GSB200_OK;
-    if(!tile_keys || !flatten_ids || !depths || !isect_ids)
-        return GSB200_E_INVALID;
-    const int64_t n_tiles = (int64_t)tile_width * tile_height;
-    cudaStream_t st       = (cudaStream_t)stream;
-    if(key_bytes == 2)
-        isect_ids_from_tilekeys_kernel<uint16_t><<<grid_for(n_isects, kThreads), kThreads, 0, st>>>(
-            n_isects, static_cast<const uint16_t *>(tile_keys), flatten_ids, depths, n_tiles, bits_for_count(n_tiles), isect_ids
-        );
-    else
-        isect_ids_from_tilekeys_kernel<uint32_t><<<grid_for(n_isects, kThreads), kThreads, 0, st>>>(
-            n_isects, static_cast<const uint32_t *>(tile_keys), flatten_ids, depths, n_tiles, bits_for_count(n_tiles), isect_ids
-        );
-    return check_launch();
-}
-
-extern "C" int gsb200_isect_offsets(
-    int64_t n_isects, const int64_t *isect_ids, int64_t I, uint32_t tile_width, uint32_t tile_height, int32_t *offsets,
-    void *stream
-)
-{
-    if(n_isects < 0 || I < 0)
-        return GSB200_E_INVALID;
-    const int64_t n_tiles = (int64_t)tile_width * tile_height;
-    const int64_t total   = I * n_tiles;
-    if(total == 0)
-        return GSB200_OK;
-    if(!offsets)
-        return GSB200_E_INVALID;
-    cudaStream_t st = (cudaStream_t)stream;
-    if(n_isects == 0)
-    {
-        GSB_CUDA_TRY(cudaMemsetAsync(offsets, 0, sizeof(int32_t) * (size_t)total, st));
-        return GSB200_OK;
-    }
-    if(!isect_ids)
-        return GSB200_E_INVALID;
-    isect_offsets_kernel<<<grid_for(n_isects, kThreads), kThreads, 0, st>>>(
-        n_isects, isect_ids, total, n_tiles, bits_for_count(n_tiles), offsets
-    );
     return check_launch();
 }
 

@@ -686,6 +686,34 @@ def _scratch_buffer(dev: torch.device, tag: str, nbytes: int) -> Tensor:
     return buf
 
 
+def _isect_rows(means2d, radii, depths, conics, opacities, tile_width, tile_height, n_images, image_ids):
+    """The projected rows as the intersection entry points take them: contiguous float32 / int32 tensors, the int64 image
+    id of each packed row (``image_ids`` given: [nnz, 2] means2d over ``n_images`` images) or None (dense
+    [..., N, 2]), and (image_dims, I, N, I_count, total, packed): I images of N rows, ``total`` = I_count * N rows for
+    the count, which sees packed rows as one flat list."""
+    means2d, depths = f32c(means2d, "means2d"), f32c(depths, "depths")
+    conics, opacities = f32c(conics, "conics"), f32c(opacities, "opacities")
+    if radii.dtype != torch.int32:
+        raise TypeError("radii must be int32")
+    radii = radii.contiguous()
+    packed = image_ids is not None
+    if packed:
+        image_dims, I, N, I_count = (), int(n_images), means2d.shape[0], 1
+        image_ids = image_ids.to(torch.int64).contiguous()
+    else:
+        image_dims = tuple(means2d.shape[:-2])
+        I, N = _prod(image_dims), means2d.shape[-2]
+        I_count = I
+    n_tiles = tile_width * tile_height
+    image_bits, tile_bits = _cabi.bits_for_count(I), _cabi.bits_for_count(n_tiles)
+    if image_bits + tile_bits > 32:
+        raise RuntimeError(
+            f"intersect_tile: (image, tile) id packing needs {image_bits + tile_bits} bits but only 32 are "
+            f"available (I={I}, n_tiles={n_tiles})."
+        )
+    return means2d, radii, depths, conics, opacities, image_ids, (image_dims, I, N, I_count, I_count * N, packed)
+
+
 @torch.no_grad()
 def isect_tiles(
     means2d: Tensor,  # [..., N, 2]
@@ -707,11 +735,6 @@ def isect_tiles(
     conservative ellipse test (AccuTile / SNUGBOX) is used, otherwise the radius AABB.
     Returns (tiles_per_gauss int32 [..., N], isect_ids int64 [n_isects], flatten_ids int32 [n_isects])."""
     dev = require_cuda(means2d, radii, depths)
-    means2d, depths = f32c(means2d, "means2d"), f32c(depths, "depths")
-    conics, opacities = f32c(conics, "conics"), f32c(opacities, "opacities")
-    if radii.dtype != torch.int32:
-        raise TypeError("radii must be int32")
-    radii = radii.contiguous()
     if packed:
         if n_images is None or image_ids is None:
             raise ValueError("n_images and image_ids are required when means2d is packed ([nnz, 2]).")
@@ -719,22 +742,10 @@ def isect_tiles(
             raise ValueError("segmented sort is not supported for packed inputs")
         if means2d.dim() != 2:
             raise ValueError(f"packed means2d must be [nnz, 2], got {tuple(means2d.shape)}")
-        image_dims, I, N = (), int(n_images), means2d.shape[0]
-        img_ids = image_ids.to(torch.int64).contiguous()
-        I_count = 1  # pass 1 sees one flat list of nnz rows
-    else:
-        image_dims = tuple(means2d.shape[:-2])
-        I, N = _prod(image_dims), means2d.shape[-2]
-        img_ids, I_count = None, I
+    means2d, radii, depths, conics, opacities, img_ids, (image_dims, I, N, I_count, total, _) = _isect_rows(
+        means2d, radii, depths, conics, opacities, tile_width, tile_height, n_images, image_ids if packed else None
+    )
     L = lib()
-    n_tiles = tile_width * tile_height
-    image_bits, tile_bits = _cabi.bits_for_count(I), _cabi.bits_for_count(n_tiles)
-    if image_bits + tile_bits > 32:
-        raise RuntimeError(
-            f"intersect_tile: (image, tile) id packing needs {image_bits + tile_bits} bits but only 32 are "
-            f"available (I={I}, n_tiles={n_tiles})."
-        )
-    total = I_count * N
     tiles_per_gauss = torch.empty(image_dims + (N,), device=dev, dtype=torch.int32)
     if total == 0:
         return (tiles_per_gauss, torch.empty(0, device=dev, dtype=torch.int64), torch.empty(0, device=dev, dtype=torch.int32))
@@ -884,31 +895,13 @@ def isect_tiles_sorted(
     earlier calls of the same shape.  ``_exact`` (isect_tiles) reads the totals first and sizes the stage exactly, and
     leaves that history alone: the call's own largest row then picks the emit kernel."""
     dev = require_cuda(means2d, radii, depths)
-    means2d, depths = f32c(means2d, "means2d"), f32c(depths, "depths")
-    conics, opacities = f32c(conics, "conics"), f32c(opacities, "opacities")
-    if radii.dtype != torch.int32:
-        raise TypeError("radii must be int32")
-    radii = radii.contiguous()
-    packed = image_ids is not None
-    if packed:
-        image_dims, I, N = (), int(n_images), means2d.shape[0]
-        image_ids = image_ids.to(torch.int64).contiguous()
-    else:
-        image_dims = tuple(means2d.shape[:-2])
-        I, N = _prod(image_dims), means2d.shape[-2]
+    means2d, radii, depths, conics, opacities, image_ids, (image_dims, I, N, I_count, total, packed) = _isect_rows(
+        means2d, radii, depths, conics, opacities, tile_width, tile_height, n_images, image_ids
+    )
     L = lib()
-    n_tiles = tile_width * tile_height
-    image_bits, tile_bits = _cabi.bits_for_count(I), _cabi.bits_for_count(n_tiles)
-    if image_bits + tile_bits > 32:
-        raise RuntimeError(
-            f"intersect_tile: (image, tile) id packing needs {image_bits + tile_bits} bits but only 32 are "
-            f"available (I={I}, n_tiles={n_tiles})."
-        )
-    key_bits = _cabi.bits_for_count(I * n_tiles)
+    key_bits = _cabi.bits_for_count(I * tile_width * tile_height)
     key_bytes = 2 if key_bits <= 16 else 4
     key_dtype = torch.int16 if key_bytes == 2 else torch.int32  # raw storage; the kernels read them unsigned
-    I_count = 1 if packed else I  # the count sees packed rows as one flat list of N rows
-    total = I_count * N
     have_counts = (
         not packed and precounted is not None and precounted.totals is not None and total > 0
         and (precounted.tile_size, precounted.tile_width, precounted.tile_height) == (tile_size, tile_width, tile_height)

@@ -219,14 +219,9 @@ extern "C"
     );
     /* Narrow keys (round 2): the rows are emitted in depth order, so the S-sized sort only needs the dense tile id
      * image * n_tiles + tile, as a key_bytes-wide (2 when I * n_tiles <= 65536, else 4) unsigned integer.
-     * gsb200_sort_tile_pairs sorts (tile id, value) pairs stably on key bits [0, end_bit).  gsb200_isect_ids_from_tilekeys
-     * rebuilds the reference's sorted int64 isect_ids ((image << tile_bits | tile) << 32 | depth bits; depths is indexed
-     * by flatten_ids) from the sorted tile ids of gsb200_isect_sorted, for callers that ask for them. */
-    size_t gsb200_sort_tile_pairs_workspace_bytes(int64_t n_isects, int key_bytes, int end_bit);
-    int gsb200_sort_tile_pairs(
-        int64_t n_isects, int key_bytes, int end_bit, const void *keys_in, const int32_t *vals_in, void *keys_out,
-        int32_t *vals_out, void *workspace, size_t workspace_bytes, void *stream
-    );
+     * gsb200_isect_ids_from_tilekeys rebuilds the reference's sorted int64 isect_ids ((image << tile_bits | tile) << 32 |
+     * depth bits; depths is indexed by flatten_ids) from the sorted tile ids of gsb200_isect_sorted, for callers that ask
+     * for them. */
     int gsb200_isect_ids_from_tilekeys(
         int64_t n_isects, int key_bytes, const void *tile_keys, const int32_t *flatten_ids, const float *depths, int64_t I,
         uint32_t tile_width, uint32_t tile_height, int64_t *isect_ids, void *stream

@@ -54,7 +54,7 @@ def test_isect_capacity_prediction():
 
 
 def test_capacity_padding_model():
-    """numpy model of the capacity-sized intersection stage (sort.cu: gsb200_isect_sorted): padding pairs carry the largest
+    """numpy model of the capacity-sized intersection stage (isect.cu: gsb200_isect_sorted): padding pairs carry the largest
     key and sit behind the real pairs, the stable sort only looks at the low `end_bit` bits, and the offsets kernel reads the
     first totals[0] sorted keys -- the result must equal the exact pipeline's, also when the number of (image, tile) cells is a
     power of two (the padding key then aliases the last real cell) and when a miss leaves garbage keys in the list."""

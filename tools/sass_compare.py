@@ -1,14 +1,17 @@
 """Checks that a change leaves the existing kernels' machine code alone.
 
-    python tools/sass_compare.py [--base REV] [--units raster.cu sort.cu pergauss.cu]
+    python tools/sass_compare.py [--base REV] [--units raster.cu isect.cu ...]
 
-Compiles each unit twice for sm_90a with the flags of gsplat_b200/build.py -- once from the sources at git revision
-``--base`` (default HEAD), once from the working tree -- disassembles both objects with ``cuobjdump -sass`` and compares
-every kernel of the base object with the kernel of the same name in the new one.  Names are compared demangled, with
-the pixel-addressing policy of the compositing kernels (``gsb::DensePixels``) removed, so that a kernel that only gained
-that template argument is matched with its old self.  Instructions and their encodings must be identical;
-address and line-info comments are ignored.  Kernels that only the new object has are listed as new.  Exit status 1
-on any difference.  Needs nvcc / cuobjdump / cu++filt (no GPU).
+Compiles the units (default: every unit of gsplat_b200/build.py) for sm_90a with the flags of build.py -- those that
+exist at git revision ``--base`` (default HEAD) from the sources at that revision, all of them from the working tree --
+disassembles the objects with ``cuobjdump -sass`` and compares every kernel of the base objects with the kernel of the
+same name in the new ones, whichever unit it is compiled in: a kernel that moved to another file is matched with its
+old self.  Names are compared demangled, with the pixel-addressing policy of the compositing kernels
+(``gsb::DensePixels``) removed, so that a kernel that only gained that template argument is matched with its old self,
+and with ``isect_count_kernel<true / false>`` under the names the two count kernels had before they became one template.
+Instructions and their encodings must be identical; address and line-info comments are ignored.  A library kernel
+(CUB) that several units instantiate must be identical in all of them.  Kernels that only the new objects have are
+listed as new.  Exit status 1 on any difference.  Needs nvcc / cuobjdump / cu++filt (no GPU).
 """
 from __future__ import annotations
 
@@ -27,6 +30,8 @@ from gsplat_b200 import build as B  # noqa: E402
 CUDA_BIN = os.path.dirname(B._nvcc()) if os.path.isabs(B._nvcc()) else "/usr/local/cuda/bin"
 # cu++filt prints the policy parameter of a kernel as `T<k>`: dropped together with the policy template argument
 POLICY_PARAM = re.compile(r",\s*T\d+\)$")
+# isect_count_kernel<TOTALS>: <true> was isect_count_totals_kernel, <false> isect_count_kernel without the totals pointer
+COUNT_KERNEL = re.compile(r"^void gsb::isect_count_kernel<\(bool\)([01])>\((.*), unsigned long long \*\)$")
 
 
 def _tree_at(rev: str, dst: str) -> None:
@@ -72,38 +77,49 @@ def kernels(obj: str):
     for n, d in zip(names, _demangle(names)):
         if "DensePixels" in n or "SparsePixels" in n:
             d = POLICY_PARAM.sub(")", d).replace(", gsb::DensePixels>", ">")
+        m = COUNT_KERNEL.match(d)
+        if m:
+            d = f"gsb::isect_count_totals_kernel({m.group(2)}, unsigned long long *)" if m.group(1) == "1" else f"gsb::isect_count_kernel({m.group(2)})"
         out[d] = raw[n]
+    return out
+
+
+def kernels_of(src_root: str, units, tmp: str, tag: str):
+    """{name: {instruction lines of every unit that has the kernel}} over the units present under src_root"""
+    out = {}
+    for unit in units:
+        if not os.path.exists(os.path.join(src_root, "gsplat_b200", "csrc", unit)):
+            continue
+        obj = os.path.join(tmp, f"{tag}_{unit}.o")
+        _compile(src_root, unit, obj)
+        for name, body in kernels(obj).items():
+            out.setdefault(name, set()).add(tuple(body))
     return out
 
 
 def main() -> int:
     ap = argparse.ArgumentParser()
     ap.add_argument("--base", default="HEAD")
-    ap.add_argument("--units", nargs="+", default=["raster.cu", "sort.cu", "pergauss.cu"])
+    ap.add_argument("--units", nargs="+", default=list(B.UNITS))
     args = ap.parse_args()
-    bad = 0
     with tempfile.TemporaryDirectory() as tmp:
         base_root = os.path.join(tmp, "base")
         _tree_at(args.base, base_root)
-        for unit in args.units:
-            o_base, o_new = os.path.join(tmp, "base_" + unit + ".o"), os.path.join(tmp, "new_" + unit + ".o")
-            _compile(base_root, unit, o_base)
-            _compile(ROOT, unit, o_new)
-            kb, kn = kernels(o_base), kernels(o_new)
-            same = [k for k in kb if k in kn and kb[k] == kn[k]]
-            missing = [k for k in kb if k not in kn]
-            changed = [k for k in kb if k in kn and kb[k] != kn[k]]
-            new = [k for k in kn if k not in kb]
-            n_instr = sum(len(kb[k]) for k in same)
-            print(f"{unit}: {len(kb)} kernels at {args.base}: {len(same)} identical ({n_instr} instructions), "
-                  f"{len(changed)} changed, {len(missing)} missing; {len(new)} new")
-            for k in changed:
-                print(f"  CHANGED {k} ({len(kb[k])} -> {len(kn[k])} instructions)")
-            for k in missing:
-                print(f"  MISSING {k}")
-            for k in new:
-                print(f"  new     {k}")
-            bad += len(changed) + len(missing)
+        kb, kn = kernels_of(base_root, args.units, tmp, "base"), kernels_of(ROOT, args.units, tmp, "new")
+    same = [k for k in kb if k in kn and kb[k] == kn[k]]
+    missing = [k for k in kb if k not in kn]
+    changed = [k for k in kb if k in kn and kb[k] != kn[k]]
+    new = [k for k in kn if k not in kb]
+    n_instr = sum(len(body) for k in same for body in kb[k])
+    print(f"{' '.join(args.units)}: {len(kb)} kernels at {args.base}: {len(same)} identical ({n_instr} instructions), "
+          f"{len(changed)} changed, {len(missing)} missing; {len(new)} new")
+    for k in changed:
+        print(f"  CHANGED {k} ({sorted(len(b) for b in kb[k])} -> {sorted(len(b) for b in kn[k])} instructions)")
+    for k in missing:
+        print(f"  MISSING {k}")
+    for k in new:
+        print(f"  new     {k}")
+    bad = len(changed) + len(missing)
     print("dense kernels unchanged" if bad == 0 else f"{bad} kernels differ")
     return 1 if bad else 0
 
