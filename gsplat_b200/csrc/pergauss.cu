@@ -553,11 +553,13 @@ __global__ void __launch_bounds__(kThreads, 4) project_sh_fwd_kernel(
             for(int d = 0; d < 3; ++d)
                 acc3[d] += Yk.v * cbuf[k * 3 + d];
         });
+        // max(x + 0.5, 0), with a colour exactly on the kink (x + 0.5 == 0) stored as -0: the backward passes the
+        // gradient there, as torch.clamp_min does, and blocks it at +0 (clamped from below).  Both zeros render alike.
 #pragma unroll
         for(int d = 0; d < 3; ++d)
         {
             const float shifted = acc3[d] + 0.5f;
-            rgb[d]              = shifted > 0.f ? shifted : 0.f;
+            rgb[d]              = shifted > 0.f ? shifted : (shifted == 0.f ? -0.f : 0.f);
         }
     }
     colors[idx * 3] = rgb[0], colors[idx * 3 + 1] = rgb[1], colors[idx * 3 + 2] = rgb[2];
@@ -643,11 +645,14 @@ __global__ void __launch_bounds__(kThreads, ONE_CAM ? 3 : 2) project_sh_bwd_kern
 #pragma unroll
             for(int k = 0; k < 9; ++k)
                 v_cov.m[k] += g.v_cov.m[k];
-            // SH part: relu mask re-derived from the stored post-activation colour
+            // SH part: the clamp's mask from the stored colour -- positive, or -0 (exactly on the kink)
             float vcol[3];
 #pragma unroll
             for(int d = 0; d < 3; ++d)
-                vcol[d] = colors[idx * 3 + d] > 0.f ? v_colors[idx * s_col + d] : 0.f;
+            {
+                const float c = colors[idx * 3 + d];
+                vcol[d]       = c > 0.f || __float_as_uint(c) == 0x80000000u ? v_colors[idx * s_col + d] : 0.f;
+            }
             float dir[3];
             sh_view_dir(mean, vm, dir);
             const float inorm = 1.f / sqrtf(dir[0] * dir[0] + dir[1] * dir[1] + dir[2] * dir[2]);
@@ -1177,6 +1182,9 @@ extern "C" int gsb200_sh_bwd(
     return check_launch();
 }
 
+// The fused kernels move quaternions and whole SH rows with 128-bit loads and stores.
+static bool misaligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
 extern "C" int gsb200_project_sh_fwd(
     int64_t C, int64_t N, int64_t K, int degrees_to_use, const float *means, const float *quats, const float *scales,
     const float *opacities, const float *sh_coeffs, const float *viewmats, const float *Ks, uint32_t image_width,
@@ -1185,7 +1193,7 @@ extern "C" int gsb200_project_sh_fwd(
 )
 {
     if(C < 0 || N < 0 || K <= 0 || degrees_to_use < 0 || degrees_to_use > 4
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K)
+       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K || misaligned16(quats) || misaligned16(sh_coeffs))
         return GSB200_E_INVALID;
     if(C * N == 0)
         return GSB200_OK;
@@ -1217,7 +1225,7 @@ extern "C" int gsb200_project_sh_fwd_rows(
 )
 {
     if(C < 0 || N < 0 || K <= 0 || degrees_to_use < 0 || degrees_to_use > 4 || tile_size == 0 || !totals
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K)
+       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K || misaligned16(quats) || misaligned16(sh_coeffs))
         return GSB200_E_INVALID;
     cudaStream_t st = (cudaStream_t)stream;
     GSB_CUDA_TRY(cudaMemsetAsync(totals, 0, 3 * sizeof(int64_t), st));
@@ -1251,7 +1259,8 @@ extern "C" int gsb200_project_sh_bwd(
 )
 {
     if(C < 0 || N < 0 || K <= 0 || degrees_to_use < 0 || degrees_to_use > 4
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K)
+       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K || misaligned16(quats) || misaligned16(sh_coeffs)
+       || misaligned16(v_quats) || misaligned16(v_sh_coeffs))
         return GSB200_E_INVALID;
     if(N == 0)
         return GSB200_OK;

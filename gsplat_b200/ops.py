@@ -548,7 +548,9 @@ def _alloc_grad(name: str, like: Tensor) -> Tensor:
     if _grad_allocator is not None:
         t = _grad_allocator(name, like)
         if t is not None:
-            if t.shape != like.shape or t.dtype != like.dtype or t.device != like.device or not t.is_contiguous():
+            # 16-byte aligned: the fused backward stores quaternion and SH gradient rows with 128-bit stores
+            if (t.shape != like.shape or t.dtype != like.dtype or t.device != like.device or not t.is_contiguous()
+                    or t.data_ptr() % 16):
                 raise RuntimeError(f"gradient allocator returned a mismatching tensor for {name!r}")
             return t
     return torch.empty_like(like)
@@ -564,6 +566,12 @@ class _ProjectSH(torch.autograd.Function):
         means, quats, scales = f32c(means, "means"), f32c(quats, "quats"), f32c(scales, "scales")
         opacities, sh_coeffs = f32c(opacities, "opacities"), f32c(sh_coeffs, "colors")
         viewmats, Ks = f32c(viewmats, "viewmats"), f32c(Ks, "Ks")
+        # the kernels read quaternions and SH rows with 128-bit loads: a contiguous VIEW with a storage offset (a
+        # parameter carved from a flat buffer) may be only 4-byte aligned
+        if quats.data_ptr() % 16:
+            quats = quats.clone()
+        if sh_coeffs.data_ptr() % 16:
+            sh_coeffs = sh_coeffs.clone()
         N, C, K = means.shape[0], viewmats.shape[0], sh_coeffs.shape[1]
         o = dict(device=dev, dtype=torch.float32)
         radii = torch.empty((C, N, 2), device=dev, dtype=torch.int32)

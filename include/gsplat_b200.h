@@ -101,7 +101,10 @@ extern "C"
     /* ---- fused projection + conic + SH->RGB : the orchestrator's default training path
      * (csrc/Rendering.cpp:976-1117: projection_ewa_3dgs_fused then assemble_proj_features with
      * color_post = max(x + 0.5, 0)).  One pass over the gaussians, B = 1, D = 3, quats/scales input.
-     * colors [C,N,3] = max(SH + 0.5, 0) for visible gaussians, 0 otherwise. */
+     * colors [C,N,3] = max(SH + 0.5, 0) for visible gaussians, 0 otherwise; a colour exactly on the kink
+     * (SH + 0.5 == 0) is stored as -0.f, one clamped from below as +0.f, and gsb200_project_sh_bwd reads that zero's sign.
+     * quats and sh_coeffs must be 16-byte aligned (128-bit loads), else GSB200_E_INVALID; the same holds for
+     * gsb200_project_sh_fwd_rows, and for quats, sh_coeffs, v_quats and v_sh_coeffs of gsb200_project_sh_bwd. */
     int gsb200_project_sh_fwd(
         int64_t C, int64_t N, int64_t K, int degrees_to_use, const float *means, const float *quats,
         const float *scales, const float *opacities, const float *sh_coeffs, const float *viewmats, const float *Ks,
@@ -124,8 +127,10 @@ extern "C"
         float *means2d, float *depths, float *conics, float *colors, void *row_records, int32_t *tiles_per_gauss,
         int64_t *totals, void *stream
     );
-    /* Backward of the fused pass.  v_colors is the gradient w.r.t. the post-activation colours
-     * (the relu mask is re-derived).  All outputs fully written; deterministic.  seen_bits (optional,
+    /* Backward of the fused pass.  v_colors is the gradient w.r.t. the post-activation colours; it passes where the
+     * stored colour is positive or -0.f (SH + 0.5 >= 0: at the kink the sub-gradient torch.clamp_min takes) and is
+     * blocked at +0.f, so colours clamped by max(x, 0) elsewhere keep the mask colour > 0.  All outputs fully written;
+     * deterministic.  seen_bits (optional,
      * ceil(N / 32) words): bit n%32 of word n/32 = gaussian n is visible in some camera of this call, i.e. its
      * gradient rows are not all zero -- the row bitmap gsb200_rows_allreduce_f32 consumes. */
     int gsb200_project_sh_bwd(

@@ -411,7 +411,7 @@ def rasterization_fwd_bwd(
         v_feat = v_feat[..., :-1]
     v_means_sh = 0
     if has_color and sh_degree is not None:
-        v_colors = (v_feat * ((raw + dt.type(0.5)) > 0)).astype(dt)
+        v_colors = (v_feat * ((raw + dt.type(0.5)) >= 0)).astype(dt)
         v_coeffs, v_means_sh = spherical_harmonics_bwd(sh_degree, means, viewmats, sh_coeffs, valid, v_colors)
         grads["v_sh"] = v_coeffs
     elif has_color:

@@ -141,7 +141,7 @@ def test_fused_project_sh_bwd_with_compensation_and_depth(gs, C):
     ov = gso.fully_fused_projection_bwd(sc["means"], None, sc["quats"], sc["scales"], vm, Ks, W, H, 0.3, o[0], o[3],
                                         o[4], cot[0], cot[1], cot[2], cot[4])
     raw = gso.spherical_harmonics(3, sc["means"], vm, sc["sh"], vis)
-    v_col = (cot[3] * ((raw + np.float32(0.5)) > 0)).astype(np.float32)
+    v_col = (cot[3] * ((raw + np.float32(0.5)) >= 0)).astype(np.float32)
     v_sh, v_m_sh = gso.spherical_harmonics_bwd(3, sc["means"], vm, sc["sh"], vis, v_col)
     for a, ref, name in ((gm, ov[0] + v_m_sh, "v_means"), (gq, ov[2], "v_quats"), (gsc, ov[3], "v_scales"),
                          (gsh, v_sh, "v_sh")):
