@@ -105,6 +105,87 @@ __device__ __forceinline__ M3 load_cov6(const float *c6)
     return S;
 }
 
+// mean and world covariance of gaussian bn.  The covariance is read from `covars` (6-entry triu) when given, else built
+// from (quat, scale), which are then left in q / s for the VJP (untouched, so keeping the caller's values, otherwise).
+__device__ __forceinline__ M3 load_gaussian(
+    int64_t bn, const float *means, const float *covars, const float *quats, const float *scales, float *mean, float *q,
+    float *s
+)
+{
+    mean[0] = means[bn * 3], mean[1] = means[bn * 3 + 1], mean[2] = means[bn * 3 + 2];
+    if(covars)
+        return load_cov6(covars + bn * 6);
+#pragma unroll
+    for(int k = 0; k < 4; ++k)
+        q[k] = quats[bn * 4 + k];
+#pragma unroll
+    for(int k = 0; k < 3; ++k)
+        s[k] = scales[bn * 3 + k];
+    return quat_scale_to_sym<false>(q, s);
+}
+
+// one projected row: radii, means2d, depth, conic and (when asked for) compensation of output row o
+__device__ __forceinline__ void store_proj(
+    const Proj &p, int64_t o, int32_t *radii, float *means2d, float *depths, float *conics, float *compensations
+)
+{
+    reinterpret_cast<int2 *>(radii)[o]     = make_int2(p.rx, p.ry);
+    reinterpret_cast<float2 *>(means2d)[o] = make_float2(p.mx, p.my);
+    depths[o]         = p.depth;
+    conics[o * 3]     = p.ca;
+    conics[o * 3 + 1] = p.cb;
+    conics[o * 3 + 2] = p.cc;
+    if(compensations)
+        compensations[o] = p.comp;
+}
+
+// v_R = v_pc mean^T + v_covc R cov^T + v_covc^T R cov ; v_t = v_pc: the 12 entries of the top three rows of the
+// viewmat gradient of one (gaussian, camera) pair, row-major
+__device__ __forceinline__ void pose_grad(const ProjGrad &g, const Cam &cam, const float *mean, const M3 &cov, float *vm)
+{
+    const M3 A2 = mul_bt(mul(g.v_covc, cam.R), cov);
+    const M3 B2 = mul(mul_at(g.v_covc, cam.R), cov);
+#pragma unroll
+    for(int i = 0; i < 3; ++i)
+    {
+#pragma unroll
+        for(int j = 0; j < 3; ++j)
+            vm[i * 4 + j] = g.v_pc[i] * mean[j] + A2.m[i * 3 + j] + B2.m[i * 3 + j];
+        vm[i * 4 + 3] = g.v_pc[i];
+    }
+}
+
+// The world-covariance gradient (full 3x3) as the gradient of what the gaussian was given as: the 6-entry triu
+// covariance when `from_covars`, else (quat, scale) -- zero when !vjp, since a gaussian no camera sees may have a zero
+// quaternion, whose normalisation VJP would turn the zero gradient into NaN.  put(dst, value) writes or adds each entry
+// of output row o.
+template<class Put>
+__device__ __forceinline__ void fold_cov_grad(
+    const M3 &v_cov, bool from_covars, bool vjp, const float *q, const float *s, int64_t o, float *v_covars,
+    float *v_quats, float *v_scales, Put put
+)
+{
+    if(from_covars)
+    {
+        put(v_covars + o * 6, v_cov.m[0]);
+        put(v_covars + o * 6 + 1, v_cov.m[1] + v_cov.m[3]);
+        put(v_covars + o * 6 + 2, v_cov.m[2] + v_cov.m[6]);
+        put(v_covars + o * 6 + 3, v_cov.m[4]);
+        put(v_covars + o * 6 + 4, v_cov.m[5] + v_cov.m[7]);
+        put(v_covars + o * 6 + 5, v_cov.m[8]);
+        return;
+    }
+    float vq[4] = {0.f, 0.f, 0.f, 0.f}, vs[3] = {0.f, 0.f, 0.f};
+    if(vjp)
+        quat_scale_sym_vjp<false>(q, s, v_cov, vq, vs);
+#pragma unroll
+    for(int k = 0; k < 4; ++k)
+        put(v_quats + o * 4 + k, vq[k]);
+#pragma unroll
+    for(int k = 0; k < 3; ++k)
+        put(v_scales + o * 3 + k, vs[k]);
+}
+
 template<int CAM>
 __global__ void __launch_bounds__(kThreads) projection_fwd_kernel(
     int64_t B, int64_t C, int64_t N, const float *__restrict__ means, const float *__restrict__ covars,
@@ -120,30 +201,15 @@ __global__ void __launch_bounds__(kThreads) projection_fwd_kernel(
     const int64_t b = idx / (C * N), c = (idx / N) % C, n = idx % N;
     const int64_t bn = b * N + n;
     const Cam cam = load_cam(viewmats + (b * C + c) * 16, Ks + (b * C + c) * 9);
-    const float mean[3] = {means[bn * 3], means[bn * 3 + 1], means[bn * 3 + 2]};
-    M3 cov;
-    if(covars)
-        cov = load_cov6(covars + bn * 6);
-    else
-    {
-        const float q[4] = {quats[bn * 4], quats[bn * 4 + 1], quats[bn * 4 + 2], quats[bn * 4 + 3]};
-        const float s[3] = {scales[bn * 3], scales[bn * 3 + 1], scales[bn * 3 + 2]};
-        cov = quat_scale_to_sym<false>(q, s);
-    }
+    float mean[3], q[4], s[3];
+    const M3 cov = load_gaussian(bn, means, covars, quats, scales, mean, q, s);
     float op = 0.f;
     if(opacities)
         op = opacities[bn];
     const Proj p = project_one<CAM>(
         mean, cov, opacities ? &op : nullptr, cam, W, H, eps2d, near_plane, far_plane, radius_clip, compensations != nullptr
     );
-    reinterpret_cast<int2 *>(radii)[idx]    = make_int2(p.rx, p.ry);
-    reinterpret_cast<float2 *>(means2d)[idx] = make_float2(p.mx, p.my);
-    depths[idx]         = p.depth;
-    conics[idx * 3]     = p.ca;
-    conics[idx * 3 + 1] = p.cb;
-    conics[idx * 3 + 2] = p.cc;
-    if(compensations)
-        compensations[idx] = p.comp;
+    store_proj(p, idx, radii, means2d, depths, conics, compensations);
 }
 
 // One thread per (b, n), looping over the C cameras: the per-gaussian sums stay in registers and
@@ -163,27 +229,14 @@ __global__ void __launch_bounds__(kThreads) projection_bwd_kernel(
     const bool active  = bn < B * N;
     const int64_t b    = active ? bn / N : 0, n = active ? bn % N : 0;
     const unsigned lane = threadIdx.x & 31;
+    // inactive lanes run the camera loop with a zero gaussian: they take part in the pose-gradient butterfly
     float mean[3] = {0.f, 0.f, 0.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
     M3 cov;
 #pragma unroll
     for(int k = 0; k < 9; ++k)
         cov.m[k] = 0.f;
     if(active)
-    {
-        mean[0] = means[bn * 3], mean[1] = means[bn * 3 + 1], mean[2] = means[bn * 3 + 2];
-        if(covars)
-            cov = load_cov6(covars + bn * 6);
-        else
-        {
-#pragma unroll
-            for(int k = 0; k < 4; ++k)
-                q[k] = quats[bn * 4 + k];
-#pragma unroll
-            for(int k = 0; k < 3; ++k)
-                s[k] = scales[bn * 3 + k];
-            cov = quat_scale_to_sym<false>(q, s);
-        }
-    }
+        cov = load_gaussian(bn, means, covars, quats, scales, mean, q, s);
     float v_mean[3] = {0.f, 0.f, 0.f};
     M3 v_cov;
 #pragma unroll
@@ -216,18 +269,7 @@ __global__ void __launch_bounds__(kThreads) projection_bwd_kernel(
             for(int k = 0; k < 9; ++k)
                 v_cov.m[k] += g.v_cov.m[k];
             if(v_viewmats)
-            { // v_R = v_pc mean^T + v_covc R cov^T + v_covc^T R cov ; v_t = v_pc
-                const M3 A2 = mul_bt(mul(g.v_covc, cam.R), cov);
-                const M3 B2 = mul(mul_at(g.v_covc, cam.R), cov);
-#pragma unroll
-                for(int i = 0; i < 3; ++i)
-                {
-#pragma unroll
-                    for(int j = 0; j < 3; ++j)
-                        vm_part[i * 4 + j] = g.v_pc[i] * mean[j] + A2.m[i * 3 + j] + B2.m[i * 3 + j];
-                    vm_part[i * 4 + 3] = g.v_pc[i];
-                }
-            }
+                pose_grad(g, cam, mean, cov, vm_part);
         }
         if(v_viewmats)
         {
@@ -253,36 +295,33 @@ __global__ void __launch_bounds__(kThreads) projection_bwd_kernel(
     }
     if(!active)
         return;
+    // a gaussian no camera sees gets a zero (quat, scale) gradient, as in the reference
+    fold_cov_grad(v_cov, covars != nullptr, seen, q, s, bn, v_covars, v_quats, v_scales, [](float *d, float v) { *d = v; });
 #pragma unroll
     for(int k = 0; k < 3; ++k)
         v_means[bn * 3 + k] = v_mean[k];
-    if(covars)
-    {
-        float *o = v_covars + bn * 6;
-        o[0] = v_cov.m[0];
-        o[1] = v_cov.m[1] + v_cov.m[3];
-        o[2] = v_cov.m[2] + v_cov.m[6];
-        o[3] = v_cov.m[4];
-        o[4] = v_cov.m[5] + v_cov.m[7];
-        o[5] = v_cov.m[8];
-    }
-    else
-    {
-        // a gaussian no camera sees gets zero, as in the reference (its quaternion may be zero, and the VJP of the
-        // normalisation would turn the zero gradient into NaN)
-        float vq[4] = {0.f, 0.f, 0.f, 0.f}, vs[3] = {0.f, 0.f, 0.f};
-        if(seen)
-            quat_scale_sym_vjp<false>(q, s, v_cov, vq, vs);
-#pragma unroll
-        for(int k = 0; k < 4; ++k)
-            v_quats[bn * 4 + k] = vq[k];
-#pragma unroll
-        for(int k = 0; k < 3; ++k)
-            v_scales[bn * 3 + k] = vs[k];
-    }
 }
 
 // ------------------------------------------------------------------ spherical harmonics
+// unit view direction u of a gaussian seen from viewmat vm; returns 1 / |dir| for sh_dir_vjp
+__device__ __forceinline__ float sh_unit_dir(const float *mean, const float *vm, float *u)
+{
+    float dir[3];
+    sh_view_dir(mean, vm, dir);
+    const float inorm = 1.f / sqrtf(dir[0] * dir[0] + dir[1] * dir[1] + dir[2] * dir[2]);
+    u[0] = dir[0] * inorm, u[1] = dir[1] * inorm, u[2] = dir[2] * inorm;
+    return inorm;
+}
+
+// VJP of u = dir / |dir|: vd = (vu - (vu . u) u) / |dir|
+__device__ __forceinline__ void sh_dir_vjp(const float *vu, const float *u, float inorm, float *vd)
+{
+    const float dot = vu[0] * u[0] + vu[1] * u[1] + vu[2] * u[2];
+#pragma unroll
+    for(int j = 0; j < 3; ++j)
+        vd[j] = (vu[j] - dot * u[j]) * inorm;
+}
+
 template<int DEG>
 __global__ void __launch_bounds__(kThreads) sh_fwd_kernel(
     int64_t B, int64_t C, int64_t N, int64_t K, int64_t D, const float *__restrict__ means,
@@ -301,13 +340,11 @@ __global__ void __launch_bounds__(kThreads) sh_fwd_kernel(
             out[d] = 0.f;
         return;
     }
-    const float mean[3] = {means[(b * N + n) * 3], means[(b * N + n) * 3 + 1], means[(b * N + n) * 3 + 2]};
-    float dir[3];
-    sh_view_dir(mean, viewmats + (b * C + c) * 16, dir);
-    const float inorm = 1.f / sqrtf(dir[0] * dir[0] + dir[1] * dir[1] + dir[2] * dir[2]);
-    constexpr int NB  = (DEG + 1) * (DEG + 1);
+    float u[3];
+    sh_unit_dir(means + (b * N + n) * 3, viewmats + (b * C + c) * 16, u);
+    constexpr int NB = (DEG + 1) * (DEG + 1);
     Dual<false> Y[NB];
-    sh_basis<DEG, false>(dir[0] * inorm, dir[1] * inorm, dir[2] * inorm, Y);
+    sh_basis<DEG, false>(u[0], u[1], u[2], Y);
     const float *cf = coeffs + n * K * D;
     for(int64_t d = 0; d < D; ++d)
     {
@@ -347,37 +384,31 @@ __global__ void __launch_bounds__(kThreads) sh_bwd_kernel(
         float vd[3]     = {0.f, 0.f, 0.f};
         if(on)
         {
-        const float *mean = means + (b * N + n) * 3;
-        float dir[3];
-        sh_view_dir(mean, viewmats + img * 16, dir);
-        const float inorm = 1.f / sqrtf(dir[0] * dir[0] + dir[1] * dir[1] + dir[2] * dir[2]);
-        const float u[3]  = {dir[0] * inorm, dir[1] * inorm, dir[2] * inorm};
-        Dual<true> Y[NB];
-        sh_basis<DEG, true>(u[0], u[1], u[2], Y);
-        const float vc = v_colors[o * D + d];
-        float vu[3] = {0.f, 0.f, 0.f};
+            float u[3];
+            const float inorm = sh_unit_dir(means + (b * N + n) * 3, viewmats + img * 16, u);
+            Dual<true> Y[NB];
+            sh_basis<DEG, true>(u[0], u[1], u[2], Y);
+            const float vc = v_colors[o * D + d];
+            float vu[3]    = {0.f, 0.f, 0.f};
 #pragma unroll
-        for(int k = 0; k < NB; ++k)
-        {
-            acc[k] += Y[k].v * vc;
-            const float g = cf[k * D + d] * vc;
-            vu[0] += g * Y[k].x;
-            vu[1] += g * Y[k].y;
-            vu[2] += g * Y[k].z;
-        }
-        if(DEG >= 1)
-        {
-            const float dot = vu[0] * u[0] + vu[1] * u[1] + vu[2] * u[2];
-#pragma unroll
-            for(int j = 0; j < 3; ++j)
-                vd[j] = (vu[j] - dot * u[j]) * inorm;
-            if(v_means != nullptr)
+            for(int k = 0; k < NB; ++k)
             {
-#pragma unroll
-                for(int j = 0; j < 3; ++j)
-                    atomicAdd(v_means + (b * N + n) * 3 + j, vd[j]);
+                acc[k] += Y[k].v * vc;
+                const float g = cf[k * D + d] * vc;
+                vu[0] += g * Y[k].x;
+                vu[1] += g * Y[k].y;
+                vu[2] += g * Y[k].z;
             }
-        }
+            if(DEG >= 1)
+            {
+                sh_dir_vjp(vu, u, inorm, vd);
+                if(v_means != nullptr)
+                {
+#pragma unroll
+                    for(int j = 0; j < 3; ++j)
+                        atomicAdd(v_means + (b * N + n) * 3 + j, vd[j]);
+                }
+            }
         }
         if(v_dirsum != nullptr && DEG >= 1)
         { // per-image sum of the view-direction gradient (for the pose gradient): warp reduce, one atomic per warp
@@ -412,13 +443,11 @@ __global__ void __launch_bounds__(kThreads) sh_rows_fwd_kernel(
         return;
     const int64_t i = idx / D, d = idx % D;
     const int64_t b = batch_ids[i], c = camera_ids[i], n = gaussian_ids[i];
-    const float mean[3] = {means[(b * N + n) * 3], means[(b * N + n) * 3 + 1], means[(b * N + n) * 3 + 2]};
-    float dir[3];
-    sh_view_dir(mean, viewmats + (b * C + c) * 16, dir);
-    const float inorm = 1.f / sqrtf(dir[0] * dir[0] + dir[1] * dir[1] + dir[2] * dir[2]);
-    constexpr int NB  = (DEG + 1) * (DEG + 1);
+    float u[3];
+    sh_unit_dir(means + (b * N + n) * 3, viewmats + (b * C + c) * 16, u);
+    constexpr int NB = (DEG + 1) * (DEG + 1);
     Dual<false> Y[NB];
-    sh_basis<DEG, false>(dir[0] * inorm, dir[1] * inorm, dir[2] * inorm, Y);
+    sh_basis<DEG, false>(u[0], u[1], u[2], Y);
     const float *cf = coeffs + n * K * D;
     float acc       = 0.f;
 #pragma unroll
@@ -442,11 +471,8 @@ __global__ void __launch_bounds__(kThreads) sh_rows_bwd_kernel(
         return;
     const int64_t i = idx / D, d = idx % D;
     const int64_t b = batch_ids[i], c = camera_ids[i], n = gaussian_ids[i];
-    const float *mean = means + (b * N + n) * 3;
-    float dir[3];
-    sh_view_dir(mean, viewmats + (b * C + c) * 16, dir);
-    const float inorm = 1.f / sqrtf(dir[0] * dir[0] + dir[1] * dir[1] + dir[2] * dir[2]);
-    const float u[3]  = {dir[0] * inorm, dir[1] * inorm, dir[2] * inorm};
+    float u[3];
+    const float inorm = sh_unit_dir(means + (b * N + n) * 3, viewmats + (b * C + c) * 16, u);
     constexpr int NB  = (DEG + 1) * (DEG + 1);
     Dual<true> Y[NB];
     sh_basis<DEG, true>(u[0], u[1], u[2], Y);
@@ -465,15 +491,15 @@ __global__ void __launch_bounds__(kThreads) sh_rows_bwd_kernel(
     }
     if(DEG >= 1 && (v_means != nullptr || v_dirsum != nullptr))
     {
-        const float dot = vu[0] * u[0] + vu[1] * u[1] + vu[2] * u[2];
+        float vd[3];
+        sh_dir_vjp(vu, u, inorm, vd);
 #pragma unroll
         for(int j = 0; j < 3; ++j)
         {
-            const float vd = (vu[j] - dot * u[j]) * inorm;
             if(v_means != nullptr)
-                atomicAdd(v_means + (b * N + n) * 3 + j, vd);
+                atomicAdd(v_means + (b * N + n) * 3 + j, vd[j]);
             if(v_dirsum != nullptr)
-                atomicAdd(v_dirsum + (b * C + c) * 3 + j, vd);
+                atomicAdd(v_dirsum + (b * C + c) * 3 + j, vd[j]);
         }
     }
 }
@@ -514,14 +540,7 @@ __global__ void __launch_bounds__(kThreads, 4) project_sh_fwd_kernel(
     const float op      = opacities[n];
     const M3 cov        = quat_scale_to_sym<false>(q, s);
     const Proj p = project_one(mean, cov, &op, cam, W, H, eps2d, near_plane, far_plane, radius_clip, compensations != nullptr);
-    reinterpret_cast<int2 *>(radii)[idx]     = make_int2(p.rx, p.ry);
-    reinterpret_cast<float2 *>(means2d)[idx] = make_float2(p.mx, p.my);
-    depths[idx]         = p.depth;
-    conics[idx * 3]     = p.ca;
-    conics[idx * 3 + 1] = p.cb;
-    conics[idx * 3 + 2] = p.cc;
-    if(compensations)
-        compensations[idx] = p.comp;
+    store_proj(p, idx, radii, means2d, depths, conics, compensations);
     float rgb[3] = {0.f, 0.f, 0.f};
     if(p.rx > 0 && p.ry > 0)
     {
@@ -653,11 +672,9 @@ __global__ void __launch_bounds__(kThreads, ONE_CAM ? 3 : 2) project_sh_bwd_kern
                 const float c = colors[idx * 3 + d];
                 vcol[d]       = c > 0.f || __float_as_uint(c) == 0x80000000u ? v_colors[idx * s_col + d] : 0.f;
             }
-            float dir[3];
-            sh_view_dir(mean, vm, dir);
-            const float inorm = 1.f / sqrtf(dir[0] * dir[0] + dir[1] * dir[1] + dir[2] * dir[2]);
-            const float u[3]  = {dir[0] * inorm, dir[1] * inorm, dir[2] * inorm};
-            float vu[3] = {0.f, 0.f, 0.f};
+            float u[3];
+            const float inorm = sh_unit_dir(mean, vm, u);
+            float vu[3]       = {0.f, 0.f, 0.f};
             // the coefficients are visited in address order: with 16-byte aligned rows they are fetched four at a time
             // into a rolling register (12 LDG.128 instead of 48 scalar loads -- the scalar stream stalled on lg_throttle)
             const bool vec4 = ((K * 3) & 3) == 0;
@@ -780,16 +797,8 @@ __global__ void __launch_bounds__(kThreads) projection_packed_kernel(
     {
         const int64_t bn = b * N + n;
         const Cam cam = load_cam(viewmats + row * 16, Ks + row * 9);
-        const float mean[3] = {means[bn * 3], means[bn * 3 + 1], means[bn * 3 + 2]};
-        M3 cov;
-        if(covars)
-            cov = load_cov6(covars + bn * 6);
-        else
-        {
-            const float q[4] = {quats[bn * 4], quats[bn * 4 + 1], quats[bn * 4 + 2], quats[bn * 4 + 3]};
-            const float s[3] = {scales[bn * 3], scales[bn * 3 + 1], scales[bn * 3 + 2]};
-            cov = quat_scale_to_sym<false>(q, s);
-        }
+        float mean[3], q[4], s[3];
+        const M3 cov = load_gaussian(bn, means, covars, quats, scales, mean, q, s);
         float op = 0.f;
         if(opacities)
             op = opacities[bn];
@@ -829,14 +838,7 @@ __global__ void __launch_bounds__(kThreads) projection_packed_kernel(
             batch_ids[o]    = b;
             camera_ids[o]   = c;
             gaussian_ids[o] = n;
-            reinterpret_cast<int2 *>(radii)[o]     = make_int2(p.rx, p.ry);
-            reinterpret_cast<float2 *>(means2d)[o] = make_float2(p.mx, p.my);
-            depths[o]         = p.depth;
-            conics[o * 3]     = p.ca;
-            conics[o * 3 + 1] = p.cb;
-            conics[o * 3 + 2] = p.cc;
-            if(compensations)
-                compensations[o] = p.comp;
+            store_proj(p, o, radii, means2d, depths, conics, compensations);
         }
     }
 }
@@ -862,21 +864,8 @@ __global__ void __launch_bounds__(kThreads) projection_packed_bwd_kernel(
     const int64_t b = batch_ids[i], c = camera_ids[i], n = gaussian_ids[i];
     const int64_t bn = b * N + n, row = b * C + c;
     const Cam cam = load_cam(viewmats + row * 16, Ks + row * 9);
-    const float mean[3] = {means[bn * 3], means[bn * 3 + 1], means[bn * 3 + 2]};
-    float q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
-    M3 cov;
-    if(covars)
-        cov = load_cov6(covars + bn * 6);
-    else
-    {
-#pragma unroll
-        for(int k = 0; k < 4; ++k)
-            q[k] = quats[bn * 4 + k];
-#pragma unroll
-        for(int k = 0; k < 3; ++k)
-            s[k] = scales[bn * 3 + k];
-        cov = quat_scale_to_sym<false>(q, s);
-    }
+    float mean[3], q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
+    const M3 cov = load_gaussian(bn, means, covars, quats, scales, mean, q, s);
     const float conic[3] = {conics[i * 3], conics[i * 3 + 1], conics[i * 3 + 2]};
     const float vc[3]    = {v_conics[i * s_c], v_conics[i * s_c + 1], v_conics[i * s_c + 2]};
     const bool has_comp  = v_compensations != nullptr;
@@ -885,63 +874,23 @@ __global__ void __launch_bounds__(kThreads) projection_packed_bwd_kernel(
         has_comp ? compensations[i] : 0.f, has_comp ? v_compensations[i] : 0.f
     );
     const int64_t o = dense_out ? bn : i;
-    float out[10];
-    int n_out;
-    out[0] = g.v_mean[0], out[1] = g.v_mean[1], out[2] = g.v_mean[2];
-    if(covars)
-    {
-        out[3] = g.v_cov.m[0], out[4] = g.v_cov.m[1] + g.v_cov.m[3], out[5] = g.v_cov.m[2] + g.v_cov.m[6];
-        out[6] = g.v_cov.m[4], out[7] = g.v_cov.m[5] + g.v_cov.m[7], out[8] = g.v_cov.m[8];
-        n_out  = 9;
-    }
-    else
-    {
-        float vq[4] = {0.f, 0.f, 0.f, 0.f}, vs[3] = {0.f, 0.f, 0.f};
-        quat_scale_sym_vjp<false>(q, s, g.v_cov, vq, vs);
-        out[3] = vq[0], out[4] = vq[1], out[5] = vq[2], out[6] = vq[3];
-        out[7] = vs[0], out[8] = vs[1], out[9] = vs[2];
-        n_out  = 10;
-    }
-    float *dst[10];
+    const auto put  = [dense_out](float *d, float v) {
+        if(dense_out)
+            atomicAdd(d, v);
+        else
+            *d = v;
+    };
 #pragma unroll
     for(int k = 0; k < 3; ++k)
-        dst[k] = v_means + o * 3 + k;
-    if(covars)
-    {
-#pragma unroll
-        for(int k = 0; k < 6; ++k)
-            dst[3 + k] = v_covars + o * 6 + k;
-    }
-    else
-    {
-#pragma unroll
-        for(int k = 0; k < 4; ++k)
-            dst[3 + k] = v_quats + o * 4 + k;
-#pragma unroll
-        for(int k = 0; k < 3; ++k)
-            dst[7 + k] = v_scales + o * 3 + k;
-    }
-#pragma unroll
-    for(int k = 0; k < 10; ++k)
-        if(k < n_out)
-        {
-            if(dense_out)
-                atomicAdd(dst[k], out[k]);
-            else
-                *dst[k] = out[k];
-        }
+        put(v_means + o * 3 + k, g.v_mean[k]);
+    fold_cov_grad(g.v_cov, covars != nullptr, true, q, s, o, v_covars, v_quats, v_scales, put);
     if(v_viewmats)
-    { // v_R = v_pc mean^T + v_covc R cov^T + v_covc^T R cov ; v_t = v_pc
-        const M3 A2 = mul_bt(mul(g.v_covc, cam.R), cov);
-        const M3 B2 = mul(mul_at(g.v_covc, cam.R), cov);
+    {
+        float vm[12];
+        pose_grad(g, cam, mean, cov, vm);
 #pragma unroll
-        for(int r = 0; r < 3; ++r)
-        {
-#pragma unroll
-            for(int j = 0; j < 3; ++j)
-                atomicAdd(v_viewmats + row * 16 + r * 4 + j, g.v_pc[r] * mean[j] + A2.m[r * 3 + j] + B2.m[r * 3 + j]);
-            atomicAdd(v_viewmats + row * 16 + r * 4 + 3, g.v_pc[r]);
-        }
+        for(int k = 0; k < 12; ++k)
+            atomicAdd(v_viewmats + row * 16 + k, vm[k]);
     }
 }
 
@@ -1027,6 +976,29 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(
 // C ABI
 using namespace gsb;
 
+// ftheta / lidar are other pipelines (3DGUT), not built
+static bool camera_model_ok(int camera_model) { return camera_model >= kCamPinhole && camera_model <= kCamFisheye; }
+
+// SH degrees 0-4, whose (degree + 1)^2 coefficients fit in the K per gaussian
+static bool sh_args_ok(int64_t K, int degrees_to_use)
+{
+    return K > 0 && degrees_to_use >= 0 && degrees_to_use <= 4 && (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) <= K;
+}
+
+#define GSB_CAM_SWITCH(model, CALL)       \
+    if((model) == kCamPinhole)            \
+    {                                     \
+        CALL(kCamPinhole);                \
+    }                                     \
+    else if((model) == kCamOrtho)         \
+    {                                     \
+        CALL(kCamOrtho);                  \
+    }                                     \
+    else                                  \
+    {                                     \
+        CALL(kCamFisheye);                \
+    }
+
 extern "C" int gsb200_quat_scale_to_covar_preci_fwd(
     int64_t N, const float *quats, const float *scales, int triu, float *covars, float *precis, void *stream
 )
@@ -1063,7 +1035,7 @@ extern "C" int gsb200_projection_fwd(
 {
     if(B < 0 || C < 0 || N < 0)
         return GSB200_E_INVALID;
-    if(camera_model < 0 || camera_model > 2) // ftheta / lidar are other pipelines (3DGUT), not built
+    if(!camera_model_ok(camera_model))
         return GSB200_E_UNSUPPORTED;
     const int64_t total = B * C * N;
     if(total == 0)
@@ -1072,18 +1044,13 @@ extern "C" int gsb200_projection_fwd(
         return GSB200_E_INVALID;
     if(!covars && (!quats || !scales))
         return GSB200_E_INVALID;
-#define GSB_LAUNCH(CAM)                                                                                                \
+#define CALL(CAM)                                                                                                      \
     projection_fwd_kernel<CAM><<<grid_for(total, kThreads), kThreads, 0, (cudaStream_t)stream>>>(                        \
         B, C, N, means, covars, quats, scales, opacities, viewmats, Ks, image_width, image_height, eps2d, near_plane,   \
         far_plane, radius_clip, radii, means2d, depths, conics, compensations                                           \
     )
-    if(camera_model == kCamPinhole)
-        GSB_LAUNCH(kCamPinhole);
-    else if(camera_model == kCamOrtho)
-        GSB_LAUNCH(kCamOrtho);
-    else
-        GSB_LAUNCH(kCamFisheye);
-#undef GSB_LAUNCH
+    GSB_CAM_SWITCH(camera_model, CALL)
+#undef CALL
     return check_launch();
 }
 
@@ -1098,7 +1065,7 @@ extern "C" int gsb200_projection_bwd(
 {
     if(B < 0 || C < 0 || N < 0)
         return GSB200_E_INVALID;
-    if(camera_model < 0 || camera_model > 2)
+    if(!camera_model_ok(camera_model))
         return GSB200_E_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
     if(v_viewmats && B * C > 0)
@@ -1111,19 +1078,14 @@ extern "C" int gsb200_projection_bwd(
         return GSB200_E_INVALID;
     if(v_compensations && !compensations)
         return GSB200_E_INVALID;
-#define GSB_LAUNCH(CAM)                                                                                                \
+#define CALL(CAM)                                                                                                      \
     projection_bwd_kernel<CAM><<<grid_for(B * N, kThreads), kThreads, 0, st>>>(                                          \
         B, C, N, means, covars, quats, scales, viewmats, Ks, image_width, image_height, eps2d, radii, conics,           \
         compensations, v_means2d, v_means2d_stride, v_depths, v_depths_stride, v_conics, v_conics_stride,               \
         v_compensations, v_means, v_covars, v_quats, v_scales, v_viewmats                                               \
     )
-    if(camera_model == kCamPinhole)
-        GSB_LAUNCH(kCamPinhole);
-    else if(camera_model == kCamOrtho)
-        GSB_LAUNCH(kCamOrtho);
-    else
-        GSB_LAUNCH(kCamFisheye);
-#undef GSB_LAUNCH
+    GSB_CAM_SWITCH(camera_model, CALL)
+#undef CALL
     return check_launch();
 }
 
@@ -1143,8 +1105,7 @@ extern "C" int gsb200_sh_fwd(
     const float *viewmats, const float *coeffs, const uint8_t *masks, float *colors, void *stream
 )
 {
-    if(B < 0 || C < 0 || N < 0 || K <= 0 || D <= 0 || degrees_to_use < 0 || degrees_to_use > 4
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K)
+    if(B < 0 || C < 0 || N < 0 || D <= 0 || !sh_args_ok(K, degrees_to_use))
         return GSB200_E_INVALID;
     const int64_t total = B * C * N;
     if(total == 0)
@@ -1164,8 +1125,7 @@ extern "C" int gsb200_sh_bwd(
     float *v_means, float *v_dirsum, void *stream
 )
 {
-    if(B < 0 || C < 0 || N < 0 || K <= 0 || D <= 0 || degrees_to_use < 0 || degrees_to_use > 4
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K)
+    if(B < 0 || C < 0 || N < 0 || D <= 0 || !sh_args_ok(K, degrees_to_use))
         return GSB200_E_INVALID;
     cudaStream_t st = (cudaStream_t)stream;
     if(v_means && B * N > 0)
@@ -1192,8 +1152,7 @@ extern "C" int gsb200_project_sh_fwd(
     int32_t *radii, float *means2d, float *depths, float *conics, float *compensations, float *colors, void *stream
 )
 {
-    if(C < 0 || N < 0 || K <= 0 || degrees_to_use < 0 || degrees_to_use > 4
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K || misaligned16(quats) || misaligned16(sh_coeffs))
+    if(C < 0 || N < 0 || !sh_args_ok(K, degrees_to_use) || misaligned16(quats) || misaligned16(sh_coeffs))
         return GSB200_E_INVALID;
     if(C * N == 0)
         return GSB200_OK;
@@ -1224,8 +1183,8 @@ extern "C" int gsb200_project_sh_fwd_rows(
     void *row_records, int32_t *tiles_per_gauss, int64_t *totals, void *stream
 )
 {
-    if(C < 0 || N < 0 || K <= 0 || degrees_to_use < 0 || degrees_to_use > 4 || tile_size == 0 || !totals
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K || misaligned16(quats) || misaligned16(sh_coeffs))
+    if(C < 0 || N < 0 || !sh_args_ok(K, degrees_to_use) || tile_size == 0 || !totals || misaligned16(quats)
+       || misaligned16(sh_coeffs))
         return GSB200_E_INVALID;
     cudaStream_t st = (cudaStream_t)stream;
     GSB_CUDA_TRY(cudaMemsetAsync(totals, 0, 3 * sizeof(int64_t), st));
@@ -1258,8 +1217,7 @@ extern "C" int gsb200_project_sh_bwd(
     const float *v_compensations, float *v_means, float *v_quats, float *v_scales, float *v_sh_coeffs, uint32_t *seen_bits, void *stream
 )
 {
-    if(C < 0 || N < 0 || K <= 0 || degrees_to_use < 0 || degrees_to_use > 4
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K || misaligned16(quats) || misaligned16(sh_coeffs)
+    if(C < 0 || N < 0 || !sh_args_ok(K, degrees_to_use) || misaligned16(quats) || misaligned16(sh_coeffs)
        || misaligned16(v_quats) || misaligned16(v_sh_coeffs))
         return GSB200_E_INVALID;
     if(N == 0)
@@ -1370,20 +1328,6 @@ PackedWs carve_packed(void *workspace, int64_t blocks)
 }
 } // namespace
 
-#define GSB_CAM_SWITCH(model, CALL)       \
-    if((model) == kCamPinhole)            \
-    {                                     \
-        CALL(kCamPinhole);                \
-    }                                     \
-    else if((model) == kCamOrtho)         \
-    {                                     \
-        CALL(kCamOrtho);                  \
-    }                                     \
-    else                                  \
-    {                                     \
-        CALL(kCamFisheye);                \
-    }
-
 // Pass 1: per-block visible counts + their inclusive scan in `workspace`; *nnz_dev (device int32) = total.
 extern "C" int gsb200_projection_packed_count(
     int64_t B, int64_t C, int64_t N, const float *means, const float *covars, const float *quats, const float *scales,
@@ -1394,7 +1338,7 @@ extern "C" int gsb200_projection_packed_count(
 {
     if(B < 0 || C < 0 || N < 0 || !nnz_dev)
         return GSB200_E_INVALID;
-    if(camera_model < 0 || camera_model > 2)
+    if(!camera_model_ok(camera_model))
         return GSB200_E_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
     if(B * C * N == 0)
@@ -1435,7 +1379,7 @@ extern "C" int gsb200_projection_packed_emit(
 {
     if(B < 0 || C < 0 || N < 0 || !indptr)
         return GSB200_E_INVALID;
-    if(camera_model < 0 || camera_model > 2)
+    if(!camera_model_ok(camera_model))
         return GSB200_E_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
     if(B * C * N == 0)
@@ -1473,7 +1417,7 @@ extern "C" int gsb200_projection_packed_bwd(
 {
     if(B < 0 || C < 0 || N < 0 || nnz < 0)
         return GSB200_E_INVALID;
-    if(camera_model < 0 || camera_model > 2)
+    if(!camera_model_ok(camera_model))
         return GSB200_E_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
     if(v_viewmats && B * C > 0)
@@ -1514,8 +1458,7 @@ extern "C" int gsb200_sh_rows_fwd(
     const int64_t *gaussian_ids, float *colors, void *stream
 )
 {
-    if(nnz < 0 || B < 0 || C < 0 || N < 0 || K <= 0 || D <= 0 || degrees_to_use < 0 || degrees_to_use > 4
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K)
+    if(nnz < 0 || B < 0 || C < 0 || N < 0 || D <= 0 || !sh_args_ok(K, degrees_to_use))
         return GSB200_E_INVALID;
     if(nnz == 0)
         return GSB200_OK;
@@ -1534,8 +1477,7 @@ extern "C" int gsb200_sh_rows_bwd(
     const int64_t *gaussian_ids, const float *v_colors, float *v_coeffs, float *v_means, float *v_dirsum, void *stream
 )
 {
-    if(nnz < 0 || B < 0 || C < 0 || N < 0 || K <= 0 || D <= 0 || degrees_to_use < 0 || degrees_to_use > 4
-       || (int64_t)(degrees_to_use + 1) * (degrees_to_use + 1) > K || !v_coeffs)
+    if(nnz < 0 || B < 0 || C < 0 || N < 0 || D <= 0 || !sh_args_ok(K, degrees_to_use) || !v_coeffs)
         return GSB200_E_INVALID;
     cudaStream_t st = (cudaStream_t)stream;
     if(N > 0)

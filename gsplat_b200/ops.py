@@ -61,6 +61,13 @@ def _rows(t: Optional[Tensor], width: int, name: str) -> Tuple[Optional[Tensor],
     return t.contiguous(), width
 
 
+def _mask_u8(masks: Optional[Tensor]) -> Optional[Tensor]:
+    """masks as the uint8 array the kernels read (a bool tensor is reinterpreted, not copied), or None"""
+    if masks is None:
+        return None
+    return masks.contiguous().view(torch.uint8) if masks.dtype == torch.bool else masks.to(torch.uint8).contiguous()
+
+
 class _Ctx:
     """device guard + stream fetch for one operator call"""
 
@@ -360,6 +367,16 @@ def fully_fused_projection(
 # spherical_harmonics (dense)
 
 
+def _v_viewmats_from_dirsum(viewmats: Tensor, v_dirsum: Tensor) -> Tensor:
+    """Pose gradient of the SH view directions.  dir = mean + R^T t  =>  dL/dR[i][j] = t[i] S[j],  dL/dt = R S, with
+    S = v_dirsum, the sum of dL/ddir over the camera's gaussians."""
+    R, t = viewmats[..., :3, :3], viewmats[..., :3, 3]
+    v_viewmats = torch.zeros_like(viewmats)
+    v_viewmats[..., :3, :3] = t[..., :, None] * v_dirsum[..., None, :]
+    v_viewmats[..., :3, 3] = torch.einsum("...ij,...j->...i", R, v_dirsum)
+    return v_viewmats
+
+
 class _SphericalHarmonics(torch.autograd.Function):
     @staticmethod
     def forward(ctx, degrees_to_use, means, viewmats, coeffs, masks):
@@ -368,9 +385,7 @@ class _SphericalHarmonics(torch.autograd.Function):
         batch = tuple(means.shape[:-2])
         B, N, C = _prod(batch), means.shape[-2], viewmats.shape[-3]
         K, D = coeffs.shape[-2:]
-        m8 = None
-        if masks is not None:
-            m8 = masks.contiguous().view(torch.uint8) if masks.dtype == torch.bool else masks.to(torch.uint8).contiguous()
+        m8 = _mask_u8(masks)
         colors = torch.empty(batch + (C, N, D), device=dev, dtype=torch.float32)
         with _Ctx(dev) as st:
             check(
@@ -400,13 +415,7 @@ class _SphericalHarmonics(torch.autograd.Function):
                 ),
                 "spherical_harmonics_bwd",
             )
-        v_viewmats = None
-        if need_vm:
-            # dir = mean + R^T t  =>  dL/dR[i][j] = t[i] S[j],  dL/dt[i] = sum_j R[i][j] S[j],  S = sum_n dL/ddir
-            R, t = viewmats[..., :3, :3], viewmats[..., :3, 3]
-            v_viewmats = torch.zeros_like(viewmats)
-            v_viewmats[..., :3, :3] = t[..., :, None] * v_dirsum[..., None, :]
-            v_viewmats[..., :3, 3] = torch.einsum("...ij,...j->...i", R, v_dirsum)
+        v_viewmats = _v_viewmats_from_dirsum(viewmats, v_dirsum) if need_vm else None
         return None, v_means, v_viewmats, v_coeffs, None
 
 
@@ -455,12 +464,7 @@ class _SphericalHarmonicsRows(torch.autograd.Function):
                 ),
                 "spherical_harmonics_bwd (rows)",
             )
-        v_viewmats = None
-        if need_vm:  # dir = mean + R^T t  =>  dL/dR[i][j] = t[i] S[j],  dL/dt = R S,  S = sum of dL/ddir over the camera's rows
-            R, t = viewmats[..., :3, :3], viewmats[..., :3, 3]
-            v_viewmats = torch.zeros_like(viewmats)
-            v_viewmats[..., :3, :3] = t[..., :, None] * v_dirsum[..., None, :]
-            v_viewmats[..., :3, 3] = torch.einsum("...ij,...j->...i", R, v_dirsum)
+        v_viewmats = _v_viewmats_from_dirsum(viewmats, v_dirsum) if need_vm else None
         return None, v_means, v_viewmats, v_coeffs, None, None, None
 
 
@@ -1070,9 +1074,7 @@ class _RasterizeToPixels(torch.autograd.Function):
         # [nnz, *] are addressed flat: ceil(R / I) keeps I * N within I - 1 rows of the real row count R.
         N = (R + I - 1) // I if I > 0 else R
         th, tw = isect_offsets.shape[-2:]
-        m8 = None
-        if masks is not None:
-            m8 = masks.contiguous().view(torch.uint8) if masks.dtype == torch.bool else masks.to(torch.uint8).contiguous()
+        m8 = _mask_u8(masks)
         offsets = isect_offsets.contiguous()
         fl = flatten_ids.contiguous()
         if offsets.dtype != torch.int32 or fl.dtype != torch.int32:
@@ -1291,9 +1293,7 @@ class _RasterizeToPixels2DGS(torch.autograd.Function):
         image_dims = tuple(isect_offsets.shape[:-2])
         I, N, D = _prod(image_dims), means2d.shape[-2], colors.shape[-1]
         th, tw = isect_offsets.shape[-2:]
-        m8 = None
-        if masks is not None:
-            m8 = masks.contiguous().view(torch.uint8) if masks.dtype == torch.bool else masks.to(torch.uint8).contiguous()
+        m8 = _mask_u8(masks)
         offsets, fl = isect_offsets.contiguous(), flatten_ids.contiguous()
         S = fl.shape[0]
         o = dict(device=dev, dtype=torch.float32)
@@ -1607,9 +1607,7 @@ class _RasterizeToPixelsSparse(torch.autograd.Function):
         backgrounds = f32c(backgrounds, "backgrounds")
         row_dims = tuple(means2d.shape[:-1])
         R, D, P = _prod(row_dims), colors.shape[-1], pixel_map.shape[0]
-        m8 = None
-        if masks is not None:
-            m8 = masks.contiguous().view(torch.uint8) if masks.dtype == torch.bool else masks.to(torch.uint8).contiguous()
+        m8 = _mask_u8(masks)
         active, offsets, fl = active_tiles.contiguous(), tile_offsets.contiguous(), flatten_ids.contiguous()
         words = tile_pixel_mask.contiguous()
         cumsum, pmap = tile_pixel_cumsum.contiguous(), pixel_map.contiguous()
