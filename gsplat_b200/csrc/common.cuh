@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/gsplat_b200.h"
 
 namespace gsb
@@ -57,6 +59,31 @@ inline uint32_t bits_for_count(int64_t count)
 }
 
 inline unsigned grid_for(int64_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
+
+// The colour channel counts the compositing kernels are built for: f(std::integral_constant<int, D>{}) for one of them,
+// GSB200_E_UNSUPPORTED for any other D.
+template<class F>
+inline int with_channels(int D, F &&f)
+{
+    switch(D)
+    {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 3: return f(std::integral_constant<int, 3>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 5: return f(std::integral_constant<int, 5>{});
+    case 8: return f(std::integral_constant<int, 8>{});
+    case 16: return f(std::integral_constant<int, 16>{});
+    case 32: return f(std::integral_constant<int, 32>{});
+    default: return GSB200_E_UNSUPPORTED;
+    }
+}
+
+// does a tw x th grid of kTile-pixel tiles cover a W x H image?
+inline bool tile_grid_covers(uint32_t tw, uint32_t th, uint32_t W, uint32_t H)
+{
+    return (uint64_t)tw * kTile >= W && (uint64_t)th * kTile >= H;
+}
 
 #ifdef __CUDACC__
 // ---- mbarrier / bulk-copy (TMA 1-D, SASS UBLKCP) wrappers

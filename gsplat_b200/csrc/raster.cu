@@ -26,6 +26,7 @@ namespace gsb
 constexpr int kBatch  = 128; // gaussians per ring stage
 constexpr int kStages = 2;
 constexpr int kWarps  = 8;
+constexpr int kPipeStages = 3; // stages of the barrier-free (PIPE) rings
 
 template<int CDIM, int BATCH = kBatch>
 struct RecLayout
@@ -45,20 +46,30 @@ struct RecordStreams
 
 static inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
+// Byte offsets of the streams in the caller's buffer (cull at 0), each 256-byte aligned, and the buffer's size
+// (gsb200_raster_records_bytes): the order stream holds n_tiles + 1 entries, and 256 bytes of slack follow it.
+struct RecordsLayout
+{
+    size_t axis, geom, color, order, bytes;
+};
+
+static inline RecordsLayout records_layout(int64_t S, int cvec4, int64_t n_tiles)
+{
+    RecordsLayout l;
+    const size_t stream = align256((size_t)S * 16);
+    l.axis  = stream;
+    l.geom  = 2 * stream;
+    l.color = 3 * stream;
+    l.order = l.color + align256((size_t)S * 16 * (size_t)cvec4);
+    l.bytes = l.order + align256((size_t)(n_tiles + 1) * 4) + 256;
+    return l;
+}
+
 static inline RecordStreams carve_records(void *base, int64_t S, int cvec4)
 {
-    RecordStreams r;
-    char *p = (char *)base;
-    r.cull  = (float4 *)p;
-    p += align256((size_t)S * 16);
-    r.axis = (float4 *)p;
-    p += align256((size_t)S * 16);
-    r.geom = (float4 *)p;
-    p += align256((size_t)S * 16);
-    r.color = (float4 *)p;
-    p += align256((size_t)S * 16 * (size_t)cvec4);
-    r.order = (int32_t *)p;
-    return r;
+    const RecordsLayout l = records_layout(S, cvec4, 0);
+    char *p               = (char *)base;
+    return {(float4 *)p, (float4 *)(p + l.axis), (float4 *)(p + l.geom), (float4 *)(p + l.color), (int32_t *)(p + l.order)};
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -295,7 +306,37 @@ struct Ring
         bulk_g2s(geom(stage), ggeom + first, n16, full(stage));
         bulk_g2s(color(stage), gcolor + first * CV, n16 * CV, full(stage));
     }
+    // one thread: one arrival per full barrier; zero the per-stage warp counters of the barrier-free rings (a ring with
+    // more stages than counters only ever zeroes counter 0)
+    __device__ __forceinline__ void init(int32_t *counters) const
+    {
+#pragma unroll
+        for(int s = 0; s < STAGES; ++s)
+        {
+            mbar_init(full(s), 1);
+            counters[s < kPipeStages ? s : 0] = 0;
+        }
+    }
 };
+
+// Survivors of one chunk of records: `mask` is the ballot of the lanes' cull tests, and the index `mine` of each hit
+// goes into the warp's list at its rank among the hits of the lanes in rank_mask (the lanes below: front to back;
+// above: back to front).  Returns the number of survivors.
+__device__ __forceinline__ int compact_survivors(uint32_t mask, bool hit, int mine, uint32_t rank_mask, int32_t *surv)
+{
+    if(hit)
+        surv[__popc(mask & rank_mask)] = mine;
+    __syncwarp();
+    return __popc(mask);
+}
+
+// Gaussian falloff of record (q = cull, g = geom) at the pixel centre (px, py); e2 = -sigma * log2(e)
+__device__ __forceinline__ float pair_vis(const float4 q, const float4 g, float px, float py, float &e2)
+{
+    const float dx = q.x - px, dy = q.y - py;
+    e2             = fmaf(g.x * dx, dx, fmaf(g.z * dy, dy, (g.y * dx) * dy));
+    return fast_ex2(e2);
+}
 
 template<int CDIM, int BATCH = kBatch, int STAGES = kStages>
 constexpr size_t ring_smem_bytes()
@@ -322,7 +363,6 @@ __device__ __forceinline__ bool block_may_touch(const float4 q, const float4 ax,
 // re-arms the barrier and fetches the batch kPipeStages ahead -- unless every warp of the tile is saturated, in which
 // case it publishes the first batch that will NOT arrive (s_stop) and all warps leave when they reach it (the tile-level
 // early exit of the barrier version).
-constexpr int kPipeStages = 3;
 
 template<int CDIM, bool PIPE = false, class Pix = DensePixels>
 __global__ void __launch_bounds__(kWarps * 32) raster_fwd_kernel(
@@ -394,12 +434,7 @@ __global__ void __launch_bounds__(kWarps * 32) raster_fwd_kernel(
 
     if(tid == 0)
     {
-#pragma unroll
-        for(int s = 0; s < KS; ++s)
-        {
-            mbar_init(ring.full(s), 1);
-            s_cnt[s < kPipeStages ? s : 0] = 0;
-        }
+        ring.init(s_cnt);
         s_alive = kWarps;
         s_stop  = 0x7fffffff;
         fence_mbar_init();
@@ -475,19 +510,15 @@ __global__ void __launch_bounds__(kWarps * 32) raster_fwd_kernel(
                 const uint32_t mask = __ballot_sync(0xffffffffu, hit);
                 if(mask == 0u)
                     continue;
-                if(hit)
-                    surv[__popc(mask & lanemask_lt)] = mine;
-                __syncwarp();
-                const int n_surv = __popc(mask);
+                const int n_surv = compact_survivors(mask, hit, mine, lanemask_lt, surv);
                 for(int i = 0; i < n_surv; ++i)
                 {
                     const int t     = surv[i];
                     const float4 q  = scull[t];
                     const float4 g  = sgeom[t];
                     const float4 cc = scol[t * CV];
-                    const float dx = q.x - px, dy = q.y - py;
-                    const float e2    = fmaf(g.x * dx, dx, fmaf(g.z * dy, dy, (g.y * dx) * dy)); // = -sigma * log2(e)
-                    const float vis   = fast_ex2(e2);
+                    float e2;
+                    const float vis   = pair_vis(q, g, px, py, e2);
                     const float alpha = fminf(kMaxAlpha, g.w * vis);
                     if(done == 0u && e2 <= 0.f && alpha >= kAlphaThreshold)
                     {
@@ -717,12 +748,7 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
     if(tid == 0)
     {
         s_tile_bin = -1;
-#pragma unroll
-        for(int s = 0; s < KS; ++s)
-        {
-            mbar_init(ring.full(s), 1);
-            s_done[s < kPipeStages ? s : 0] = 0;
-        }
+        ring.init(s_done);
         fence_mbar_init();
     }
     __syncthreads();
@@ -893,18 +919,14 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
                 if(mask == 0u)
                     continue;
                 // survivors compacted back to front into the per-warp list (one LDS per survivor instead of walking the mask)
-                if(hit)
-                    surv[__popc(mask & lanemask_gt)] = mine;
-                __syncwarp();
-                const int n_surv = __popc(mask);
+                const int n_surv = compact_survivors(mask, hit, mine, lanemask_gt, surv);
                 for(int si = 0; si < n_surv; ++si)
                 {
                     const int t    = surv[si];
                     const float4 q = scull[t];
                     const float4 g = sgeom[t];
-                    const float dx = q.x - px, dy = q.y - py;
-                    const float e2    = fmaf(g.x * dx, dx, fmaf(g.z * dy, dy, (g.y * dx) * dy)); // = -sigma * log2(e)
-                    const float vis   = fast_ex2(e2);
+                    float e2;
+                    const float vis   = pair_vis(q, g, px, py, e2);
                     const float ov    = g.w * vis;
                     const float alpha = fminf(kMaxAlpha, ov);
                     const bool valid  = (t <= lim) && e2 <= 0.f && alpha >= kAlphaThreshold;
@@ -1040,12 +1062,15 @@ static int launch_pack(
     if(want_order)
         side_lock.lock();
     SideLane *lane = want_order ? side_lane() : nullptr;
+    auto order_tiles = [&](cudaStream_t on) {
+        tile_order_kernel<<<1, 1024, 0, on>>>(offsets, (int32_t)n_tiles, (int32_t)S, r.order);
+        return check_launch();
+    };
     if(lane != nullptr)
     {
         GSB_CUDA_TRY(cudaEventRecord(lane->fork, st));
         GSB_CUDA_TRY(cudaStreamWaitEvent(lane->stream, lane->fork, 0));
-        tile_order_kernel<<<1, 1024, 0, lane->stream>>>(offsets, (int32_t)n_tiles, (int32_t)S, r.order);
-        if(int rc = check_launch())
+        if(int rc = order_tiles(lane->stream))
             return rc;
         GSB_CUDA_TRY(cudaEventRecord(lane->join, lane->stream));
     }
@@ -1063,11 +1088,7 @@ static int launch_pack(
     if(lane != nullptr)
         GSB_CUDA_TRY(cudaStreamWaitEvent(st, lane->join, 0));
     else if(want_order)
-    {
-        tile_order_kernel<<<1, 1024, 0, st>>>(offsets, (int32_t)n_tiles, (int32_t)S, r.order);
-        if(int rc = check_launch())
-            return rc;
-    }
+        return order_tiles(st); // no side stream: after the pack, on the caller's stream
     return GSB200_OK;
 }
 
@@ -1129,28 +1150,17 @@ static int launch_bwd(
 
 // ---------------------------------------------------------------------------------------------
 // C ABI
-#define GSB_FOR_CHANNELS(X) X(1) X(2) X(3) X(4) X(5) X(8) X(16) X(32)
 
 extern "C" int gsb200_raster_supports_channels(int D)
 {
-    switch(D)
-    {
-#define X(n) case n:
-        GSB_FOR_CHANNELS(X)
-#undef X
-        return 1;
-    default:
-        return 0;
-    }
+    return gsb::with_channels(D, [](auto) { return GSB200_OK; }) == GSB200_OK;
 }
 
 extern "C" size_t gsb200_raster_records_bytes(int64_t n_isects, int D, int64_t n_tiles)
 {
     if(n_isects < 0 || D <= 0 || n_tiles < 0)
         return 0;
-    const size_t cv = (size_t)((D + 3) / 4);
-    return 3 * gsb::align256((size_t)n_isects * 16) + gsb::align256((size_t)n_isects * 16 * cv)
-         + gsb::align256((size_t)(n_tiles + 1) * 4) + 256;
+    return gsb::records_layout(n_isects, (D + 3) / 4, n_tiles).bytes;
 }
 
 extern "C" int gsb200_raster_pack(
@@ -1166,17 +1176,41 @@ extern "C" int gsb200_raster_pack(
     if(!means2d || !conics || !colors || !opacities || !flatten_ids || !records)
         return GSB200_E_INVALID;
     const unsigned n_tiles = (unsigned)(I * tile_width * tile_height);
-    cudaStream_t st        = (cudaStream_t)stream;
-    switch(D)
-    {
-#define X(n)                                                                                                         \
-    case n:                                                                                                          \
-        return gsb::launch_pack<n>(means2d, conics, colors, opacities, offsets, flatten_ids, n_isects, n_tiles, records, st);
-        GSB_FOR_CHANNELS(X)
-#undef X
-    default:
+    return gsb::with_channels(D, [&](auto C) {
+        return gsb::launch_pack<C>(means2d, conics, colors, opacities, offsets, flatten_ids, n_isects, n_tiles, records, (cudaStream_t)stream);
+    });
+}
+
+// gsb200_raster_fwd (rows == nullptr: the per-gaussian inputs) and gsb200_raster_fwd_rows (the 64-byte row records,
+// D <= 4).  The checks run in the same order for both.
+static int raster_fwd(
+    int64_t I, int64_t N, int D, const float *means2d, const float *conics, const float *colors, const float *opacities,
+    const void *row_records, bool from_rows, const float *backgrounds, const uint8_t *masks, uint32_t image_width,
+    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+    const int32_t *flatten_ids, int64_t n_isects, void *records, float *render_colors, float *render_alphas,
+    int32_t *last_ids, void *stream
+)
+{
+    if(I < 0 || N < 0 || n_isects < 0 || !offsets || !render_colors || !render_alphas || !last_ids)
+        return GSB200_E_INVALID;
+    const bool inputs = from_rows ? row_records && (reinterpret_cast<uintptr_t>(row_records) & 15) == 0
+                                  : means2d && conics && colors && opacities;
+    if(n_isects > 0 && (!inputs || !flatten_ids || !records))
+        return GSB200_E_INVALID;
+    if(tile_size != (uint32_t)gsb::kTile || (from_rows && D > 4))
         return GSB200_E_UNSUPPORTED;
-    }
+    if(I == 0 || image_width == 0 || image_height == 0)
+        return GSB200_OK;
+    if(!gsb::tile_grid_covers(tile_width, tile_height, image_width, image_height))
+        return GSB200_E_INVALID;
+    const unsigned n_tiles = (unsigned)(I * tile_width * tile_height);
+    return gsb::with_channels(D, [&](auto C) {
+        return gsb::launch_fwd<C>(
+            n_tiles, (uint32_t)I, means2d, conics, colors, opacities, backgrounds, masks, image_width, image_height, tile_width,
+            tile_height, offsets, flatten_ids, n_isects, gsb::DensePixels{}, records, render_colors, render_alphas, last_ids,
+            (cudaStream_t)stream, static_cast<const float4 *>(row_records)
+        );
+    });
 }
 
 extern "C" int gsb200_raster_fwd(
@@ -1187,32 +1221,10 @@ extern "C" int gsb200_raster_fwd(
     int32_t *last_ids, void *stream
 )
 {
-    if(I < 0 || N < 0 || n_isects < 0 || !offsets || !render_colors || !render_alphas || !last_ids)
-        return GSB200_E_INVALID;
-    if(n_isects > 0 && (!means2d || !conics || !colors || !opacities || !flatten_ids || !records))
-        return GSB200_E_INVALID;
-    if(tile_size != (uint32_t)gsb::kTile)
-        return GSB200_E_UNSUPPORTED;
-    if(I == 0 || image_width == 0 || image_height == 0)
-        return GSB200_OK;
-    if((uint64_t)tile_width * gsb::kTile < image_width || (uint64_t)tile_height * gsb::kTile < image_height)
-        return GSB200_E_INVALID;
-    const unsigned n_tiles = (unsigned)(I * tile_width * tile_height);
-    cudaStream_t st        = (cudaStream_t)stream;
-    switch(D)
-    {
-#define X(n)                                                                                                         \
-    case n:                                                                                                          \
-        return gsb::launch_fwd<n>(                                                                                   \
-            n_tiles, (uint32_t)I, means2d, conics, colors, opacities, backgrounds, masks, image_width, image_height, \
-            tile_width, tile_height, offsets, flatten_ids, n_isects, gsb::DensePixels{}, records, render_colors,      \
-            render_alphas, last_ids, st                                                                              \
-        );
-        GSB_FOR_CHANNELS(X)
-#undef X
-    default:
-        return GSB200_E_UNSUPPORTED;
-    }
+    return raster_fwd(
+        I, N, D, means2d, conics, colors, opacities, nullptr, false, backgrounds, masks, image_width, image_height, tile_size,
+        tile_width, tile_height, offsets, flatten_ids, n_isects, records, render_colors, render_alphas, last_ids, stream
+    );
 }
 
 // Forward from the 64-byte row records {cull | axis | geom | color} that gsb200_project_sh_fwd_rows wrote (D <= 4).
@@ -1223,33 +1235,10 @@ extern "C" int gsb200_raster_fwd_rows(
     int32_t *last_ids, void *stream
 )
 {
-    if(I < 0 || N < 0 || n_isects < 0 || !offsets || !render_colors || !render_alphas || !last_ids)
-        return GSB200_E_INVALID;
-    if(n_isects > 0 && (!row_records || !flatten_ids || !records || (reinterpret_cast<uintptr_t>(row_records) & 15) != 0))
-        return GSB200_E_INVALID;
-    if(tile_size != (uint32_t)gsb::kTile || D > 4)
-        return GSB200_E_UNSUPPORTED;
-    if(I == 0 || image_width == 0 || image_height == 0)
-        return GSB200_OK;
-    if((uint64_t)tile_width * gsb::kTile < image_width || (uint64_t)tile_height * gsb::kTile < image_height)
-        return GSB200_E_INVALID;
-    const unsigned n_tiles = (unsigned)(I * tile_width * tile_height);
-    cudaStream_t st        = (cudaStream_t)stream;
-    const float4 *rr       = static_cast<const float4 *>(row_records);
-    switch(D)
-    {
-#define X(n)                                                                                                         \
-    case n:                                                                                                          \
-        return gsb::launch_fwd<n>(                                                                                   \
-            n_tiles, (uint32_t)I, nullptr, nullptr, nullptr, nullptr, backgrounds, masks, image_width, image_height, \
-            tile_width, tile_height, offsets, flatten_ids, n_isects, gsb::DensePixels{}, records, render_colors,      \
-            render_alphas, last_ids, st, rr                                                                          \
-        );
-        X(1) X(2) X(3) X(4)
-#undef X
-    default:
-        return GSB200_E_UNSUPPORTED;
-    }
+    return raster_fwd(
+        I, N, D, nullptr, nullptr, nullptr, nullptr, row_records, true, backgrounds, masks, image_width, image_height, tile_size,
+        tile_width, tile_height, offsets, flatten_ids, n_isects, records, render_colors, render_alphas, last_ids, stream
+    );
 }
 
 // The gradient records of the backward (include/gsplat_b200.h): a 16-byte aligned base, and rows * row width below 2^32
@@ -1283,21 +1272,13 @@ extern "C" int gsb200_raster_bwd(
     if(int rc = grad_records_ok((double)I * (double)N, D, absgrad, v_grad_records))
         return rc;
     const unsigned n_tiles = (unsigned)(I * tile_width * tile_height);
-    cudaStream_t st        = (cudaStream_t)stream;
-    switch(D)
-    {
-#define X(n)                                                                                                       \
-    case n:                                                                                                        \
-        return gsb::launch_bwd<n>(                                                                                 \
-            n_tiles, (uint32_t)I, backgrounds, masks, image_width, image_height, tile_width, tile_height, offsets, \
-            flatten_ids, n_isects, gsb::DensePixels{}, records, render_alphas, last_ids, v_render_colors,           \
-            v_render_alphas, absgrad != 0, v_grad_records, st                                                      \
+    return gsb::with_channels(D, [&](auto C) {
+        return gsb::launch_bwd<C>(
+            n_tiles, (uint32_t)I, backgrounds, masks, image_width, image_height, tile_width, tile_height, offsets, flatten_ids,
+            n_isects, gsb::DensePixels{}, records, render_alphas, last_ids, v_render_colors, v_render_alphas, absgrad != 0,
+            v_grad_records, (cudaStream_t)stream
         );
-        GSB_FOR_CHANNELS(X)
-#undef X
-    default:
-        return GSB200_E_UNSUPPORTED;
-    }
+    });
 }
 
 // ---- sparse pixels: one CTA per active tile of the layout of gsb200_sparse_layout_*, outputs [P, D] / [P] in the original
@@ -1311,7 +1292,7 @@ static int sparse_args_ok(
         return GSB200_E_INVALID;
     if(n_active > 0 && (!active_tiles || !tile_offsets || !tile_pixel_mask || !tile_pixel_cumsum || !pixel_map))
         return GSB200_E_INVALID;
-    if((uint64_t)tw * gsb::kTile < W || (uint64_t)th * gsb::kTile < H)
+    if(!gsb::tile_grid_covers(tw, th, W, H))
         return GSB200_E_INVALID;
     return GSB200_OK;
 }
@@ -1337,21 +1318,13 @@ extern "C" int gsb200_raster_sparse_fwd(
     if(n_isects > 0 && (!means2d || !conics || !colors || !opacities || !flatten_ids))
         return GSB200_E_INVALID;
     const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
-    cudaStream_t st = (cudaStream_t)stream;
-    switch(D)
-    {
-#define X(n)                                                                                                         \
-    case n:                                                                                                          \
-        return gsb::launch_fwd<n>(                                                                                   \
-            (unsigned)n_active, 1u, means2d, conics, colors, opacities, backgrounds, masks, image_width, image_height, \
-            tile_width, tile_height, tile_offsets, flatten_ids, n_isects, pm, records, render_colors, render_alphas, \
-            last_ids, st                                                                                             \
+    return gsb::with_channels(D, [&](auto C) {
+        return gsb::launch_fwd<C>(
+            (unsigned)n_active, 1u, means2d, conics, colors, opacities, backgrounds, masks, image_width, image_height, tile_width,
+            tile_height, tile_offsets, flatten_ids, n_isects, pm, records, render_colors, render_alphas, last_ids,
+            (cudaStream_t)stream
         );
-        GSB_FOR_CHANNELS(X)
-#undef X
-    default:
-        return GSB200_E_UNSUPPORTED;
-    }
+    });
 }
 
 extern "C" int gsb200_raster_sparse_bwd(
@@ -1376,19 +1349,11 @@ extern "C" int gsb200_raster_sparse_bwd(
     if(int rc = grad_records_ok((double)n_rows, D, absgrad, v_grad_records))
         return rc;
     const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
-    cudaStream_t st = (cudaStream_t)stream;
-    switch(D)
-    {
-#define X(n)                                                                                                       \
-    case n:                                                                                                        \
-        return gsb::launch_bwd<n>(                                                                                 \
-            (unsigned)n_active, 1u, backgrounds, masks, image_width, image_height, tile_width, tile_height,        \
-            tile_offsets, flatten_ids, n_isects, pm, records, render_alphas, last_ids, v_render_colors,            \
-            v_render_alphas, absgrad != 0, v_grad_records, st                                                      \
+    return gsb::with_channels(D, [&](auto C) {
+        return gsb::launch_bwd<C>(
+            (unsigned)n_active, 1u, backgrounds, masks, image_width, image_height, tile_width, tile_height, tile_offsets,
+            flatten_ids, n_isects, pm, records, render_alphas, last_ids, v_render_colors, v_render_alphas, absgrad != 0,
+            v_grad_records, (cudaStream_t)stream
         );
-        GSB_FOR_CHANNELS(X)
-#undef X
-    default:
-        return GSB200_E_UNSUPPORTED;
-    }
+    });
 }

@@ -711,8 +711,6 @@ int launch_surfel_bwd(
 
 // ---------------------------------------------------------------------------------------------
 // C ABI
-#define GSB_SURFEL_CHANNELS(X) X(1) X(2) X(3) X(4) X(5) X(8) X(16) X(32)
-
 extern "C" int gsb200_surfel_projection_fwd(
     int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *viewmats,
     const float *Ks, uint32_t image_width, uint32_t image_height, float near_plane, float far_plane, float radius_clip,
@@ -774,25 +772,17 @@ extern "C" int gsb200_surfel_raster_fwd(
         return GSB200_E_UNSUPPORTED;
     if(I == 0 || image_width == 0 || image_height == 0)
         return GSB200_OK;
-    if((uint64_t)tile_width * gsb::kTile < image_width || (uint64_t)tile_height * gsb::kTile < image_height)
+    if(!gsb::tile_grid_covers(tile_width, tile_height, image_width, image_height))
         return GSB200_E_INVALID;
     if((double)I * (double)N * 9.0 >= 2147483648.0 || (double)I * tile_width * tile_height >= 2147483648.0)
         return GSB200_E_UNSUPPORTED;
-    cudaStream_t st = (cudaStream_t)stream;
-    switch(D)
-    {
-#define X(n)                                                                                                                \
-    case n:                                                                                                                 \
-        return gsb::launch_surfel_fwd<n>(                                                                                   \
-            (uint32_t)I, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height, \
-            tile_width, tile_height, offsets, flatten_ids, n_isects, render_colors, render_alphas, render_normals,           \
-            render_distort, render_median, last_ids, median_ids, st                                                         \
+    return gsb::with_channels(D, [&](auto C) {
+        return gsb::launch_surfel_fwd<C>(
+            (uint32_t)I, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height,
+            tile_width, tile_height, offsets, flatten_ids, n_isects, render_colors, render_alphas, render_normals,
+            render_distort, render_median, last_ids, median_ids, (cudaStream_t)stream
         );
-        GSB_SURFEL_CHANNELS(X)
-#undef X
-    default:
-        return GSB200_E_UNSUPPORTED;
-    }
+    });
 }
 
 extern "C" int gsb200_surfel_raster_bwd(
@@ -816,24 +806,16 @@ extern "C" int gsb200_surfel_raster_bwd(
        || !render_alphas || !last_ids || !median_ids || !v_render_colors || !v_means2d || !v_ray_transforms || !v_colors
        || !v_opacities || !v_normals || !v_densify)
         return GSB200_E_INVALID;
-    if((uint64_t)tile_width * gsb::kTile < image_width || (uint64_t)tile_height * gsb::kTile < image_height)
+    if(!gsb::tile_grid_covers(tile_width, tile_height, image_width, image_height))
         return GSB200_E_INVALID;
     if((double)I * (double)N * 9.0 >= 2147483648.0 || (double)I * tile_width * tile_height >= 2147483648.0)
         return GSB200_E_UNSUPPORTED;
-    gsb::SurfGradDst dst{v_means2d, v_ray_transforms, v_colors, v_opacities, v_normals, v_densify, v_means2d_abs};
-    cudaStream_t st = (cudaStream_t)stream;
-    switch(D)
-    {
-#define X(n)                                                                                                                \
-    case n:                                                                                                                 \
-        return gsb::launch_surfel_bwd<n>(                                                                                   \
-            (uint32_t)I, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height, \
-            tile_width, tile_height, offsets, flatten_ids, n_isects, render_colors, render_alphas, last_ids, median_ids,    \
-            v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst, st                  \
+    const gsb::SurfGradDst dst{v_means2d, v_ray_transforms, v_colors, v_opacities, v_normals, v_densify, v_means2d_abs};
+    return gsb::with_channels(D, [&](auto C) {
+        return gsb::launch_surfel_bwd<C>(
+            (uint32_t)I, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height,
+            tile_width, tile_height, offsets, flatten_ids, n_isects, render_colors, render_alphas, last_ids, median_ids,
+            v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst, (cudaStream_t)stream
         );
-        GSB_SURFEL_CHANNELS(X)
-#undef X
-    default:
-        return GSB200_E_UNSUPPORTED;
-    }
+    });
 }

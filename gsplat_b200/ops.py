@@ -1027,6 +1027,26 @@ def _split_grad_records(rec: Tensor, D: int, absgrad: bool):
     return rec[..., 0:2], rec[..., 2:5], rec[..., 6 : 6 + D], rec[..., 5], (rec[..., 6 + D : 8 + D] if absgrad else None)
 
 
+def _composite_backward(ctx, render_alphas, v_render_colors, v_render_alphas, D, row_dims, run):
+    """Both compositing backwards around their C call run(v_render_colors, v_render_alphas, absgrad, rec, stream).
+    Returns the contiguous v_render_colors and the (v_means2d, v_conics, v_colors, v_opacities) gradients."""
+    dev = render_alphas.device
+    # set_materialize_grads(False): an output the loss does not use arrives as None instead of a zero-filled tensor
+    # (render_alphas in a plain photometric loss: 8 MB of zeros per 1080p step); the kernel takes a null pointer for it
+    if v_render_colors is None:
+        v_render_colors = torch.zeros(render_alphas.shape[:-1] + (D,), device=dev, dtype=torch.float32)
+    v_render_colors = v_render_colors.contiguous()
+    v_render_alphas = v_render_alphas.contiguous() if v_render_alphas is not None else None
+    absgrad = ctx.absgrad_holder is not None
+    rec = _grad_records(row_dims, D, absgrad, dev)
+    with _Ctx(dev) as st:
+        run(v_render_colors, v_render_alphas, absgrad, rec, st)
+    v_means2d, v_conics, v_colors, v_opacities, v_abs = _split_grad_records(rec, D, absgrad)
+    if absgrad:
+        ctx.absgrad_holder.copy_(v_abs)
+    return v_render_colors, (v_means2d, v_conics, v_colors, v_opacities)
+
+
 def _rasterize_padded(means2d, colors, backgrounds, tile_size, packed, absgrad, composite):
     """Shared by the compositing entry points: checks the arguments, pads colors / backgrounds with zero channels up to
     the next count the kernels are built for, runs composite(colors, backgrounds, absgrad_holder, padded), sets
@@ -1113,18 +1133,8 @@ class _RasterizeToPixels(torch.autograd.Function):
     @staticmethod
     def backward(ctx, v_render_colors, v_render_alphas):
         backgrounds, m8, offsets, fl, records, render_alphas, last_ids = ctx.saved_tensors
-        absgrad_holder = ctx.absgrad_holder
         row_dims, I, N, D, width, height, tile_size, tw, th, S = ctx.meta
-        dev = render_alphas.device
-        # set_materialize_grads(False): an output the loss does not use arrives as None instead of a zero-filled tensor
-        # (render_alphas in a plain photometric loss: 8 MB of zeros per 1080p step); the kernel takes a null pointer for it
-        if v_render_colors is None:
-            v_render_colors = torch.zeros(render_alphas.shape[:-1] + (D,), device=dev, dtype=torch.float32)
-        v_render_colors = v_render_colors.contiguous()
-        v_render_alphas = v_render_alphas.contiguous() if v_render_alphas is not None else None
-        absgrad = absgrad_holder is not None
-        rec = _grad_records(row_dims, D, absgrad, dev)
-        with _Ctx(dev) as st:
+        def run(v_render_colors, v_render_alphas, absgrad, rec, st):
             check(
                 lib().gsb200_raster_bwd(
                     I, N, D, ptr(backgrounds), ptr(m8), width, height, tile_size, tw, th, ptr(offsets), ptr(fl), S,
@@ -1133,13 +1143,11 @@ class _RasterizeToPixels(torch.autograd.Function):
                 ),
                 "rasterize_to_pixels_3dgs_bwd",
             )
-        v_means2d, v_conics, v_colors, v_opacities, v_abs = _split_grad_records(rec, D, absgrad)
-        if absgrad:
-            absgrad_holder.copy_(v_abs)
+        v_render_colors, grads = _composite_backward(ctx, render_alphas, v_render_colors, v_render_alphas, D, row_dims, run)
         v_backgrounds = None
         if backgrounds is not None and ctx.needs_input_grad[4]:
             v_backgrounds = (v_render_colors * (1.0 - render_alphas)).sum(dim=(-3, -2))
-        return (v_means2d, v_conics, v_colors, v_opacities, v_backgrounds) + (None,) * 8
+        return grads + (v_backgrounds,) + (None,) * 8
 
 
 def rasterize_to_pixels(
@@ -1635,16 +1643,8 @@ class _RasterizeToPixelsSparse(torch.autograd.Function):
     @staticmethod
     def backward(ctx, v_render_colors, v_render_alphas):
         backgrounds, m8, image_ids, active, offsets, fl, words, cumsum, pmap, records, render_alphas, last_ids = ctx.saved_tensors
-        absgrad_holder = ctx.absgrad_holder
         row_dims, R, D, width, height, tw, th = ctx.meta
-        dev = render_alphas.device
-        if v_render_colors is None:
-            v_render_colors = torch.zeros(render_alphas.shape[:-1] + (D,), device=dev, dtype=torch.float32)
-        v_render_colors = v_render_colors.contiguous()
-        v_render_alphas = v_render_alphas.contiguous() if v_render_alphas is not None else None
-        absgrad = absgrad_holder is not None
-        rec = _grad_records(row_dims, D, absgrad, dev)
-        with _Ctx(dev) as st:
+        def run(v_render_colors, v_render_alphas, absgrad, rec, st):
             check(
                 lib().gsb200_raster_sparse_bwd(
                     R, D, ptr(backgrounds), ptr(m8), width, height, 16, tw, th, active.shape[0], ptr(active), ptr(offsets), ptr(fl),
@@ -1653,13 +1653,11 @@ class _RasterizeToPixelsSparse(torch.autograd.Function):
                 ),
                 "rasterize_to_pixels_sparse_bwd",
             )
-        v_means2d, v_conics, v_colors, v_opacities, v_abs = _split_grad_records(rec, D, absgrad)
-        if absgrad:
-            absgrad_holder.copy_(v_abs)
+        v_render_colors, grads = _composite_backward(ctx, render_alphas, v_render_colors, v_render_alphas, D, row_dims, run)
         v_backgrounds = None
         if backgrounds is not None and ctx.needs_input_grad[4]:
             v_backgrounds = torch.zeros_like(backgrounds).index_add_(0, image_ids.long(), v_render_colors * (1.0 - render_alphas))
-        return (v_means2d, v_conics, v_colors, v_opacities, v_backgrounds) + (None,) * 13
+        return grads + (v_backgrounds,) + (None,) * 13
 
 
 def rasterize_to_pixels_sparse(

@@ -19,7 +19,7 @@ import torch
 from ._cabi import stream as _raw_stream
 
 from ._cabi import check, lib, ptr
-from .ops import _grad_records, _split_grad_records
+from .ops import _grad_records, _prod, _split_grad_records
 
 _libs = []
 
@@ -69,10 +69,7 @@ def rasterize_to_pixels_3dgs_bwd(means2d, conics, colors, opacities, backgrounds
     I, th, tw, D, S = _geom(tile_offsets, flatten_ids, colors)
     dev = means2d.device
     rows = tuple(means2d.shape[:-1])
-    R = 1
-    for d in rows:
-        R *= d
-    N = (R + max(I, 1) - 1) // max(I, 1)
+    N = (_prod(rows) + max(I, 1) - 1) // max(I, 1)
     means2d, conics, colors, opacities = means2d.contiguous(), conics.contiguous(), colors.contiguous(), opacities.contiguous()
     offsets, fl = tile_offsets.contiguous(), flatten_ids.contiguous()
     g = _grad_records(rows, D, absgrad, dev)
