@@ -4,7 +4,8 @@ Public names mirror /root/reference/gsplat/__init__.py:19-104 for the hot path:
 rasterization, fully_fused_projection, spherical_harmonics, isect_tiles, isect_offset_encode,
 rasterize_to_pixels, quat_scale_to_covar_preci, the sparse-pixel ops build_sparse_tile_layout,
 isect_tiles_sparse, rasterize_to_pixels_sparse, and 2DGS: rasterization_2dgs, fully_fused_projection_2dgs,
-rasterize_to_pixels_2dgs (dense layout).  Importing the package does not need a GPU; calling an
+rasterize_to_pixels_2dgs (dense layout), and the pair queries rasterize_to_indices_in_range /
+rasterize_to_indices_in_range_2dgs.  Importing the package does not need a GPU; calling an
 operator does (and needs gsplat_b200/libgsplat_b200.so, built by ``python -m gsplat_b200.build``).
 """
 from .ops import (  # noqa: F401
@@ -19,6 +20,8 @@ from .ops import (  # noqa: F401
     isect_tiles,
     isect_tiles_sparse,
     quat_scale_to_covar_preci,
+    rasterize_to_indices_in_range,
+    rasterize_to_indices_in_range_2dgs,
     rasterize_to_pixels,
     rasterize_to_pixels_2dgs,
     rasterize_to_pixels_sparse,
@@ -79,6 +82,8 @@ __all__ = [
     "rasterization_2dgs",
     "fully_fused_projection_2dgs",
     "rasterize_to_pixels_2dgs",
+    "rasterize_to_indices_in_range",
+    "rasterize_to_indices_in_range_2dgs",
     "quat_scale_to_covar_preci",
     "compute_relocation",
     "mcmc_perturb_positions",

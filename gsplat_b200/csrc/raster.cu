@@ -19,6 +19,7 @@
 #include <mutex>
 
 #include "common.cuh"
+#include "indices.cuh"
 #include "rowrec.cuh"
 
 namespace gsb
@@ -999,6 +1000,103 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------
+// rasterize_to_indices_in_range: the (pixel, gaussian) pairs the forward composites, walking only the kIndexBatch-record
+// batches [b0, b1) of each tile's list from the pixel's given transmittance.  One CTA per tile, each batch's records
+// built by row_record and staged in shared memory; every decision is raster_fwd_kernel's: its warp -> 8x4 pixel block
+// mapping, block_may_touch, pair_vis and its alpha, threshold and stop expressions.  EMIT = false writes every pixel's
+// pair count; EMIT = true writes its pairs, front to back, from its scanned start.
+template<bool EMIT>
+__global__ void __launch_bounds__(kWarps * 32) raster_indices_kernel(
+    const uint32_t I, const int64_t N, const int64_t n_isects, const float *__restrict__ means2d,
+    const float *__restrict__ conics, const float *__restrict__ opacities, const float *__restrict__ transmittances,
+    const uint32_t W, const uint32_t H, const uint32_t tw, const uint32_t th, const int32_t *__restrict__ offsets,
+    const int32_t *__restrict__ flatten_ids, const int32_t b0, const int32_t b1, int32_t *__restrict__ counts,
+    const int64_t *__restrict__ starts, int64_t *__restrict__ gaussian_ids, int64_t *__restrict__ pixel_ids,
+    int64_t *__restrict__ image_ids
+)
+{
+    static_assert(kWarps * 32 == kIndexBatch, "one record of a batch per thread");
+    __shared__ float4 s_cull[kIndexBatch], s_axis[kIndexBatch], s_geom[kIndexBatch];
+    __shared__ int32_t s_id[kIndexBatch];
+    const TileGeom tg   = decode_block(blockIdx.x, tw, th);
+    const unsigned tid  = threadIdx.x;
+    const unsigned warp = tid >> 5, lane = tid & 31;
+    const int bx0 = tg.tile_x * kTile + (warp & 1) * 8;
+    const int by0 = tg.tile_y * kTile + (warp >> 1) * 4;
+    const int px_i = bx0 + (lane & 7), py_i = by0 + (lane >> 3);
+    const float px = (float)px_i + 0.5f, py = (float)py_i + 0.5f;
+    const float cx = (float)bx0 + 4.0f, cy = (float)by0 + 2.0f;
+    const bool inside      = (px_i < (int)W) && (py_i < (int)H);
+    const int64_t pix_in   = (int64_t)py_i * W + px_i;
+    const int64_t pix      = (int64_t)tg.image_id * H * W + pix_in;
+    const int64_t tile_lin = (int64_t)tg.image_id * tw * th + tg.tile_id;
+    const int32_t range_start = offsets[tile_lin];
+    const int32_t range_end   = (tile_lin == (int64_t)I * tw * th - 1) ? (int32_t)n_isects : offsets[tile_lin + 1];
+    const int b_end           = min(b1, (range_end - range_start + kIndexBatch - 1) / kIndexBatch);
+
+    float T        = inside ? transmittances[pix] : 1.f;
+    bool done      = !inside;
+    int32_t cnt    = 0;
+    const int64_t base = (EMIT && inside) ? starts[pix] : 0;
+    for(int b = b0; b < b_end; ++b)
+    {
+        if(__syncthreads_count(done) == kIndexBatch)
+            break; // every pixel of the tile has stopped (also the barrier before the stage is overwritten)
+        const int32_t first = range_start + b * kIndexBatch;
+        const int count     = min(kIndexBatch, (int)(range_end - first));
+        if((int)tid < count)
+        {
+            const int32_t g = flatten_ids[first + (int)tid];
+            const float2 m  = *reinterpret_cast<const float2 *>(means2d + (int64_t)g * 2);
+            float4 rc, ra, rg;
+            row_record(m.x, m.y, conics[(int64_t)g * 3], conics[(int64_t)g * 3 + 1], conics[(int64_t)g * 3 + 2], opacities[g], rc, ra, rg);
+            s_cull[tid] = rc;
+            s_axis[tid] = ra;
+            s_geom[tid] = rg;
+            s_id[tid]   = g;
+        }
+        __syncthreads();
+        for(int c0 = 0; c0 < count; c0 += 32)
+        {
+            if(__all_sync(0xffffffffu, done))
+                break;
+            const int mine = c0 + (int)lane;
+            const bool hit = mine < count && block_may_touch(s_cull[mine], s_axis[mine], cx, cy);
+            for(uint32_t mask = __ballot_sync(0xffffffffu, hit); mask != 0u; mask &= mask - 1u)
+            {
+                const int t = c0 + __ffs(mask) - 1;
+                if(done)
+                    continue;
+                const float4 q = s_cull[t];
+                const float4 g = s_geom[t];
+                float e2;
+                const float vis   = pair_vis(q, g, px, py, e2);
+                const float alpha = fminf(kMaxAlpha, g.w * vis);
+                if(e2 <= 0.f && alpha >= kAlphaThreshold)
+                {
+                    const float next_T = T * (1.0f - alpha);
+                    if(next_T <= kTransmittanceThreshold)
+                        done = true; // exclusive of the current gaussian
+                    else
+                    {
+                        if constexpr(EMIT)
+                        {
+                            gaussian_ids[base + cnt] = (int64_t)s_id[t] % N;
+                            pixel_ids[base + cnt]    = pix_in;
+                            image_ids[base + cnt]    = tg.image_id;
+                        }
+                        ++cnt;
+                        T = next_T;
+                    }
+                }
+            }
+        }
+    }
+    if(!EMIT && inside)
+        counts[pix] = cnt;
+}
+
+// ---------------------------------------------------------------------------------------------
 // record streams + tile dispatch order of one view batch (the first stage of the forward; also callable on its own,
 // gsb200_raster_pack, for bindings that rebuild the records in their backward instead of keeping them alive)
 // The tile dispatch order (one CTA, ~9 us) depends only on the offsets: it runs on a side stream next to the pack pass
@@ -1356,4 +1454,29 @@ extern "C" int gsb200_raster_sparse_bwd(
             v_grad_records, (cudaStream_t)stream
         );
     });
+}
+
+// ---- rasterize_to_indices_in_range: count pass (emit = 0) and emit pass (emit = 1) over one workspace (indices.cuh)
+extern "C" int gsb200_raster_indices(
+    int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities, const float *transmittances,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+    const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t range_start, int64_t range_end, int emit,
+    void *workspace, size_t workspace_bytes, int64_t *total, int64_t *gaussian_ids, int64_t *pixel_ids, int64_t *image_ids,
+    void *stream
+)
+{
+    const cudaStream_t st = (cudaStream_t)stream;
+    const bool inputs_ok  = means2d && conics && opacities && transmittances && offsets && flatten_ids;
+    return gsb::run_index_pass(
+        I, N, image_width, image_height, tile_size, tile_width, tile_height, n_isects, range_start, range_end, inputs_ok, emit,
+        workspace, workspace_bytes, total, gaussian_ids && pixel_ids && image_ids, st,
+        [&](unsigned n_tiles, int32_t b0, int32_t b1, const gsb::PixelCounts &pc) {
+            auto kernel = emit ? gsb::raster_indices_kernel<true> : gsb::raster_indices_kernel<false>;
+            kernel<<<n_tiles, gsb::kWarps * 32, 0, st>>>(
+                (uint32_t)I, N, n_isects, means2d, conics, opacities, transmittances, image_width, image_height, tile_width,
+                tile_height, offsets, flatten_ids, b0, b1, pc.counts, pc.starts, gaussian_ids, pixel_ids, image_ids
+            );
+            return gsb::check_launch();
+        }
+    );
 }

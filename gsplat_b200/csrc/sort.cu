@@ -1,9 +1,10 @@
-// sort.cu -- the library-level functions (version, error strings, last CUDA error) and the sparse pixel layout, a
-// cub::DeviceRadixSort::SortPairs over one key per requested pixel.
+// sort.cu -- the library-level functions (version, error strings, last CUDA error), the sparse pixel layout, a
+// cub::DeviceRadixSort::SortPairs over one key per requested pixel, and the pixel-count scan of the index queries.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
+#include "indices.cuh"
 
 namespace gsb
 {
@@ -210,4 +211,50 @@ extern "C" int gsb200_sparse_layout_finish(
         reinterpret_cast<unsigned long long *>(tile_pixel_mask), tile_pixel_cumsum, pixel_map
     );
     return gsb::check_launch();
+}
+
+// ---- per-pixel pair counts of the index queries (indices.cuh): exclusive int64 scan of int32 counts
+namespace gsb
+{
+static size_t align256_bytes(size_t b) { return (b + 255) & ~(size_t)255; }
+
+static size_t pixel_scan_scratch(int64_t P)
+{
+    size_t bytes = 0;
+    cub::DeviceScan::ExclusiveScan(
+        (void *)nullptr, bytes, (const int32_t *)nullptr, (int64_t *)nullptr, cuda::std::plus<int64_t>{}, (int64_t)0, P + 1
+    );
+    return bytes;
+}
+
+size_t pixel_counts_bytes(int64_t P)
+{
+    return align256_bytes(sizeof(int32_t) * (size_t)(P + 1)) + align256_bytes(sizeof(int64_t) * (size_t)(P + 1))
+         + align256_bytes(pixel_scan_scratch(P));
+}
+
+PixelCounts carve_pixel_counts(void *workspace, int64_t P)
+{
+    char *p             = (char *)workspace;
+    const size_t counts = align256_bytes(sizeof(int32_t) * (size_t)(P + 1));
+    const size_t starts = align256_bytes(sizeof(int64_t) * (size_t)(P + 1));
+    return {(int32_t *)p, (int64_t *)(p + counts), p + counts + starts, pixel_scan_scratch(P)};
+}
+
+int scan_pixel_counts(const PixelCounts &pc, int64_t P, int64_t *total, cudaStream_t st)
+{
+    size_t bytes = pc.scratch_bytes;
+    GSB_CUDA_TRY(cub::DeviceScan::ExclusiveScan(
+        pc.scratch, bytes, (const int32_t *)pc.counts, pc.starts, cuda::std::plus<int64_t>{}, (int64_t)0, P + 1, st
+    ));
+    GSB_CUDA_TRY(cudaMemcpyAsync(total, pc.starts + P, sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+    return GSB200_OK;
+}
+} // namespace gsb
+
+extern "C" size_t gsb200_indices_workspace_bytes(int64_t n_pixels)
+{
+    if(n_pixels < 0)
+        return 0;
+    return gsb::pixel_counts_bytes(n_pixels);
 }

@@ -6,6 +6,7 @@
 // Reference semantics: csrc/Projection2DGSFused.cu (projection and VJP), csrc/Projection2DGS.cuh (ray-transform VJP),
 // csrc/RasterizeToPixels2DGSSerialBatchFwd.cu / Bwd.cu (compositing), include/Common.h and csrc/Rasterization.h (constants).
 #include "gaussmath.cuh"
+#include "indices.cuh"
 
 namespace gsb
 {
@@ -449,6 +450,73 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_raster_fwd_kernel(
     median_ids[pix]     = median_idx;
 }
 
+// rasterize_to_indices_in_range_2dgs: the (pixel, surfel) pairs surfel_raster_fwd_kernel composites, walking only the
+// batches [b0, b1) of each tile's list from the pixel's given transmittance; the pixel mapping, staging, surf_eval and
+// the stop rule are the forward's.  EMIT = false writes every pixel's pair count; EMIT = true writes its pairs, front to
+// back, from its scanned start.
+template<bool EMIT>
+__global__ void __launch_bounds__(kSurfThreads) surfel_indices_kernel(
+    uint32_t I, int64_t N, const float *__restrict__ means2d, const float *__restrict__ rt, const float *__restrict__ opacities,
+    const float *__restrict__ transmittances, uint32_t W, uint32_t H, uint32_t tw, uint32_t th,
+    const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids, int64_t n_isects, int32_t b0, int32_t b1,
+    int32_t *__restrict__ counts, const int64_t *__restrict__ starts, int64_t *__restrict__ gaussian_ids,
+    int64_t *__restrict__ pixel_ids, int64_t *__restrict__ image_ids
+)
+{
+    static_assert(kSurfThreads == kIndexBatch, "one record of a batch per thread");
+    __shared__ SurfRec rec[kSurfThreads];
+    const uint32_t tile  = blockIdx.x; // image * th * tw + tile row * tw + tile col
+    const uint32_t img   = tile / (tw * th);
+    const uint32_t tin   = tile - img * tw * th;
+    const uint32_t tr    = threadIdx.x;
+    const uint32_t i     = (tin / tw) * kTile + tr / kTile;
+    const uint32_t j     = (tin % tw) * kTile + tr % kTile;
+    const bool inside    = i < H && j < W;
+    const int64_t pix_in = (int64_t)i * W + j;
+    const int64_t pix    = (int64_t)img * H * W + pix_in;
+    const int64_t start  = offsets[tile];
+    const int64_t end    = (tile + 1 == I * tw * th) ? n_isects : offsets[tile + 1];
+    const int64_t b_end  = min((int64_t)b1, (end - start + kSurfThreads - 1) / kSurfThreads);
+    const float px = (float)j + 0.5f, py = (float)i + 0.5f;
+
+    float T            = inside ? transmittances[pix] : 1.f;
+    bool done          = !inside;
+    int32_t cnt        = 0;
+    const int64_t base = (EMIT && inside) ? starts[pix] : 0;
+    for(int64_t b = b0; b < b_end; ++b)
+    {
+        if(__syncthreads_count(done) == kSurfThreads)
+            break;
+        const int64_t batch = start + b * kSurfThreads;
+        if(batch + tr < end)
+            stage(rec[tr], flatten_ids[batch + tr], means2d, opacities, rt);
+        __syncthreads();
+        const int n_b = (int)min((int64_t)kSurfThreads, end - batch);
+        for(int t = 0; t < n_b && !done; ++t)
+        {
+            const SurfHit h = surf_eval(rec[t], px, py);
+            if(!h.ok)
+                continue;
+            const float next_T = T * (1.f - h.alpha);
+            if(next_T <= kTransmittanceThreshold)
+            { // exclusive: this surfel does not contribute
+                done = true;
+                break;
+            }
+            if constexpr(EMIT)
+            {
+                gaussian_ids[base + cnt] = (int64_t)rec[t].id % N;
+                pixel_ids[base + cnt]    = pix_in;
+                image_ids[base + cnt]    = img;
+            }
+            ++cnt;
+            T = next_T;
+        }
+    }
+    if(!EMIT && inside)
+        counts[pix] = cnt;
+}
+
 struct SurfGradDst
 {
     float *means2d, *rt, *colors, *opacities, *normals, *densify, *abs;
@@ -818,4 +886,29 @@ extern "C" int gsb200_surfel_raster_bwd(
             v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst, (cudaStream_t)stream
         );
     });
+}
+
+// ---- rasterize_to_indices_in_range_2dgs: count pass (emit = 0) and emit pass (emit = 1) over one workspace (indices.cuh)
+extern "C" int gsb200_surfel_indices(
+    int64_t I, int64_t N, const float *means2d, const float *ray_transforms, const float *opacities,
+    const float *transmittances, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
+    uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t range_start,
+    int64_t range_end, int emit, void *workspace, size_t workspace_bytes, int64_t *total, int64_t *gaussian_ids,
+    int64_t *pixel_ids, int64_t *image_ids, void *stream
+)
+{
+    const cudaStream_t st = (cudaStream_t)stream;
+    const bool inputs_ok  = means2d && ray_transforms && opacities && transmittances && offsets && flatten_ids;
+    return gsb::run_index_pass(
+        I, N, image_width, image_height, tile_size, tile_width, tile_height, n_isects, range_start, range_end, inputs_ok, emit,
+        workspace, workspace_bytes, total, gaussian_ids && pixel_ids && image_ids, st,
+        [&](unsigned n_tiles, int32_t b0, int32_t b1, const gsb::PixelCounts &pc) {
+            auto kernel = emit ? gsb::surfel_indices_kernel<true> : gsb::surfel_indices_kernel<false>;
+            kernel<<<n_tiles, gsb::kSurfThreads, 0, st>>>(
+                (uint32_t)I, N, means2d, ray_transforms, opacities, transmittances, image_width, image_height, tile_width,
+                tile_height, offsets, flatten_ids, n_isects, b0, b1, pc.counts, pc.starts, gaussian_ids, pixel_ids, image_ids
+            );
+            return gsb::check_launch();
+        }
+    );
 }

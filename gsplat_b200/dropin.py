@@ -8,6 +8,8 @@ executable form).  ``apply()`` rebinds, in place, the names the reference's call
                         rasterize_to_pixels_sparse}                          (_wrapper.py:1433,1352,1566)
   gsplat.rasterization_2dgs / gsplat.rendering.rasterization_2dgs            (rendering.py:1358)
   gsplat.cuda._wrapper.{fully_fused_projection_2dgs, rasterize_to_pixels_2dgs} (_wrapper.py:2633,2918)
+  gsplat.cuda._wrapper.{rasterize_to_indices_in_range,
+                        rasterize_to_indices_in_range_2dgs}                  (_wrapper.py:2486,3154)
   gsplat.<the same re-exports>                                               (__init__.py:23-62)
   gsplat.relocation.compute_relocation (+ its import in gsplat.strategy.ops) (relocation.py:25, strategy/ops.py:26)
   gsplat.strategy.ops._cuda_fused_mcmc_perturb                               (strategy/ops.py:405)
@@ -46,6 +48,8 @@ _OPS = (
 )
 # rebound only where the package has them (its build may leave 2DGS out)
 _OPS_2DGS = ("fully_fused_projection_2dgs", "rasterize_to_pixels_2dgs")
+# the pair queries, rebound only where the package has them: the pairs are then those this library's compositing renders
+_OPS_INDICES = ("rasterize_to_indices_in_range", "rasterize_to_indices_in_range_2dgs")
 
 _saved: List[Tuple[object, str, object]] = []
 
@@ -99,13 +103,13 @@ def apply(losses: bool = True, ops: bool = True) -> Dict[str, object]:
         _apply_ops(B, G)
     if losses:
         _apply_losses(G)
-    return {"package": G.__file__, "ops": (list(_OPS + _OPS_2DGS) + ["adam", "rasterization", "rasterization_2dgs", "compute_relocation"]) if ops else [], "losses": losses}
+    return {"package": G.__file__, "ops": (list(_OPS + _OPS_2DGS + _OPS_INDICES) + ["adam", "rasterization", "rasterization_2dgs", "compute_relocation"]) if ops else [], "losses": losses}
 
 
 def _apply_ops(B, G) -> None:
     W = importlib.import_module("gsplat.cuda._wrapper")
     R = importlib.import_module("gsplat.rendering")
-    for name in _OPS + tuple(n for n in _OPS_2DGS if hasattr(W, n)):
+    for name in _OPS + tuple(n for n in _OPS_2DGS + _OPS_INDICES if hasattr(W, n)):
         fn = _delegating(name, getattr(B, name), getattr(W, name))
         _set(W, name, fn)
         if hasattr(G, name):

@@ -13,6 +13,7 @@ hand-written sm_90a kernels.
 from __future__ import annotations
 
 import math
+import operator
 from typing import Optional, Tuple
 
 import torch
@@ -1438,6 +1439,132 @@ def rasterize_to_pixels_2dgs(
     if absgrad:
         means2d.absgrad = holder
     return outs
+
+
+# --------------------------------------------------------------------------------------------
+# rasterize_to_indices_in_range / rasterize_to_indices_in_range_2dgs (reference wrappers gsplat/cuda/_wrapper.py:2486,
+# :3154): the pairs the compositing forward of this library composites, for iterative rasterization and picking.
+
+_RANGE_MAX = 1 << 62  # any range end past the last batch means "to the end"
+
+
+def _batch_index(v, name: str) -> int:
+    """A batch index: an integer, or an integral float such as the reference docs' 1e10; negative is a ValueError."""
+    if isinstance(v, float):
+        if not math.isfinite(v) or not v.is_integer():
+            raise ValueError(f"{name} must be a whole number of batches, got {v!r}")
+        v = int(v)
+    else:
+        try:
+            v = operator.index(v)
+        except TypeError:
+            raise TypeError(f"{name} must be an integer, got {type(v).__name__}") from None
+    if v < 0:
+        raise ValueError(f"{name} must be >= 0, got {v}")
+    return min(v, _RANGE_MAX)
+
+
+def _indices_in_range(
+    what, entry, range_start, range_end, transmittances, means2d, rows, rows_tail, rows_name, opacities, image_width,
+    image_height, tile_size, isect_offsets, flatten_ids,
+):
+    rs, re_ = _batch_index(range_start, "range_start"), _batch_index(range_end, "range_end")
+    W, H = int(image_width), int(image_height)
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    if means2d.dim() < 2 or means2d.shape[-1] != 2:
+        raise ValueError(f"means2d must be [..., N, 2], got {tuple(means2d.shape)}")
+    image_dims, N = tuple(means2d.shape[:-2]), means2d.shape[-2]
+    _check_shape(rows, image_dims + (N,) + rows_tail, rows_name)
+    _check_shape(opacities, image_dims + (N,), "opacities")
+    _check_shape(transmittances, image_dims + (H, W), "transmittances")
+    if isect_offsets.dim() != means2d.dim() or tuple(isect_offsets.shape[:-2]) != image_dims:
+        raise ValueError(f"isect_offsets must be {image_dims + ('tile_height', 'tile_width')}, got {tuple(isect_offsets.shape)}")
+    th, tw = isect_offsets.shape[-2:]
+    if th * 16 < H or tw * 16 < W:
+        raise ValueError(f"isect_offsets tile grid {tw}x{th} does not cover a {W}x{H} image")
+    if flatten_ids.dim() != 1:
+        raise ValueError(f"flatten_ids must be one-dimensional, got {tuple(flatten_ids.shape)}")
+    if isect_offsets.dtype != torch.int32 or flatten_ids.dtype != torch.int32:
+        raise TypeError("isect_offsets and flatten_ids must be int32")
+    for t, name in ((transmittances, "transmittances"), (means2d, "means2d"), (rows, rows_name), (opacities, "opacities")):
+        if t.dtype != torch.float32:
+            raise TypeError(f"{name}: expected float32, got {t.dtype} (gsplat_b200 computes in fp32 only)")
+    dev = require_cuda(transmittances, means2d, rows, opacities, isect_offsets, flatten_ids)
+    I, S = _prod(image_dims), flatten_ids.shape[0]
+    P = I * H * W
+    if N == 0 or S == 0 or P == 0 or re_ <= rs:
+        return tuple(torch.empty(0, device=dev, dtype=torch.int64) for _ in range(3))
+    tr, m2, rw, op = (t.contiguous() for t in (transmittances, means2d, rows, opacities))
+    off, fl = isect_offsets.contiguous(), flatten_ids.contiguous()
+    L = lib()
+    ws = torch.empty(L.gsb200_indices_workspace_bytes(P), device=dev, dtype=torch.uint8)
+    total = torch.empty(1, device=dev, dtype=torch.int64)
+    fn = getattr(L, entry)
+    with _Ctx(dev) as st:
+
+        def run(emit, outs):
+            check(
+                fn(I, N, ptr(m2), ptr(rw), ptr(op), ptr(tr), W, H, 16, tw, th, ptr(off), ptr(fl), S, rs, re_, emit, ptr(ws),
+                   ws.numel(), ptr(total), *(ptr(o) for o in outs), st),
+                what,
+            )
+
+        run(0, (None, None, None))
+        M = int(total.item())  # the host sync between the two passes (reference: csrc/Rasterization.cpp:1050)
+        outs = tuple(torch.empty(M, device=dev, dtype=torch.int64) for _ in range(3))
+        if M > 0:
+            run(1, outs)
+    return outs
+
+
+@torch.no_grad()
+def rasterize_to_indices_in_range(
+    range_start: int,
+    range_end: int,
+    transmittances: Tensor,  # [..., image_height, image_width]
+    means2d: Tensor,  # [..., N, 2]
+    conics: Tensor,  # [..., N, 3]
+    opacities: Tensor,  # [..., N]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    isect_offsets: Tensor,  # [..., tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+) -> Tuple[Tensor, Tensor, Tensor]:
+    """The (gaussian, pixel) pairs ``rasterize_to_pixels`` composites when every pixel starts from its transmittance
+    and walks only the batches ``[range_start, range_end)`` of ``tile_size**2`` gaussians of its tile's depth-sorted list
+    (``range_end`` past the last batch, e.g. 1e10, means "to the end").  A gaussian that would bring the transmittance
+    to 1e-4 or below stops the pixel and is not returned.  The decisions are the compositing kernel's own.
+
+    Returns int64 ``(gaussian_ids, pixel_ids, image_ids)`` [M]: ``gaussian_ids`` in [0, N), ``pixel_ids`` row-major
+    within the image, ``image_ids`` the flattened image index; ordered by (image, row, col), front to back per pixel."""
+    return _indices_in_range(
+        "rasterize_to_indices_3dgs", "gsb200_raster_indices", range_start, range_end, transmittances, means2d, conics, (3,),
+        "conics", opacities, image_width, image_height, tile_size, isect_offsets, flatten_ids,
+    )
+
+
+@torch.no_grad()
+def rasterize_to_indices_in_range_2dgs(
+    range_start: int,
+    range_end: int,
+    transmittances: Tensor,  # [..., image_height, image_width]
+    means2d: Tensor,  # [..., N, 2]
+    ray_transforms: Tensor,  # [..., N, 3, 3]
+    opacities: Tensor,  # [..., N]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    isect_offsets: Tensor,  # [..., tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+) -> Tuple[Tensor, Tensor, Tensor]:
+    """``rasterize_to_indices_in_range`` for surfels: the pairs ``rasterize_to_pixels_2dgs`` composites, with the same
+    ranges, outputs and order."""
+    return _indices_in_range(
+        "rasterize_to_indices_2dgs", "gsb200_surfel_indices", range_start, range_end, transmittances, means2d,
+        ray_transforms, (3, 3), "ray_transforms", opacities, image_width, image_height, tile_size, isect_offsets, flatten_ids,
+    )
 
 
 # --------------------------------------------------------------------------------------------

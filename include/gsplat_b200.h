@@ -421,6 +421,33 @@ extern "C"
         float *v_normals, float *v_densify, float *v_means2d_abs, void *stream
     );
 
+    /* ---- rasterize_to_indices_in_range / _2dgs (_wrapper.py:2486, :3154; kernels
+     * csrc/RasterizeToIndices{3,2}DGSSerialBatch.cu, host csrc/Rasterization.cpp:954-1090) ----
+     * The (pixel, gaussian) pairs the compositing forward (gsb200_raster_fwd / gsb200_surfel_raster_fwd) composites when
+     * each pixel walks only the batches [range_start, range_end) of 256 records of its tile's list, starting from its
+     * transmittance (float32 [I,H,W]).  A pair whose next transmittance is <= 1e-4 stops the pixel and is not a pair.
+     * Dense rows: means2d [I,N,2], conics [I,N,3] / ray_transforms [I,N,3,3], opacities [I,N]; offsets [I,th,tw];
+     * tile_size must be 16.  range_start / range_end >= 0; range_end past every list means "to the end".
+     * Two calls with one workspace of gsb200_indices_workspace_bytes(I*H*W) bytes: emit = 0 counts every pixel's
+     * pairs and writes their total to total (device int64 [1]); the caller reads it, then emit = 1 writes gaussian_ids
+     * (flatten id % N), pixel_ids (row-major in the image) and image_ids, int64 [total], pixel-major over
+     * (image, row, col) and front to back within a pixel. */
+    size_t gsb200_indices_workspace_bytes(int64_t n_pixels);
+    int gsb200_raster_indices(
+        int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities,
+        const float *transmittances, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
+        uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t range_start,
+        int64_t range_end, int emit, void *workspace, size_t workspace_bytes, int64_t *total, int64_t *gaussian_ids,
+        int64_t *pixel_ids, int64_t *image_ids, void *stream
+    );
+    int gsb200_surfel_indices(
+        int64_t I, int64_t N, const float *means2d, const float *ray_transforms, const float *opacities,
+        const float *transmittances, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
+        uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t range_start,
+        int64_t range_end, int emit, void *workspace, size_t workspace_bytes, int64_t *total, int64_t *gaussian_ids,
+        int64_t *pixel_ids, int64_t *image_ids, void *stream
+    );
+
     /* ---- MCMC strategy ops ("next" row): relocation (ext.cpp `relocation`, gsplat/relocation.py:64,
      * csrc/RelocationCUDA.cu:36-80) and in-place position perturbation (csrc/MCMCPerturbCUDA.cu:28-60,
      * gsplat/strategy/ops.py).  ratios int32 [N] already clamped to [1, n_max]; binoms [n_max, n_max]. */

@@ -1,0 +1,34 @@
+#!/usr/bin/env python
+"""Write tests/golden/ref_signatures_indices.json: the parameter lists of the reference's rasterize_to_indices_in_range
+and rasterize_to_indices_in_range_2dgs (gsplat/cuda/_wrapper.py), parsed with ast from a gsplat source checkout.
+
+    python tests/golden/make_golden_indices.py GSPLAT_CHECKOUT      (the directory that holds gsplat/)
+
+tests/golden/make_ref_indices_golden.py records the reference op's outputs (ref_indices.npz) on a GPU.
+"""
+import ast
+import json
+import os
+import sys
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+NAMES = ("rasterize_to_indices_in_range", "rasterize_to_indices_in_range_2dgs")
+
+
+def main():
+    if len(sys.argv) != 2:
+        sys.exit(__doc__)
+    path = os.path.join(sys.argv[1], "gsplat", "cuda", "_wrapper.py")
+    out = {}
+    for node in ast.walk(ast.parse(open(path).read())):
+        if isinstance(node, ast.FunctionDef) and node.name in NAMES:
+            a = node.args
+            out[node.name] = {"params": [x.arg for x in a.posonlyargs + a.args + a.kwonlyargs], "n_defaults": len(a.defaults)}
+    assert sorted(out) == sorted(NAMES), f"found {sorted(out)} in {path}"
+    with open(os.path.join(HERE, "ref_signatures_indices.json"), "w") as f:
+        json.dump({"params": out}, f, indent=1)
+    print("wrote ref_signatures_indices.json")
+
+
+if __name__ == "__main__":
+    main()
