@@ -4,8 +4,11 @@ Public names mirror /root/reference/gsplat/__init__.py:19-104 for the hot path:
 rasterization, fully_fused_projection, spherical_harmonics, isect_tiles, isect_offset_encode,
 rasterize_to_pixels, quat_scale_to_covar_preci, the sparse-pixel ops build_sparse_tile_layout,
 isect_tiles_sparse, rasterize_to_pixels_sparse, and 2DGS: rasterization_2dgs, fully_fused_projection_2dgs,
-rasterize_to_pixels_2dgs (dense layout), and the pair queries rasterize_to_indices_in_range /
-rasterize_to_indices_in_range_2dgs.  Importing the package does not need a GPU; calling an
+rasterize_to_pixels_2dgs (dense layout), the pair queries rasterize_to_indices_in_range /
+rasterize_to_indices_in_range_2dgs, and the per-pixel contributor queries rasterize_num_contributing_gaussians,
+rasterize_contributing_gaussian_ids, rasterize_top_contributing_gaussian_ids and their _sparse forms (the pair query's
+walk with the compositing kernel's decisions: against the reference's ops they can differ only at pairs on the 1/255
+and 1e-4 thresholds).  Importing the package does not need a GPU; calling an
 operator does (and needs gsplat_b200/libgsplat_b200.so, built by ``python -m gsplat_b200.build``).
 """
 from .ops import (  # noqa: F401
@@ -20,11 +23,17 @@ from .ops import (  # noqa: F401
     isect_tiles,
     isect_tiles_sparse,
     quat_scale_to_covar_preci,
+    rasterize_contributing_gaussian_ids,
+    rasterize_contributing_gaussian_ids_sparse,
+    rasterize_num_contributing_gaussians,
+    rasterize_num_contributing_gaussians_sparse,
     rasterize_to_indices_in_range,
     rasterize_to_indices_in_range_2dgs,
     rasterize_to_pixels,
     rasterize_to_pixels_2dgs,
     rasterize_to_pixels_sparse,
+    rasterize_top_contributing_gaussian_ids,
+    rasterize_top_contributing_gaussian_ids_sparse,
     spherical_harmonics,
 )
 from .losses import l1_loss, ssim_loss  # noqa: F401
@@ -84,6 +93,12 @@ __all__ = [
     "rasterize_to_pixels_2dgs",
     "rasterize_to_indices_in_range",
     "rasterize_to_indices_in_range_2dgs",
+    "rasterize_num_contributing_gaussians",
+    "rasterize_num_contributing_gaussians_sparse",
+    "rasterize_contributing_gaussian_ids",
+    "rasterize_contributing_gaussian_ids_sparse",
+    "rasterize_top_contributing_gaussian_ids",
+    "rasterize_top_contributing_gaussian_ids_sparse",
     "quat_scale_to_covar_preci",
     "compute_relocation",
     "mcmc_perturb_positions",

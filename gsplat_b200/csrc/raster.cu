@@ -16,6 +16,7 @@
 //    (exact: the skipped pairs are `continue`d by the reference too); finished warps drop out by ballot;
 //  * the backward walks the same ring back to front and reduces each gaussian's gradients over a warp's
 //    pixels in two phases, pixel-major then gaussian-major (raster_bwd2_kernel).
+#include <algorithm>
 #include <mutex>
 
 #include "common.cuh"
@@ -1000,25 +1001,166 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------
-// rasterize_to_indices_in_range: the (pixel, gaussian) pairs the forward composites, walking only the kIndexBatch-record
-// batches [b0, b1) of each tile's list from the pixel's given transmittance.  One CTA per tile, each batch's records
-// built by row_record and staged in shared memory; every decision is raster_fwd_kernel's: its warp -> 8x4 pixel block
-// mapping, block_may_touch, pair_vis and its alpha, threshold and stop expressions.  EMIT = false writes every pixel's
-// pair count; EMIT = true writes its pairs, front to back, from its scanned start.
-template<bool EMIT>
+// The pair-query walk: which (pixel, gaussian) pairs the forward composites, walking only the kIndexBatch-record
+// batches [b0, b1) of each tile's list from the pixel's given transmittance (null: T = 1).  One CTA per tile of the pixel
+// policy (DensePixels: every tile of the [I, th, tw] grid; SparsePixels: every active tile, its live pixels only), each
+// batch's records built by row_record and staged in shared memory; every decision is raster_fwd_kernel's: its
+// warp -> 8x4 pixel block mapping, block_may_touch, pair_vis and its alpha, threshold and stop expressions.  What the
+// walk does with a pixel's pairs is the Sink's:
+//   begin(live, pix, pix_in, image_id)  once per lane (pix: the output row, pix_in: the row-major pixel in its image)
+//   pair(k, g, w)                        the pixel's k-th pair: flatten id g, weight w = alpha * T before the pair
+//   end(pix, count, T)                   once per live pixel, after the walk
+struct CountSink // rasterize_to_indices_in_range's count pass and rasterize_num_contributing_gaussians
+{
+    int32_t *counts; // [rows] pairs per pixel
+    float *alphas;   // [rows] 1 - final T, or null
+    __device__ __forceinline__ void begin(bool, int64_t, int64_t, int) {}
+    __device__ __forceinline__ void pair(int32_t, int32_t, float) {}
+    __device__ __forceinline__ void end(int64_t pix, int32_t count, float T) const
+    {
+        counts[pix] = count;
+        if(alphas != nullptr)
+            alphas[pix] = 1.0f - T;
+    }
+};
+
+struct PairSink // rasterize_to_indices_in_range's emit pass: the pairs from the pixel's scanned start
+{
+    int64_t N;
+    const int64_t *starts;
+    int64_t *gaussian_ids, *pixel_ids, *image_ids;
+    int64_t base, pix_in;
+    int image_id;
+    __device__ __forceinline__ void begin(bool live, int64_t pix, int64_t in_image, int image)
+    {
+        base     = live ? starts[pix] : 0;
+        pix_in   = in_image;
+        image_id = image;
+    }
+    __device__ __forceinline__ void pair(int32_t k, int32_t g, float) const
+    {
+        gaussian_ids[base + k] = (int64_t)g % N;
+        pixel_ids[base + k]    = pix_in;
+        image_ids[base + k]    = image_id;
+    }
+    __device__ __forceinline__ void end(int64_t, int32_t, float) const {}
+};
+
+// rasterize_contributing_gaussian_ids: the first K pairs of a pixel at [pix, k] (later ones are dropped, as the
+// reference drops them), -1 / 0 after its last pair; nothing outside the pixel's row of K.
+struct IdsSink
+{
+    int32_t N, K;
+    int32_t *ids;   // [rows, K] g % N
+    float *weights; // [rows, K] alpha * T before the pair
+    int64_t row;
+    __device__ __forceinline__ void begin(bool, int64_t pix, int64_t, int) { row = pix * K; }
+    __device__ __forceinline__ void pair(int32_t k, int32_t g, float w) const
+    {
+        if(k < K)
+        {
+            ids[row + k]     = g % N;
+            weights[row + k] = w;
+        }
+    }
+    __device__ __forceinline__ void end(int64_t, int32_t count, float) const
+    {
+        for(int32_t k = count < K ? count : K; k < K; ++k)
+        {
+            ids[row + k]     = -1;
+            weights[row + k] = 0.f;
+        }
+    }
+};
+
+// rasterize_top_contributing_gaussian_ids: K slots per pixel in dynamic shared memory ({id, weight, walk position},
+// slot k of thread t at [k * kIndexBatch + t]: conflict-free).  The reference's rule: empty slots hold -1, 0, +inf; a
+// pair replaces the lowest-weight slot (the first on ties) only when strictly heavier; at the end the slots are sorted
+// by walk position (stable), i.e. front to back with the empty ones last.
+struct TopSink
+{
+    static constexpr size_t kSlotBytes = sizeof(int32_t) + sizeof(float) + sizeof(uint32_t);
+    int32_t N, K;
+    int32_t *ids;   // [rows, K]
+    float *weights; // [rows, K]
+    int64_t row;
+    int32_t *s_id;
+    float *s_w;
+    uint32_t *s_pos;
+    __device__ __forceinline__ void begin(bool, int64_t pix, int64_t, int)
+    {
+        extern __shared__ __align__(16) int32_t s_top_slots[];
+        const size_t plane = (size_t)K * kIndexBatch;
+        s_id  = s_top_slots + threadIdx.x;
+        s_w   = reinterpret_cast<float *>(s_top_slots + plane) + threadIdx.x;
+        s_pos = reinterpret_cast<uint32_t *>(s_top_slots + 2 * plane) + threadIdx.x;
+        row   = pix * K;
+        for(int32_t k = 0; k < K; ++k)
+        {
+            s_id[k * kIndexBatch]  = -1;
+            s_w[k * kIndexBatch]   = 0.f;
+            s_pos[k * kIndexBatch] = 0xffffffffu;
+        }
+    }
+    __device__ __forceinline__ void pair(int32_t k, int32_t g, float w) const
+    {
+        int32_t m = 0;
+        float wm  = s_w[0];
+        for(int32_t j = 1; j < K; ++j)
+        {
+            const float v = s_w[j * kIndexBatch];
+            if(v < wm)
+            {
+                wm = v;
+                m  = j;
+            }
+        }
+        if(w > wm)
+        {
+            s_w[m * kIndexBatch]   = w;
+            s_id[m * kIndexBatch]  = g % N;
+            s_pos[m * kIndexBatch] = (uint32_t)k;
+        }
+    }
+    __device__ __forceinline__ void end(int64_t, int32_t, float) const
+    {
+        for(int32_t i = 1; i < K; ++i)
+        {
+            const uint32_t p = s_pos[i * kIndexBatch];
+            const float w    = s_w[i * kIndexBatch];
+            const int32_t id = s_id[i * kIndexBatch];
+            int32_t j        = i - 1;
+            for(; j >= 0 && s_pos[j * kIndexBatch] > p; --j)
+            {
+                s_pos[(j + 1) * kIndexBatch] = s_pos[j * kIndexBatch];
+                s_w[(j + 1) * kIndexBatch]   = s_w[j * kIndexBatch];
+                s_id[(j + 1) * kIndexBatch]  = s_id[j * kIndexBatch];
+            }
+            s_pos[(j + 1) * kIndexBatch] = p;
+            s_w[(j + 1) * kIndexBatch]   = w;
+            s_id[(j + 1) * kIndexBatch]  = id;
+        }
+        for(int32_t k = 0; k < K; ++k)
+        {
+            ids[row + k]     = s_id[k * kIndexBatch];
+            weights[row + k] = s_w[k * kIndexBatch];
+        }
+    }
+};
+
+template<class Sink, class Pix = DensePixels>
 __global__ void __launch_bounds__(kWarps * 32) raster_indices_kernel(
-    const uint32_t I, const int64_t N, const int64_t n_isects, const float *__restrict__ means2d,
-    const float *__restrict__ conics, const float *__restrict__ opacities, const float *__restrict__ transmittances,
-    const uint32_t W, const uint32_t H, const uint32_t tw, const uint32_t th, const int32_t *__restrict__ offsets,
-    const int32_t *__restrict__ flatten_ids, const int32_t b0, const int32_t b1, int32_t *__restrict__ counts,
-    const int64_t *__restrict__ starts, int64_t *__restrict__ gaussian_ids, int64_t *__restrict__ pixel_ids,
-    int64_t *__restrict__ image_ids
+    const uint32_t I, const int64_t n_isects, const float *__restrict__ means2d, const float *__restrict__ conics,
+    const float *__restrict__ opacities, const float *__restrict__ transmittances, const uint32_t W, const uint32_t H,
+    const uint32_t tw, const uint32_t th, const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids,
+    const int32_t b0, const int32_t b1, Sink sink, const Pix pixmap = Pix{}
 )
 {
     static_assert(kWarps * 32 == kIndexBatch, "one record of a batch per thread");
     __shared__ float4 s_cull[kIndexBatch], s_axis[kIndexBatch], s_geom[kIndexBatch];
     __shared__ int32_t s_id[kIndexBatch];
-    const TileGeom tg   = decode_block(blockIdx.x, tw, th);
+    uint32_t ord;
+    const TileGeom tg   = block_tile(nullptr, tw, th, pixmap, ord);
     const unsigned tid  = threadIdx.x;
     const unsigned warp = tid >> 5, lane = tid & 31;
     const int bx0 = tg.tile_x * kTile + (warp & 1) * 8;
@@ -1026,18 +1168,30 @@ __global__ void __launch_bounds__(kWarps * 32) raster_indices_kernel(
     const int px_i = bx0 + (lane & 7), py_i = by0 + (lane >> 3);
     const float px = (float)px_i + 0.5f, py = (float)py_i + 0.5f;
     const float cx = (float)bx0 + 4.0f, cy = (float)by0 + 2.0f;
-    const bool inside      = (px_i < (int)W) && (py_i < (int)H);
-    const int64_t pix_in   = (int64_t)py_i * W + px_i;
-    const int64_t pix      = (int64_t)tg.image_id * H * W + pix_in;
-    const int64_t tile_lin = (int64_t)tg.image_id * tw * th + tg.tile_id;
-    const int32_t range_start = offsets[tile_lin];
-    const int32_t range_end   = (tile_lin == (int64_t)I * tw * th - 1) ? (int32_t)n_isects : offsets[tile_lin + 1];
-    const int b_end           = min(b1, (range_end - range_start + kIndexBatch - 1) / kIndexBatch);
+    const int64_t pix_in = (int64_t)py_i * W + px_i;
+    bool inside;
+    int64_t pix;
+    int32_t range_start, range_end;
+    if constexpr(Pix::kSparse)
+    {
+        pix         = pixmap.slot(ord, (int)(((warp >> 1) * 4 + (lane >> 3)) * kTile + (warp & 1) * 8 + (lane & 7)), inside);
+        range_start = offsets[ord];
+        range_end   = offsets[ord + 1];
+    }
+    else
+    {
+        inside                 = (px_i < (int)W) && (py_i < (int)H);
+        pix                    = (int64_t)tg.image_id * H * W + pix_in;
+        const int64_t tile_lin = (int64_t)tg.image_id * tw * th + tg.tile_id;
+        range_start            = offsets[tile_lin];
+        range_end              = (tile_lin == (int64_t)I * tw * th - 1) ? (int32_t)n_isects : offsets[tile_lin + 1];
+    }
+    const int b_end = min(b1, (range_end - range_start + kIndexBatch - 1) / kIndexBatch);
 
-    float T        = inside ? transmittances[pix] : 1.f;
-    bool done      = !inside;
-    int32_t cnt    = 0;
-    const int64_t base = (EMIT && inside) ? starts[pix] : 0;
+    float T     = (inside && transmittances != nullptr) ? transmittances[pix] : 1.f;
+    bool done   = !inside;
+    int32_t cnt = 0;
+    sink.begin(inside, pix, pix_in, tg.image_id);
     for(int b = b0; b < b_end; ++b)
     {
         if(__syncthreads_count(done) == kIndexBatch)
@@ -1079,12 +1233,7 @@ __global__ void __launch_bounds__(kWarps * 32) raster_indices_kernel(
                         done = true; // exclusive of the current gaussian
                     else
                     {
-                        if constexpr(EMIT)
-                        {
-                            gaussian_ids[base + cnt] = (int64_t)s_id[t] % N;
-                            pixel_ids[base + cnt]    = pix_in;
-                            image_ids[base + cnt]    = tg.image_id;
-                        }
+                        sink.pair(cnt, s_id[t], alpha * T);
                         ++cnt;
                         T = next_T;
                     }
@@ -1092,8 +1241,8 @@ __global__ void __launch_bounds__(kWarps * 32) raster_indices_kernel(
             }
         }
     }
-    if(!EMIT && inside)
-        counts[pix] = cnt;
+    if(inside)
+        sink.end(pix, cnt, T);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1471,12 +1620,134 @@ extern "C" int gsb200_raster_indices(
         I, N, image_width, image_height, tile_size, tile_width, tile_height, n_isects, range_start, range_end, inputs_ok, emit,
         workspace, workspace_bytes, total, gaussian_ids && pixel_ids && image_ids, st,
         [&](unsigned n_tiles, int32_t b0, int32_t b1, const gsb::PixelCounts &pc) {
-            auto kernel = emit ? gsb::raster_indices_kernel<true> : gsb::raster_indices_kernel<false>;
-            kernel<<<n_tiles, gsb::kWarps * 32, 0, st>>>(
-                (uint32_t)I, N, n_isects, means2d, conics, opacities, transmittances, image_width, image_height, tile_width,
-                tile_height, offsets, flatten_ids, b0, b1, pc.counts, pc.starts, gaussian_ids, pixel_ids, image_ids
-            );
-            return gsb::check_launch();
+            auto launch = [&](auto sink) {
+                gsb::raster_indices_kernel<<<n_tiles, gsb::kWarps * 32, 0, st>>>(
+                    (uint32_t)I, n_isects, means2d, conics, opacities, transmittances, image_width, image_height, tile_width,
+                    tile_height, offsets, flatten_ids, b0, b1, sink
+                );
+                return gsb::check_launch();
+            };
+            if(emit)
+                return launch(gsb::PairSink{N, pc.starts, gaussian_ids, pixel_ids, image_ids});
+            return launch(gsb::CountSink{pc.counts, nullptr});
         }
     );
 }
+
+// ---- per-pixel contributor queries: the full walk from T = 1 with one sink, over every tile (dense) or over the active
+// tiles of a sparse layout (active_tiles != null).  The checks run in run_index_pass's order with its return codes;
+// every pixel is written, also when there are no intersections.
+namespace gsb
+{
+template<class Sink>
+static int run_contrib(
+    int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities, uint32_t W, uint32_t H,
+    uint32_t tile_size, uint32_t tw, uint32_t th, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects,
+    int64_t n_active, const int32_t *active_tiles, const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum,
+    const int64_t *pixel_map, bool outputs_ok, size_t smem, const Sink &sink, cudaStream_t st
+)
+{
+    const bool sparse = active_tiles != nullptr;
+    if(I < 0 || N < 0 || n_isects < 0 || n_active < 0)
+        return GSB200_E_INVALID;
+    if(tile_size != (uint32_t)kTile)
+        return GSB200_E_UNSUPPORTED;
+    const int64_t n_tiles = sparse ? n_active : I * (int64_t)tw * th;
+    if(n_tiles == 0 || W == 0 || H == 0)
+        return GSB200_OK; // no pixels
+    const bool inputs_ok = offsets && (n_isects == 0 || (means2d && conics && opacities && flatten_ids))
+                        && (!sparse || (tile_pixel_mask && tile_pixel_cumsum && pixel_map));
+    if(!inputs_ok || !outputs_ok || !tile_grid_covers(tw, th, W, H))
+        return GSB200_E_INVALID;
+    if(n_tiles >= 2147483648LL || n_isects >= 2147483648LL)
+        return GSB200_E_UNSUPPORTED;
+    auto launch = [&](auto kernel, const auto &pm) {
+        if(smem > 0)
+            GSB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kernel<<<(unsigned)n_tiles, kWarps * 32, smem, st>>>(
+            (uint32_t)I, n_isects, means2d, conics, opacities, nullptr, W, H, tw, th, offsets, flatten_ids, 0, 0x7fffffff,
+            sink, pm
+        );
+        return check_launch();
+    };
+    if(sparse)
+        return launch(raster_indices_kernel<Sink, SparsePixels>, SparsePixels{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map});
+    return launch(raster_indices_kernel<Sink, DensePixels>, DensePixels{});
+}
+
+// largest K of the top-K query on the current device: its opt-in shared memory per block, less the kernels' staging
+// arrays, over the K slots of every thread
+static int contrib_max_samples()
+{
+    int dev = 0, optin = 0;
+    GSB_CUDA_TRY(cudaGetDevice(&dev));
+    GSB_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    size_t staging = 0;
+    for(const void *k : {(const void *)raster_indices_kernel<TopSink, DensePixels>, (const void *)raster_indices_kernel<TopSink, SparsePixels>})
+    {
+        cudaFuncAttributes a;
+        GSB_CUDA_TRY(cudaFuncGetAttributes(&a, k));
+        staging = std::max(staging, a.sharedSizeBytes);
+    }
+    if((size_t)optin <= staging)
+        return 0;
+    return (int)(((size_t)optin - staging) / ((size_t)kIndexBatch * TopSink::kSlotBytes));
+}
+} // namespace gsb
+
+#define GSB200_CONTRIB_ARGS                                                                                              \
+    I, N, means2d, conics, opacities, image_width, image_height, tile_size, tile_width, tile_height, offsets, flatten_ids, \
+        n_isects, n_active, active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map
+
+extern "C" int gsb200_contrib_max_samples(void)
+{
+    return gsb::contrib_max_samples();
+}
+
+extern "C" int gsb200_contrib_count(
+    int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities, uint32_t image_width,
+    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+    const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int32_t *counts,
+    float *alphas, void *stream
+)
+{
+    return gsb::run_contrib(GSB200_CONTRIB_ARGS, counts != nullptr, 0, gsb::CountSink{counts, alphas}, (cudaStream_t)stream);
+}
+
+extern "C" int gsb200_contrib_ids(
+    int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities, uint32_t image_width,
+    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+    const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int max_samples,
+    int32_t *ids, float *weights, void *stream
+)
+{
+    if(max_samples < 0 || N > 0x7fffffffLL)
+        return GSB200_E_INVALID;
+    if(max_samples == 0)
+        return GSB200_OK;
+    const gsb::IdsSink sink{(int32_t)N, max_samples, ids, weights, 0};
+    return gsb::run_contrib(GSB200_CONTRIB_ARGS, ids && weights, 0, sink, (cudaStream_t)stream);
+}
+
+extern "C" int gsb200_contrib_top(
+    int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities, uint32_t image_width,
+    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+    const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int num_samples,
+    int32_t *ids, float *weights, void *stream
+)
+{
+    if(num_samples <= 0 || N > 0x7fffffffLL)
+        return GSB200_E_INVALID;
+    const int bound = gsb::contrib_max_samples();
+    if(bound < 0)
+        return bound;
+    if(num_samples > bound)
+        return GSB200_E_UNSUPPORTED;
+    const gsb::TopSink sink{(int32_t)N, num_samples, ids, weights, 0, nullptr, nullptr, nullptr};
+    const size_t smem = (size_t)num_samples * gsb::kIndexBatch * gsb::TopSink::kSlotBytes;
+    return gsb::run_contrib(GSB200_CONTRIB_ARGS, ids && weights, smem, sink, (cudaStream_t)stream);
+}
+#undef GSB200_CONTRIB_ARGS

@@ -10,6 +10,9 @@ executable form).  ``apply()`` rebinds, in place, the names the reference's call
   gsplat.cuda._wrapper.{fully_fused_projection_2dgs, rasterize_to_pixels_2dgs} (_wrapper.py:2633,2918)
   gsplat.cuda._wrapper.{rasterize_to_indices_in_range,
                         rasterize_to_indices_in_range_2dgs}                  (_wrapper.py:2486,3154)
+  gsplat.cuda._wrapper.{rasterize_num_contributing_gaussians,
+                        rasterize_contributing_gaussian_ids,
+                        rasterize_top_contributing_gaussian_ids, + _sparse}  (_wrapper.py:1668-2008)
   gsplat.<the same re-exports>                                               (__init__.py:23-62)
   gsplat.relocation.compute_relocation (+ its import in gsplat.strategy.ops) (relocation.py:25, strategy/ops.py:26)
   gsplat.strategy.ops._cuda_fused_mcmc_perturb                               (strategy/ops.py:405)
@@ -50,6 +53,15 @@ _OPS = (
 _OPS_2DGS = ("fully_fused_projection_2dgs", "rasterize_to_pixels_2dgs")
 # the pair queries, rebound only where the package has them: the pairs are then those this library's compositing renders
 _OPS_INDICES = ("rasterize_to_indices_in_range", "rasterize_to_indices_in_range_2dgs")
+# the per-pixel contributor queries, likewise: their counts, ids and weights are then those of this library's render
+_OPS_CONTRIB = (
+    "rasterize_num_contributing_gaussians",
+    "rasterize_num_contributing_gaussians_sparse",
+    "rasterize_contributing_gaussian_ids",
+    "rasterize_contributing_gaussian_ids_sparse",
+    "rasterize_top_contributing_gaussian_ids",
+    "rasterize_top_contributing_gaussian_ids_sparse",
+)
 
 _saved: List[Tuple[object, str, object]] = []
 
@@ -103,13 +115,13 @@ def apply(losses: bool = True, ops: bool = True) -> Dict[str, object]:
         _apply_ops(B, G)
     if losses:
         _apply_losses(G)
-    return {"package": G.__file__, "ops": (list(_OPS + _OPS_2DGS + _OPS_INDICES) + ["adam", "rasterization", "rasterization_2dgs", "compute_relocation"]) if ops else [], "losses": losses}
+    return {"package": G.__file__, "ops": (list(_OPS + _OPS_2DGS + _OPS_INDICES + _OPS_CONTRIB) + ["adam", "rasterization", "rasterization_2dgs", "compute_relocation"]) if ops else [], "losses": losses}
 
 
 def _apply_ops(B, G) -> None:
     W = importlib.import_module("gsplat.cuda._wrapper")
     R = importlib.import_module("gsplat.rendering")
-    for name in _OPS + tuple(n for n in _OPS_2DGS + _OPS_INDICES if hasattr(W, n)):
+    for name in _OPS + tuple(n for n in _OPS_2DGS + _OPS_INDICES + _OPS_CONTRIB if hasattr(W, n)):
         fn = _delegating(name, getattr(B, name), getattr(W, name))
         _set(W, name, fn)
         if hasattr(G, name):

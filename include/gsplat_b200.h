@@ -448,6 +448,45 @@ extern "C"
         int64_t *pixel_ids, int64_t *image_ids, void *stream
     );
 
+    /* ---- per-pixel contributor queries: rasterize_num_contributing_gaussians, rasterize_contributing_gaussian_ids,
+     * rasterize_top_contributing_gaussian_ids and their _sparse forms (_wrapper.py:1668-2008, host
+     * csrc/Rasterization.cpp:1380-1620).  Each pixel walks its tile's full list from T = 1 with the decisions of
+     * gsb200_raster_indices (and so of gsb200_raster_fwd).  Rows: means2d [R,2], conics [R,3], opacities [R]; ids are
+     * flatten id % N (dense rows [I,N,*]: the gaussian index; packed rows [nnz,*]: pass N = nnz, the row index).
+     * Dense: offsets [I,th,tw], active_tiles = null, outputs row (image, y, x) of I*H*W.  Sparse (active_tiles non-null):
+     * the layout of gsb200_sparse_layout_* and the per-active-tile offsets [n_active + 1] of gsb200_isect_sparse_emit,
+     * outputs row = the pixel's index in the caller's list [P].  tile_size must be 16.  Every pixel is written.
+     *   count: counts int32 [rows] contributing pairs, alphas float32 [rows] (nullable) 1 - final T.
+     *   ids:   ids int32 / weights float32 [rows, max_samples]: the first max_samples pairs front to back (later ones
+     *          are dropped), weight alpha * T before the pair; -1 / 0 after a pixel's last pair.
+     *   top:   ids / weights [rows, num_samples]: the num_samples heaviest pairs (a pair replaces the lightest slot,
+     *          the first on ties, only when strictly heavier), front to back, -1 / 0 for empty slots.  num_samples must
+     *          lie in [1, gsb200_contrib_max_samples()] (GSB200_E_UNSUPPORTED above it).
+     * gsb200_contrib_max_samples: the largest num_samples the current device's opt-in shared memory per block holds, or
+     * GSB200_E_CUDA without a device. */
+    int gsb200_contrib_max_samples(void);
+    int gsb200_contrib_count(
+        int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities, uint32_t image_width,
+        uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+        const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int32_t *counts,
+        float *alphas, void *stream
+    );
+    int gsb200_contrib_ids(
+        int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities, uint32_t image_width,
+        uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+        const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int max_samples,
+        int32_t *ids, float *weights, void *stream
+    );
+    int gsb200_contrib_top(
+        int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities, uint32_t image_width,
+        uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+        const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int num_samples,
+        int32_t *ids, float *weights, void *stream
+    );
+
     /* ---- MCMC strategy ops ("next" row): relocation (ext.cpp `relocation`, gsplat/relocation.py:64,
      * csrc/RelocationCUDA.cu:36-80) and in-place position perturbation (csrc/MCMCPerturbCUDA.cu:28-60,
      * gsplat/strategy/ops.py).  ratios int32 [N] already clamped to [1, n_max]; binoms [n_max, n_max]. */

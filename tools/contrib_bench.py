@@ -1,0 +1,82 @@
+"""Times the per-pixel contributor queries on bench.py's scene (the garden crop tiled 3 x 3, 1M Gaussians, one
+1920x1080 view, seed 42): rasterize_num_contributing_gaussians, rasterize_contributing_gaussian_ids,
+rasterize_top_contributing_gaussian_ids with K = 8 and 32, and the three _sparse forms on 4096 seeded pixels, with one
+rasterize_to_pixels forward on the same intersections for scale.
+
+    python tools/contrib_bench.py [--steps 20] [--warmup 5]
+
+Each call is timed with CUDA events after `warmup` untimed calls; the ids query includes its host read of the largest
+count.  Projection, tile intersection and the sparse layout run once, outside the timed calls.  Prints one JSON line
+with the median times (ms), the pair count, and the device name and power limit.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
+sys.path.insert(0, ROOT)
+
+import gsplat_b200 as gs  # noqa: E402
+from tests import scene  # noqa: E402
+from tools.indices_bench import device_info, timed  # noqa: E402
+
+W, H, SCENE_GRID, N_SPARSE = 1920, 1080, 3, 4096
+TW, TH = (W + 15) // 16, (H + 15) // 16
+
+
+def main() -> int:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("contrib_bench needs a GPU")
+    dev = "cuda:0"
+    sc = scene.make_scene(scene_grid=SCENE_GRID, sh_degree=0)
+    Ks = scene.rescale_K(sc["Ks"], sc["width"], sc["height"], W, H)[:1]
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)  # noqa: E731
+    vm = t(sc["viewmats"][:1])
+    opac = t(sc["opacities"])[None].contiguous()
+    colors = t(sc["colors"])[None].contiguous()
+    rec = {"image": f"{W}x{H}", "n_gaussians": int(sc["means"].shape[0]), "sparse_pixels": N_SPARSE, "steps": args.steps}
+    ms = lambda fn: timed(fn, args.steps, args.warmup)[0]  # noqa: E731
+    with torch.no_grad():
+        radii, m2, depths, conics, _ = gs.fully_fused_projection(t(sc["means"]), None, t(sc["quats"]), t(sc["scales"]), vm, t(Ks), W, H)
+        _, ids, fl = gs.isect_tiles(m2, radii, depths, 16, TW, TH, conics=conics, opacities=opac)
+        off = gs.isect_offset_encode(ids, 1, TW, TH)
+        a = (m2, conics, opac, off, fl, W, H, 16)
+        counts, _ = gs.rasterize_num_contributing_gaussians(*a)
+        rec["isects"] = int(fl.shape[0])
+        rec["pairs"] = int(counts.sum())
+        rec["max_count"] = int(counts.max())
+        rec["raster_fwd_ms"] = ms(lambda: gs.rasterize_to_pixels(m2, conics, colors, opac, W, H, 16, off, fl))
+        rec["num_ms"] = ms(lambda: gs.rasterize_num_contributing_gaussians(*a))
+        rec["ids_ms"] = ms(lambda: gs.rasterize_contributing_gaussian_ids(*a, counts))
+        for k in (8, 32):
+            rec[f"top{k}_ms"] = ms(lambda: gs.rasterize_top_contributing_gaussian_ids(*a, k))
+
+        rng = np.random.RandomState(42)
+        flat = rng.choice(W * H, N_SPARSE, replace=False)
+        pixels = t(np.stack([flat // W, flat % W], -1).astype(np.int32))
+        image_ids = torch.zeros(N_SPARSE, device=dev, dtype=torch.int32)
+        active, amask, words, cum, pmap = gs.build_sparse_tile_layout(pixels, image_ids, 1, 16, TW, TH)
+        s_off, s_fl = gs.isect_tiles_sparse(m2, radii, depths, amask, active, 1, 16, TW, TH)
+        s = (m2, conics, opac, active, s_off, s_fl, words, cum, pmap)
+        grid = (W, H, 16, TW, TH)
+        s_counts, _ = gs.rasterize_num_contributing_gaussians_sparse(*s, *grid)
+        rec["sparse_num_ms"] = ms(lambda: gs.rasterize_num_contributing_gaussians_sparse(*s, *grid))
+        rec["sparse_ids_ms"] = ms(lambda: gs.rasterize_contributing_gaussian_ids_sparse(*s, s_counts, *grid))
+        rec["sparse_top8_ms"] = ms(lambda: gs.rasterize_top_contributing_gaussian_ids_sparse(*s, *grid, 8))
+    rec.update(device_info())
+    print(json.dumps(rec), flush=True)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
