@@ -1006,45 +1006,7 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
 // policy (DensePixels: every tile of the [I, th, tw] grid; SparsePixels: every active tile, its live pixels only), each
 // batch's records built by row_record and staged in shared memory; every decision is raster_fwd_kernel's: its
 // warp -> 8x4 pixel block mapping, block_may_touch, pair_vis and its alpha, threshold and stop expressions.  What the
-// walk does with a pixel's pairs is the Sink's:
-//   begin(live, pix, pix_in, image_id)  once per lane (pix: the output row, pix_in: the row-major pixel in its image)
-//   pair(k, g, w)                        the pixel's k-th pair: flatten id g, weight w = alpha * T before the pair
-//   end(pix, count, T)                   once per live pixel, after the walk
-struct CountSink // rasterize_to_indices_in_range's count pass and rasterize_num_contributing_gaussians
-{
-    int32_t *counts; // [rows] pairs per pixel
-    float *alphas;   // [rows] 1 - final T, or null
-    __device__ __forceinline__ void begin(bool, int64_t, int64_t, int) {}
-    __device__ __forceinline__ void pair(int32_t, int32_t, float) {}
-    __device__ __forceinline__ void end(int64_t pix, int32_t count, float T) const
-    {
-        counts[pix] = count;
-        if(alphas != nullptr)
-            alphas[pix] = 1.0f - T;
-    }
-};
-
-struct PairSink // rasterize_to_indices_in_range's emit pass: the pairs from the pixel's scanned start
-{
-    int64_t N;
-    const int64_t *starts;
-    int64_t *gaussian_ids, *pixel_ids, *image_ids;
-    int64_t base, pix_in;
-    int image_id;
-    __device__ __forceinline__ void begin(bool live, int64_t pix, int64_t in_image, int image)
-    {
-        base     = live ? starts[pix] : 0;
-        pix_in   = in_image;
-        image_id = image;
-    }
-    __device__ __forceinline__ void pair(int32_t k, int32_t g, float) const
-    {
-        gaussian_ids[base + k] = (int64_t)g % N;
-        pixel_ids[base + k]    = pix_in;
-        image_ids[base + k]    = image_id;
-    }
-    __device__ __forceinline__ void end(int64_t, int32_t, float) const {}
-};
+// walk does with a pixel's pairs is the Sink's (indices.cuh: CountSink, PairSink; below: IdsSink, TopSink).
 
 // rasterize_contributing_gaussian_ids: the first K pairs of a pixel at [pix, k] (later ones are dropped, as the
 // reference drops them), -1 / 0 after its last pair; nothing outside the pixel's row of K.
@@ -1618,18 +1580,13 @@ extern "C" int gsb200_raster_indices(
     const bool inputs_ok  = means2d && conics && opacities && transmittances && offsets && flatten_ids;
     return gsb::run_index_pass(
         I, N, image_width, image_height, tile_size, tile_width, tile_height, n_isects, range_start, range_end, inputs_ok, emit,
-        workspace, workspace_bytes, total, gaussian_ids && pixel_ids && image_ids, st,
-        [&](unsigned n_tiles, int32_t b0, int32_t b1, const gsb::PixelCounts &pc) {
-            auto launch = [&](auto sink) {
-                gsb::raster_indices_kernel<<<n_tiles, gsb::kWarps * 32, 0, st>>>(
-                    (uint32_t)I, n_isects, means2d, conics, opacities, transmittances, image_width, image_height, tile_width,
-                    tile_height, offsets, flatten_ids, b0, b1, sink
-                );
-                return gsb::check_launch();
-            };
-            if(emit)
-                return launch(gsb::PairSink{N, pc.starts, gaussian_ids, pixel_ids, image_ids});
-            return launch(gsb::CountSink{pc.counts, nullptr});
+        workspace, workspace_bytes, total, gaussian_ids, pixel_ids, image_ids, st,
+        [&](unsigned n_tiles, int32_t b0, int32_t b1, auto sink) {
+            gsb::raster_indices_kernel<<<n_tiles, gsb::kWarps * 32, 0, st>>>(
+                (uint32_t)I, n_isects, means2d, conics, opacities, transmittances, image_width, image_height, tile_width,
+                tile_height, offsets, flatten_ids, b0, b1, sink
+            );
+            return gsb::check_launch();
         }
     );
 }

@@ -452,15 +452,13 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_raster_fwd_kernel(
 
 // rasterize_to_indices_in_range_2dgs: the (pixel, surfel) pairs surfel_raster_fwd_kernel composites, walking only the
 // batches [b0, b1) of each tile's list from the pixel's given transmittance; the pixel mapping, staging, surf_eval and
-// the stop rule are the forward's.  EMIT = false writes every pixel's pair count; EMIT = true writes its pairs, front to
-// back, from its scanned start.
-template<bool EMIT>
+// the stop rule are the forward's.  What the walk does with a pixel's pairs is the Sink's (indices.cuh).
+template<class Sink>
 __global__ void __launch_bounds__(kSurfThreads) surfel_indices_kernel(
-    uint32_t I, int64_t N, const float *__restrict__ means2d, const float *__restrict__ rt, const float *__restrict__ opacities,
+    uint32_t I, const float *__restrict__ means2d, const float *__restrict__ rt, const float *__restrict__ opacities,
     const float *__restrict__ transmittances, uint32_t W, uint32_t H, uint32_t tw, uint32_t th,
     const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids, int64_t n_isects, int32_t b0, int32_t b1,
-    int32_t *__restrict__ counts, const int64_t *__restrict__ starts, int64_t *__restrict__ gaussian_ids,
-    int64_t *__restrict__ pixel_ids, int64_t *__restrict__ image_ids
+    Sink sink
 )
 {
     static_assert(kSurfThreads == kIndexBatch, "one record of a batch per thread");
@@ -479,10 +477,10 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_indices_kernel(
     const int64_t b_end  = min((int64_t)b1, (end - start + kSurfThreads - 1) / kSurfThreads);
     const float px = (float)j + 0.5f, py = (float)i + 0.5f;
 
-    float T            = inside ? transmittances[pix] : 1.f;
-    bool done          = !inside;
-    int32_t cnt        = 0;
-    const int64_t base = (EMIT && inside) ? starts[pix] : 0;
+    float T     = inside ? transmittances[pix] : 1.f;
+    bool done   = !inside;
+    int32_t cnt = 0;
+    sink.begin(inside, pix, pix_in, img);
     for(int64_t b = b0; b < b_end; ++b)
     {
         if(__syncthreads_count(done) == kSurfThreads)
@@ -503,18 +501,13 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_indices_kernel(
                 done = true;
                 break;
             }
-            if constexpr(EMIT)
-            {
-                gaussian_ids[base + cnt] = (int64_t)rec[t].id % N;
-                pixel_ids[base + cnt]    = pix_in;
-                image_ids[base + cnt]    = img;
-            }
+            sink.pair(cnt, rec[t].id, h.alpha * T);
             ++cnt;
             T = next_T;
         }
     }
-    if(!EMIT && inside)
-        counts[pix] = cnt;
+    if(inside)
+        sink.end(pix, cnt, T);
 }
 
 struct SurfGradDst
@@ -522,8 +515,44 @@ struct SurfGradDst
     float *means2d, *rt, *colors, *opacities, *normals, *densify, *abs;
 };
 
+// Butterfly-reduces gv[OFF, OFF + 32) across the warp and adds each owned slot to its gradient row; recurses over the
+// remaining 32-value chunks (a lane owns at most one slot of a chunk).
 template<int OFF, int NV>
-__device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, const SurfRec &r, const SurfGradDst &dst, int CDIM);
+__device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, const SurfRec &r, const SurfGradDst &dst, int CDIM)
+{
+    constexpr int M = (NV - OFF) < 32 ? (NV - OFF) : 32;
+    float v[M];
+#pragma unroll
+    for(int k = 0; k < M; ++k)
+        v[k] = gv[OFF + k];
+    Butterfly<M, 16>::run(v, lane);
+    const int s = butterfly_slot<M>(lane);
+    if(s >= 0 && v[0] != 0.f)
+    {
+        const int slot  = OFF + s;
+        const int64_t g = r.id;
+        const float val = v[0];
+        if(slot < CDIM)
+            atomicAdd(dst.colors + g * CDIM + slot, val);
+        else if(slot < CDIM + 3)
+            atomicAdd(dst.normals + g * 3 + (slot - CDIM), val);
+        else if(slot < CDIM + 12)
+        {
+            const int e = slot - CDIM - 3;
+            atomicAdd(dst.rt + g * 9 + e, val);
+            if(e == 2 || e == 5)
+                atomicAdd(dst.densify + g * 2 + (e == 5), val * r.m[8]);
+        }
+        else if(slot < CDIM + 14)
+            atomicAdd(dst.means2d + g * 2 + (slot - CDIM - 12), val);
+        else if(slot == CDIM + 14)
+            atomicAdd(dst.opacities + g, val);
+        else if(dst.abs)
+            atomicAdd(dst.abs + g * 2 + (slot - CDIM - 15), val);
+    }
+    if constexpr(OFF + 32 < NV)
+        reduce_emit<OFF + 32, NV>(gv, lane, r, dst, CDIM);
+}
 
 // Back to front over each tile's list.  Per gaussian, the warp's per-pixel gradients (colours, normals, ray transform,
 // screen mean, opacity, |screen mean|) are butterfly-reduced and added with one atomic per value; v_densify is the
@@ -701,78 +730,15 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_raster_bwd_kernel(
     }
 }
 
-// Butterfly-reduces gv[OFF, OFF + 32) across the warp and adds each owned slot to its gradient row; recurses over the
-// remaining 32-value chunks (a lane owns at most one slot of a chunk).
-template<int OFF, int NV>
-__device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, const SurfRec &r, const SurfGradDst &dst, int CDIM)
+// The checks both compositing entries make last, in this order: the tile grid covers the image, and the flattened
+// row and tile indices fit in int32.
+int surfel_raster_limits(int64_t I, int64_t N, uint32_t W, uint32_t H, uint32_t tw, uint32_t th)
 {
-    constexpr int M = (NV - OFF) < 32 ? (NV - OFF) : 32;
-    float v[M];
-#pragma unroll
-    for(int k = 0; k < M; ++k)
-        v[k] = gv[OFF + k];
-    Butterfly<M, 16>::run(v, lane);
-    const int s = butterfly_slot<M>(lane);
-    if(s >= 0 && v[0] != 0.f)
-    {
-        const int slot  = OFF + s;
-        const int64_t g = r.id;
-        const float val = v[0];
-        {
-            {
-                if(slot < CDIM)
-                    atomicAdd(dst.colors + g * CDIM + slot, val);
-                else if(slot < CDIM + 3)
-                    atomicAdd(dst.normals + g * 3 + (slot - CDIM), val);
-                else if(slot < CDIM + 12)
-                {
-                    const int e = slot - CDIM - 3;
-                    atomicAdd(dst.rt + g * 9 + e, val);
-                    if(e == 2 || e == 5)
-                        atomicAdd(dst.densify + g * 2 + (e == 5), val * r.m[8]);
-                }
-                else if(slot < CDIM + 14)
-                    atomicAdd(dst.means2d + g * 2 + (slot - CDIM - 12), val);
-                else if(slot == CDIM + 14)
-                    atomicAdd(dst.opacities + g, val);
-                else if(dst.abs)
-                    atomicAdd(dst.abs + g * 2 + (slot - CDIM - 15), val);
-            }
-        }
-    }
-    if constexpr(OFF + 32 < NV)
-        reduce_emit<OFF + 32, NV>(gv, lane, r, dst, CDIM);
-}
-
-template<int CDIM>
-int launch_surfel_fwd(
-    uint32_t I, const float *means2d, const float *rt, const float *colors, const float *opacities, const float *normals,
-    const float *backgrounds, const uint8_t *masks, uint32_t W, uint32_t H, uint32_t tw, uint32_t th, const int32_t *offsets,
-    const int32_t *flatten_ids, int64_t n_isects, float *rc, float *ra, float *rn, float *rd, float *rm, int32_t *last_ids,
-    int32_t *median_ids, cudaStream_t st
-)
-{
-    surfel_raster_fwd_kernel<CDIM><<<I * tw * th, kSurfThreads, 0, st>>>(
-        I, means2d, rt, colors, opacities, normals, backgrounds, masks, W, H, tw, th, offsets, flatten_ids, n_isects, rc, ra, rn,
-        rd, rm, last_ids, median_ids
-    );
-    return check_launch();
-}
-
-template<int CDIM>
-int launch_surfel_bwd(
-    uint32_t I, const float *means2d, const float *rt, const float *colors, const float *opacities, const float *normals,
-    const float *backgrounds, const uint8_t *masks, uint32_t W, uint32_t H, uint32_t tw, uint32_t th, const int32_t *offsets,
-    const int32_t *flatten_ids, int64_t n_isects, const float *rc, const float *ra, const int32_t *last_ids,
-    const int32_t *median_ids, const float *v_rc, const float *v_ra, const float *v_rn, const float *v_rd, const float *v_rm,
-    const SurfGradDst &dst, cudaStream_t st
-)
-{
-    surfel_raster_bwd_kernel<CDIM><<<I * tw * th, kSurfThreads, 0, st>>>(
-        I, means2d, rt, colors, opacities, normals, backgrounds, masks, W, H, tw, th, offsets, flatten_ids, n_isects, rc, ra,
-        last_ids, median_ids, v_rc, v_ra, v_rn, v_rd, v_rm, dst
-    );
-    return check_launch();
+    if(!tile_grid_covers(tw, th, W, H))
+        return GSB200_E_INVALID;
+    if((double)I * (double)N * 9.0 >= 2147483648.0 || (double)I * tw * th >= 2147483648.0)
+        return GSB200_E_UNSUPPORTED;
+    return GSB200_OK;
 }
 } // namespace
 } // namespace gsb
@@ -840,16 +806,15 @@ extern "C" int gsb200_surfel_raster_fwd(
         return GSB200_E_UNSUPPORTED;
     if(I == 0 || image_width == 0 || image_height == 0)
         return GSB200_OK;
-    if(!gsb::tile_grid_covers(tile_width, tile_height, image_width, image_height))
-        return GSB200_E_INVALID;
-    if((double)I * (double)N * 9.0 >= 2147483648.0 || (double)I * tile_width * tile_height >= 2147483648.0)
-        return GSB200_E_UNSUPPORTED;
+    if(int rc = gsb::surfel_raster_limits(I, N, image_width, image_height, tile_width, tile_height))
+        return rc;
     return gsb::with_channels(D, [&](auto C) {
-        return gsb::launch_surfel_fwd<C>(
+        gsb::surfel_raster_fwd_kernel<C><<<(uint32_t)I * tile_width * tile_height, gsb::kSurfThreads, 0, (cudaStream_t)stream>>>(
             (uint32_t)I, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height,
             tile_width, tile_height, offsets, flatten_ids, n_isects, render_colors, render_alphas, render_normals,
-            render_distort, render_median, last_ids, median_ids, (cudaStream_t)stream
+            render_distort, render_median, last_ids, median_ids
         );
+        return gsb::check_launch();
     });
 }
 
@@ -874,17 +839,16 @@ extern "C" int gsb200_surfel_raster_bwd(
        || !render_alphas || !last_ids || !median_ids || !v_render_colors || !v_means2d || !v_ray_transforms || !v_colors
        || !v_opacities || !v_normals || !v_densify)
         return GSB200_E_INVALID;
-    if(!gsb::tile_grid_covers(tile_width, tile_height, image_width, image_height))
-        return GSB200_E_INVALID;
-    if((double)I * (double)N * 9.0 >= 2147483648.0 || (double)I * tile_width * tile_height >= 2147483648.0)
-        return GSB200_E_UNSUPPORTED;
+    if(int rc = gsb::surfel_raster_limits(I, N, image_width, image_height, tile_width, tile_height))
+        return rc;
     const gsb::SurfGradDst dst{v_means2d, v_ray_transforms, v_colors, v_opacities, v_normals, v_densify, v_means2d_abs};
     return gsb::with_channels(D, [&](auto C) {
-        return gsb::launch_surfel_bwd<C>(
+        gsb::surfel_raster_bwd_kernel<C><<<(uint32_t)I * tile_width * tile_height, gsb::kSurfThreads, 0, (cudaStream_t)stream>>>(
             (uint32_t)I, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height,
             tile_width, tile_height, offsets, flatten_ids, n_isects, render_colors, render_alphas, last_ids, median_ids,
-            v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst, (cudaStream_t)stream
+            v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst
         );
+        return gsb::check_launch();
     });
 }
 
@@ -901,12 +865,11 @@ extern "C" int gsb200_surfel_indices(
     const bool inputs_ok  = means2d && ray_transforms && opacities && transmittances && offsets && flatten_ids;
     return gsb::run_index_pass(
         I, N, image_width, image_height, tile_size, tile_width, tile_height, n_isects, range_start, range_end, inputs_ok, emit,
-        workspace, workspace_bytes, total, gaussian_ids && pixel_ids && image_ids, st,
-        [&](unsigned n_tiles, int32_t b0, int32_t b1, const gsb::PixelCounts &pc) {
-            auto kernel = emit ? gsb::surfel_indices_kernel<true> : gsb::surfel_indices_kernel<false>;
-            kernel<<<n_tiles, gsb::kSurfThreads, 0, st>>>(
-                (uint32_t)I, N, means2d, ray_transforms, opacities, transmittances, image_width, image_height, tile_width,
-                tile_height, offsets, flatten_ids, n_isects, b0, b1, pc.counts, pc.starts, gaussian_ids, pixel_ids, image_ids
+        workspace, workspace_bytes, total, gaussian_ids, pixel_ids, image_ids, st,
+        [&](unsigned n_tiles, int32_t b0, int32_t b1, auto sink) {
+            gsb::surfel_indices_kernel<<<n_tiles, gsb::kSurfThreads, 0, st>>>(
+                (uint32_t)I, means2d, ray_transforms, opacities, transmittances, image_width, image_height, tile_width,
+                tile_height, offsets, flatten_ids, n_isects, b0, b1, sink
             );
             return gsb::check_launch();
         }

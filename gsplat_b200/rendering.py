@@ -98,6 +98,42 @@ def _unsupported(name: str, why: str = "out of scope for the gsplat_b200 hot pat
     raise NotImplementedError(f"rasterization({name}): {why}")
 
 
+def _check_colors(colors, sh_degree, batch_dims, C, N):
+    """The colour shapes both rasterizers accept: post-activation [..., N, D] or [..., C, N, D], or SH [N, K, D]."""
+    nb = len(batch_dims)
+    if sh_degree is None:
+        ok = (colors.dim() == nb + 2 and tuple(colors.shape[:-1]) == batch_dims + (N,)) or (
+            colors.dim() == nb + 3 and tuple(colors.shape[:-1]) == batch_dims + (C, N)
+        )
+        if not ok:
+            raise ValueError(f"colors must be [..., N, D] or [..., C, N, D], got {tuple(colors.shape)}")
+    else:
+        if colors.dim() != 3 or colors.shape[0] != N:
+            raise ValueError(f"SH colors must be [N, K, D], got {tuple(colors.shape)}")
+        if (sh_degree + 1) ** 2 > colors.shape[-2]:
+            raise ValueError(f"sh_degree={sh_degree} needs K >= {(sh_degree + 1) ** 2}, got {colors.shape[-2]}")
+
+
+def _color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N):
+    """[..., C, N, D] features of the dense rows: the post-activation colours broadcast over the cameras, or the SH
+    colours evaluated for every visible row."""
+    if sh_degree is None:
+        if colors.dim() == len(batch_dims) + 2:
+            return torch.broadcast_to(colors[..., None, :, :], batch_dims + (C, N, colors.shape[-1]))
+        return colors
+    valid = (radii > 0).all(dim=-1)
+    feat = spherical_harmonics(sh_degree, means, viewmats, colors, masks=valid)
+    return torch.clamp_min(feat + 0.5, 0.0)
+
+
+def _normalize_expected_depth(render_colors, render_alphas, render_mode):
+    """ED / RGB+ED: the last channel is the accumulated depth; divide it by the alpha."""
+    if render_mode not in _EXPECTED_MODES:
+        return render_colors
+    depth = render_colors[..., -1:] / render_alphas.clamp(min=1e-10)
+    return torch.cat([render_colors[..., :-1], depth], dim=-1)
+
+
 def _project_dense(
     means, covars, quats, scales, opacities, colors, viewmats, Ks, width, height, sh_degree, eps2d, near_plane, far_plane,
     radius_clip, antialiased, camera_model, has_color, nb, batch_dims, C, N, rows_out=None,
@@ -118,16 +154,7 @@ def _project_dense(
             far_plane=far_plane, radius_clip=radius_clip, packed=False, calc_compensations=antialiased,
             camera_model=camera_model, opacities=opacities,
         )
-        feat = None
-        if has_color:
-            if sh_degree is None:
-                feat = colors
-                if feat.dim() == nb + 2:
-                    feat = torch.broadcast_to(feat[..., None, :, :], batch_dims + (C, N, feat.shape[-1]))
-            else:
-                valid = (radii > 0).all(dim=-1)
-                feat = spherical_harmonics(sh_degree, means, viewmats, colors, masks=valid)
-                feat = torch.clamp_min(feat + 0.5, 0.0)
+        feat = _color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N) if has_color else None
 
     opac = torch.broadcast_to(opacities[..., None, :], batch_dims + (C, N))
     if compensations is not None:
@@ -266,21 +293,11 @@ def rasterization(
     if has_color:
         if colors is None:
             raise ValueError(f"render_mode={render_mode!r} needs colors")
-        if sh_degree is None:
-            ok = (colors.dim() == nb + 2 and tuple(colors.shape[:-1]) == batch_dims + (N,)) or (
-                colors.dim() == nb + 3 and tuple(colors.shape[:-1]) == batch_dims + (C, N)
-            )
-            if not ok:
-                raise ValueError(f"colors must be [..., N, D] or [..., C, N, D], got {tuple(colors.shape)}")
-        else:
-            if colors.dim() != 3 or colors.shape[0] != N:
-                raise ValueError(f"SH colors must be [N, K, D], got {tuple(colors.shape)}")
-            if (sh_degree + 1) ** 2 > colors.shape[-2]:
-                raise ValueError(f"sh_degree={sh_degree} needs K >= {(sh_degree + 1) ** 2}, got {colors.shape[-2]}")
-            if colors.dtype in (torch.float16, torch.bfloat16):
-                # half-precision SH storage: evaluated in fp32 on every path (as ops.spherical_harmonics does); the
-                # cast is differentiable, so the gradient comes back in the storage dtype
-                colors = colors.float()
+        _check_colors(colors, sh_degree, batch_dims, C, N)
+        if sh_degree is not None and colors.dtype in (torch.float16, torch.bfloat16):
+            # half-precision SH storage: evaluated in fp32 on every path (as ops.spherical_harmonics does); the cast is
+            # differentiable, so the gradient comes back in the storage dtype
+            colors = colors.float()
 
     antialiased = rasterize_mode == "antialiased"
 
@@ -423,9 +440,7 @@ def rasterization(
             packed=packed, absgrad=absgrad, _row_records=rows_out.rows if (rows_out is not None and n_ch == 3) else None,
         )
 
-    if render_mode in _EXPECTED_MODES:  # ED / RGB+ED: normalise accumulated depth
-        depth = render_colors[..., -1:] / render_alphas.clamp(min=1e-10)
-        render_colors = torch.cat([render_colors[..., :-1], depth], dim=-1)
+    render_colors = _normalize_expected_depth(render_colors, render_alphas, render_mode)
 
     meta = _Meta({
         "batch_ids": batch_ids,
@@ -531,17 +546,7 @@ def rasterization_2dgs(
     if tuple(opacities.shape) != batch_dims + (N,):
         raise ValueError(f"opacities must be [..., N], got {tuple(opacities.shape)}")
     if has_color:
-        if sh_degree is None:
-            ok = (colors.dim() == nb + 2 and tuple(colors.shape[:-1]) == batch_dims + (N,)) or (
-                colors.dim() == nb + 3 and tuple(colors.shape[:-1]) == batch_dims + (C, N)
-            )
-            if not ok:
-                raise ValueError(f"colors must be [..., N, D] or [..., C, N, D], got {tuple(colors.shape)}")
-        else:
-            if colors.dim() != 3 or colors.shape[0] != N:
-                raise ValueError(f"SH colors must be [N, K, D], got {tuple(colors.shape)}")
-            if (sh_degree + 1) ** 2 > colors.shape[-2]:
-                raise ValueError(f"sh_degree={sh_degree} needs K >= {(sh_degree + 1) ** 2}, got {colors.shape[-2]}")
+        _check_colors(colors, sh_degree, batch_dims, C, N)
 
     # ---- projection (ray-splat transforms), reference Rendering.cpp:1802-1814
     radii, means2d, depths, ray_transforms, normals = fully_fused_projection_2dgs(
@@ -560,16 +565,7 @@ def rasterization_2dgs(
     isect_offsets = hits.isect_offsets.reshape(batch_dims + (C, tile_height, tile_width))
 
     # ---- channels: [colour | depth]
-    feat = None
-    if has_color:
-        if sh_degree is None:
-            feat = colors
-            if feat.dim() == nb + 2:
-                feat = torch.broadcast_to(feat[..., None, :, :], batch_dims + (C, N, feat.shape[-1]))
-        else:
-            valid = (radii > 0).all(dim=-1)
-            feat = spherical_harmonics(sh_degree, means, viewmats, colors, masks=valid)
-            feat = torch.clamp_min(feat + 0.5, 0.0)
+    feat = _color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N) if has_color else None
     if has_depth:
         if has_color:
             feat = torch.cat((feat, depths[..., None]), dim=-1)
@@ -583,9 +579,7 @@ def rasterization_2dgs(
         backgrounds=backgrounds, absgrad=absgrad, distloss=distloss,
     )
 
-    if render_mode in _EXPECTED_MODES:  # ED / RGB+ED: normalise the accumulated depth
-        depth = render_colors[..., -1:] / render_alphas.clamp(min=1e-10)
-        render_colors = torch.cat([render_colors[..., :-1], depth], dim=-1)
+    render_colors = _normalize_expected_depth(render_colors, render_alphas, render_mode)
 
     camtoworlds = torch.linalg.inv(viewmats)
     surf_normals = None

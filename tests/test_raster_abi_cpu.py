@@ -1,12 +1,13 @@
 """The compositing entry points of the C ABI, checked on the CPU: gsb200_raster_records_bytes against sizes recorded
 before the record-stream layout was written once for both the carving and the size query, and the return code of every
-gsb200_raster_* entry and of the two surfel compositing entries for invalid or early-return arguments, including
-which check fires first.  Every call here returns before a kernel is launched: the pointers are fake and never read."""
+gsb200_raster_* entry, of the two surfel compositing entries and of the two pair-query entries (gsb200_raster_indices,
+gsb200_surfel_indices) for invalid or early-return arguments, including which check fires first.  Every call here
+returns before a kernel is launched or the device is touched: the pointers are fake and never read."""
 import pytest
 
 from gsplat_b200 import _cabi
 
-OK, INVALID, UNSUPPORTED = 0, -1, -2
+OK, INVALID, UNSUPPORTED, WORKSPACE = 0, -1, -2, -4
 FAKE = 1 << 20  # 16-byte aligned, never dereferenced
 CHANNELS = (1, 2, 3, 4, 5, 8, 16, 32)
 
@@ -66,9 +67,14 @@ PARAMS = {
     "v_render_normals v_render_distort v_render_median v_means2d v_ray_transforms v_colors v_opacities v_normals v_densify "
     "v_means2d_abs stream",
 }
+# rows: conics [R, 3] for gsb200_raster_indices, ray transforms [R, 3, 3] for gsb200_surfel_indices
+INDICES_PARAMS = ("I N means2d rows opacities transmittances W H tile_size tw th offsets flatten_ids n_isects range_start "
+                  "range_end emit workspace workspace_bytes total gaussian_ids pixel_ids image_ids stream")
+PARAMS["gsb200_raster_indices"] = PARAMS["gsb200_surfel_indices"] = INDICES_PARAMS
 # a 16 x 16 image of one tile, one intersection, D = 3; every other pointer fake and 16-byte aligned
 BASE = dict(I=1, N=4, D=3, W=16, H=16, tile_size=16, tw=1, th=1, n_isects=1, n_active=1, n_rows=4, absgrad=0,
-            backgrounds=None, masks=None, v_render_alphas=None, stream=None)
+            backgrounds=None, masks=None, v_render_alphas=None, stream=None,
+            range_start=0, range_end=1, emit=1, workspace_bytes=1 << 62)
 
 GRID_SMALL = dict(W=17)  # one 16-pixel tile column for a 17-pixel wide image
 
@@ -189,6 +195,60 @@ CASES = [
     ("gsb200_surfel_raster_bwd", dict(N=1 << 28), UNSUPPORTED),
     ("gsb200_surfel_raster_bwd", dict(D=6), UNSUPPORTED),
 ]
+
+# Both pair-query entries share their checks and pass sequence.  BASE is an emit pass (emit = 1) with a large enough
+# workspace; the count pass (emit = 0) zeroes *total on the device when there are no pairs, so its early return is not
+# called here.
+INDICES_CASES = [
+    (dict(I=-1), INVALID),
+    (dict(N=-1), INVALID),
+    (dict(n_isects=-1), INVALID),
+    (dict(range_start=-1), INVALID),
+    (dict(range_end=-1), INVALID),
+    (dict(range_end=-1, tile_size=8), INVALID),
+    (dict(tile_size=8), UNSUPPORTED),
+    (dict(tile_size=8, n_isects=0), UNSUPPORTED),
+    (dict(emit=0, total=None), INVALID),
+    (dict(emit=0, total=None, n_isects=0), INVALID),
+    (dict(emit=0, total=None, range_end=0), INVALID),
+    (dict(emit=0, total=None, tile_size=8), UNSUPPORTED),
+    (dict(total=None, workspace_bytes=1), WORKSPACE),
+    (dict(n_isects=0), OK),
+    (dict(I=0), OK),
+    (dict(N=0), OK),
+    (dict(W=0), OK),
+    (dict(H=0, means2d=None), OK),
+    (dict(range_end=0), OK),
+    (dict(range_start=3, range_end=3), OK),
+    (dict(range_start=5, range_end=2), OK),
+    (dict(GRID_SMALL, range_end=0), OK),
+    (dict(range_end=0, gaussian_ids=None), OK),
+    (dict(n_isects=0, workspace=None), OK),
+    (dict(means2d=None), INVALID),
+    (dict(rows=None), INVALID),
+    (dict(opacities=None), INVALID),
+    (dict(transmittances=None), INVALID),
+    (dict(offsets=None), INVALID),
+    (dict(flatten_ids=None), INVALID),
+    (dict(gaussian_ids=None), INVALID),
+    (dict(pixel_ids=None), INVALID),
+    (dict(image_ids=None), INVALID),
+    (dict(emit=0, gaussian_ids=None, workspace_bytes=1), WORKSPACE),
+    (dict(GRID_SMALL), INVALID),
+    (dict(GRID_SMALL, workspace=None), INVALID),
+    (dict(GRID_SMALL, emit=0), INVALID),
+    (dict(means2d=None, workspace=None), INVALID),
+    (dict(workspace=None), WORKSPACE),
+    (dict(workspace_bytes=1), WORKSPACE),
+    (dict(emit=0, workspace_bytes=1), WORKSPACE),
+    (dict(workspace_bytes=1, n_isects=1 << 31), WORKSPACE),
+    (dict(n_isects=(1 << 31) - 1, workspace_bytes=1), WORKSPACE),
+    (dict(n_isects=1 << 31), UNSUPPORTED),
+    (dict(emit=0, n_isects=1 << 31), UNSUPPORTED),
+    (dict(I=1 << 31), UNSUPPORTED),
+    (dict(emit=0, I=1 << 31), UNSUPPORTED),
+]
+CASES += [(entry, changes, code) for entry in ("gsb200_raster_indices", "gsb200_surfel_indices") for changes, code in INDICES_CASES]
 
 
 def _call(entry, changes):

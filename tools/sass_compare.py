@@ -9,8 +9,8 @@ same name in the new ones, whichever unit it is compiled in: a kernel that moved
 old self.  Names are compared demangled, with the pixel-addressing policy of the compositing kernels
 (``gsb::DensePixels``) removed, so that a kernel that only gained that template argument is matched with its old self,
 with ``isect_count_kernel<true / false>`` under the names the two count kernels had before they became one template, and
-with the pair-query kernel ``raster_indices_kernel`` named by its sink without its parameter list (``<false / true>``
-became the ``CountSink`` / ``PairSink`` instantiations when the walk took a sink).
+with the pair-query kernels ``raster_indices_kernel`` and ``surfel_indices_kernel`` named by their sink without their
+parameter list (``<false / true>`` became the ``CountSink`` / ``PairSink`` instantiations when each walk took a sink).
 Instructions and their encodings must be identical; address and line-info comments are ignored.  A library kernel
 (CUB) that several units instantiate must be identical in all of them.  Kernels that only the new objects have are
 listed as new.  Exit status 1 on any difference.  Needs nvcc / cuobjdump / cu++filt (no GPU).
@@ -34,8 +34,9 @@ CUDA_BIN = os.path.dirname(B._nvcc()) if os.path.isabs(B._nvcc()) else "/usr/loc
 POLICY_PARAM = re.compile(r",\s*T\d+\)$")
 # isect_count_kernel<TOTALS>: <true> was isect_count_totals_kernel, <false> isect_count_kernel without the totals pointer
 COUNT_KERNEL = re.compile(r"^void gsb::isect_count_kernel<\(bool\)([01])>\((.*), unsigned long long \*\)$")
-# raster_indices_kernel<EMIT> became raster_indices_kernel<Sink, Pix>: <false> is the CountSink walk, <true> the PairSink
-INDICES_KERNEL = re.compile(r"^void gsb::raster_indices_kernel<(.*)>\(.*\)$")
+# raster_indices_kernel<EMIT> became raster_indices_kernel<Sink, Pix> and surfel_indices_kernel<EMIT> became
+# surfel_indices_kernel<Sink>: <false> is the CountSink walk, <true> the PairSink
+INDICES_KERNEL = re.compile(r"^void (gsb::(?:<unnamed>::)?(?:raster|surfel)_indices_kernel)<(.*)>\(.*\)$")
 INDICES_SINK = {"(bool)0": "gsb::CountSink", "(bool)1": "gsb::PairSink"}
 
 
@@ -87,7 +88,7 @@ def kernels(obj: str):
             d = f"gsb::isect_count_totals_kernel({m.group(2)}, unsigned long long *)" if m.group(1) == "1" else f"gsb::isect_count_kernel({m.group(2)})"
         m = INDICES_KERNEL.match(d)
         if m:
-            d = f"gsb::raster_indices_kernel<{INDICES_SINK.get(m.group(1), m.group(1))}>"
+            d = f"{m.group(1)}<{INDICES_SINK.get(m.group(2), m.group(2))}>"
         out[d] = raw[n]
     return out
 
