@@ -163,6 +163,17 @@ _SIGNATURES = {
         [c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64,
          c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     ),
+    "gsb200_surfel_raster_sparse_fwd": (
+        c_int,
+        [c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp,
+         c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    ),
+    "gsb200_surfel_raster_sparse_bwd": (
+        c_int,
+        [c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp,
+         c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+         c_vp, c_vp],
+    ),
     "gsb200_indices_workspace_bytes": (c_sz, [c_i64]),
     "gsb200_raster_indices": (
         c_int,

@@ -29,7 +29,7 @@ UNITS = {
     "loss.cu": [],
     "surfel.cu": ["-fmad=false"],
 }
-HEADERS = ["common.cuh", "gaussmath.cuh", "indices.cuh", "isect.cuh", "rowrec.cuh", os.path.join("..", "..", "include", "gsplat_b200.h")]
+HEADERS = ["common.cuh", "gaussmath.cuh", "indices.cuh", "isect.cuh", "pixels.cuh", "rowrec.cuh", os.path.join("..", "..", "include", "gsplat_b200.h")]
 
 
 def _nvcc() -> str:

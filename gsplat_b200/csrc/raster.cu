@@ -21,6 +21,7 @@
 
 #include "common.cuh"
 #include "indices.cuh"
+#include "pixels.cuh"
 #include "rowrec.cuh"
 
 namespace gsb
@@ -186,82 +187,6 @@ __global__ void __launch_bounds__(256) pack_rows_kernel(
         const int64_t s = base + u * 64;
         if(s < S)
             dst[s] = v[u];
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-struct TileGeom
-{
-    int image_id, tile_id, tile_x, tile_y;
-};
-
-__device__ __forceinline__ TileGeom decode_block(const uint32_t block, uint32_t tw, uint32_t th)
-{
-    TileGeom t;
-    const uint32_t per = tw * th;
-    t.image_id         = block / per;
-    t.tile_id          = block % per;
-    t.tile_x           = t.tile_id % tw;
-    t.tile_y           = t.tile_id / tw;
-    return t;
-}
-
-__device__ __forceinline__ TileGeom decode_tile(const int32_t *__restrict__ order, uint32_t tw, uint32_t th)
-{
-    return decode_block(order ? (uint32_t)order[blockIdx.x] : blockIdx.x, tw, th);
-}
-
-// ---------------------------------------------------------------------------------------------
-// Pixel addressing of the compositing kernels, a compile-time policy.
-//  DensePixels: one CTA per tile of the [I, th, tw] grid; offsets [I * th * tw] (the last range ends at n_isects); the
-//    pixel (x, y) of image i is live when it lies inside the W x H image and is stored at (i * H + y) * W + x.
-//  SparsePixels: one CTA per ACTIVE tile ord (rasterize_to_pixels_sparse); the tile is active_tiles[ord], its list is
-//    offsets[ord] .. offsets[ord + 1], and a pixel is live when its bit in the tile's raster-order mask is set.  Its
-//    output slot is pixel_map[start + rank], start = the live pixels of the tiles before (inclusive cumsum[ord - 1])
-//    and rank = the live pixels before it in the tile.  Live margin pixels of a partial tile are rendered too.
-struct DensePixels
-{
-    static constexpr bool kSparse = false;
-};
-
-struct SparsePixels
-{
-    static constexpr bool kSparse = true;
-    const int32_t *active_tiles;      // [AT] dense tile ids image * th * tw + ty * tw + tx, ascending
-    const uint64_t *tile_pixel_mask;  // [AT, 4] bit (y % 16) * 16 + x % 16 of word >> 6
-    const int64_t *tile_pixel_cumsum; // [AT] inclusive prefix sum of the live pixels per tile
-    const int64_t *pixel_map;         // [P] (tile, in-tile) order -> output row
-
-    // output row of in-tile position `pos` of active tile `ord`; live = false (and row 0) if the pixel was not requested
-    __device__ __forceinline__ int64_t slot(const uint32_t ord, const int pos, bool &live) const
-    {
-        const uint64_t *words = tile_pixel_mask + (size_t)ord * 4;
-        const int w = pos >> 6, bit = pos & 63;
-        const uint64_t mw = words[w];
-        live = ((mw >> bit) & 1ull) != 0ull;
-        if(!live)
-            return 0;
-        int rank = __popcll(mw & ((1ull << bit) - 1ull));
-        for(int q = 0; q < w; ++q)
-            rank += __popcll(words[q]);
-        const int64_t start = ord == 0 ? 0 : tile_pixel_cumsum[ord - 1];
-        return pixel_map[start + rank];
-    }
-};
-
-// tile of this CTA; ord = its position in the launch's tile list (the block index after the tile order)
-template<class Pix>
-__device__ __forceinline__ TileGeom block_tile(const int32_t *__restrict__ order, uint32_t tw, uint32_t th, const Pix &pm, uint32_t &ord)
-{
-    if constexpr(Pix::kSparse)
-    {
-        ord = order ? (uint32_t)order[blockIdx.x] : blockIdx.x;
-        return decode_block((uint32_t)pm.active_tiles[ord], tw, th);
-    }
-    else
-    {
-        ord = 0;
-        return decode_tile(order, tw, th);
     }
 }
 
@@ -1492,20 +1417,6 @@ extern "C" int gsb200_raster_bwd(
 
 // ---- sparse pixels: one CTA per active tile of the layout of gsb200_sparse_layout_*, outputs [P, D] / [P] in the original
 // pixel order.  `records` is caller scratch of gsb200_raster_records_bytes(n_isects, D, n_active).
-static int sparse_args_ok(
-    int64_t n_active, const int32_t *active_tiles, const int32_t *tile_offsets, const uint64_t *tile_pixel_mask,
-    const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, uint32_t W, uint32_t H, uint32_t tw, uint32_t th
-)
-{
-    if(n_active < 0 || n_active > 0x7fffffffLL)
-        return GSB200_E_INVALID;
-    if(n_active > 0 && (!active_tiles || !tile_offsets || !tile_pixel_mask || !tile_pixel_cumsum || !pixel_map))
-        return GSB200_E_INVALID;
-    if(!gsb::tile_grid_covers(tw, th, W, H))
-        return GSB200_E_INVALID;
-    return GSB200_OK;
-}
-
 extern "C" int gsb200_raster_sparse_fwd(
     int D, const float *means2d, const float *conics, const float *colors, const float *opacities, const float *backgrounds,
     const uint8_t *masks, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
@@ -1518,7 +1429,7 @@ extern "C" int gsb200_raster_sparse_fwd(
         return GSB200_E_UNSUPPORTED;
     if(n_isects < 0)
         return GSB200_E_INVALID;
-    if(int rc = sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_width, tile_height))
+    if(int rc = gsb::sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_width, tile_height))
         return rc;
     if(n_active == 0)
         return GSB200_OK;
@@ -1549,7 +1460,7 @@ extern "C" int gsb200_raster_sparse_bwd(
         return GSB200_E_UNSUPPORTED;
     if(n_rows < 0 || n_isects < 0)
         return GSB200_E_INVALID;
-    if(int rc = sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_width, tile_height))
+    if(int rc = gsb::sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_width, tile_height))
         return rc;
     if(n_isects == 0 || n_active == 0)
         return GSB200_OK;

@@ -7,6 +7,7 @@
 // csrc/RasterizeToPixels2DGSSerialBatchFwd.cu / Bwd.cu (compositing), include/Common.h and csrc/Rasterization.h (constants).
 #include "gaussmath.cuh"
 #include "indices.cuh"
+#include "pixels.cuh"
 
 namespace gsb
 {
@@ -343,25 +344,35 @@ __device__ __forceinline__ SurfHit surf_eval(const SurfRec &r, float px, float p
     return h;
 }
 
-template<int CDIM>
+// One CTA per tile of the pixel policy (pixels.cuh): every tile of the [I, th, tw] grid (DensePixels), or every active
+// tile with its requested pixels only (SparsePixels).  A pixel that is not live stages records and meets every barrier
+// but composites and writes nothing.
+template<int CDIM, class Pix = DensePixels>
 __global__ void __launch_bounds__(kSurfThreads) surfel_raster_fwd_kernel(
     uint32_t I, const float *__restrict__ means2d, const float *__restrict__ rt, const float *__restrict__ colors,
     const float *__restrict__ opacities, const float *__restrict__ normals, const float *__restrict__ backgrounds,
     const uint8_t *__restrict__ masks, uint32_t W, uint32_t H, uint32_t tw, uint32_t th, const int32_t *__restrict__ offsets,
     const int32_t *__restrict__ flatten_ids, int64_t n_isects, float *__restrict__ render_colors, float *__restrict__ render_alphas,
     float *__restrict__ render_normals, float *__restrict__ render_distort, float *__restrict__ render_median,
-    int32_t *__restrict__ last_ids, int32_t *__restrict__ median_ids
+    int32_t *__restrict__ last_ids, int32_t *__restrict__ median_ids, const Pix pixmap = Pix{}
 )
 {
     __shared__ SurfRec rec[kSurfThreads];
-    const uint32_t tile = blockIdx.x; // image * th * tw + tile row * tw + tile col
+    const uint32_t tile = pixmap.tile(blockIdx.x); // image * th * tw + tile row * tw + tile col
     const uint32_t img  = tile / (tw * th);
     const uint32_t tin  = tile - img * tw * th;
     const uint32_t tr   = threadIdx.x;
     const uint32_t i    = (tin / tw) * kTile + tr / kTile;
     const uint32_t j    = (tin % tw) * kTile + tr % kTile;
-    const bool inside   = i < H && j < W;
-    const int64_t pix   = (int64_t)img * H * W + (int64_t)i * W + j;
+    bool inside;
+    int64_t pix;
+    if constexpr(Pix::kSparse)
+        pix = pixmap.slot(blockIdx.x, (int)tr, inside);
+    else
+    {
+        inside = i < H && j < W;
+        pix    = (int64_t)img * H * W + (int64_t)i * W + j;
+    }
     const float *bg     = backgrounds ? backgrounds + (int64_t)img * CDIM : nullptr;
 
     if(masks && !masks[tile])
@@ -382,8 +393,17 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_raster_fwd_kernel(
         }
         return;
     }
-    const int64_t start = offsets[tile];
-    const int64_t end   = (tile + 1 == I * tw * th) ? n_isects : offsets[tile + 1];
+    int64_t start, end;
+    if constexpr(Pix::kSparse)
+    {
+        start = offsets[blockIdx.x];
+        end   = offsets[blockIdx.x + 1];
+    }
+    else
+    {
+        start = offsets[tile];
+        end   = (tile + 1 == I * tw * th) ? n_isects : offsets[tile + 1];
+    }
     const float px = (float)j + 0.5f, py = (float)i + 0.5f;
 
     float T = 1.f, distort = 0.f, accum_vis_depth = 0.f, median_depth = 0.f;
@@ -437,6 +457,8 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_raster_fwd_kernel(
     }
     if(!inside)
         return;
+    if constexpr(Pix::kSparse)
+        pix = pixmap.slot(blockIdx.x, (int)tr, inside); // looked up again: the row is not held across the walk
     render_alphas[pix] = 1.f - T;
 #pragma unroll
     for(int k = 0; k < CDIM; ++k)
@@ -557,7 +579,7 @@ __device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, cons
 // Back to front over each tile's list.  Per gaussian, the warp's per-pixel gradients (colours, normals, ray transform,
 // screen mean, opacity, |screen mean|) are butterfly-reduced and added with one atomic per value; v_densify is the
 // z-column of the ray-transform gradient times M[2][2], the same for every pixel of the gaussian.
-template<int CDIM>
+template<int CDIM, class Pix = DensePixels>
 __global__ void __launch_bounds__(kSurfThreads) surfel_raster_bwd_kernel(
     uint32_t I, const float *__restrict__ means2d, const float *__restrict__ rt, const float *__restrict__ colors,
     const float *__restrict__ opacities, const float *__restrict__ normals, const float *__restrict__ backgrounds,
@@ -566,14 +588,14 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_raster_bwd_kernel(
     const float *__restrict__ render_alphas, const int32_t *__restrict__ last_ids, const int32_t *__restrict__ median_ids,
     const float *__restrict__ v_render_colors, const float *__restrict__ v_render_alphas,
     const float *__restrict__ v_render_normals, const float *__restrict__ v_render_distort,
-    const float *__restrict__ v_render_median, SurfGradDst dst
+    const float *__restrict__ v_render_median, SurfGradDst dst, const Pix pixmap = Pix{}
 )
 {
     constexpr int NV = CDIM + 17; // colours | normals 3 | ray transform 9 | xy 2 | opacity 1 | abs xy 2
     __shared__ SurfRec rec[kSurfThreads];
     __shared__ float s_col[kSurfThreads * CDIM];
     __shared__ float s_nrm[kSurfThreads * 3];
-    const uint32_t tile = blockIdx.x;
+    const uint32_t tile = pixmap.tile(blockIdx.x);
     if(masks && !masks[tile])
         return;
     const uint32_t img  = tile / (tw * th);
@@ -582,11 +604,29 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_raster_bwd_kernel(
     const unsigned lane = tr & 31;
     const uint32_t i    = (tin / tw) * kTile + tr / kTile;
     const uint32_t j    = (tin % tw) * kTile + tr % kTile;
-    const bool inside   = i < H && j < W;
-    const int64_t pix   = inside ? (int64_t)img * H * W + (int64_t)i * W + j : (int64_t)img * H * W;
-    const float *bg     = backgrounds ? backgrounds + (int64_t)img * CDIM : nullptr;
-    const int64_t start = offsets[tile];
-    const int64_t end   = (tile + 1 == I * tw * th) ? n_isects : offsets[tile + 1];
+    // a pixel that is not live reads the row of a live one (the image's first pixel; sparse: row 0) and adds nothing
+    bool inside;
+    int64_t pix;
+    if constexpr(Pix::kSparse)
+        pix = pixmap.slot(blockIdx.x, (int)tr, inside);
+    else
+    {
+        inside = i < H && j < W;
+        pix    = inside ? (int64_t)img * H * W + (int64_t)i * W + j : (int64_t)img * H * W;
+    }
+    // the list range after bg, as before the pixel policy: read in the other order, the dense kernel's code changes
+    const float *bg = backgrounds ? backgrounds + (int64_t)img * CDIM : nullptr;
+    int64_t start, end;
+    if constexpr(Pix::kSparse)
+    {
+        start = offsets[blockIdx.x];
+        end   = offsets[blockIdx.x + 1];
+    }
+    else
+    {
+        start = offsets[tile];
+        end   = (tile + 1 == I * tw * th) ? n_isects : offsets[tile + 1];
+    }
     const float px = (float)j + 0.5f, py = (float)i + 0.5f;
 
     const float T_final = 1.f - render_alphas[pix];
@@ -847,6 +887,86 @@ extern "C" int gsb200_surfel_raster_bwd(
             (uint32_t)I, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height,
             tile_width, tile_height, offsets, flatten_ids, n_isects, render_colors, render_alphas, last_ids, median_ids,
             v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst
+        );
+        return gsb::check_launch();
+    });
+}
+
+// ---- sparse pixels (rasterize_to_pixels_2dgs_sparse): one CTA per active tile of the layout of gsb200_sparse_layout_*,
+// outputs [P, *] in the original pixel order.  The checks run in the order of gsb200_raster_sparse_fwd / _bwd, then the
+// row limit of the dense entries.
+static int surfel_rows_ok(int64_t n_rows)
+{
+    return (double)n_rows * 9.0 >= 2147483648.0 ? GSB200_E_UNSUPPORTED : GSB200_OK;
+}
+
+extern "C" int gsb200_surfel_raster_sparse_fwd(
+    int64_t n_rows, int D, const float *means2d, const float *ray_transforms, const float *colors, const float *opacities,
+    const float *normals, const float *backgrounds, const uint8_t *masks, uint32_t image_width, uint32_t image_height,
+    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t n_active, const int32_t *active_tiles,
+    const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t n_isects, const uint64_t *tile_pixel_mask,
+    const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, float *render_colors, float *render_alphas,
+    float *render_normals, float *render_distort, float *render_median, int32_t *last_ids, int32_t *median_ids, void *stream
+)
+{
+    if(tile_size != (uint32_t)gsb::kTile)
+        return GSB200_E_UNSUPPORTED;
+    if(n_rows < 0 || n_isects < 0)
+        return GSB200_E_INVALID;
+    if(int rc = gsb::sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_width, tile_height))
+        return rc;
+    if(n_active == 0)
+        return GSB200_OK;
+    if(!render_colors || !render_alphas || !render_normals || !render_distort || !render_median || !last_ids || !median_ids)
+        return GSB200_E_INVALID;
+    if(n_isects > 0 && (!means2d || !ray_transforms || !colors || !opacities || !normals || !flatten_ids))
+        return GSB200_E_INVALID;
+    if(int rc = surfel_rows_ok(n_rows))
+        return rc;
+    const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
+    return gsb::with_channels(D, [&](auto C) {
+        gsb::surfel_raster_fwd_kernel<C, gsb::SparsePixels><<<(uint32_t)n_active, gsb::kSurfThreads, 0, (cudaStream_t)stream>>>(
+            1u, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height, tile_width,
+            tile_height, tile_offsets, flatten_ids, n_isects, render_colors, render_alphas, render_normals, render_distort,
+            render_median, last_ids, median_ids, pm
+        );
+        return gsb::check_launch();
+    });
+}
+
+extern "C" int gsb200_surfel_raster_sparse_bwd(
+    int64_t n_rows, int D, const float *means2d, const float *ray_transforms, const float *colors, const float *opacities,
+    const float *normals, const float *backgrounds, const uint8_t *masks, uint32_t image_width, uint32_t image_height,
+    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t n_active, const int32_t *active_tiles,
+    const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t n_isects, const uint64_t *tile_pixel_mask,
+    const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, const float *render_colors, const float *render_alphas,
+    const int32_t *last_ids, const int32_t *median_ids, const float *v_render_colors, const float *v_render_alphas,
+    const float *v_render_normals, const float *v_render_distort, const float *v_render_median, float *v_means2d,
+    float *v_ray_transforms, float *v_colors, float *v_opacities, float *v_normals, float *v_densify, float *v_means2d_abs,
+    void *stream
+)
+{
+    if(tile_size != (uint32_t)gsb::kTile)
+        return GSB200_E_UNSUPPORTED;
+    if(n_rows < 0 || n_isects < 0)
+        return GSB200_E_INVALID;
+    if(int rc = gsb::sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_width, tile_height))
+        return rc;
+    if(n_isects == 0 || n_active == 0)
+        return GSB200_OK;
+    if(!means2d || !ray_transforms || !colors || !opacities || !normals || !flatten_ids || !render_colors || !render_alphas
+       || !last_ids || !median_ids || !v_render_colors || !v_means2d || !v_ray_transforms || !v_colors || !v_opacities
+       || !v_normals || !v_densify)
+        return GSB200_E_INVALID;
+    if(int rc = surfel_rows_ok(n_rows))
+        return rc;
+    const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
+    const gsb::SurfGradDst dst{v_means2d, v_ray_transforms, v_colors, v_opacities, v_normals, v_densify, v_means2d_abs};
+    return gsb::with_channels(D, [&](auto C) {
+        gsb::surfel_raster_bwd_kernel<C, gsb::SparsePixels><<<(uint32_t)n_active, gsb::kSurfThreads, 0, (cudaStream_t)stream>>>(
+            1u, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height, tile_width,
+            tile_height, tile_offsets, flatten_ids, n_isects, render_colors, render_alphas, last_ids, median_ids,
+            v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst, pm
         );
         return gsb::check_launch();
     });

@@ -1731,6 +1731,26 @@ def isect_tiles_sparse(
     return tile_offsets, flatten_ids
 
 
+def _check_sparse_layout(image_ids, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map,
+                         image_width, image_height, tile_width, tile_height) -> Tuple[int, int]:
+    """The layout checks of the sparse compositing ops, before anything is launched.  Returns (AT, P)."""
+    AT, P = active_tiles.shape[0] if active_tiles.dim() == 1 else -1, pixel_map.shape[0] if pixel_map.dim() == 1 else -1
+    if AT < 0 or P < 0 or active_tiles.dtype != torch.int32:
+        raise ValueError("active_tiles must be int32 [AT] and pixel_map [P]")
+    if tuple(tile_offsets.shape) != (AT + 1,) or tile_offsets.dtype != torch.int32 or flatten_ids.dtype != torch.int32:
+        raise ValueError(f"tile_offsets must be int32 [{AT + 1}] and flatten_ids int32 (isect_tiles_sparse)")
+    if tuple(tile_pixel_mask.shape) != (AT, _TILE_WORDS) or tile_pixel_mask.element_size() != 8:
+        raise ValueError(f"tile_pixel_mask must be 64-bit [{AT}, {_TILE_WORDS}], got {tile_pixel_mask.dtype} {tuple(tile_pixel_mask.shape)}")
+    n_cum = tile_pixel_cumsum.shape[0] if tile_pixel_cumsum.dim() == 1 else -1
+    if n_cum not in ((AT,) if AT > 0 else (0, 1)) or tile_pixel_cumsum.dtype != torch.int64 or pixel_map.dtype != torch.int64:
+        raise ValueError("tile_pixel_cumsum must be int64 [AT] and pixel_map int64 [P] (build_sparse_tile_layout)")
+    if tuple(image_ids.shape) != (P,):
+        raise ValueError(f"image_ids must be [{P}], got {tuple(image_ids.shape)}")
+    if tile_width * 16 < image_width or tile_height * 16 < image_height:
+        raise ValueError(f"a {tile_width} x {tile_height} tile grid does not cover {image_width} x {image_height} pixels")
+    return AT, P
+
+
 class _RasterizeToPixelsSparse(torch.autograd.Function):
     @staticmethod
     def forward(
@@ -1813,20 +1833,10 @@ def rasterize_to_pixels_sparse(
     isect_tiles_sparse.  Returns (render_colors [P, channels], render_alphas [P, 1]) in the original pixel order; each
     value is the dense rendering's at that pixel (requested pixels in the margin of a partial tile included).  With
     ``absgrad`` the backward fills ``means2d.absgrad``."""
-    AT, P = active_tiles.shape[0] if active_tiles.dim() == 1 else -1, pixel_map.shape[0] if pixel_map.dim() == 1 else -1
-    if AT < 0 or P < 0 or active_tiles.dtype != torch.int32:
-        raise ValueError("active_tiles must be int32 [AT] and pixel_map [P]")
-    if tuple(tile_offsets.shape) != (AT + 1,) or tile_offsets.dtype != torch.int32 or flatten_ids.dtype != torch.int32:
-        raise ValueError(f"tile_offsets must be int32 [{AT + 1}] and flatten_ids int32 (isect_tiles_sparse)")
-    if tuple(tile_pixel_mask.shape) != (AT, _TILE_WORDS) or tile_pixel_mask.element_size() != 8:
-        raise ValueError(f"tile_pixel_mask must be 64-bit [{AT}, {_TILE_WORDS}], got {tile_pixel_mask.dtype} {tuple(tile_pixel_mask.shape)}")
-    n_cum = tile_pixel_cumsum.shape[0] if tile_pixel_cumsum.dim() == 1 else -1
-    if n_cum not in ((AT,) if AT > 0 else (0, 1)) or tile_pixel_cumsum.dtype != torch.int64 or pixel_map.dtype != torch.int64:
-        raise ValueError("tile_pixel_cumsum must be int64 [AT] and pixel_map int64 [P] (build_sparse_tile_layout)")
-    if tuple(image_ids.shape) != (P,):
-        raise ValueError(f"image_ids must be [{P}], got {tuple(image_ids.shape)}")
-    if tile_width * 16 < image_width or tile_height * 16 < image_height:
-        raise ValueError(f"a {tile_width} x {tile_height} tile grid does not cover {image_width} x {image_height} pixels")
+    _check_sparse_layout(
+        image_ids, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width,
+        image_height, tile_width, tile_height,
+    )
 
     def composite(colors, backgrounds, holder, padded):
         return _RasterizeToPixelsSparse.apply(
@@ -1836,6 +1846,167 @@ def rasterize_to_pixels_sparse(
         )
 
     return _rasterize_padded(means2d, colors, backgrounds, tile_size, packed, absgrad, composite)
+
+
+class _RasterizeToPixels2DGSSparse(torch.autograd.Function):
+    @staticmethod
+    def forward(
+        ctx, means2d, ray_transforms, colors, opacities, normals, densify, backgrounds, masks, image_ids, active_tiles,
+        tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, width, height, tile_width, tile_height,
+        absgrad_holder,
+    ):
+        dev = require_cuda(means2d, ray_transforms, colors, opacities, normals, active_tiles, tile_offsets, flatten_ids, pixel_map)
+        means2d, ray_transforms = f32c(means2d, "means2d"), f32c(ray_transforms, "ray_transforms")
+        colors, opacities, normals = f32c(colors, "colors"), f32c(opacities, "opacities"), f32c(normals, "normals")
+        backgrounds = f32c(backgrounds, "backgrounds")
+        R, D, P = _prod(means2d.shape[:-1]), colors.shape[-1], pixel_map.shape[0]
+        m8 = _mask_u8(masks)
+        active, offsets, fl = active_tiles.contiguous(), tile_offsets.contiguous(), flatten_ids.contiguous()
+        words, cumsum, pmap = tile_pixel_mask.contiguous(), tile_pixel_cumsum.contiguous(), pixel_map.contiguous()
+        AT, S = active.shape[0], fl.shape[0]
+        o = dict(device=dev, dtype=torch.float32)
+        if P == 0 or S == 0:
+            # no requested pixel, or nothing listed in any active tile: the background alone, no kernel launch
+            if backgrounds is not None and P > 0:
+                render_colors = backgrounds[image_ids.long()]
+            else:
+                render_colors = torch.zeros((P, D), **o)
+            render_alphas, render_distort, render_median = (torch.zeros((P, 1), **o) for _ in range(3))
+            render_normals = torch.zeros((P, 3), **o)
+            last_ids = median_ids = torch.zeros(P, device=dev, dtype=torch.int32)
+        else:
+            render_colors = torch.empty((P, D), **o)
+            render_alphas, render_distort, render_median = (torch.empty((P, 1), **o) for _ in range(3))
+            render_normals = torch.empty((P, 3), **o)
+            last_ids = torch.empty(P, device=dev, dtype=torch.int32)
+            median_ids = torch.empty(P, device=dev, dtype=torch.int32)
+            with _Ctx(dev) as st:
+                check(
+                    lib().gsb200_surfel_raster_sparse_fwd(
+                        R, D, ptr(means2d), ptr(ray_transforms), ptr(colors), ptr(opacities), ptr(normals), ptr(backgrounds),
+                        ptr(m8), width, height, 16, tile_width, tile_height, AT, ptr(active), ptr(offsets), ptr(fl), S,
+                        ptr(words), ptr(cumsum), ptr(pmap), ptr(render_colors), ptr(render_alphas), ptr(render_normals),
+                        ptr(render_distort), ptr(render_median), ptr(last_ids), ptr(median_ids), st,
+                    ),
+                    "rasterize_to_pixels_2dgs_sparse",
+                )
+        ctx.save_for_backward(
+            means2d, ray_transforms, colors, opacities, normals, backgrounds, m8, image_ids, active, offsets, fl, words, cumsum,
+            pmap, render_colors, render_alphas, last_ids, median_ids,
+        )
+        ctx.set_materialize_grads(False)
+        ctx.absgrad_holder = absgrad_holder  # filled in place by backward; deliberately not a saved tensor
+        ctx.meta = (R, D, width, height, tile_width, tile_height, tuple(densify.shape))
+        return render_colors, render_alphas, render_normals, render_distort, render_median
+
+    @staticmethod
+    def backward(ctx, v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median):
+        (means2d, ray_transforms, colors, opacities, normals, backgrounds, m8, image_ids, active, offsets, fl, words, cumsum,
+         pmap, render_colors, render_alphas, last_ids, median_ids) = ctx.saved_tensors
+        R, D, width, height, tw, th, densify_shape = ctx.meta
+        dev = render_alphas.device
+        if v_render_colors is None:
+            v_render_colors = torch.zeros_like(render_colors)
+        v_render_colors = v_render_colors.contiguous()
+        c = lambda g: None if g is None else g.contiguous()  # noqa: E731
+        v_render_alphas, v_render_normals = c(v_render_alphas), c(v_render_normals)
+        v_render_distort, v_render_median = c(v_render_distort), c(v_render_median)
+        v_means2d, v_ray_transforms = torch.zeros_like(means2d), torch.zeros_like(ray_transforms)
+        v_colors, v_opacities, v_normals = torch.zeros_like(colors), torch.zeros_like(opacities), torch.zeros_like(normals)
+        v_densify = torch.zeros(densify_shape, device=dev, dtype=torch.float32)
+        holder = ctx.absgrad_holder
+        v_abs = torch.zeros_like(means2d) if holder is not None else None
+        if fl.shape[0] > 0 and pmap.shape[0] > 0:
+            with _Ctx(dev) as st:
+                check(
+                    lib().gsb200_surfel_raster_sparse_bwd(
+                        R, D, ptr(means2d), ptr(ray_transforms), ptr(colors), ptr(opacities), ptr(normals), ptr(backgrounds),
+                        ptr(m8), width, height, 16, tw, th, active.shape[0], ptr(active), ptr(offsets), ptr(fl), fl.shape[0],
+                        ptr(words), ptr(cumsum), ptr(pmap), ptr(render_colors), ptr(render_alphas), ptr(last_ids),
+                        ptr(median_ids), ptr(v_render_colors), ptr(v_render_alphas), ptr(v_render_normals),
+                        ptr(v_render_distort), ptr(v_render_median), ptr(v_means2d), ptr(v_ray_transforms), ptr(v_colors),
+                        ptr(v_opacities), ptr(v_normals), ptr(v_densify), ptr(v_abs), st,
+                    ),
+                    "rasterize_to_pixels_2dgs_sparse_bwd",
+                )
+        if holder is not None:
+            holder.copy_(v_abs)
+        v_backgrounds = None
+        if backgrounds is not None and ctx.needs_input_grad[6]:
+            v_backgrounds = torch.zeros_like(backgrounds).index_add_(0, image_ids.long(), v_render_colors * (1.0 - render_alphas))
+        return (v_means2d, v_ray_transforms, v_colors, v_opacities, v_normals, v_densify, v_backgrounds) + (None,) * 13
+
+
+def rasterize_to_pixels_2dgs_sparse(
+    means2d: Tensor,  # [..., N, 2]
+    ray_transforms: Tensor,  # [..., N, 3, 3]
+    colors: Tensor,  # [..., N, channels]
+    opacities: Tensor,  # [..., N]
+    normals: Tensor,  # [..., N, 3]
+    densify: Tensor,  # [..., N, 2]
+    image_ids: Tensor,  # [P]
+    active_tiles: Tensor,  # [AT]
+    tile_offsets: Tensor,  # [AT + 1]
+    flatten_ids: Tensor,  # [n_isects]
+    tile_pixel_mask: Tensor,  # [AT, 4]
+    tile_pixel_cumsum: Tensor,  # [AT]
+    pixel_map: Tensor,  # [P]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+    backgrounds: Optional[Tensor] = None,  # [n_images, channels]
+    masks: Optional[Tensor] = None,  # [n_images, tile_height, tile_width]
+    absgrad: bool = False,
+    distloss: bool = False,
+) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """rasterize_to_pixels_2dgs at the pixels of a build_sparse_tile_layout layout only, with the lists of
+    isect_tiles_sparse (conics=None) on the surfel rows.  The images are the leading dimensions of the rows, flattened:
+    image ``i`` of the layout is row block ``i`` of ``means2d.reshape(-1, N, 2)``.  Returns (render_colors [P, channels],
+    render_alphas [P, 1], render_normals [P, 3], render_distort [P, 1], render_median [P, 1]) in the original pixel
+    order; each value is the dense rendering's at that pixel (requested pixels in the margin of a partial tile
+    included).  The last colour channel is the depth that the distortion and the median depth are taken from.
+    ``densify`` receives the densification gradient; with ``absgrad`` the backward fills ``means2d.absgrad``.
+    ``distloss`` is accepted for symmetry with rasterize_to_pixels_2dgs: the distortion is always computed."""
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    AT, P = _check_sparse_layout(
+        image_ids, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width,
+        image_height, tile_width, tile_height,
+    )
+    if flatten_ids.dim() != 1:
+        raise ValueError(f"flatten_ids must be one-dimensional, got {tuple(flatten_ids.shape)}")
+    if means2d.dim() < 2 or means2d.shape[-1] != 2:
+        raise ValueError(f"means2d must be [..., N, 2], got {tuple(means2d.shape)}")
+    lead, N = tuple(means2d.shape[:-2]), means2d.shape[-2]
+    n_images = _prod(lead)
+    if colors.dim() != means2d.dim():
+        raise ValueError(f"colors must be [..., N, channels], got {tuple(colors.shape)}")
+    D = colors.shape[-1]
+    _check_shape(ray_transforms, lead + (N, 3, 3), "ray_transforms")
+    _check_shape(colors, lead + (N, D), "colors")
+    _check_shape(opacities, lead + (N,), "opacities")
+    _check_shape(normals, lead + (N, 3), "normals")
+    _check_shape(densify, lead + (N, 2), "densify")
+    if backgrounds is not None:
+        _check_shape(backgrounds, (n_images, D), "backgrounds")
+    if masks is not None:
+        _check_shape(masks, (n_images, tile_height, tile_width), "masks")
+    if D not in _SUPPORTED_CHANNELS:
+        raise NotImplementedError(
+            f"rasterize_to_pixels_2dgs_sparse: {D} channels; the 2DGS kernels are built for {_SUPPORTED_CHANNELS} (the last "
+            "channel is the depth, so the channels cannot be padded)"
+        )
+    holder = torch.zeros_like(means2d) if absgrad else None
+    outs = _RasterizeToPixels2DGSSparse.apply(
+        means2d, ray_transforms, colors, opacities, normals, densify, backgrounds, masks, image_ids, active_tiles,
+        tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, int(image_width), int(image_height),
+        int(tile_width), int(tile_height), holder,
+    )
+    if absgrad:
+        means2d.absgrad = holder
+    return outs
 
 # --------------------------------------------------------------------------------------------
 # per-pixel contributor queries (reference wrappers gsplat/cuda/_wrapper.py:1668-2008): the pairs

@@ -420,6 +420,33 @@ extern "C"
         const float *v_render_median, float *v_means2d, float *v_ray_transforms, float *v_colors, float *v_opacities,
         float *v_normals, float *v_densify, float *v_means2d_abs, void *stream
     );
+    /* Surfel compositing of the requested pixels only (rasterize_to_pixels_2dgs_sparse; no reference counterpart): one
+     * CTA per active tile, the layout and lists of gsb200_raster_sparse_fwd.  The surfel rows, backgrounds [n_images, D]
+     * and masks [n_images, th, tw] are those of gsb200_surfel_raster_fwd with n_rows rows in all (n_rows * 9 < 2^31).
+     * Outputs in the original pixel order: render_colors [P, D], render_alphas, render_distort, render_median [P],
+     * render_normals [P, 3], last_ids and median_ids int32 [P]; each the dense forward's value at that pixel.  The
+     * backward ACCUMULATES into the gradient rows of gsb200_surfel_raster_bwd ([n_rows, *], caller zero-initialises);
+     * v_render_* [P, *] with the same NULL rules. */
+    int gsb200_surfel_raster_sparse_fwd(
+        int64_t n_rows, int D, const float *means2d, const float *ray_transforms, const float *colors,
+        const float *opacities, const float *normals, const float *backgrounds, const uint8_t *masks, uint32_t image_width,
+        uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t n_active,
+        const int32_t *active_tiles, const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t n_isects,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, float *render_colors,
+        float *render_alphas, float *render_normals, float *render_distort, float *render_median, int32_t *last_ids,
+        int32_t *median_ids, void *stream
+    );
+    int gsb200_surfel_raster_sparse_bwd(
+        int64_t n_rows, int D, const float *means2d, const float *ray_transforms, const float *colors,
+        const float *opacities, const float *normals, const float *backgrounds, const uint8_t *masks, uint32_t image_width,
+        uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int64_t n_active,
+        const int32_t *active_tiles, const int32_t *tile_offsets, const int32_t *flatten_ids, int64_t n_isects,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map,
+        const float *render_colors, const float *render_alphas, const int32_t *last_ids, const int32_t *median_ids,
+        const float *v_render_colors, const float *v_render_alphas, const float *v_render_normals,
+        const float *v_render_distort, const float *v_render_median, float *v_means2d, float *v_ray_transforms,
+        float *v_colors, float *v_opacities, float *v_normals, float *v_densify, float *v_means2d_abs, void *stream
+    );
 
     /* ---- rasterize_to_indices_in_range / _2dgs (_wrapper.py:2486, :3154; kernels
      * csrc/RasterizeToIndices{3,2}DGSSerialBatch.cu, host csrc/Rasterization.cpp:954-1090) ----

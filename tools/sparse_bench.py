@@ -1,12 +1,17 @@
 """Sparse-pixel rendering against the dense pipeline on bench.py's scene (1M Gaussians, one 1920x1080 view, seed 42).
 
-    python tools/sparse_bench.py [--steps 20] [--warmup 5] [--out FILE]
+    python tools/sparse_bench.py [--2dgs] [--steps 20] [--warmup 5] [--out FILE]
 
 One step of each pipeline, timed on the host around a device synchronise (both pipelines read one count back to the
 host, so a step is not asynchronous anyway):
   sparse: build_sparse_tile_layout + isect_tiles_sparse + rasterize_to_pixels_sparse forward + backward;
   dense:  isect_tiles(conics=None) + isect_offset_encode + rasterize_to_pixels forward + backward over the whole image
           (the same radius-AABB tile lists), the loss on the requested pixels only.
+With --2dgs the same scene is projected as surfels (fully_fused_projection_2dgs, RGB + depth channel) and the pipelines
+are the 2DGS ones:
+  sparse: build_sparse_tile_layout + isect_tiles_sparse + rasterize_to_pixels_2dgs_sparse forward + backward;
+  dense:  isect_tiles_sorted + rasterize_to_pixels_2dgs forward + backward over the whole image (the same lists), the
+          loss on all five outputs at the requested pixels only.
 Workloads: (a) 4096 random pixels, (b) sixteen 64x64 patches, (c) every pixel.  The projection runs once, outside the
 timed steps.  Prints one JSON line per workload with the median step times, and the device name and power limit.
 """
@@ -62,6 +67,7 @@ def main() -> int:
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--out", help="also append the JSON lines to this file")
+    ap.add_argument("--2dgs", dest="surfels", action="store_true", help="the 2DGS pipelines on the scene's surfels")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("sparse_bench needs a GPU")
@@ -70,6 +76,8 @@ def main() -> int:
     Ks = scene.rescale_K(sc["Ks"], sc["width"], sc["height"], W, H)
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)  # noqa: E731
     N = sc["means"].shape[0]
+    if args.surfels:
+        return main_2dgs(args, sc, Ks, t, N, dev)
     with torch.no_grad():
         radii, m2, depths, conics, _ = gs.fully_fused_projection(
             t(sc["means"]), None, t(sc["quats"]), t(sc["scales"]), t(sc["viewmats"][:1]), t(Ks[:1]), W, H
@@ -79,18 +87,6 @@ def main() -> int:
     params = [x.detach().clone().requires_grad_(True) for x in (m2, conics, colors, opac)]
     info = device_info()
     lines = []
-
-    def timed(fn):
-        for _ in range(args.warmup):
-            fn()
-        torch.cuda.synchronize()
-        ts = []
-        for _ in range(args.steps):
-            t0 = time.perf_counter()
-            fn()
-            torch.cuda.synchronize()
-            ts.append(time.perf_counter() - t0)
-        return statistics.median(ts) * 1e3, min(ts) * 1e3
 
     for name, pix in workloads(np.random.RandomState(42)).items():
         pixels = t(pix.astype(np.int32))
@@ -115,8 +111,8 @@ def main() -> int:
             (rc * v_img).sum().backward()
             stats.update(dense_isects=int(fl.shape[0]))
 
-        sparse_ms, sparse_min = timed(sparse_step)
-        dense_ms, dense_min = timed(dense_step)
+        sparse_ms, sparse_min = _timed(sparse_step, args.steps, args.warmup)
+        dense_ms, dense_min = _timed(dense_step, args.steps, args.warmup)
         rec = dict(
             workload=name, pixels=P, n_gaussians=N, image=f"{W}x{H}", steps=args.steps, sparse_ms=round(sparse_ms, 3),
             sparse_min_ms=round(sparse_min, 3), dense_ms=round(dense_ms, 3), dense_min_ms=round(dense_min, 3),
@@ -125,9 +121,81 @@ def main() -> int:
         line = json.dumps(rec)
         print(line, flush=True)
         lines.append(line)
+    _write(args, lines)
+    return 0
+
+
+def _write(args, lines):
     if args.out:
         with open(args.out, "a") as f:
             f.write("\n".join(lines) + "\n")
+
+
+def _timed(fn, steps, warmup):
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(steps):
+        t0 = time.perf_counter()
+        fn()
+        torch.cuda.synchronize()
+        ts.append(time.perf_counter() - t0)
+    return statistics.median(ts) * 1e3, min(ts) * 1e3
+
+
+def main_2dgs(args, sc, Ks, t, N, dev) -> int:
+    D = 4  # RGB + the depth channel that distortion and median depth are taken from
+    with torch.no_grad():
+        radii, m2, depths, rt, nrm = gs.fully_fused_projection_2dgs(
+            t(sc["means"]), t(sc["quats"]), t(sc["scales"]), t(sc["viewmats"][:1]), t(Ks[:1]), W, H
+        )
+        colors = torch.cat([t(sc["colors"])[None], depths[..., None]], -1).contiguous()
+        opac = t(sc["opacities"])[None].contiguous()
+    params = [x.detach().clone().requires_grad_(True) for x in (m2, rt, colors, opac, nrm)]
+    densify = torch.zeros_like(m2, requires_grad=True)
+    info = device_info()
+    lines = []
+    for name, pix in workloads(np.random.RandomState(42)).items():
+        pixels = t(pix.astype(np.int32))
+        image_ids = torch.zeros(pixels.shape[0], device=dev, dtype=torch.int32)
+        P = pixels.shape[0]
+        g = torch.Generator(device=dev).manual_seed(0)
+        v = [torch.randn((P, k), device=dev, generator=g) for k in (D, 1, 3, 1, 1)]
+        v_img = []
+        for x in v:
+            img = torch.zeros((1, H, W, x.shape[-1]), device=dev)
+            img[0, pixels[:, 0].long(), pixels[:, 1].long()] = x
+            v_img.append(img)
+        stats = {}
+
+        def sparse_step():
+            active, amask, words, cum, pmap = gs.build_sparse_tile_layout(pixels, image_ids, 1, 16, TW, TH)
+            toff, fl = gs.isect_tiles_sparse(m2, radii, depths, amask, active, 1, 16, TW, TH)
+            outs = gs.rasterize_to_pixels_2dgs_sparse(
+                *params, densify, image_ids, active, toff, fl, words, cum, pmap, W, H, 16, TW, TH, distloss=True
+            )
+            sum((o * c).sum() for o, c in zip(outs, v)).backward()
+            stats.update(n_active=int(active.shape[0]), n_isects=int(fl.shape[0]))
+
+        def dense_step():
+            hits = gs.ops.isect_tiles_sorted(m2, radii, depths, 16, TW, TH)
+            off = hits.isect_offsets.reshape(1, TH, TW)
+            outs = gs.rasterize_to_pixels_2dgs(*params, densify, W, H, 16, off, hits.flatten_ids, distloss=True)
+            sum((o * c).sum() for o, c in zip(outs, v_img)).backward()
+            stats.update(dense_isects=int(hits.flatten_ids.shape[0]))
+
+        sparse_ms, sparse_min = _timed(sparse_step, args.steps, args.warmup)
+        dense_ms, dense_min = _timed(dense_step, args.steps, args.warmup)
+        rec = dict(
+            pipeline="2dgs", workload=name, pixels=P, n_gaussians=N, image=f"{W}x{H}", channels=D, steps=args.steps,
+            sparse_ms=round(sparse_ms, 3), sparse_min_ms=round(sparse_min, 3), dense_ms=round(dense_ms, 3),
+            dense_min_ms=round(dense_min, 3), sparse_over_dense=round(sparse_ms / dense_ms, 3), **stats, **info,
+        )
+        line = json.dumps(rec)
+        print(line, flush=True)
+        lines.append(line)
+    _write(args, lines)
     return 0
 
 
