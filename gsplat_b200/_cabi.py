@@ -90,7 +90,7 @@ _SIGNATURES = {
     "gsb200_nvls_allreduce_f32": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp]),
     "gsb200_p2p_allreduce_f32": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp]),
     "gsb200_rows_allreduce_f32": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp, c_vp]),
-    "gsb200_isect_count_totals": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp]),
+    "gsb200_isect_count_totals": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp]),
     "gsb200_project_sh_fwd_rows": (
         c_int,
         [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32, c_f32, c_u32,
@@ -104,8 +104,8 @@ _SIGNATURES = {
     "gsb200_isect_sorted_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_i64, c_int, c_u32, c_u32]),
     "gsb200_isect_sorted": (
         c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_vp,
-         c_vp, c_vp, c_sz, c_vp],
+        [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp,
+         c_vp, c_vp, c_vp, c_sz, c_vp],
     ),
     "gsb200_isect_ids_from_tilekeys": (c_int, [c_i64, c_int, c_vp, c_vp, c_vp, c_i64, c_u32, c_u32, c_vp, c_vp]),
     "gsb200_isect_offsets": (c_int, [c_i64, c_vp, c_i64, c_u32, c_u32, c_vp, c_vp]),
@@ -126,15 +126,7 @@ _SIGNATURES = {
     "gsb200_sparse_layout_workspace_bytes": (c_sz, [c_i64, c_i64, c_u32, c_u32]),
     "gsb200_sparse_layout_sort": (c_int, [c_i64, c_vp, c_vp, c_i64, c_u32, c_u32, c_u32, c_vp, c_sz, c_vp, c_vp]),
     "gsb200_sparse_layout_finish": (c_int, [c_i64, c_i64, c_u32, c_u32, c_i64, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_isect_sparse_count_workspace_bytes": (c_sz, [c_i64, c_i64]),
-    "gsb200_isect_sparse_count": (
-        c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp, c_sz, c_vp],
-    ),
-    "gsb200_isect_sparse_emit_workspace_bytes": (c_sz, [c_i64, c_i64, c_u32, c_u32]),
-    "gsb200_isect_sparse_emit": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp],
-    ),
+    "gsb200_isect_active_offsets": (c_int, [c_i64, c_vp, c_i64, c_u32, c_u32, c_vp, c_i64, c_vp, c_vp]),
     "gsb200_raster_sparse_fwd": (
         c_int,
         [c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp,

@@ -3,8 +3,9 @@
 // (isect.cuh), and the counts of the two units must agree bit for bit.
 //
 // In pipeline order: the per-row tile count, the depth order of the rows, the scan of the counts in that order, the
-// emission of (tile id, row) pairs, their stable sort on the tile id and the per-tile offsets; then the same stages
-// restricted to the tiles of a mask (isect_tiles_sparse).  gsb200_isect_sorted runs the dense stage in one call.
+// emission of (tile id, row) pairs, their stable sort on the tile id and the per-tile offsets.  gsb200_isect_sorted runs
+// the stages after the count in one call.  Given a tile mask (isect_tiles_sparse), the count and the emission see only
+// the tiles the mask sets, and gsb200_isect_active_offsets picks the offsets of the active tiles.
 // The sorts are cub::DeviceRadixSort::SortPairs (the library call the reference makes, csrc/IntersectTile.cu:1078-1121;
 // its onesweep kernels are compiled here for sm_90a), used twice: once over the rows that have tiles on (image, depth)
 // and once over the S intersections on the dense (image, tile) id only.
@@ -22,265 +23,9 @@ namespace gsb
 {
 constexpr int kThreads = 256;
 
-// ------------------------------------------------------------------ count
-// Row-order tile count of every row.  TOTALS: also the totals the host reads once (block_tile_totals); without them
-// this is the first pass of the unsorted intersection.
-template<bool TOTALS>
-__global__ void __launch_bounds__(kThreads) isect_count_kernel(
-    int64_t total, const float *__restrict__ means2d, const int32_t *__restrict__ radii, const float *__restrict__ conics,
-    const float *__restrict__ opacities, uint32_t tile_size, uint32_t tw, uint32_t th, int32_t *__restrict__ tiles_per_gauss,
-    unsigned long long *__restrict__ totals
-)
-{
-    unsigned long long *s_tot = nullptr;
-    if constexpr(TOTALS)
-        s_tot = block_tile_totals_begin();
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int cnt         = 0;
-    if(i < total)
-    {
-        const int2 r = reinterpret_cast<const int2 *>(radii)[i];
-        if(r.x > 0 && r.y > 0)
-        {
-            const float2 m = reinterpret_cast<const float2 *>(means2d)[i];
-            float cn[3] = {0.f, 0.f, 0.f}, op = 0.f;
-            const bool accu = conics != nullptr && opacities != nullptr;
-            if(accu)
-                cn[0] = conics[i * 3], cn[1] = conics[i * 3 + 1], cn[2] = conics[i * 3 + 2], op = opacities[i];
-            cnt = tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [](int64_t) {});
-        }
-        tiles_per_gauss[i] = cnt;
-    }
-    if constexpr(TOTALS)
-        block_tile_totals(cnt, s_tot, totals);
-}
-
-// ------------------------------------------------------------------ depth order
-// The reference sorts all S intersections on (image, tile, depth) = 45+ key bits.  Sorting the rows ONCE by
-// (image, depth) and emitting the intersections in that order leaves only the (image, tile) bits for the
-// S-sized sort: both sorts are stable, so inside a tile the result is (depth, then row index) -- exactly the
-// order the reference's single stable sort produces (csrc/Intersect.cpp:283-326).
-// keys of every projected row (the masked tile intersection orders all rows)
-__global__ void __launch_bounds__(256) depth_key_kernel(
-    int64_t total, int64_t N, const int32_t *__restrict__ radii, const float *__restrict__ depths,
-    const int64_t *__restrict__ image_ids, uint64_t *__restrict__ keys, int32_t *__restrict__ rows
-)
-{
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(i >= total)
-        return;
-    const int2 r = reinterpret_cast<const int2 *>(radii)[i];
-    uint64_t k   = ~0ull; // culled rows go last
-    if(r.x > 0 && r.y > 0)
-        k = ((uint64_t)(image_ids ? image_ids[i] : i / N) << 32) | (uint64_t)__float_as_uint(depths[i]);
-    keys[i] = k;
-    rows[i] = (int32_t)i;
-}
-
-// single image: the key is the depth's bit pattern alone (culled rows 0xffffffff sort last; a visible depth is a
-// positive finite float, never that pattern) -- 8 instead of 12 bytes per row and pass
-__global__ void __launch_bounds__(256) depth_key32_kernel(
-    int64_t total, const int32_t *__restrict__ radii, const float *__restrict__ depths, uint32_t *__restrict__ keys,
-    int32_t *__restrict__ rows
-)
-{
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(i >= total)
-        return;
-    const int2 r = reinterpret_cast<const int2 *>(radii)[i];
-    keys[i]      = (r.x > 0 && r.y > 0) ? __float_as_uint(depths[i]) : 0xffffffffu;
-    rows[i]      = (int32_t)i;
-}
-
-struct DepthOrderLayout
-{
-    size_t keys_in, keys_out, rows_in, cub, total;
-};
-static DepthOrderLayout depth_order_layout(int64_t total, int end_bit)
-{
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    DepthOrderLayout L;
-    size_t cub_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(
-        (void *)nullptr, cub_bytes, (const uint64_t *)nullptr, (uint64_t *)nullptr, (const int32_t *)nullptr, (int32_t *)nullptr,
-        total, 0, end_bit
-    );
-    L.keys_in  = 0;
-    L.keys_out = L.keys_in + al(sizeof(uint64_t) * (size_t)total);
-    L.rows_in  = L.keys_out + al(sizeof(uint64_t) * (size_t)total);
-    L.cub      = L.rows_in + al(sizeof(int32_t) * (size_t)total);
-    L.total    = L.cub + al(cub_bytes) + 256;
-    return L;
-}
-
-static size_t depth_order_workspace_bytes(int64_t I, int64_t total_rows)
-{
-    if(total_rows <= 0 || I <= 0)
-        return 0;
-    return depth_order_layout(total_rows, 32 + (int)bits_for_count(I)).total;
-}
-
-// order int32 [rows] = the projected rows in ascending (image, depth bits, row) order, culled rows (radii <= 0) last.
-// rows = I * N, or N when image_ids (packed layout) is given.
-static int depth_order(
-    int64_t I, int64_t N, const int32_t *radii, const float *depths, const int64_t *image_ids, int32_t *order,
-    void *workspace, size_t workspace_bytes, cudaStream_t st
-)
-{
-    if(I < 0 || N < 0)
-        return GSB200_E_INVALID;
-    const int64_t total = image_ids ? N : I * N; // packed: N rows in total
-    if(total == 0)
-        return GSB200_OK;
-    if(!radii || !depths || !order || !workspace || total > 0x7fffffffLL)
-        return GSB200_E_INVALID;
-    const int end_bit = 32 + (int)bits_for_count(I);
-    const auto L      = depth_order_layout(total, end_bit);
-    if(L.total > workspace_bytes)
-        return GSB200_E_WORKSPACE;
-    char *ws         = static_cast<char *>(workspace);
-    uint64_t *k_in   = reinterpret_cast<uint64_t *>(ws + L.keys_in), *k_out = reinterpret_cast<uint64_t *>(ws + L.keys_out);
-    int32_t *rows_in = reinterpret_cast<int32_t *>(ws + L.rows_in);
-    size_t cub_bytes = L.total - L.cub;
-    if(I == 1 && image_ids == nullptr)
-    { // 32-bit keys in the (larger) 64-bit key buffers; the CUB temp storage sized for 64-bit keys is ample
-        uint32_t *k32_in = reinterpret_cast<uint32_t *>(k_in), *k32_out = reinterpret_cast<uint32_t *>(k_out);
-        depth_key32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(total, radii, depths, k32_in, rows_in);
-        if(int rc = check_launch())
-            return rc;
-        size_t need = 0;
-        cub::DeviceRadixSort::SortPairs((void *)nullptr, need, k32_in, k32_out, rows_in, order, total, 0, 32, st);
-        if(need > cub_bytes)
-            return GSB200_E_WORKSPACE;
-        GSB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(ws + L.cub, need, k32_in, k32_out, rows_in, order, total, 0, 32, st));
-        return GSB200_OK;
-    }
-    depth_key_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(total, N, radii, depths, image_ids, k_in, rows_in);
-    if(int rc = check_launch())
-        return rc;
-    GSB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(ws + L.cub, cub_bytes, k_in, k_out, rows_in, order, total, 0, end_bit, st));
-    return GSB200_OK;
-}
-
-// the dense stage sorts only the rows that have tiles (gsb200_isect_sorted): their compaction, keys and counts
-struct HasTiles
-{
-    const int32_t *tiles;
-    __host__ __device__ bool operator()(const int32_t &i) const { return tiles[i] > 0; }
-};
-struct CountOfBounded
-{
-    const int32_t *tiles, *order;
-    const int64_t *totals;
-    int64_t cap;
-    __host__ __device__ int64_t operator()(const int32_t &j) const
-    {
-        const int64_t n = totals[1] < cap ? totals[1] : cap;
-        return (int64_t)j < n ? (int64_t)tiles[order[j]] : 0;
-    }
-};
-
-__global__ void __launch_bounds__(256) depth_key_rows_bounded_kernel(
-    int64_t cap_vis, int64_t N, const int32_t *__restrict__ rows, const float *__restrict__ depths,
-    const int64_t *__restrict__ image_ids, bool single_image, const int64_t *__restrict__ totals, void *__restrict__ keys
-)
-{
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(j >= cap_vis)
-        return;
-    const bool real  = j < totals[1];
-    const int64_t i  = real ? rows[j] : 0;
-    const uint32_t d = real ? __float_as_uint(depths[i]) : 0xffffffffu;
-    if(single_image)
-        static_cast<uint32_t *>(keys)[j] = d;
-    else
-        static_cast<uint64_t *>(keys)[j] = real ? (((uint64_t)(image_ids ? image_ids[i] : i / N) << 32) | (uint64_t)d) : ~0ull;
-}
-
-// ------------------------------------------------------------------ emission
-// Key of one (gaussian, tile) intersection.  int64_t: the reference's isect id, (image | tile) << 32 | depth bits
-// (csrc/IntersectTile.cu:925-988).  uint16_t / uint32_t: the dense tile id image * n_tiles + tile alone -- the rows are
-// emitted in depth order already, so the S-sized sort only needs those bits, and moving 2 + 4 instead of 8 + 4 bytes per
-// intersection and pass halves its traffic (the 64-bit ids are rebuilt on demand: isect_ids_from_tilekeys_kernel).
-template<class KeyT>
-struct IsectKey
-{
-    uint32_t base;
-    __device__ __forceinline__ IsectKey(int64_t image, uint32_t, uint32_t, int64_t n_tiles) : base((uint32_t)(image * n_tiles)) {}
-    __device__ __forceinline__ KeyT operator()(int64_t tile) const { return (KeyT)(base + (uint32_t)tile); }
-};
-template<>
-struct IsectKey<int64_t>
-{
-    int64_t hi_db;
-    __device__ __forceinline__ IsectKey(int64_t image, uint32_t dbits, uint32_t tile_n_bits, int64_t)
-        : hi_db((image << (32 + tile_n_bits)) | (int64_t)dbits)
-    {
-    }
-    __device__ __forceinline__ int64_t operator()(int64_t tile) const { return hi_db | (tile << 32); }
-};
-
-// Capacity-bounded emission (gsb200_isect_sorted): the launch covers `total` = capacity row slots and writes into
-// capacity-sized outputs, while the real counts sit in device memory (totals[0] intersections, totals[1] rows with
-// tiles).  Returns the number of real row slots; the slots between the real intersections and the capacity get padding
-// pairs (largest key: the stable sort leaves them behind every real pair; row 0: any valid row).
-template<class KeyT>
-__device__ __forceinline__ int64_t emit_bounded_rows(
-    int64_t j, int64_t n_threads, int64_t total, const int64_t *__restrict__ totals, int64_t cap_isects,
-    KeyT *__restrict__ isect_ids, int32_t *__restrict__ flatten_ids
-)
-{
-    const int64_t n_real = totals[0] < cap_isects ? totals[0] : cap_isects;
-    for(int64_t s = n_real + j; s < cap_isects; s += n_threads)
-    {
-        isect_ids[s]   = (KeyT)~(KeyT)0;
-        flatten_ids[s] = 0;
-    }
-    return totals[1] < total ? totals[1] : total;
-}
-
-template<class KeyT>
-__global__ void __launch_bounds__(kThreads) isect_emit_kernel(
-    int64_t total, int64_t N, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
-    const float *__restrict__ depths, const float *__restrict__ conics, const float *__restrict__ opacities,
-    const int64_t *__restrict__ cum_tiles, const int64_t *__restrict__ image_ids, const int32_t *__restrict__ order,
-    uint32_t tile_size, uint32_t tw, uint32_t th, uint32_t tile_n_bits, KeyT *__restrict__ isect_ids,
-    int32_t *__restrict__ flatten_ids, const int64_t *__restrict__ totals = nullptr, int64_t cap_isects = 0
-)
-{
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(totals != nullptr)
-        total = emit_bounded_rows<KeyT>(j, (int64_t)gridDim.x * blockDim.x, total, totals, cap_isects, isect_ids, flatten_ids);
-    if(j >= total)
-        return;
-    if(totals != nullptr && cum_tiles[j] > cap_isects)
-        return; // beyond the speculative capacity: the host sees totals[0] > capacity and redoes the stage
-    const int64_t i = order ? (int64_t)order[j] : j;
-    const int2 r    = reinterpret_cast<const int2 *>(radii)[i];
-    if(r.x <= 0 || r.y <= 0)
-        return;
-    const float2 m = reinterpret_cast<const float2 *>(means2d)[i];
-    float cn[3] = {0.f, 0.f, 0.f}, op = 0.f;
-    const bool accu = conics != nullptr && opacities != nullptr;
-    if(accu)
-        cn[0] = conics[i * 3], cn[1] = conics[i * 3 + 1], cn[2] = conics[i * 3 + 2], op = opacities[i];
-    int64_t cur         = (j == 0) ? 0 : cum_tiles[j - 1];
-    // packed rows carry their image id
-    const IsectKey<KeyT> key(image_ids ? image_ids[i] : (i / N), __float_as_uint(depths[i]), tile_n_bits, (int64_t)tw * th);
-    tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [&](int64_t tile) {
-        isect_ids[cur]   = key(tile);
-        flatten_ids[cur] = (int32_t)i;
-        ++cur;
-    });
-}
-
-// ---- warp-cooperative emit.  One thread per gaussian with a loop over ITS tiles (isect_emit_kernel) leaves a warp
-// waiting for its largest gaussian and writes 8 + 4 byte records at lane-dependent strides: at S = 20 M (large
-// screen-space gaussians) it took 444 us for 240 MB of output.  Here a gaussian with more than kSmallTiles tiles is
-// handed to its whole warp: the tile interval of every tile row is a closed form of the row index (the incremental
-// scheme of tiles_of_gaussian only carries the previous row's far line over as the next row's near line), so lane r
-// computes row ru0 + r, a warp scan places the rows, and the lanes then write the tiles round-robin -- consecutive
-// lanes, consecutive addresses -- in the same order as the sequential enumeration.
+// ------------------------------------------------------------------ tile rows
+// The tiles of one gaussian row by row, each row's tile interval in closed form: how a warp shares the rows of a
+// gaussian with many tiles (the masked count, isect_emit_coop_kernel).
 constexpr int kSmallTiles = 64; // measured: below ~2 warps' worth of tiles the per-gaussian warp hand-over costs more than it saves
 
 struct AccuGauss
@@ -381,6 +126,228 @@ __device__ __forceinline__ void accu_row(const AccuGauss &g, int u, int &v0, int
         v1 = v0;
 }
 
+// ------------------------------------------------------------------ count
+// A masked row with more tiles than this is counted by its whole warp.  Measured on an H100 80GB HBM3 at 700 W, bench.py's
+// scene (1M rows, one 1080p view): handing over rows above 64 tiles, the masked count of the 3DGS rows took 29 us, above
+// 256 tiles 23 us (the same up to 1024); that of the surfel rows takes 100 us either way, 230 us without any hand-over.
+constexpr int kManyMaskedTiles = 256;
+
+// Row-order tile count of every row.  TOTALS: also the totals the host reads once (block_tile_totals); without them
+// this is the first pass of the unsorted intersection.  MASKED: only the tiles whose byte in tile_mask [I, th, tw] is
+// set count; row i belongs to image image_ids[i], or i / N without image_ids.
+template<bool TOTALS, bool MASKED = false>
+__global__ void __launch_bounds__(kThreads) isect_count_kernel(
+    int64_t total, const float *__restrict__ means2d, const int32_t *__restrict__ radii, const float *__restrict__ conics,
+    const float *__restrict__ opacities, uint32_t tile_size, uint32_t tw, uint32_t th, int32_t *__restrict__ tiles_per_gauss,
+    unsigned long long *__restrict__ totals, int64_t N = 0, int64_t I = 0, const int64_t *__restrict__ image_ids = nullptr,
+    const uint8_t *__restrict__ tile_mask = nullptr
+)
+{
+    unsigned long long *s_tot = nullptr;
+    if constexpr(TOTALS)
+        s_tot = block_tile_totals_begin();
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int cnt         = 0;
+    bool many       = false; // MASKED: a row of more than kManyMaskedTiles tiles
+    if(i < total)
+    {
+        const int2 r = reinterpret_cast<const int2 *>(radii)[i];
+        if(r.x > 0 && r.y > 0)
+        {
+            const float2 m = reinterpret_cast<const float2 *>(means2d)[i];
+            float cn[3] = {0.f, 0.f, 0.f}, op = 0.f;
+            const bool accu = conics != nullptr && opacities != nullptr;
+            if(accu)
+                cn[0] = conics[i * 3], cn[1] = conics[i * 3 + 1], cn[2] = conics[i * 3 + 2], op = opacities[i];
+            if constexpr(MASKED)
+            {
+                // the mask has no bytes for an image outside [0, I): such a row counts no tile, so the compaction drops
+                // it and no later pass reads its image
+                const int64_t img = image_ids ? image_ids[i] : i / N;
+                if(img >= 0 && img < I)
+                {
+                    const uint8_t *tm = tile_mask + img * (int64_t)tw * th;
+                    many = tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [](int64_t) {})
+                           > kManyMaskedTiles;
+                    if(!many)
+                        tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [&](int64_t t) {
+                            cnt += tm[t] != 0;
+                        });
+                }
+            }
+            else
+                cnt = tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [](int64_t) {});
+        }
+        if constexpr(!MASKED)
+            tiles_per_gauss[i] = cnt;
+    }
+    if constexpr(MASKED)
+    {
+        // Rows with many tiles (large gaussians near the camera) lie scattered over the row order: one lane looping over
+        // all the tiles of such a row would hold its warp for each of them.  Here the warp counts the row, one tile row per
+        // lane, with the row intervals of accu_row (the tiles of tiles_of_gaussian).
+        const unsigned lane = threadIdx.x & 31;
+        for(uint32_t big = __ballot_sync(0xffffffffu, many); big; big &= big - 1)
+        {
+            const int src      = __ffs(big) - 1;
+            const int64_t b    = i - (int64_t)lane + src;
+            const int2 r       = reinterpret_cast<const int2 *>(radii)[b];
+            const float2 m     = reinterpret_cast<const float2 *>(means2d)[b];
+            const bool accu    = conics != nullptr && opacities != nullptr;
+            const AccuGauss g  = accu_setup(
+                m.x, m.y, r.x, r.y, accu, accu ? conics[b * 3] : 0.f, accu ? conics[b * 3 + 1] : 0.f,
+                accu ? conics[b * 3 + 2] : 0.f, accu ? opacities[b] : 0.f, tile_size, tw, th
+            );
+            const uint8_t *tm = tile_mask + (image_ids ? image_ids[b] : b / N) * (int64_t)tw * th;
+            int c             = 0;
+            for(int u = g.ru0 + (int)lane; u < g.ru1; u += 32)
+            {
+                int v0 = 0, v1 = 0;
+                accu_row(g, u, v0, v1);
+                for(int v = v0; v < v1; ++v)
+                    c += tm[g.isY ? (int64_t)u * tw + v : (int64_t)v * tw + u] != 0;
+            }
+            c = __reduce_add_sync(0xffffffffu, c);
+            if((int)lane == src)
+                cnt = c;
+        }
+        if(i < total)
+            tiles_per_gauss[i] = cnt;
+    }
+    if constexpr(TOTALS)
+        block_tile_totals(cnt, s_tot, totals);
+}
+
+// ------------------------------------------------------------------ depth order
+// The reference sorts all S intersections on (image, tile, depth) = 45+ key bits.  Sorting the rows ONCE by
+// (image, depth) and emitting the intersections in that order leaves only the (image, tile) bits for the
+// S-sized sort: both sorts are stable, so inside a tile the result is (depth, then row index) -- exactly the
+// order the reference's single stable sort produces (csrc/Intersect.cpp:283-326).
+// gsb200_isect_sorted sorts only the rows that have tiles: their compaction, keys and counts
+struct HasTiles
+{
+    const int32_t *tiles;
+    __host__ __device__ bool operator()(const int32_t &i) const { return tiles[i] > 0; }
+};
+struct CountOfBounded
+{
+    const int32_t *tiles, *order;
+    const int64_t *totals;
+    int64_t cap;
+    __host__ __device__ int64_t operator()(const int32_t &j) const
+    {
+        const int64_t n = totals[1] < cap ? totals[1] : cap;
+        return (int64_t)j < n ? (int64_t)tiles[order[j]] : 0;
+    }
+};
+
+__global__ void __launch_bounds__(256) depth_key_rows_bounded_kernel(
+    int64_t cap_vis, int64_t N, const int32_t *__restrict__ rows, const float *__restrict__ depths,
+    const int64_t *__restrict__ image_ids, bool single_image, const int64_t *__restrict__ totals, void *__restrict__ keys
+)
+{
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(j >= cap_vis)
+        return;
+    const bool real  = j < totals[1];
+    const int64_t i  = real ? rows[j] : 0;
+    const uint32_t d = real ? __float_as_uint(depths[i]) : 0xffffffffu;
+    if(single_image)
+        static_cast<uint32_t *>(keys)[j] = d;
+    else
+        static_cast<uint64_t *>(keys)[j] = real ? (((uint64_t)(image_ids ? image_ids[i] : i / N) << 32) | (uint64_t)d) : ~0ull;
+}
+
+// ------------------------------------------------------------------ emission
+// Key of one (gaussian, tile) intersection.  int64_t: the reference's isect id, (image | tile) << 32 | depth bits
+// (csrc/IntersectTile.cu:925-988).  uint16_t / uint32_t: the dense tile id image * n_tiles + tile alone -- the rows are
+// emitted in depth order already, so the S-sized sort only needs those bits, and moving 2 + 4 instead of 8 + 4 bytes per
+// intersection and pass halves its traffic (the 64-bit ids are rebuilt on demand: isect_ids_from_tilekeys_kernel).
+template<class KeyT>
+struct IsectKey
+{
+    uint32_t base;
+    __device__ __forceinline__ IsectKey(int64_t image, uint32_t, uint32_t, int64_t n_tiles) : base((uint32_t)(image * n_tiles)) {}
+    __device__ __forceinline__ KeyT operator()(int64_t tile) const { return (KeyT)(base + (uint32_t)tile); }
+};
+template<>
+struct IsectKey<int64_t>
+{
+    int64_t hi_db;
+    __device__ __forceinline__ IsectKey(int64_t image, uint32_t dbits, uint32_t tile_n_bits, int64_t)
+        : hi_db((image << (32 + tile_n_bits)) | (int64_t)dbits)
+    {
+    }
+    __device__ __forceinline__ int64_t operator()(int64_t tile) const { return hi_db | (tile << 32); }
+};
+
+// Capacity-bounded emission (gsb200_isect_sorted): the launch covers `total` = capacity row slots and writes into
+// capacity-sized outputs, while the real counts sit in device memory (totals[0] intersections, totals[1] rows with
+// tiles).  Returns the number of real row slots; the slots between the real intersections and the capacity get padding
+// pairs (largest key: the stable sort leaves them behind every real pair; row 0: any valid row).
+template<class KeyT>
+__device__ __forceinline__ int64_t emit_bounded_rows(
+    int64_t j, int64_t n_threads, int64_t total, const int64_t *__restrict__ totals, int64_t cap_isects,
+    KeyT *__restrict__ isect_ids, int32_t *__restrict__ flatten_ids
+)
+{
+    const int64_t n_real = totals[0] < cap_isects ? totals[0] : cap_isects;
+    for(int64_t s = n_real + j; s < cap_isects; s += n_threads)
+    {
+        isect_ids[s]   = (KeyT)~(KeyT)0;
+        flatten_ids[s] = 0;
+    }
+    return totals[1] < total ? totals[1] : total;
+}
+
+// MASKED: only the tiles whose byte in tile_mask [I, th, tw] is set are emitted, as the masked count counted them.
+template<class KeyT, bool MASKED = false>
+__global__ void __launch_bounds__(kThreads) isect_emit_kernel(
+    int64_t total, int64_t N, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
+    const float *__restrict__ depths, const float *__restrict__ conics, const float *__restrict__ opacities,
+    const int64_t *__restrict__ cum_tiles, const int64_t *__restrict__ image_ids, const int32_t *__restrict__ order,
+    uint32_t tile_size, uint32_t tw, uint32_t th, uint32_t tile_n_bits, KeyT *__restrict__ isect_ids,
+    int32_t *__restrict__ flatten_ids, const int64_t *__restrict__ totals = nullptr, int64_t cap_isects = 0,
+    const uint8_t *__restrict__ tile_mask = nullptr
+)
+{
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(totals != nullptr)
+        total = emit_bounded_rows<KeyT>(j, (int64_t)gridDim.x * blockDim.x, total, totals, cap_isects, isect_ids, flatten_ids);
+    if(j >= total)
+        return;
+    if(totals != nullptr && cum_tiles[j] > cap_isects)
+        return; // beyond the speculative capacity: the host sees totals[0] > capacity and redoes the stage
+    const int64_t i = order ? (int64_t)order[j] : j;
+    const int2 r    = reinterpret_cast<const int2 *>(radii)[i];
+    if(r.x <= 0 || r.y <= 0)
+        return;
+    const float2 m = reinterpret_cast<const float2 *>(means2d)[i];
+    float cn[3] = {0.f, 0.f, 0.f}, op = 0.f;
+    const bool accu = conics != nullptr && opacities != nullptr;
+    if(accu)
+        cn[0] = conics[i * 3], cn[1] = conics[i * 3 + 1], cn[2] = conics[i * 3 + 2], op = opacities[i];
+    int64_t cur         = (j == 0) ? 0 : cum_tiles[j - 1];
+    // packed rows carry their image id
+    const int64_t img = image_ids ? image_ids[i] : (i / N);
+    const IsectKey<KeyT> key(img, __float_as_uint(depths[i]), tile_n_bits, (int64_t)tw * th);
+    const uint8_t *tm = MASKED ? tile_mask + img * (int64_t)tw * th : nullptr;
+    tiles_of_gaussian(m.x, m.y, r.x, r.y, accu ? cn : nullptr, accu ? &op : nullptr, tile_size, tw, th, [&](int64_t tile) {
+        if(MASKED && tm[tile] == 0)
+            return;
+        isect_ids[cur]   = key(tile);
+        flatten_ids[cur] = (int32_t)i;
+        ++cur;
+    });
+}
+
+// ---- warp-cooperative emit.  One thread per gaussian with a loop over ITS tiles (isect_emit_kernel) leaves a warp
+// waiting for its largest gaussian and writes 8 + 4 byte records at lane-dependent strides: at S = 20 M (large
+// screen-space gaussians) it took 444 us for 240 MB of output.  Here a gaussian with more than kSmallTiles tiles is
+// handed to its whole warp: the tile interval of every tile row is a closed form of the row index (the incremental
+// scheme of tiles_of_gaussian only carries the previous row's far line over as the next row's near line), so lane r
+// computes row ru0 + r, a warp scan places the rows, and the lanes then write the tiles round-robin -- consecutive
+// lanes, consecutive addresses -- in the same order as the sequential enumeration.
 template<class KeyT>
 __global__ void __launch_bounds__(kThreads) isect_emit_coop_kernel(
     int64_t total, int64_t N, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
@@ -505,9 +472,9 @@ static auto with_key_type(int key_bytes, F &&f)
 // capacity-sized outputs, real counts in `totals` (device)
 static int emit_tilekeys_bounded(
     int64_t N, int64_t cap_vis, int64_t max_tiles_hint, const float *means2d, const int32_t *radii, const float *depths,
-    const float *conics, const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, const int32_t *order,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int key_bytes, void *keys, int32_t *flatten_ids,
-    const int64_t *totals, int64_t cap_isects, cudaStream_t st
+    const float *conics, const float *opacities, const int64_t *cum_tiles, const int64_t *image_ids, const uint8_t *tile_mask,
+    const int32_t *order, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int key_bytes, void *keys,
+    int32_t *flatten_ids, const int64_t *totals, int64_t cap_isects, cudaStream_t st
 )
 {
     const uint32_t tile_bits = bits_for_count((int64_t)tile_width * tile_height);
@@ -517,7 +484,13 @@ static int emit_tilekeys_bounded(
     const bool serial = max_tiles_hint > 0 && max_tiles_hint <= 96;
     return with_key_type(key_bytes, [&](auto key) {
         using KeyT = decltype(key);
-        if(serial)
+        // a mask breaks the contiguous per-row tile intervals the cooperative kernel places: one thread per row
+        if(tile_mask != nullptr)
+            isect_emit_kernel<KeyT, true><<<grid_for(cap_vis, kThreads), kThreads, 0, st>>>(
+                cap_vis, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width,
+                tile_height, tile_bits, static_cast<KeyT *>(keys), flatten_ids, totals, cap_isects, tile_mask
+            );
+        else if(serial)
             isect_emit_kernel<KeyT><<<grid_for(cap_vis, kThreads), kThreads, 0, st>>>(
                 cap_vis, N, means2d, radii, depths, conics, opacities, cum_tiles, image_ids, order, tile_size, tile_width,
                 tile_height, tile_bits, static_cast<KeyT *>(keys), flatten_ids, totals, cap_isects
@@ -627,6 +600,20 @@ static int offsets_tilekeys_bounded(
     });
 }
 
+// tile_offsets[a] = offsets[active_tiles[a]] for a < n_active, tile_offsets[n_active] = n_isects.  The ids come from the
+// caller unchecked: one outside [0, total_tiles) gets n_isects, as if it were a tile past the last one.
+__global__ void __launch_bounds__(kThreads) isect_active_offsets_kernel(
+    int64_t n_active, const int32_t *__restrict__ active_tiles, int64_t total_tiles, const int32_t *__restrict__ offsets,
+    int64_t n_isects, int32_t *__restrict__ tile_offsets
+)
+{
+    const int64_t a = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(a > n_active)
+        return;
+    const int64_t t = a < n_active ? (int64_t)active_tiles[a] : -1;
+    tile_offsets[a] = t >= 0 && t < total_tiles ? offsets[t] : (int32_t)n_isects;
+}
+
 // the reference's 64-bit intersection ids, rebuilt from the sorted tile ids and the rows' depths
 template<class KeyT>
 __global__ void __launch_bounds__(kThreads) isect_ids_from_tilekeys_kernel(
@@ -691,140 +678,6 @@ __global__ void publish_totals_kernel(const int64_t *__restrict__ totals, volati
     __syncwarp();
     if(threadIdx.x == 0)
         host[3] = seq;
-}
-
-// ------------------------------------------------------------------ masked tile intersection
-// Tile intersection restricted to the tiles of a mask (isect_tiles_sparse).  Same enumeration as the dense AABB
-// path (tiles_of_gaussian without conics), in the depth order of depth_order above; a tile whose tile_mask entry
-// is 0 is neither counted nor emitted.  Keys are dense tile ids image * th * tw + tile (32 bits).
-__device__ __forceinline__ int64_t masked_row_image(int64_t i, int64_t N, const int64_t *__restrict__ image_ids)
-{
-    return image_ids ? image_ids[i] : i / N;
-}
-
-__global__ void __launch_bounds__(kThreads) isect_count_masked_kernel(
-    int64_t total, int64_t N, int64_t I, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
-    const int64_t *__restrict__ image_ids, const uint8_t *__restrict__ tile_mask, const int32_t *__restrict__ order,
-    uint32_t tile_size, uint32_t tw, uint32_t th, int32_t *__restrict__ counts_in_order
-)
-{
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(j >= total)
-        return;
-    const int64_t i = order[j];
-    const int2 r    = reinterpret_cast<const int2 *>(radii)[i];
-    int cnt         = 0;
-    const int64_t img = masked_row_image(i, N, image_ids);
-    if(r.x > 0 && r.y > 0 && img >= 0 && img < I)
-    {
-        const float2 m     = reinterpret_cast<const float2 *>(means2d)[i];
-        const uint8_t *tm  = tile_mask + img * (int64_t)tw * th;
-        tiles_of_gaussian(m.x, m.y, r.x, r.y, nullptr, nullptr, tile_size, tw, th, [&](int64_t t) { cnt += tm[t] != 0; });
-    }
-    counts_in_order[j] = cnt;
-}
-
-__global__ void __launch_bounds__(kThreads) isect_emit_masked_kernel(
-    int64_t total, int64_t N, int64_t I, const float *__restrict__ means2d, const int32_t *__restrict__ radii,
-    const int64_t *__restrict__ image_ids, const uint8_t *__restrict__ tile_mask, const int32_t *__restrict__ order,
-    const int64_t *__restrict__ cum_tiles, uint32_t tile_size, uint32_t tw, uint32_t th, uint32_t *__restrict__ keys,
-    int32_t *__restrict__ flatten_ids
-)
-{
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(j >= total)
-        return;
-    int64_t cur       = j == 0 ? 0 : cum_tiles[j - 1];
-    const int64_t end = cum_tiles[j];
-    if(end == cur)
-        return;
-    const int64_t i   = order[j];
-    const int2 r      = reinterpret_cast<const int2 *>(radii)[i];
-    const float2 m    = reinterpret_cast<const float2 *>(means2d)[i];
-    const int64_t img = masked_row_image(i, N, image_ids);
-    const uint8_t *tm = tile_mask + img * (int64_t)tw * th;
-    const uint32_t base = (uint32_t)(img * (int64_t)tw * th);
-    tiles_of_gaussian(m.x, m.y, r.x, r.y, nullptr, nullptr, tile_size, tw, th, [&](int64_t t) {
-        if(tm[t] != 0 && cur < end)
-        {
-            keys[cur]        = base + (uint32_t)t;
-            flatten_ids[cur] = (int32_t)i;
-            ++cur;
-        }
-    });
-}
-
-// tile_offsets[a] = first sorted intersection of active tile a (lower bound of its id in the sorted keys), a < AT;
-// tile_offsets[AT] = n_isects
-__global__ void __launch_bounds__(kThreads) isect_offsets_sparse_kernel(
-    int64_t n_active, const int32_t *__restrict__ active_tiles, int64_t n_isects, const uint32_t *__restrict__ keys,
-    int32_t *__restrict__ tile_offsets
-)
-{
-    const int64_t a = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if(a > n_active)
-        return;
-    if(a == n_active)
-    {
-        tile_offsets[a] = (int32_t)n_isects;
-        return;
-    }
-    const uint32_t t = (uint32_t)active_tiles[a];
-    int64_t lo = 0, hi = n_isects;
-    while(lo < hi)
-    {
-        const int64_t mid = (lo + hi) >> 1;
-        if(keys[mid] < t)
-            lo = mid + 1;
-        else
-            hi = mid;
-    }
-    tile_offsets[a] = (int32_t)lo;
-}
-
-struct SparseCountLayout
-{
-    size_t depth, counts, scan, total;
-};
-static SparseCountLayout sparse_count_layout(int64_t I, int64_t total)
-{
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    SparseCountLayout L;
-    size_t scan = 0;
-    cub::DeviceScan::InclusiveSum((void *)nullptr, scan, (const int32_t *)nullptr, (int64_t *)nullptr, total);
-    L.depth  = 0;
-    L.counts = L.depth + al(depth_order_workspace_bytes(I, total));
-    L.scan   = L.counts + al(sizeof(int32_t) * (size_t)total);
-    L.total  = L.scan + al(scan) + 256;
-    return L;
-}
-
-struct SparseEmitLayout
-{
-    size_t keys_in, vals_in, keys_out, sort, total;
-};
-static SparseEmitLayout sparse_emit_layout(int64_t n_isects, int end_bit)
-{
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    SparseEmitLayout L;
-    L.keys_in  = 0;
-    L.vals_in  = L.keys_in + al(sizeof(uint32_t) * (size_t)n_isects);
-    L.keys_out = L.vals_in + al(sizeof(int32_t) * (size_t)n_isects);
-    L.sort     = L.keys_out + al(sizeof(uint32_t) * (size_t)n_isects);
-    L.total    = L.sort + al(sort_tile_pairs_workspace_bytes<uint32_t>(n_isects, end_bit) + 256) + 256;
-    return L;
-}
-
-static int sparse_isect_args(int64_t I, int64_t N, const int64_t *image_ids, uint32_t tile_size, uint32_t tw, uint32_t th, int64_t &total)
-{
-    if(I < 0 || N < 0 || tile_size == 0)
-        return GSB200_E_INVALID;
-    total = image_ids ? N : I * N; // packed: N rows, image_ids[i] in [0, I)
-    if(total > 0x7fffffffLL)
-        return GSB200_E_INVALID;
-    if(bits_for_count(I) + bits_for_count((int64_t)tw * th) > 32)
-        return GSB200_E_KEYBITS;
-    return GSB200_OK;
 }
 
 } // namespace gsb
@@ -897,24 +750,32 @@ extern "C" int gsb200_isect_emit(
 
 extern "C" int gsb200_isect_count_totals(
     int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *conics, const float *opacities,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *tiles_per_gauss, int64_t *totals, void *stream
+    const int64_t *image_ids, const uint8_t *tile_mask, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+    int32_t *tiles_per_gauss, int64_t *totals, void *stream
 )
 {
     if(I < 0 || N < 0 || tile_size == 0 || !totals)
         return GSB200_E_INVALID;
     cudaStream_t st = (cudaStream_t)stream;
     GSB_CUDA_TRY(cudaMemsetAsync(totals, 0, 3 * sizeof(int64_t), st));
-    const int64_t total = I * N;
+    // the rows of gsb200_isect_sorted: N rows in total when image_ids is given, else I * N
+    const int64_t total = image_ids ? N : I * N;
     if(total == 0)
         return GSB200_OK;
     if(!means2d || !radii || !tiles_per_gauss || total > 0x7fffffffLL)
         return GSB200_E_INVALID;
     if(bits_for_count(I) + bits_for_count((int64_t)tile_width * tile_height) > 32)
         return GSB200_E_KEYBITS;
-    isect_count_kernel<true><<<grid_for(total, kThreads), kThreads, 0, st>>>(
-        total, means2d, radii, conics, opacities, tile_size, tile_width, tile_height, tiles_per_gauss,
-        reinterpret_cast<unsigned long long *>(totals)
-    );
+    unsigned long long *tot = reinterpret_cast<unsigned long long *>(totals);
+    if(tile_mask != nullptr)
+        isect_count_kernel<true, true><<<grid_for(total, kThreads), kThreads, 0, st>>>(
+            total, means2d, radii, conics, opacities, tile_size, tile_width, tile_height, tiles_per_gauss, tot, N, I, image_ids,
+            tile_mask
+        );
+    else
+        isect_count_kernel<true><<<grid_for(total, kThreads), kThreads, 0, st>>>(
+            total, means2d, radii, conics, opacities, tile_size, tile_width, tile_height, tiles_per_gauss, tot
+        );
     return check_launch();
 }
 
@@ -943,10 +804,10 @@ extern "C" size_t gsb200_isect_sorted_workspace_bytes(
 
 extern "C" int gsb200_isect_sorted(
     int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const float *conics,
-    const float *opacities, const int64_t *image_ids, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
-    const int32_t *tiles_per_gauss, const int64_t *totals, int64_t cap_vis, int64_t cap_isects, int64_t max_tiles_hint,
-    int key_bytes, void *tile_keys, int32_t *flatten_ids, int32_t *offsets, void *workspace, size_t workspace_bytes,
-    void *stream
+    const float *opacities, const int64_t *image_ids, const uint8_t *tile_mask, uint32_t tile_size, uint32_t tile_width,
+    uint32_t tile_height, const int32_t *tiles_per_gauss, const int64_t *totals, int64_t cap_vis, int64_t cap_isects,
+    int64_t max_tiles_hint, int key_bytes, void *tile_keys, int32_t *flatten_ids, int32_t *offsets, void *workspace,
+    size_t workspace_bytes, void *stream
 )
 {
     if(I <= 0 || N <= 0 || cap_vis <= 0 || cap_isects <= 0 || tile_size == 0 || (key_bytes != 2 && key_bytes != 4))
@@ -1003,8 +864,8 @@ extern "C" int gsb200_isect_sorted(
     GSB_CUDA_TRY(cub::DeviceScan::InclusiveSum(ws + L.cub, cub_bytes, it, cum, cap_vis, st));
     // 4. emission in depth order, (dense tile id, row) pairs; 5. stable sort on the tile id; 6. offsets
     if(int rc = emit_tilekeys_bounded(
-           N, cap_vis, max_tiles_hint, means2d, radii, depths, conics, opacities, cum, image_ids, order, tile_size, tile_width,
-           tile_height, key_bytes, tkeys, tvals, totals, cap_isects, st
+           N, cap_vis, max_tiles_hint, means2d, radii, depths, conics, opacities, cum, image_ids, tile_mask, order, tile_size,
+           tile_width, tile_height, key_bytes, tkeys, tvals, totals, cap_isects, st
        ))
         return rc;
     if(int rc = with_key_type(key_bytes, [&](auto key) {
@@ -1077,93 +938,17 @@ extern "C" int gsb200_isect_offsets(
     return check_launch();
 }
 
-extern "C" size_t gsb200_isect_sparse_count_workspace_bytes(int64_t I, int64_t total_rows)
-{
-    if(I <= 0 || total_rows <= 0)
-        return 0;
-    return sparse_count_layout(I, total_rows).total;
-}
-
-extern "C" int gsb200_isect_sparse_count(
-    int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const int64_t *image_ids,
-    const uint8_t *tile_mask, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *order,
-    int64_t *cum_tiles, void *workspace, size_t workspace_bytes, void *stream
+extern "C" int gsb200_isect_active_offsets(
+    int64_t n_active, const int32_t *active_tiles, int64_t I, uint32_t tile_width, uint32_t tile_height,
+    const int32_t *offsets, int64_t n_isects, int32_t *tile_offsets, void *stream
 )
 {
-    int64_t total = 0;
-    if(int rc = sparse_isect_args(I, N, image_ids, tile_size, tile_width, tile_height, total))
-        return rc;
-    if(total == 0)
-        return GSB200_OK;
-    if(!means2d || !radii || !depths || !tile_mask || !order || !cum_tiles || !workspace)
+    const int64_t total_tiles = I * (int64_t)tile_width * tile_height;
+    if(n_active < 0 || I < 0 || n_isects < 0 || n_isects > 0x7fffffffLL || !tile_offsets || (n_active > 0 && !active_tiles)
+       || (total_tiles > 0 && !offsets))
         return GSB200_E_INVALID;
-    const auto L = sparse_count_layout(I, total);
-    if(L.total > workspace_bytes)
-        return GSB200_E_WORKSPACE;
-    char *ws        = static_cast<char *>(workspace);
-    cudaStream_t st = (cudaStream_t)stream;
-    // 1. rows in (image, depth) order
-    if(int rc = depth_order(I, N, radii, depths, image_ids, order, ws + L.depth, L.counts - L.depth, st))
-        return rc;
-    // 2. masked tile counts in that order; 3. inclusive scan
-    int32_t *counts = reinterpret_cast<int32_t *>(ws + L.counts);
-    isect_count_masked_kernel<<<grid_for(total, kThreads), kThreads, 0, st>>>(
-        total, N, I, means2d, radii, image_ids, tile_mask, order, tile_size, tile_width, tile_height, counts
-    );
-    if(int rc = check_launch())
-        return rc;
-    size_t scan_bytes = L.total - L.scan;
-    GSB_CUDA_TRY(cub::DeviceScan::InclusiveSum(ws + L.scan, scan_bytes, counts, cum_tiles, total, st));
-    return GSB200_OK;
-}
-
-extern "C" size_t gsb200_isect_sparse_emit_workspace_bytes(int64_t I, int64_t n_isects, uint32_t tile_width, uint32_t tile_height)
-{
-    if(I <= 0 || n_isects <= 0)
-        return 0;
-    const int end_bit = (int)bits_for_count(I * (int64_t)tile_width * tile_height);
-    return sparse_emit_layout(n_isects, end_bit > 0 ? end_bit : 1).total;
-}
-
-extern "C" int gsb200_isect_sparse_emit(
-    int64_t I, int64_t N, const float *means2d, const int32_t *radii, const int64_t *image_ids, const uint8_t *tile_mask,
-    uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *order, const int64_t *cum_tiles,
-    int64_t n_isects, int64_t n_active, const int32_t *active_tiles, int32_t *tile_offsets, int32_t *flatten_ids,
-    void *workspace, size_t workspace_bytes, void *stream
-)
-{
-    int64_t total = 0;
-    if(int rc = sparse_isect_args(I, N, image_ids, tile_size, tile_width, tile_height, total))
-        return rc;
-    if(n_isects < 0 || n_isects > 0x7fffffffLL || n_active < 0 || !tile_offsets || (n_active > 0 && !active_tiles))
-        return GSB200_E_INVALID;
-    cudaStream_t st = (cudaStream_t)stream;
-    const uint32_t *sorted = nullptr;
-    if(n_isects > 0)
-    {
-        if(total == 0 || !means2d || !radii || !tile_mask || !order || !cum_tiles || !flatten_ids || !workspace)
-            return GSB200_E_INVALID;
-        int end_bit  = (int)bits_for_count(I * (int64_t)tile_width * tile_height);
-        end_bit      = end_bit > 0 ? end_bit : 1;
-        const auto L = sparse_emit_layout(n_isects, end_bit);
-        if(L.total > workspace_bytes)
-            return GSB200_E_WORKSPACE;
-        char *ws          = static_cast<char *>(workspace);
-        uint32_t *keys_in = reinterpret_cast<uint32_t *>(ws + L.keys_in), *keys_out = reinterpret_cast<uint32_t *>(ws + L.keys_out);
-        int32_t *vals_in  = reinterpret_cast<int32_t *>(ws + L.vals_in);
-        // 4. emission in depth order; 5. stable sort on the (image, tile) bits
-        isect_emit_masked_kernel<<<grid_for(total, kThreads), kThreads, 0, st>>>(
-            total, N, I, means2d, radii, image_ids, tile_mask, order, cum_tiles, tile_size, tile_width, tile_height, keys_in, vals_in
-        );
-        if(int rc = check_launch())
-            return rc;
-        if(int rc = sort_tile_pairs<uint32_t>(n_isects, end_bit, keys_in, vals_in, keys_out, flatten_ids, ws + L.sort, L.total - L.sort, st))
-            return rc;
-        sorted = keys_out;
-    }
-    // 6. per-active-tile offsets from the sorted keys
-    isect_offsets_sparse_kernel<<<grid_for(n_active + 1, kThreads), kThreads, 0, st>>>(
-        n_active, active_tiles, n_isects, sorted, tile_offsets
+    isect_active_offsets_kernel<<<grid_for(n_active + 1, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
+        n_active, active_tiles, total_tiles, offsets, n_isects, tile_offsets
     );
     return check_launch();
 }

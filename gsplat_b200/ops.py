@@ -900,15 +900,17 @@ def isect_tiles_sorted(
     means2d: Tensor, radii: Tensor, depths: Tensor, tile_size: int, tile_width: int, tile_height: int,
     conics: Optional[Tensor] = None, opacities: Optional[Tensor] = None, precounted: Optional[RowSideOutputs] = None,
     n_images: Optional[int] = None, image_ids: Optional[Tensor] = None, _exact: bool = False,
+    _tile_mask: Optional[Tensor] = None,
 ) -> SortedIntersections:
     """Sorted tile intersection + offsets, the reference's sorted ``isect_tiles`` + ``isect_offset_encode``
     (csrc/Intersect.cpp:203-326, 330-382), with the S-sized sort done on 2- or 4-byte dense tile ids instead of the
     8-byte (image | tile | depth) ids.  Rows are dense ([..., N, 2] means2d), or packed ([nnz, 2] means2d with
     ``n_images`` and the image of each row in ``image_ids``).  The stage is launched on capacities predicted from the
     earlier calls of the same shape.  ``_exact`` (isect_tiles) reads the totals first and sizes the stage exactly, and
-    leaves that history alone: the call's own largest row then picks the emit kernel."""
+    leaves that history alone: the call's own largest row then picks the emit kernel.  ``_tile_mask`` (isect_tiles_sparse,
+    with ``_exact``): uint8 [I, th, tw]; only the tiles it sets are counted and listed."""
     dev = require_cuda(means2d, radii, depths)
-    means2d, radii, depths, conics, opacities, image_ids, (image_dims, I, N, I_count, total, packed) = _isect_rows(
+    means2d, radii, depths, conics, opacities, image_ids, (image_dims, I, N, _, total, packed) = _isect_rows(
         means2d, radii, depths, conics, opacities, tile_width, tile_height, n_images, image_ids
     )
     L = lib()
@@ -916,7 +918,7 @@ def isect_tiles_sorted(
     key_bytes = 2 if key_bits <= 16 else 4
     key_dtype = torch.int16 if key_bytes == 2 else torch.int32  # raw storage; the kernels read them unsigned
     have_counts = (
-        not packed and precounted is not None and precounted.totals is not None and total > 0
+        _tile_mask is None and not packed and precounted is not None and precounted.totals is not None and total > 0
         and (precounted.tile_size, precounted.tile_width, precounted.tile_height) == (tile_size, tile_width, tile_height)
         and precounted.tiles_per_gauss.numel() == total and conics is not None and opacities is not None
     )
@@ -943,8 +945,8 @@ def isect_tiles_sorted(
         if not have_counts:
             check(
                 L.gsb200_isect_count_totals(
-                    I_count, N, ptr(means2d), ptr(radii), ptr(conics) if accu else None, ptr(opacities) if accu else None, tile_size,
-                    tile_width, tile_height, ptr(tiles_per_gauss), ptr(totals), st,
+                    I, N, ptr(means2d), ptr(radii), ptr(conics) if accu else None, ptr(opacities) if accu else None, ptr(image_ids),
+                    ptr(_tile_mask), tile_size, tile_width, tile_height, ptr(tiles_per_gauss), ptr(totals), st,
                 ),
                 "intersect_tile (count)",
             )
@@ -957,8 +959,8 @@ def isect_tiles_sorted(
             check(
                 L.gsb200_isect_sorted(
                     I, N, ptr(means2d), ptr(radii), ptr(depths), ptr(conics) if accu else None, ptr(opacities) if accu else None,
-                    ptr(image_ids), tile_size, tile_width, tile_height, ptr(tiles_per_gauss), ptr(totals), cap_vis, cap_isects, max_tiles, key_bytes,
-                    ptr(keys_out), ptr(vals_out), ptr(offsets), ptr(ws), ws.numel(), st,
+                    ptr(image_ids), ptr(_tile_mask), tile_size, tile_width, tile_height, ptr(tiles_per_gauss), ptr(totals), cap_vis, cap_isects,
+                    max_tiles, key_bytes, ptr(keys_out), ptr(vals_out), ptr(offsets), ptr(ws), ws.numel(), st,
                 ),
                 "intersect_tile (sorted)",
             )
@@ -1698,37 +1700,23 @@ def isect_tiles_sparse(
             f"available (I={n_images}, n_tiles={tile_width * tile_height})."
         )
     dev = require_cuda(means2d, radii, depths, tile_mask, active_tiles, image_ids)
-    means2d, depths = f32c(means2d, "means2d"), f32c(depths, "depths")
-    radii, tm = radii.contiguous(), tile_mask.contiguous().view(torch.uint8)
     active = active_tiles.contiguous()
-    img = image_ids.to(torch.int64).contiguous() if packed else None
-    AT, total = active.shape[0], N if packed else I * N
-    L = lib()
+    AT = active.shape[0]
+    # without rows the sorted stage lists nothing, and every tile offset is 0
+    hits = isect_tiles_sorted(
+        means2d, radii, depths, tile_size, tile_width, tile_height, n_images=n_images if packed else None,
+        image_ids=image_ids if packed else None, _exact=True, _tile_mask=tile_mask.contiguous().view(torch.uint8),
+    )
     tile_offsets = torch.empty(AT + 1, device=dev, dtype=torch.int32)
     with _Ctx(dev) as st:
-        n_isects = 0
-        order = torch.empty(total, device=dev, dtype=torch.int32)
-        cum = torch.empty(total, device=dev, dtype=torch.int64)
-        if total > 0:
-            ws = _scratch_buffer(dev, "sparse_count", L.gsb200_isect_sparse_count_workspace_bytes(I, total))
-            check(
-                L.gsb200_isect_sparse_count(
-                    I, N, ptr(means2d), ptr(radii), ptr(depths), ptr(img), ptr(tm), tile_size, tile_width, tile_height, ptr(order),
-                    ptr(cum), ptr(ws), ws.numel(), st,
-                ),
-                "intersect_tile_sparse (count)",
-            )
-            n_isects = int(cum[-1].item())  # the one host sync (as in isect_tiles)
-        flatten_ids = torch.empty(n_isects, device=dev, dtype=torch.int32)
-        ws = _scratch_buffer(dev, "sparse_emit", L.gsb200_isect_sparse_emit_workspace_bytes(I, n_isects, tile_width, tile_height))
         check(
-            L.gsb200_isect_sparse_emit(
-                I, N, ptr(means2d), ptr(radii), ptr(img), ptr(tm), tile_size, tile_width, tile_height, ptr(order), ptr(cum),
-                n_isects, AT, ptr(active), ptr(tile_offsets), ptr(flatten_ids), ptr(ws), ws.numel(), st,
+            lib().gsb200_isect_active_offsets(
+                AT, ptr(active), n_images, tile_width, tile_height, ptr(hits.isect_offsets), hits.flatten_ids.shape[0],
+                ptr(tile_offsets), st,
             ),
-            "intersect_tile_sparse (emit)",
+            "intersect_tile_sparse (offsets)",
         )
-    return tile_offsets, flatten_ids
+    return tile_offsets, hits.flatten_ids
 
 
 def _check_sparse_layout(image_ids, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map,

@@ -215,12 +215,13 @@ extern "C"
     );
     /* Sorted output, first pass: the row-order count, and the totals the host reads -- totals[0] = n_isects,
      * totals[1] = rows that have tiles, totals[2] = largest tile count of a row (max_tiles_hint of gsb200_isect_sorted:
-     * picks the one-thread-per-gaussian or the warp-cooperative emit kernel).  totals is int64 [3].  Packed layout:
-     * call with I = 1, N = the number of rows. */
+     * picks the one-thread-per-gaussian or the warp-cooperative emit kernel).  totals is int64 [3].  Rows as in
+     * gsb200_isect_sorted: I*N, or N when image_ids int64 [N] is given.  tile_mask NULL, or uint8 [I, th, tw]: a row
+     * then counts only the tiles whose byte is set, and a row whose image lies outside [0, I) counts none. */
     int gsb200_isect_count_totals(
         int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *conics, const float *opacities,
-        uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *tiles_per_gauss, int64_t *totals,
-        void *stream
+        const int64_t *image_ids, const uint8_t *tile_mask, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        int32_t *tiles_per_gauss, int64_t *totals, void *stream
     );
     /* Narrow keys (round 2): the rows are emitted in depth order, so the S-sized sort only needs the dense tile id
      * image * n_tiles + tile, as a key_bytes-wide (2 when I * n_tiles <= 65536, else 4) unsigned integer.
@@ -242,17 +243,18 @@ extern "C"
      * therefore launch with PREDICTED capacities before it has read the totals (the host read then overlaps this work
      * instead of idling the GPU: the sync being hidden is the reference's csrc/Intersect.cpp:258-259), use the first
      * totals[0] entries if both counts fit, and otherwise call again with capacities = totals.  key_bytes: 2 when
-     * I * th * tw <= 65536, else 4. */
+     * I * th * tw <= 65536, else 4.  tile_mask NULL, or the uint8 [I, th, tw] mask the counts were taken with: only the
+     * tiles it sets are emitted. */
     size_t gsb200_isect_sorted_workspace_bytes(
         int64_t I, int64_t total_rows, int64_t cap_vis, int64_t cap_isects, int key_bytes, uint32_t tile_width,
         uint32_t tile_height
     );
     int gsb200_isect_sorted(
         int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const float *conics,
-        const float *opacities, const int64_t *image_ids, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
-        const int32_t *tiles_per_gauss, const int64_t *totals, int64_t cap_vis, int64_t cap_isects, int64_t max_tiles_hint,
-        int key_bytes, void *tile_keys, int32_t *flatten_ids, int32_t *offsets, void *workspace, size_t workspace_bytes,
-        void *stream
+        const float *opacities, const int64_t *image_ids, const uint8_t *tile_mask, uint32_t tile_size, uint32_t tile_width,
+        uint32_t tile_height, const int32_t *tiles_per_gauss, const int64_t *totals, int64_t cap_vis, int64_t cap_isects,
+        int64_t max_tiles_hint, int key_bytes, void *tile_keys, int32_t *flatten_ids, int32_t *offsets, void *workspace,
+        size_t workspace_bytes, void *stream
     );
     /* Publishes totals (int64 [3], device) into host_mapped (int64 [4], pinned / mapped host memory) with system-scope
      * stores from a one-warp kernel, then writes seq into host_mapped[3]: the host polls that word instead of waiting for
@@ -328,29 +330,19 @@ extern "C"
         size_t workspace_bytes, int32_t *active_tiles, uint8_t *active_tile_mask, uint64_t *tile_pixel_mask,
         int64_t *tile_pixel_cumsum, int64_t *pixel_map, void *stream
     );
-    /* Tile intersection restricted to the tiles whose tile_mask [I, th, tw] byte is set (radius AABB test).  Dense rows
-     * [I, N] (image_ids NULL) or packed rows [N] with int64 image_ids.  gsb200_isect_sparse_count orders the rows by
-     * (image, depth) into order int32 [rows] and writes the inclusive scan of their masked tile counts to cum_tiles
-     * int64 [rows]; the caller reads n_isects = cum_tiles[rows - 1], then gsb200_isect_sparse_emit emits, stably sorts
-     * by (image, tile) into flatten_ids int32 [n_isects] and writes tile_offsets int32 [n_active + 1] (the start of
-     * each active tile's range, and n_isects). */
-    size_t gsb200_isect_sparse_count_workspace_bytes(int64_t I, int64_t total_rows);
-    int gsb200_isect_sparse_count(
-        int64_t I, int64_t N, const float *means2d, const int32_t *radii, const float *depths, const int64_t *image_ids,
-        const uint8_t *tile_mask, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, int32_t *order,
-        int64_t *cum_tiles, void *workspace, size_t workspace_bytes, void *stream
+    /* Tile intersection restricted to the tiles of active_tile_mask: gsb200_isect_count_totals and gsb200_isect_sorted
+     * with that mask as tile_mask (dense rows [I, N], or packed rows [N] with int64 image_ids), then
+     * gsb200_isect_active_offsets: tile_offsets int32 [n_active + 1] = the sorted stage's offsets [I, th, tw] at each
+     * of active_tiles int32 [n_active], and n_isects.  An active tile id outside [0, I * th * tw) gets n_isects. */
+    int gsb200_isect_active_offsets(
+        int64_t n_active, const int32_t *active_tiles, int64_t I, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, int64_t n_isects, int32_t *tile_offsets, void *stream
     );
-    size_t gsb200_isect_sparse_emit_workspace_bytes(int64_t I, int64_t n_isects, uint32_t tile_width, uint32_t tile_height);
-    int gsb200_isect_sparse_emit(
-        int64_t I, int64_t N, const float *means2d, const int32_t *radii, const int64_t *image_ids, const uint8_t *tile_mask,
-        uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *order, const int64_t *cum_tiles,
-        int64_t n_isects, int64_t n_active, const int32_t *active_tiles, int32_t *tile_offsets, int32_t *flatten_ids,
-        void *workspace, size_t workspace_bytes, void *stream
-    );
-    /* Compositing of the requested pixels only: one CTA per active tile, tile_offsets [n_active + 1] and flatten_ids
-     * from gsb200_isect_sparse_emit, the layout tensors from gsb200_sparse_layout_finish.  Gaussian rows and
-     * backgrounds [n_images, D] / masks [n_images, th, tw] as in gsb200_raster_fwd; `records` of
-     * gsb200_raster_records_bytes(n_isects, D, n_active).  Outputs in the original pixel order: render_colors [P, D],
+    /* Compositing of the requested pixels only: one CTA per active tile, tile_offsets [n_active + 1] of
+     * gsb200_isect_active_offsets and flatten_ids of the masked gsb200_isect_sorted, the layout tensors from
+     * gsb200_sparse_layout_finish.  Gaussian rows and backgrounds [n_images, D] / masks [n_images, th, tw] as in
+     * gsb200_raster_fwd; `records` of gsb200_raster_records_bytes(n_isects, D, n_active).  Outputs in the original
+     * pixel order: render_colors [P, D],
      * render_alphas [P], last_ids int32 [P].  The backward accumulates into the gradient records of gsb200_raster_bwd,
      * one per gaussian row g in [0, n_rows); v_render_colors [P, D], v_render_alphas [P] or NULL. */
     int gsb200_raster_sparse_fwd(
@@ -481,7 +473,7 @@ extern "C"
      * gsb200_raster_indices (and so of gsb200_raster_fwd).  Rows: means2d [R,2], conics [R,3], opacities [R]; ids are
      * flatten id % N (dense rows [I,N,*]: the gaussian index; packed rows [nnz,*]: pass N = nnz, the row index).
      * Dense: offsets [I,th,tw], active_tiles = null, outputs row (image, y, x) of I*H*W.  Sparse (active_tiles non-null):
-     * the layout of gsb200_sparse_layout_* and the per-active-tile offsets [n_active + 1] of gsb200_isect_sparse_emit,
+     * the layout of gsb200_sparse_layout_* and the per-active-tile offsets [n_active + 1] of gsb200_isect_active_offsets,
      * outputs row = the pixel's index in the caller's list [P].  tile_size must be 16.  Every pixel is written.
      *   count: counts int32 [rows] contributing pairs, alphas float32 [rows] (nullable) 1 - final T.
      *   ids:   ids int32 / weights float32 [rows, max_samples]: the first max_samples pairs front to back (later ones

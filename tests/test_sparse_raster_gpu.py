@@ -55,13 +55,25 @@ def _project(gs, garden, C, packed):
     )
 
 
-def _dense_lists(gs, rows, C):
+def _dense_lists(gs, rows, C, tw=TW, th=TH):
     packed = rows["image_ids"] is not None
     _, isect_ids, flatten_ids = gs.isect_tiles(
-        rows["means2d"], rows["radii"], rows["depths"], 16, TW, TH, packed=packed, n_images=C if packed else None,
+        rows["means2d"], rows["radii"], rows["depths"], 16, tw, th, packed=packed, n_images=C if packed else None,
         image_ids=rows["image_ids"],
     )
-    return gs.isect_offset_encode(isect_ids, C, TW, TH), flatten_ids
+    return gs.isect_offset_encode(isect_ids, C, tw, th), flatten_ids
+
+
+def _assert_active_lists(gs, rows, C, active, tile_offsets, flatten_ids, tw=TW, th=TH):
+    """the sparse lists are the dense pipeline's lists of the active tiles, in its order"""
+    offsets, fl = _dense_lists(gs, rows, C, tw, th)
+    off = np.concatenate([offsets.cpu().numpy().reshape(-1), [fl.shape[0]]])
+    fl = fl.cpu().numpy()
+    exp_ids = [fl[off[t] : off[t + 1]] for t in active]
+    exp_off = np.concatenate([[0], np.cumsum([len(x) for x in exp_ids])]).astype(np.int32)
+    assert tile_offsets.dtype == torch.int32 and np.array_equal(tile_offsets.cpu().numpy(), exp_off)
+    exp_fl = np.concatenate(exp_ids) if exp_ids else np.zeros(0, np.int32)
+    assert np.array_equal(flatten_ids.cpu().numpy(), exp_fl)
 
 
 def _pixel_set(kind, C, rng):
@@ -152,14 +164,32 @@ def test_layout_and_intersections(gs, garden, kind, C, packed):
     assert cumsum.dtype == torch.int64 and np.array_equal(cumsum.cpu().numpy(), m_cumsum)
     assert pmap.dtype == torch.int64 and np.array_equal(pmap.cpu().numpy(), m_pmap)
     # the intersections of the active tiles, in the dense pipeline's order
-    offsets, fl = _dense_lists(gs, rows, C)
-    off = np.concatenate([offsets.cpu().numpy().reshape(-1), [fl.shape[0]]])
-    fl = fl.cpu().numpy()
-    exp_ids = [fl[off[t] : off[t + 1]] for t in m_active]
-    exp_off = np.concatenate([[0], np.cumsum([len(x) for x in exp_ids])]).astype(np.int32)
-    assert tile_offsets.dtype == torch.int32 and np.array_equal(tile_offsets.cpu().numpy(), exp_off)
-    exp_fl = np.concatenate(exp_ids) if exp_ids else np.zeros(0, np.int32)
-    assert np.array_equal(flatten_ids.cpu().numpy(), exp_fl)
+    _assert_active_lists(gs, rows, C, m_active, tile_offsets, flatten_ids)
+
+
+@pytest.mark.parametrize("packed", [False, True], ids=["dense", "packed"])
+def test_intersections_wide_tile_ids(gs, packed):
+    """One image on a 300 x 256 tile grid: more than 65536 tiles, so the masked lists are sorted on 4-byte tile ids (the
+    grid of the other tests fits 2-byte ids)."""
+    tw, th, n = 300, 256, 4000
+    rng = np.random.RandomState(5)
+    m2 = rng.uniform(-40.0, [tw * 16 + 40.0, th * 16 + 40.0], (n, 2)).astype(np.float32)
+    radii = rng.randint(1, 90, (n, 2)).astype(np.int32)
+    radii[rng.rand(n) < 0.3] = 0  # culled rows
+    depths = rng.choice(np.linspace(1.0, 40.0, 300), n).astype(np.float32)  # many equal depths: the row index decides
+    t = lambda a: torch.from_numpy(a).to(DEV)  # noqa: E731
+    if packed:
+        rows = dict(means2d=t(m2), radii=t(radii), depths=t(depths), image_ids=torch.zeros(n, device=DEV, dtype=torch.int64))
+    else:
+        rows = dict(means2d=t(m2[None]), radii=t(radii[None]), depths=t(depths[None]), image_ids=None)
+    flat = rng.choice(tw * 16 * th * 16, 20000, replace=False)
+    pixels = t(np.stack([flat // (tw * 16), flat % (tw * 16)], -1).astype(np.int32))
+    active, amask = gs.build_sparse_tile_layout(pixels, torch.zeros(len(flat), device=DEV, dtype=torch.int32), 1, 16, tw, th)[:2]
+    tile_offsets, flatten_ids = gs.isect_tiles_sparse(
+        rows["means2d"], rows["radii"], rows["depths"], amask, active, 1, 16, tw, th, image_ids=rows["image_ids"]
+    )
+    assert flatten_ids.shape[0] > 0
+    _assert_active_lists(gs, rows, 1, active.cpu().numpy(), tile_offsets, flatten_ids, tw, th)
 
 
 def _features(rows, D, seed):

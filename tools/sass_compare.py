@@ -8,12 +8,13 @@ disassembles the objects with ``cuobjdump -sass`` and compares every kernel of t
 same name in the new ones, whichever unit it is compiled in: a kernel that moved to another file is matched with its
 old self.  Names are compared demangled, with the pixel-addressing policy of the compositing kernels
 (``gsb::DensePixels``) removed, so that a kernel that only gained that template argument is matched with its old self,
-with ``isect_count_kernel<true / false>`` under the names the two count kernels had before they became one template, and
-with the pair-query kernels ``raster_indices_kernel`` and ``surfel_indices_kernel`` named by their sink without their
-parameter list (``<false / true>`` became the ``CountSink`` / ``PairSink`` instantiations when each walk took a sink).
-Instructions and their encodings must be identical; address and line-info comments are ignored.  A library kernel
-(CUB) that several units instantiate must be identical in all of them.  Kernels that only the new objects have are
-listed as new.  Exit status 1 on any difference.  Needs nvcc / cuobjdump / cu++filt (no GPU).
+with ``isect_count_kernel<true / false>`` under the names the two count kernels had before they became one template,
+with the unmasked ``isect_count_kernel`` and ``isect_emit_kernel`` (``MASKED`` = false) without that template argument
+and the tile-mask parameters that came with it, and with the pair-query kernels ``raster_indices_kernel`` and
+``surfel_indices_kernel`` named by their sink without their parameter list (``<false / true>`` became the
+``CountSink`` / ``PairSink`` instantiations when each walk took a sink).  Instructions and their encodings must be
+identical; address and line-info comments are ignored.  A library kernel (CUB) that several units instantiate must be
+identical in all of them.  Kernels that only the new objects have are listed as new.  Exit status 1 on any difference.  Needs nvcc / cuobjdump / cu++filt (no GPU).
 """
 from __future__ import annotations
 
@@ -32,6 +33,11 @@ from gsplat_b200 import build as B  # noqa: E402
 CUDA_BIN = os.path.dirname(B._nvcc()) if os.path.isabs(B._nvcc()) else "/usr/local/cuda/bin"
 # cu++filt prints the policy parameter of a kernel as `T<k>`: dropped together with the policy template argument
 POLICY_PARAM = re.compile(r",\s*T\d+\)$")
+# isect_count_kernel<TOTALS> and isect_emit_kernel<KeyT> gained a MASKED template argument and appended parameters
+# (count: N, I, image_ids, tile_mask; emit: tile_mask): <..., false> is the kernel as it was
+MASKED_KERNEL = re.compile(
+    r"^void (gsb::isect_(?:count|emit)_kernel)<(.*), \(bool\)0>\((.*?), (?:long, long, const long \*, )?const unsigned char \*\)$"
+)
 # isect_count_kernel<TOTALS>: <true> was isect_count_totals_kernel, <false> isect_count_kernel without the totals pointer
 COUNT_KERNEL = re.compile(r"^void gsb::isect_count_kernel<\(bool\)([01])>\((.*), unsigned long long \*\)$")
 # raster_indices_kernel<EMIT> became raster_indices_kernel<Sink, Pix> and surfel_indices_kernel<EMIT> became
@@ -83,6 +89,9 @@ def kernels(obj: str):
     for n, d in zip(names, _demangle(names)):
         if "DensePixels" in n or "SparsePixels" in n:
             d = POLICY_PARAM.sub(")", d).replace(", gsb::DensePixels>", ">")
+        m = MASKED_KERNEL.match(d)
+        if m:
+            d = f"void {m.group(1)}<{m.group(2)}>({m.group(3)})"
         m = COUNT_KERNEL.match(d)
         if m:
             d = f"gsb::isect_count_totals_kernel({m.group(2)}, unsigned long long *)" if m.group(1) == "1" else f"gsb::isect_count_kernel({m.group(2)})"
