@@ -9,7 +9,10 @@ the reference has no such op), the pair queries rasterize_to_indices_in_range /
 rasterize_to_indices_in_range_2dgs, and the per-pixel contributor queries rasterize_num_contributing_gaussians,
 rasterize_contributing_gaussian_ids, rasterize_top_contributing_gaussian_ids and their _sparse forms (the pair query's
 walk with the compositing kernel's decisions: against the reference's ops they can differ only at pairs on the 1/255
-and 1e-4 thresholds).  Importing the package does not need a GPU; calling an
+and 1e-4 thresholds), and their 2DGS forms rasterize_num_contributing_gaussians_2dgs,
+rasterize_contributing_gaussian_ids_2dgs, rasterize_top_contributing_gaussian_ids_2dgs and their _2dgs_sparse forms
+(this library's own: the reference has no such ops; the surfel walk takes rasterize_to_pixels_2dgs's decisions, so
+their alphas equal its render_alphas bit for bit).  Importing the package does not need a GPU; calling an
 operator does (and needs gsplat_b200/libgsplat_b200.so, built by ``python -m gsplat_b200.build``).
 """
 from .ops import (  # noqa: F401
@@ -25,8 +28,12 @@ from .ops import (  # noqa: F401
     isect_tiles_sparse,
     quat_scale_to_covar_preci,
     rasterize_contributing_gaussian_ids,
+    rasterize_contributing_gaussian_ids_2dgs,
+    rasterize_contributing_gaussian_ids_2dgs_sparse,
     rasterize_contributing_gaussian_ids_sparse,
     rasterize_num_contributing_gaussians,
+    rasterize_num_contributing_gaussians_2dgs,
+    rasterize_num_contributing_gaussians_2dgs_sparse,
     rasterize_num_contributing_gaussians_sparse,
     rasterize_to_indices_in_range,
     rasterize_to_indices_in_range_2dgs,
@@ -35,6 +42,8 @@ from .ops import (  # noqa: F401
     rasterize_to_pixels_2dgs_sparse,
     rasterize_to_pixels_sparse,
     rasterize_top_contributing_gaussian_ids,
+    rasterize_top_contributing_gaussian_ids_2dgs,
+    rasterize_top_contributing_gaussian_ids_2dgs_sparse,
     rasterize_top_contributing_gaussian_ids_sparse,
     spherical_harmonics,
 )
@@ -102,6 +111,12 @@ __all__ = [
     "rasterize_contributing_gaussian_ids_sparse",
     "rasterize_top_contributing_gaussian_ids",
     "rasterize_top_contributing_gaussian_ids_sparse",
+    "rasterize_num_contributing_gaussians_2dgs",
+    "rasterize_num_contributing_gaussians_2dgs_sparse",
+    "rasterize_contributing_gaussian_ids_2dgs",
+    "rasterize_contributing_gaussian_ids_2dgs_sparse",
+    "rasterize_top_contributing_gaussian_ids_2dgs",
+    "rasterize_top_contributing_gaussian_ids_2dgs_sparse",
     "quat_scale_to_covar_preci",
     "compute_relocation",
     "mcmc_perturb_positions",

@@ -1,12 +1,16 @@
 // indices.cuh -- sinks and host side of the index queries (gsb200_raster_indices, gsb200_surfel_indices): which
-// gaussians each pixel composites, walking only the batches [range_start, range_end) of kIndexBatch records of its list.
+// gaussians each pixel composites, walking only the batches [range_start, range_end) of kIndexBatch records of its list;
+// and of the per-pixel contributor queries of both walks (gsb200_contrib_*, gsb200_surfel_contrib_*).
 //
 // Two passes over the same workspace: the count pass writes the pair count of every pixel and their exclusive int64
 // scan (sort.cu) and copies the total to the caller; the emit pass writes each pixel's pairs, front to back, at its
 // scanned start.  The output is pixel-major over (image, row, col).
 #pragma once
 
+#include <algorithm>
+
 #include "common.cuh"
+#include "pixels.cuh"
 
 namespace gsb
 {
@@ -26,7 +30,7 @@ PixelCounts carve_pixel_counts(void *workspace, int64_t P);
 int scan_pixel_counts(const PixelCounts &pc, int64_t P, int64_t *total, cudaStream_t st);
 
 // What a pair-query walk (raster_indices_kernel of raster.cu, surfel_indices_kernel of surfel.cu) does with a pixel's
-// pairs is its Sink's:
+// pairs is its Sink's (both walks run kIndexBatch threads per CTA, one pixel per thread):
 //   begin(live, pix, pix_in, image_id)  once per thread (pix: the output row, pix_in: the row-major pixel in its image)
 //   pair(k, g, w)                        the pixel's k-th pair: flatten id g, weight w = alpha * T before the pair
 //   end(pix, count, T)                   once per live pixel, after the walk
@@ -64,6 +68,108 @@ struct PairSink // rasterize_to_indices_in_range's emit pass: the pairs from the
         image_ids[base + k]    = image_id;
     }
     __device__ __forceinline__ void end(int64_t, int32_t, float) const {}
+};
+
+// rasterize_contributing_gaussian_ids: the first K pairs of a pixel at [pix, k] (later ones are dropped, as the
+// reference drops them), -1 / 0 after its last pair; nothing outside the pixel's row of K.
+struct IdsSink
+{
+    int32_t N, K;
+    int32_t *ids;   // [rows, K] g % N
+    float *weights; // [rows, K] alpha * T before the pair
+    int64_t row;
+    __device__ __forceinline__ void begin(bool, int64_t pix, int64_t, int) { row = pix * K; }
+    __device__ __forceinline__ void pair(int32_t k, int32_t g, float w) const
+    {
+        if(k < K)
+        {
+            ids[row + k]     = g % N;
+            weights[row + k] = w;
+        }
+    }
+    __device__ __forceinline__ void end(int64_t, int32_t count, float) const
+    {
+        for(int32_t k = count < K ? count : K; k < K; ++k)
+        {
+            ids[row + k]     = -1;
+            weights[row + k] = 0.f;
+        }
+    }
+};
+
+// rasterize_top_contributing_gaussian_ids: K slots per pixel in dynamic shared memory ({id, weight, walk position},
+// slot k of thread t at [k * kIndexBatch + t]: conflict-free).  The reference's rule: empty slots hold -1, 0, +inf; a
+// pair replaces the lowest-weight slot (the first on ties) only when strictly heavier; at the end the slots are sorted
+// by walk position (stable), i.e. front to back with the empty ones last.
+struct TopSink
+{
+    static constexpr size_t kSlotBytes = sizeof(int32_t) + sizeof(float) + sizeof(uint32_t);
+    int32_t N, K;
+    int32_t *ids;   // [rows, K]
+    float *weights; // [rows, K]
+    int64_t row;
+    int32_t *s_id;
+    float *s_w;
+    uint32_t *s_pos;
+    __device__ __forceinline__ void begin(bool, int64_t pix, int64_t, int)
+    {
+        extern __shared__ __align__(16) int32_t s_top_slots[];
+        const size_t plane = (size_t)K * kIndexBatch;
+        s_id  = s_top_slots + threadIdx.x;
+        s_w   = reinterpret_cast<float *>(s_top_slots + plane) + threadIdx.x;
+        s_pos = reinterpret_cast<uint32_t *>(s_top_slots + 2 * plane) + threadIdx.x;
+        row   = pix * K;
+        for(int32_t k = 0; k < K; ++k)
+        {
+            s_id[k * kIndexBatch]  = -1;
+            s_w[k * kIndexBatch]   = 0.f;
+            s_pos[k * kIndexBatch] = 0xffffffffu;
+        }
+    }
+    __device__ __forceinline__ void pair(int32_t k, int32_t g, float w) const
+    {
+        int32_t m = 0;
+        float wm  = s_w[0];
+        for(int32_t j = 1; j < K; ++j)
+        {
+            const float v = s_w[j * kIndexBatch];
+            if(v < wm)
+            {
+                wm = v;
+                m  = j;
+            }
+        }
+        if(w > wm)
+        {
+            s_w[m * kIndexBatch]   = w;
+            s_id[m * kIndexBatch]  = g % N;
+            s_pos[m * kIndexBatch] = (uint32_t)k;
+        }
+    }
+    __device__ __forceinline__ void end(int64_t, int32_t, float) const
+    {
+        for(int32_t i = 1; i < K; ++i)
+        {
+            const uint32_t p = s_pos[i * kIndexBatch];
+            const float w    = s_w[i * kIndexBatch];
+            const int32_t id = s_id[i * kIndexBatch];
+            int32_t j        = i - 1;
+            for(; j >= 0 && s_pos[j * kIndexBatch] > p; --j)
+            {
+                s_pos[(j + 1) * kIndexBatch] = s_pos[j * kIndexBatch];
+                s_w[(j + 1) * kIndexBatch]   = s_w[j * kIndexBatch];
+                s_id[(j + 1) * kIndexBatch]  = s_id[j * kIndexBatch];
+            }
+            s_pos[(j + 1) * kIndexBatch] = p;
+            s_w[(j + 1) * kIndexBatch]   = w;
+            s_id[(j + 1) * kIndexBatch]  = id;
+        }
+        for(int32_t k = 0; k < K; ++k)
+        {
+            ids[row + k]     = s_id[k * kIndexBatch];
+            weights[row + k] = s_w[k * kIndexBatch];
+        }
+    }
 };
 
 // Argument checks and the pass sequence shared by both index queries.  `inputs_ok`: the gaussian rows, the
@@ -106,5 +212,119 @@ int run_index_pass(
     if(int rc = launch(n_tiles, b0, b1, CountSink{pc.counts, nullptr}))
         return rc;
     return scan_pixel_counts(pc, P, total, st);
+}
+
+// ---- per-pixel contributor queries: the full walk from T = 1 with one sink, over every tile (dense) or over the active
+// tiles of a sparse layout (active_tiles != null).  The checks run in run_index_pass's order with its return codes;
+// every pixel is written, also when there are no intersections.
+//
+// The arguments of the C entries of both walks: `rows` is conics [R, 3] (raster.cu) or ray_transforms [R, 3, 3]
+// (surfel.cu).
+struct ContribArgs
+{
+    int64_t I, N;
+    const float *means2d, *rows, *opacities;
+    uint32_t W, H, tile_size, tw, th;
+    const int32_t *offsets, *flatten_ids;
+    int64_t n_isects, n_active;
+    const int32_t *active_tiles;
+    const uint64_t *tile_pixel_mask;
+    const int64_t *tile_pixel_cumsum, *pixel_map;
+};
+
+// ContribArgs from the parameters of a contributor entry, named as gsb200_contrib_count's with `rows` for conics
+#define GSB200_CONTRIB_ARGS(rows)                                                                                       \
+    gsb::ContribArgs                                                                                                    \
+    {                                                                                                                   \
+        I, N, means2d, rows, opacities, image_width, image_height, tile_size, tile_width, tile_height, offsets,         \
+            flatten_ids, n_isects, n_active, active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map                \
+    }
+
+// A Walk is one unit's pair-query kernel:
+//   Walk::launch(a, n_tiles, pixmap, sink, smem, st)  launches it over n_tiles CTAs from T = 1 through the whole lists
+//   Walk::max_samples()                             the largest K of its TopSink on the current device (top_max_samples)
+// launch_walk and top_max_samples are the steps both walks take.
+template<class... Params, class... Args>
+int launch_walk(void (*kernel)(Params...), unsigned n_tiles, size_t smem, cudaStream_t st, const Args &...args)
+{
+    if(smem > 0) // TopSink's slots
+        GSB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<n_tiles, kIndexBatch, smem, st>>>(args...);
+    return check_launch();
+}
+
+// largest K of a top-K walk on the current device: its opt-in shared memory per block, less the static shared memory
+// (the staging arrays) of the larger of its two TopSink instantiations, over the K slots of every thread
+inline int top_max_samples(const void *dense_walk, const void *sparse_walk)
+{
+    int dev = 0, optin = 0;
+    GSB_CUDA_TRY(cudaGetDevice(&dev));
+    GSB_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    size_t staging = 0;
+    for(const void *k : {dense_walk, sparse_walk})
+    {
+        cudaFuncAttributes a;
+        GSB_CUDA_TRY(cudaFuncGetAttributes(&a, k));
+        staging = std::max(staging, a.sharedSizeBytes);
+    }
+    if((size_t)optin <= staging)
+        return 0;
+    return (int)(((size_t)optin - staging) / ((size_t)kIndexBatch * TopSink::kSlotBytes));
+}
+
+template<class Walk, class Sink>
+int run_contrib(const ContribArgs &a, bool outputs_ok, size_t smem, const Sink &sink, cudaStream_t st)
+{
+    const bool sparse = a.active_tiles != nullptr;
+    if(a.I < 0 || a.N < 0 || a.n_isects < 0 || a.n_active < 0)
+        return GSB200_E_INVALID;
+    if(a.tile_size != (uint32_t)kTile)
+        return GSB200_E_UNSUPPORTED;
+    const int64_t n_tiles = sparse ? a.n_active : a.I * (int64_t)a.tw * a.th;
+    if(n_tiles == 0 || a.W == 0 || a.H == 0)
+        return GSB200_OK; // no pixels
+    const bool inputs_ok = a.offsets && (a.n_isects == 0 || (a.means2d && a.rows && a.opacities && a.flatten_ids))
+                        && (!sparse || (a.tile_pixel_mask && a.tile_pixel_cumsum && a.pixel_map));
+    if(!inputs_ok || !outputs_ok || !tile_grid_covers(a.tw, a.th, a.W, a.H))
+        return GSB200_E_INVALID;
+    if(n_tiles >= 2147483648LL || a.n_isects >= 2147483648LL)
+        return GSB200_E_UNSUPPORTED;
+    if(sparse)
+        return Walk::launch(a, (unsigned)n_tiles, SparsePixels{a.active_tiles, a.tile_pixel_mask, a.tile_pixel_cumsum, a.pixel_map}, sink, smem, st);
+    return Walk::launch(a, (unsigned)n_tiles, DensePixels{}, sink, smem, st);
+}
+
+// count: CountSink
+template<class Walk>
+int contrib_count(const ContribArgs &a, int32_t *counts, float *alphas, cudaStream_t st)
+{
+    return run_contrib<Walk>(a, counts != nullptr, 0, CountSink{counts, alphas}, st);
+}
+
+// ids: IdsSink; max_samples = 0 writes nothing
+template<class Walk>
+int contrib_ids(const ContribArgs &a, int max_samples, int32_t *ids, float *weights, cudaStream_t st)
+{
+    if(max_samples < 0 || a.N > 0x7fffffffLL)
+        return GSB200_E_INVALID;
+    if(max_samples == 0)
+        return GSB200_OK;
+    return run_contrib<Walk>(a, ids && weights, 0, IdsSink{(int32_t)a.N, max_samples, ids, weights, 0}, st);
+}
+
+// top: TopSink, num_samples in [1, Walk::max_samples()]
+template<class Walk>
+int contrib_top(const ContribArgs &a, int num_samples, int32_t *ids, float *weights, cudaStream_t st)
+{
+    if(num_samples <= 0 || a.N > 0x7fffffffLL)
+        return GSB200_E_INVALID;
+    const int bound = Walk::max_samples();
+    if(bound < 0)
+        return bound;
+    if(num_samples > bound)
+        return GSB200_E_UNSUPPORTED;
+    const TopSink sink{(int32_t)a.N, num_samples, ids, weights, 0, nullptr, nullptr, nullptr};
+    const size_t smem = (size_t)num_samples * kIndexBatch * TopSink::kSlotBytes;
+    return run_contrib<Walk>(a, ids && weights, smem, sink, st);
 }
 } // namespace gsb

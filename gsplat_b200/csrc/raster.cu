@@ -931,110 +931,7 @@ __global__ void __launch_bounds__(kWarps * 32, MINB) raster_bwd2_kernel(
 // policy (DensePixels: every tile of the [I, th, tw] grid; SparsePixels: every active tile, its live pixels only), each
 // batch's records built by row_record and staged in shared memory; every decision is raster_fwd_kernel's: its
 // warp -> 8x4 pixel block mapping, block_may_touch, pair_vis and its alpha, threshold and stop expressions.  What the
-// walk does with a pixel's pairs is the Sink's (indices.cuh: CountSink, PairSink; below: IdsSink, TopSink).
-
-// rasterize_contributing_gaussian_ids: the first K pairs of a pixel at [pix, k] (later ones are dropped, as the
-// reference drops them), -1 / 0 after its last pair; nothing outside the pixel's row of K.
-struct IdsSink
-{
-    int32_t N, K;
-    int32_t *ids;   // [rows, K] g % N
-    float *weights; // [rows, K] alpha * T before the pair
-    int64_t row;
-    __device__ __forceinline__ void begin(bool, int64_t pix, int64_t, int) { row = pix * K; }
-    __device__ __forceinline__ void pair(int32_t k, int32_t g, float w) const
-    {
-        if(k < K)
-        {
-            ids[row + k]     = g % N;
-            weights[row + k] = w;
-        }
-    }
-    __device__ __forceinline__ void end(int64_t, int32_t count, float) const
-    {
-        for(int32_t k = count < K ? count : K; k < K; ++k)
-        {
-            ids[row + k]     = -1;
-            weights[row + k] = 0.f;
-        }
-    }
-};
-
-// rasterize_top_contributing_gaussian_ids: K slots per pixel in dynamic shared memory ({id, weight, walk position},
-// slot k of thread t at [k * kIndexBatch + t]: conflict-free).  The reference's rule: empty slots hold -1, 0, +inf; a
-// pair replaces the lowest-weight slot (the first on ties) only when strictly heavier; at the end the slots are sorted
-// by walk position (stable), i.e. front to back with the empty ones last.
-struct TopSink
-{
-    static constexpr size_t kSlotBytes = sizeof(int32_t) + sizeof(float) + sizeof(uint32_t);
-    int32_t N, K;
-    int32_t *ids;   // [rows, K]
-    float *weights; // [rows, K]
-    int64_t row;
-    int32_t *s_id;
-    float *s_w;
-    uint32_t *s_pos;
-    __device__ __forceinline__ void begin(bool, int64_t pix, int64_t, int)
-    {
-        extern __shared__ __align__(16) int32_t s_top_slots[];
-        const size_t plane = (size_t)K * kIndexBatch;
-        s_id  = s_top_slots + threadIdx.x;
-        s_w   = reinterpret_cast<float *>(s_top_slots + plane) + threadIdx.x;
-        s_pos = reinterpret_cast<uint32_t *>(s_top_slots + 2 * plane) + threadIdx.x;
-        row   = pix * K;
-        for(int32_t k = 0; k < K; ++k)
-        {
-            s_id[k * kIndexBatch]  = -1;
-            s_w[k * kIndexBatch]   = 0.f;
-            s_pos[k * kIndexBatch] = 0xffffffffu;
-        }
-    }
-    __device__ __forceinline__ void pair(int32_t k, int32_t g, float w) const
-    {
-        int32_t m = 0;
-        float wm  = s_w[0];
-        for(int32_t j = 1; j < K; ++j)
-        {
-            const float v = s_w[j * kIndexBatch];
-            if(v < wm)
-            {
-                wm = v;
-                m  = j;
-            }
-        }
-        if(w > wm)
-        {
-            s_w[m * kIndexBatch]   = w;
-            s_id[m * kIndexBatch]  = g % N;
-            s_pos[m * kIndexBatch] = (uint32_t)k;
-        }
-    }
-    __device__ __forceinline__ void end(int64_t, int32_t, float) const
-    {
-        for(int32_t i = 1; i < K; ++i)
-        {
-            const uint32_t p = s_pos[i * kIndexBatch];
-            const float w    = s_w[i * kIndexBatch];
-            const int32_t id = s_id[i * kIndexBatch];
-            int32_t j        = i - 1;
-            for(; j >= 0 && s_pos[j * kIndexBatch] > p; --j)
-            {
-                s_pos[(j + 1) * kIndexBatch] = s_pos[j * kIndexBatch];
-                s_w[(j + 1) * kIndexBatch]   = s_w[j * kIndexBatch];
-                s_id[(j + 1) * kIndexBatch]  = s_id[j * kIndexBatch];
-            }
-            s_pos[(j + 1) * kIndexBatch] = p;
-            s_w[(j + 1) * kIndexBatch]   = w;
-            s_id[(j + 1) * kIndexBatch]  = id;
-        }
-        for(int32_t k = 0; k < K; ++k)
-        {
-            ids[row + k]     = s_id[k * kIndexBatch];
-            weights[row + k] = s_w[k * kIndexBatch];
-        }
-    }
-};
-
+// walk does with a pixel's pairs is the Sink's (indices.cuh: CountSink, PairSink, IdsSink, TopSink).
 template<class Sink, class Pix = DensePixels>
 __global__ void __launch_bounds__(kWarps * 32) raster_indices_kernel(
     const uint32_t I, const int64_t n_isects, const float *__restrict__ means2d, const float *__restrict__ conics,
@@ -1502,74 +1399,31 @@ extern "C" int gsb200_raster_indices(
     );
 }
 
-// ---- per-pixel contributor queries: the full walk from T = 1 with one sink, over every tile (dense) or over the active
-// tiles of a sparse layout (active_tiles != null).  The checks run in run_index_pass's order with its return codes;
-// every pixel is written, also when there are no intersections.
+// ---- per-pixel contributor queries over raster_indices_kernel (indices.cuh: run_contrib and its checks)
 namespace gsb
 {
-template<class Sink>
-static int run_contrib(
-    int64_t I, int64_t N, const float *means2d, const float *conics, const float *opacities, uint32_t W, uint32_t H,
-    uint32_t tile_size, uint32_t tw, uint32_t th, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects,
-    int64_t n_active, const int32_t *active_tiles, const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum,
-    const int64_t *pixel_map, bool outputs_ok, size_t smem, const Sink &sink, cudaStream_t st
-)
+struct RasterWalk
 {
-    const bool sparse = active_tiles != nullptr;
-    if(I < 0 || N < 0 || n_isects < 0 || n_active < 0)
-        return GSB200_E_INVALID;
-    if(tile_size != (uint32_t)kTile)
-        return GSB200_E_UNSUPPORTED;
-    const int64_t n_tiles = sparse ? n_active : I * (int64_t)tw * th;
-    if(n_tiles == 0 || W == 0 || H == 0)
-        return GSB200_OK; // no pixels
-    const bool inputs_ok = offsets && (n_isects == 0 || (means2d && conics && opacities && flatten_ids))
-                        && (!sparse || (tile_pixel_mask && tile_pixel_cumsum && pixel_map));
-    if(!inputs_ok || !outputs_ok || !tile_grid_covers(tw, th, W, H))
-        return GSB200_E_INVALID;
-    if(n_tiles >= 2147483648LL || n_isects >= 2147483648LL)
-        return GSB200_E_UNSUPPORTED;
-    auto launch = [&](auto kernel, const auto &pm) {
-        if(smem > 0)
-            GSB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kernel<<<(unsigned)n_tiles, kWarps * 32, smem, st>>>(
-            (uint32_t)I, n_isects, means2d, conics, opacities, nullptr, W, H, tw, th, offsets, flatten_ids, 0, 0x7fffffff,
-            sink, pm
-        );
-        return check_launch();
-    };
-    if(sparse)
-        return launch(raster_indices_kernel<Sink, SparsePixels>, SparsePixels{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map});
-    return launch(raster_indices_kernel<Sink, DensePixels>, DensePixels{});
-}
-
-// largest K of the top-K query on the current device: its opt-in shared memory per block, less the kernels' staging
-// arrays, over the K slots of every thread
-static int contrib_max_samples()
-{
-    int dev = 0, optin = 0;
-    GSB_CUDA_TRY(cudaGetDevice(&dev));
-    GSB_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    size_t staging = 0;
-    for(const void *k : {(const void *)raster_indices_kernel<TopSink, DensePixels>, (const void *)raster_indices_kernel<TopSink, SparsePixels>})
+    template<class Pix, class Sink>
+    static int launch(const ContribArgs &a, unsigned n_tiles, const Pix &pm, const Sink &sink, size_t smem, cudaStream_t st)
     {
-        cudaFuncAttributes a;
-        GSB_CUDA_TRY(cudaFuncGetAttributes(&a, k));
-        staging = std::max(staging, a.sharedSizeBytes);
+        return launch_walk(
+            raster_indices_kernel<Sink, Pix>, n_tiles, smem, st, (uint32_t)a.I, a.n_isects, a.means2d, a.rows, a.opacities,
+            (const float *)nullptr, a.W, a.H, a.tw, a.th, a.offsets, a.flatten_ids, (int32_t)0, (int32_t)0x7fffffff, sink, pm
+        );
     }
-    if((size_t)optin <= staging)
-        return 0;
-    return (int)(((size_t)optin - staging) / ((size_t)kIndexBatch * TopSink::kSlotBytes));
-}
+    static int max_samples()
+    {
+        return top_max_samples(
+            (const void *)raster_indices_kernel<TopSink, DensePixels>, (const void *)raster_indices_kernel<TopSink, SparsePixels>
+        );
+    }
+};
 } // namespace gsb
-
-#define GSB200_CONTRIB_ARGS                                                                                              \
-    I, N, means2d, conics, opacities, image_width, image_height, tile_size, tile_width, tile_height, offsets, flatten_ids, \
-        n_isects, n_active, active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map
 
 extern "C" int gsb200_contrib_max_samples(void)
 {
-    return gsb::contrib_max_samples();
+    return gsb::RasterWalk::max_samples();
 }
 
 extern "C" int gsb200_contrib_count(
@@ -1580,7 +1434,7 @@ extern "C" int gsb200_contrib_count(
     float *alphas, void *stream
 )
 {
-    return gsb::run_contrib(GSB200_CONTRIB_ARGS, counts != nullptr, 0, gsb::CountSink{counts, alphas}, (cudaStream_t)stream);
+    return gsb::contrib_count<gsb::RasterWalk>(GSB200_CONTRIB_ARGS(conics), counts, alphas, (cudaStream_t)stream);
 }
 
 extern "C" int gsb200_contrib_ids(
@@ -1591,12 +1445,7 @@ extern "C" int gsb200_contrib_ids(
     int32_t *ids, float *weights, void *stream
 )
 {
-    if(max_samples < 0 || N > 0x7fffffffLL)
-        return GSB200_E_INVALID;
-    if(max_samples == 0)
-        return GSB200_OK;
-    const gsb::IdsSink sink{(int32_t)N, max_samples, ids, weights, 0};
-    return gsb::run_contrib(GSB200_CONTRIB_ARGS, ids && weights, 0, sink, (cudaStream_t)stream);
+    return gsb::contrib_ids<gsb::RasterWalk>(GSB200_CONTRIB_ARGS(conics), max_samples, ids, weights, (cudaStream_t)stream);
 }
 
 extern "C" int gsb200_contrib_top(
@@ -1607,15 +1456,5 @@ extern "C" int gsb200_contrib_top(
     int32_t *ids, float *weights, void *stream
 )
 {
-    if(num_samples <= 0 || N > 0x7fffffffLL)
-        return GSB200_E_INVALID;
-    const int bound = gsb::contrib_max_samples();
-    if(bound < 0)
-        return bound;
-    if(num_samples > bound)
-        return GSB200_E_UNSUPPORTED;
-    const gsb::TopSink sink{(int32_t)N, num_samples, ids, weights, 0, nullptr, nullptr, nullptr};
-    const size_t smem = (size_t)num_samples * gsb::kIndexBatch * gsb::TopSink::kSlotBytes;
-    return gsb::run_contrib(GSB200_CONTRIB_ARGS, ids && weights, smem, sink, (cudaStream_t)stream);
+    return gsb::contrib_top<gsb::RasterWalk>(GSB200_CONTRIB_ARGS(conics), num_samples, ids, weights, (cudaStream_t)stream);
 }
-#undef GSB200_CONTRIB_ARGS

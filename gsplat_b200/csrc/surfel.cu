@@ -472,34 +472,47 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_raster_fwd_kernel(
     median_ids[pix]     = median_idx;
 }
 
-// rasterize_to_indices_in_range_2dgs: the (pixel, surfel) pairs surfel_raster_fwd_kernel composites, walking only the
-// batches [b0, b1) of each tile's list from the pixel's given transmittance; the pixel mapping, staging, surf_eval and
-// the stop rule are the forward's.  What the walk does with a pixel's pairs is the Sink's (indices.cuh).
-template<class Sink>
+// The pair-query walk of rasterize_to_indices_in_range_2dgs and the 2DGS contributor queries: the (pixel, surfel) pairs
+// surfel_raster_fwd_kernel composites, walking only the batches [b0, b1) of each tile's list from the pixel's given
+// transmittance (null: T = 1).  One CTA per tile of the pixel policy (DensePixels: every tile of the [I, th, tw] grid;
+// SparsePixels: every active tile, its live pixels only); the pixel mapping, staging, surf_eval and the stop rule are
+// the forward's.  What the walk does with a pixel's pairs is the Sink's (indices.cuh).
+template<class Sink, class Pix = DensePixels>
 __global__ void __launch_bounds__(kSurfThreads) surfel_indices_kernel(
     uint32_t I, const float *__restrict__ means2d, const float *__restrict__ rt, const float *__restrict__ opacities,
     const float *__restrict__ transmittances, uint32_t W, uint32_t H, uint32_t tw, uint32_t th,
     const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids, int64_t n_isects, int32_t b0, int32_t b1,
-    Sink sink
+    Sink sink, const Pix pixmap = Pix{}
 )
 {
     static_assert(kSurfThreads == kIndexBatch, "one record of a batch per thread");
     __shared__ SurfRec rec[kSurfThreads];
-    const uint32_t tile  = blockIdx.x; // image * th * tw + tile row * tw + tile col
+    const uint32_t tile  = pixmap.tile(blockIdx.x); // image * th * tw + tile row * tw + tile col
     const uint32_t img   = tile / (tw * th);
     const uint32_t tin   = tile - img * tw * th;
     const uint32_t tr    = threadIdx.x;
     const uint32_t i     = (tin / tw) * kTile + tr / kTile;
     const uint32_t j     = (tin % tw) * kTile + tr % kTile;
-    const bool inside    = i < H && j < W;
     const int64_t pix_in = (int64_t)i * W + j;
-    const int64_t pix    = (int64_t)img * H * W + pix_in;
-    const int64_t start  = offsets[tile];
-    const int64_t end    = (tile + 1 == I * tw * th) ? n_isects : offsets[tile + 1];
-    const int64_t b_end  = min((int64_t)b1, (end - start + kSurfThreads - 1) / kSurfThreads);
+    bool inside;
+    int64_t pix, start, end;
+    if constexpr(Pix::kSparse)
+    {
+        pix   = pixmap.slot(blockIdx.x, (int)tr, inside);
+        start = offsets[blockIdx.x];
+        end   = offsets[blockIdx.x + 1];
+    }
+    else
+    {
+        inside = i < H && j < W;
+        pix    = (int64_t)img * H * W + pix_in;
+        start  = offsets[tile];
+        end    = (tile + 1 == I * tw * th) ? n_isects : offsets[tile + 1];
+    }
+    const int64_t b_end = min((int64_t)b1, (end - start + kSurfThreads - 1) / kSurfThreads);
     const float px = (float)j + 0.5f, py = (float)i + 0.5f;
 
-    float T     = inside ? transmittances[pix] : 1.f;
+    float T     = (inside && transmittances != nullptr) ? transmittances[pix] : 1.f;
     bool done   = !inside;
     int32_t cnt = 0;
     sink.begin(inside, pix, pix_in, img);
@@ -994,4 +1007,66 @@ extern "C" int gsb200_surfel_indices(
             return gsb::check_launch();
         }
     );
+}
+
+// ---- 2DGS per-pixel contributor queries over surfel_indices_kernel (indices.cuh: run_contrib and its checks, in the
+// order and with the return codes of gsb200_contrib_*)
+namespace gsb
+{
+struct SurfelWalk
+{
+    template<class Pix, class Sink>
+    static int launch(const ContribArgs &a, unsigned n_tiles, const Pix &pm, const Sink &sink, size_t smem, cudaStream_t st)
+    {
+        return launch_walk(
+            surfel_indices_kernel<Sink, Pix>, n_tiles, smem, st, (uint32_t)a.I, a.means2d, a.rows, a.opacities,
+            (const float *)nullptr, a.W, a.H, a.tw, a.th, a.offsets, a.flatten_ids, a.n_isects, (int32_t)0,
+            (int32_t)0x7fffffff, sink, pm
+        );
+    }
+    static int max_samples()
+    {
+        return top_max_samples(
+            (const void *)surfel_indices_kernel<TopSink, DensePixels>, (const void *)surfel_indices_kernel<TopSink, SparsePixels>
+        );
+    }
+};
+} // namespace gsb
+
+extern "C" int gsb200_surfel_contrib_max_samples(void)
+{
+    return gsb::SurfelWalk::max_samples();
+}
+
+extern "C" int gsb200_surfel_contrib_count(
+    int64_t I, int64_t N, const float *means2d, const float *ray_transforms, const float *opacities, uint32_t image_width,
+    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+    const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int32_t *counts,
+    float *alphas, void *stream
+)
+{
+    return gsb::contrib_count<gsb::SurfelWalk>(GSB200_CONTRIB_ARGS(ray_transforms), counts, alphas, (cudaStream_t)stream);
+}
+
+extern "C" int gsb200_surfel_contrib_ids(
+    int64_t I, int64_t N, const float *means2d, const float *ray_transforms, const float *opacities, uint32_t image_width,
+    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+    const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int max_samples,
+    int32_t *ids, float *weights, void *stream
+)
+{
+    return gsb::contrib_ids<gsb::SurfelWalk>(GSB200_CONTRIB_ARGS(ray_transforms), max_samples, ids, weights, (cudaStream_t)stream);
+}
+
+extern "C" int gsb200_surfel_contrib_top(
+    int64_t I, int64_t N, const float *means2d, const float *ray_transforms, const float *opacities, uint32_t image_width,
+    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+    const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int num_samples,
+    int32_t *ids, float *weights, void *stream
+)
+{
+    return gsb::contrib_top<gsb::SurfelWalk>(GSB200_CONTRIB_ARGS(ray_transforms), num_samples, ids, weights, (cudaStream_t)stream);
 }

@@ -14,7 +14,7 @@ from __future__ import annotations
 
 import math
 import operator
-from typing import Optional, Tuple
+from typing import NamedTuple, Optional, Tuple
 
 import torch
 from torch import Tensor
@@ -2000,20 +2000,39 @@ def rasterize_to_pixels_2dgs_sparse(
 # per-pixel contributor queries (reference wrappers gsplat/cuda/_wrapper.py:1668-2008): the pairs
 # rasterize_to_indices_in_range(0, inf) composites from T = 1, per pixel, as counts, padded id lists or the K heaviest.
 # Every query is one walk of the pair-query kernel (csrc/raster.cu, raster_indices_kernel) with its own per-pair sink,
-# dense over every tile or sparse over the active tiles of a build_sparse_tile_layout layout.
+# dense over every tile or sparse over the active tiles of a build_sparse_tile_layout layout.  The _2dgs forms (the
+# reference has none) are the same queries over the surfel walk (csrc/surfel.cu, surfel_indices_kernel).
+
+class _ContribWalk(NamedTuple):
+    """One pair-query walk of the contributor queries: its rows (tail and name) and its C entries."""
+
+    rows_tail: tuple  # (3,) conics or (3, 3) ray_transforms
+    rows_name: str
+    packed: bool  # whether the dense form also takes packed [nnz, *] rows
+    count: str
+    ids: str
+    top: str
+    max_samples: str
+
+
+_CONTRIB_3DGS = _ContribWalk((3,), "conics", True, "gsb200_contrib_count", "gsb200_contrib_ids", "gsb200_contrib_top",
+                             "gsb200_contrib_max_samples")
+_CONTRIB_2DGS = _ContribWalk((3, 3), "ray_transforms", False, "gsb200_surfel_contrib_count", "gsb200_surfel_contrib_ids",
+                             "gsb200_surfel_contrib_top", "gsb200_surfel_contrib_max_samples")
 
 _max_samples_cache = {}
 
 
-def _max_depth_samples(dev: torch.device) -> int:
-    """The largest num_depth_samples the top-K kernel holds on this device (its opt-in shared memory per block)."""
+def _max_depth_samples(dev: torch.device, entry: str = _CONTRIB_3DGS.max_samples) -> int:
+    """The largest num_depth_samples the top-K kernel of a walk (its ``*_max_samples`` entry) holds on this device (its
+    opt-in shared memory per block), cached per walk and device."""
     idx = dev.index if dev.index is not None else torch.cuda.current_device()
-    if idx not in _max_samples_cache:
+    if (entry, idx) not in _max_samples_cache:
         with torch.cuda.device(idx):
-            rc = lib().gsb200_contrib_max_samples()
-        check(min(rc, 0), "gsb200_contrib_max_samples")
-        _max_samples_cache[idx] = rc
-    return _max_samples_cache[idx]
+            rc = getattr(lib(), entry)()
+        check(min(rc, 0), entry)
+        _max_samples_cache[entry, idx] = rc
+    return _max_samples_cache[entry, idx]
 
 
 def _depth_samples(num_depth_samples) -> int:
@@ -2026,14 +2045,16 @@ def _depth_samples(num_depth_samples) -> int:
     return K
 
 
-def _contrib_rows(means2d, conics, opacities, image_dims=None) -> int:
-    """Checks dense [..., N, *] or packed [nnz, *] rows; returns N (nnz when packed: ids are then row indices)."""
+def _contrib_rows(walk, means2d, rows, opacities, image_dims=None) -> int:
+    """Checks dense [..., N, *] rows, or packed [nnz, *] rows where the walk takes them; returns N (nnz when packed: ids
+    are then row indices)."""
     if means2d.dim() < 2 or means2d.shape[-1] != 2:
-        raise ValueError(f"means2d must be [..., N, 2] or [nnz, 2], got {tuple(means2d.shape)}")
+        shapes = "[..., N, 2] or [nnz, 2]" if walk.packed else "[..., N, 2]"
+        raise ValueError(f"means2d must be {shapes}, got {tuple(means2d.shape)}")
     lead = tuple(means2d.shape[:-1])
-    if means2d.dim() > 2 and image_dims is not None and lead[:-1] != tuple(image_dims):
+    if (means2d.dim() > 2 or not walk.packed) and image_dims is not None and lead[:-1] != tuple(image_dims):
         raise ValueError(f"means2d must be {tuple(image_dims) + ('N', 2)} to match tile_offsets, got {tuple(means2d.shape)}")
-    _check_shape(conics, lead + (3,), "conics")
+    _check_shape(rows, lead + walk.rows_tail, walk.rows_name)
     _check_shape(opacities, lead, "opacities")
     return lead[-1]
 
@@ -2057,9 +2078,10 @@ def _check_counts(num_contributing_gaussians, dims) -> None:
         raise TypeError(f"num_contributing_gaussians must have dtype int32, got {nc.dtype}")
 
 
-def _contrib_dense(means2d, conics, opacities, tile_offsets, flatten_ids, image_width, image_height, tile_size, counts=None):
-    """Checks the dense-layout arguments (and the per-pixel counts, if given); returns (the output dims [..., H, W],
-    (the C arguments before the outputs, the tensors they point into), the device)."""
+def _contrib_dense(walk, means2d, rows, opacities, tile_offsets, flatten_ids, image_width, image_height, tile_size,
+                   counts=None):
+    """Checks the dense-layout arguments (and the per-pixel counts, if given); returns (the walk, the output dims
+    [..., H, W], (the C arguments before the outputs, the tensors they point into), the device)."""
     W, H = int(image_width), int(image_height)
     if tile_size != 16:
         raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
@@ -2067,32 +2089,34 @@ def _contrib_dense(means2d, conics, opacities, tile_offsets, flatten_ids, image_
         raise ValueError(f"tile_offsets must be [..., tile_height, tile_width], got {tuple(tile_offsets.shape)}")
     image_dims = tuple(tile_offsets.shape[:-2])
     th, tw = tile_offsets.shape[-2:]
-    N = _contrib_rows(means2d, conics, opacities, image_dims)
+    N = _contrib_rows(walk, means2d, rows, opacities, image_dims)
     if th * 16 < H or tw * 16 < W:
         raise ValueError(f"tile_offsets tile grid {tw}x{th} does not cover a {W}x{H} image")
     if flatten_ids.dim() != 1:
         raise ValueError(f"flatten_ids must be one-dimensional, got {tuple(flatten_ids.shape)}")
-    _contrib_dtypes(((means2d, "means2d"), (conics, "conics"), (opacities, "opacities")),
+    _contrib_dtypes(((means2d, "means2d"), (rows, walk.rows_name), (opacities, "opacities")),
                     ((tile_offsets, "tile_offsets", torch.int32), (flatten_ids, "flatten_ids", torch.int32)))
     _check_counts(counts, image_dims + (H, W))
-    dev = require_cuda(means2d, conics, opacities, tile_offsets, flatten_ids, counts)
-    keep = [t.contiguous() for t in (means2d, conics, opacities, tile_offsets, flatten_ids)]
-    m2, con, op, off, fl = keep
-    args = (_prod(image_dims), N, ptr(m2), ptr(con), ptr(op), W, H, 16, tw, th, ptr(off), ptr(fl), fl.shape[0], 0, None, None,
+    dev = require_cuda(means2d, rows, opacities, tile_offsets, flatten_ids, counts)
+    keep = [t.contiguous() for t in (means2d, rows, opacities, tile_offsets, flatten_ids)]
+    m2, rw, op, off, fl = keep
+    args = (_prod(image_dims), N, ptr(m2), ptr(rw), ptr(op), W, H, 16, tw, th, ptr(off), ptr(fl), fl.shape[0], 0, None, None,
             None, None)
-    return image_dims + (H, W), (args, keep), dev
+    return walk, image_dims + (H, W), (args, keep), dev
 
 
-def _contrib_sparse(means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum,
-                    pixel_map, image_width, image_height, tile_size, tile_width, tile_height, counts=None):
+def _contrib_sparse(walk, means2d, rows, opacities, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask,
+                    tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size, tile_width, tile_height, counts=None):
     """_contrib_dense for a sparse layout: the output dims are [P]."""
     W, H, tw, th = int(image_width), int(image_height), int(tile_width), int(tile_height)
     if tile_size != 16:
         raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
-    N = _contrib_rows(means2d, conics, opacities)
+    N = _contrib_rows(walk, means2d, rows, opacities)
     if active_tiles.dim() != 1 or pixel_map.dim() != 1 or flatten_ids.dim() != 1:
         raise ValueError("active_tiles [AT], pixel_map [P] and flatten_ids [n_isects] must be one-dimensional")
     AT, P = active_tiles.shape[0], pixel_map.shape[0]
+    if AT == 0 and P > 0:
+        raise ValueError(f"pixel_map lists {P} pixels but the layout has no active tile (build_sparse_tile_layout)")
     _check_shape(tile_offsets, (AT + 1,), "tile_offsets")
     _check_shape(tile_pixel_mask, (AT, _TILE_WORDS), "tile_pixel_mask")
     if tuple(tile_pixel_cumsum.shape) not in (((AT,),) if AT > 0 else ((0,), (1,))):
@@ -2101,32 +2125,33 @@ def _contrib_sparse(means2d, conics, opacities, active_tiles, tile_offsets, flat
         raise ValueError(f"a {tw} x {th} tile grid does not cover {W} x {H} pixels")
     if tile_pixel_mask.element_size() != 8 or tile_pixel_mask.is_floating_point():
         raise TypeError(f"tile_pixel_mask must be a 64-bit integer tensor, got {tile_pixel_mask.dtype}")
-    _contrib_dtypes(((means2d, "means2d"), (conics, "conics"), (opacities, "opacities")),
+    _contrib_dtypes(((means2d, "means2d"), (rows, walk.rows_name), (opacities, "opacities")),
                     ((active_tiles, "active_tiles", torch.int32), (tile_offsets, "tile_offsets", torch.int32),
                      (flatten_ids, "flatten_ids", torch.int32), (tile_pixel_cumsum, "tile_pixel_cumsum", torch.int64),
                      (pixel_map, "pixel_map", torch.int64)))
     _check_counts(counts, (P,))
-    dev = require_cuda(means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum,
+    dev = require_cuda(means2d, rows, opacities, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum,
                        pixel_map, counts)
-    keep = [t.contiguous() for t in (means2d, conics, opacities, tile_offsets, flatten_ids, active_tiles, tile_pixel_mask,
+    keep = [t.contiguous() for t in (means2d, rows, opacities, tile_offsets, flatten_ids, active_tiles, tile_pixel_mask,
                                      tile_pixel_cumsum, pixel_map)]
-    m2, con, op, off, fl, act, words, cum, pmap = keep
-    args = (1, N, ptr(m2), ptr(con), ptr(op), W, H, 16, tw, th, ptr(off), ptr(fl), fl.shape[0], AT, ptr(act), ptr(words),
+    m2, rw, op, off, fl, act, words, cum, pmap = keep
+    args = (1, N, ptr(m2), ptr(rw), ptr(op), W, H, 16, tw, th, ptr(off), ptr(fl), fl.shape[0], AT, ptr(act), ptr(words),
             ptr(cum), ptr(pmap))
-    return (P,), (args, keep), dev
+    return walk, (P,), (args, keep), dev
 
 
 def _contrib_count(what, checked):
-    dims, (args, _keep), dev = checked
+    walk, dims, (args, _keep), dev = checked
     counts = torch.empty(dims, device=dev, dtype=torch.int32)
     alphas = torch.empty(dims, device=dev, dtype=torch.float32)
-    with _Ctx(dev) as st:
-        check(lib().gsb200_contrib_count(*args, ptr(counts), ptr(alphas), st), what)
+    if counts.numel() > 0:  # a sparse layout without pixels has no active tile either: nothing to launch
+        with _Ctx(dev) as st:
+            check(getattr(lib(), walk.count)(*args, ptr(counts), ptr(alphas), st), what)
     return counts, alphas
 
 
 def _contrib_ids(what, checked, nc):
-    dims, (args, _keep), dev = checked
+    walk, dims, (args, _keep), dev = checked
     K = 0
     if nc.numel() > 0:
         lo, K = (int(v) for v in torch.stack(torch.aminmax(nc)).tolist())  # the one host read
@@ -2136,19 +2161,21 @@ def _contrib_ids(what, checked, nc):
     weights = torch.empty(dims + (K,), device=dev, dtype=torch.float32)
     if ids.numel() > 0:
         with _Ctx(dev) as st:
-            check(lib().gsb200_contrib_ids(*args, K, ptr(ids), ptr(weights), st), what)
+            check(getattr(lib(), walk.ids)(*args, K, ptr(ids), ptr(weights), st), what)
     return ids, weights
 
 
 def _contrib_top(what, checked, K):
-    dims, (args, _keep), dev = checked
-    bound = _max_depth_samples(dev)
+    walk, dims, (args, _keep), dev = checked
+    # the 3DGS walk's bound is _max_depth_samples' default
+    bound = _max_depth_samples(dev) if walk is _CONTRIB_3DGS else _max_depth_samples(dev, walk.max_samples)
     if K > bound:
         raise ValueError(f"num_depth_samples {K} exceeds {bound}, the most the top-K kernel holds in shared memory on {dev}")
     ids = torch.empty(dims + (K,), device=dev, dtype=torch.int32)
     weights = torch.empty(dims + (K,), device=dev, dtype=torch.float32)
-    with _Ctx(dev) as st:
-        check(lib().gsb200_contrib_top(*args, K, ptr(ids), ptr(weights), st), what)
+    if ids.numel() > 0:
+        with _Ctx(dev) as st:
+            check(getattr(lib(), walk.top)(*args, K, ptr(ids), ptr(weights), st), what)
     return ids, weights
 
 
@@ -2166,7 +2193,8 @@ def rasterize_num_contributing_gaussians(
     """Per pixel, the number of Gaussians ``rasterize_to_pixels`` composites and its accumulated alpha.  The decisions
     are the compositing kernel's own, so the alphas equal ``render_alphas``.  Returns (counts int32 [..., H, W],
     alphas float32 [..., H, W])."""
-    checked = _contrib_dense(means2d, conics, opacities, tile_offsets, flatten_ids, image_width, image_height, tile_size)
+    checked = _contrib_dense(_CONTRIB_3DGS, means2d, conics, opacities, tile_offsets, flatten_ids, image_width,
+                             image_height, tile_size)
     return _contrib_count("rasterize_num_contributing_gaussians", checked)
 
 
@@ -2189,8 +2217,9 @@ def rasterize_num_contributing_gaussians_sparse(
 ) -> Tuple[Tensor, Tensor]:
     """``rasterize_num_contributing_gaussians`` at the pixels of a build_sparse_tile_layout layout, with the lists of
     isect_tiles_sparse.  Returns (counts int32 [P], alphas float32 [P]) in the original pixel order."""
-    checked = _contrib_sparse(means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask,
-                              tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size, tile_width, tile_height)
+    checked = _contrib_sparse(_CONTRIB_3DGS, means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids,
+                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
+                              tile_width, tile_height)
     return _contrib_count("rasterize_num_contributing_gaussians_sparse", checked)
 
 
@@ -2209,8 +2238,8 @@ def rasterize_contributing_gaussian_ids(
     """Every Gaussian each pixel composites, front to back, with its weight ``alpha * T`` (T before it).  Returns
     (ids int32, weights float32) [..., H, W, K] with K = ``num_contributing_gaussians.max()`` (read back to the host
     once): a pixel's first K pairs (later ones are dropped), then -1 / 0.  Ids index N (dense rows) or nnz (packed)."""
-    checked = _contrib_dense(means2d, conics, opacities, tile_offsets, flatten_ids, image_width, image_height, tile_size,
-                             num_contributing_gaussians)
+    checked = _contrib_dense(_CONTRIB_3DGS, means2d, conics, opacities, tile_offsets, flatten_ids, image_width,
+                             image_height, tile_size, num_contributing_gaussians)
     return _contrib_ids("rasterize_contributing_gaussian_ids", checked, num_contributing_gaussians)
 
 
@@ -2234,9 +2263,9 @@ def rasterize_contributing_gaussian_ids_sparse(
 ) -> Tuple[Tensor, Tensor]:
     """``rasterize_contributing_gaussian_ids`` at the pixels of a sparse layout: (ids, weights) [P, K] in the original
     pixel order."""
-    checked = _contrib_sparse(means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask,
-                              tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size, tile_width, tile_height,
-                              num_contributing_gaussians)
+    checked = _contrib_sparse(_CONTRIB_3DGS, means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids,
+                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
+                              tile_width, tile_height, num_contributing_gaussians)
     return _contrib_ids("rasterize_contributing_gaussian_ids_sparse", checked, num_contributing_gaussians)
 
 
@@ -2257,7 +2286,8 @@ def rasterize_top_contributing_gaussian_ids(
     strictly heavier, as in the reference.  K must lie in [1, the device's bound] (about 71 on an H100: K slots per pixel
     live in shared memory); outside it a ValueError is raised before anything runs."""
     K = _depth_samples(num_depth_samples)
-    checked = _contrib_dense(means2d, conics, opacities, tile_offsets, flatten_ids, image_width, image_height, tile_size)
+    checked = _contrib_dense(_CONTRIB_3DGS, means2d, conics, opacities, tile_offsets, flatten_ids, image_width,
+                             image_height, tile_size)
     return _contrib_top("rasterize_top_contributing_gaussian_ids", checked, K)
 
 
@@ -2282,9 +2312,151 @@ def rasterize_top_contributing_gaussian_ids_sparse(
     """``rasterize_top_contributing_gaussian_ids`` at the pixels of a sparse layout: (ids, weights) [P, K] in the
     original pixel order."""
     K = _depth_samples(num_depth_samples)
-    checked = _contrib_sparse(means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask,
-                              tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size, tile_width, tile_height)
+    checked = _contrib_sparse(_CONTRIB_3DGS, means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids,
+                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
+                              tile_width, tile_height)
     return _contrib_top("rasterize_top_contributing_gaussian_ids_sparse", checked, K)
+
+
+@torch.no_grad()
+def rasterize_num_contributing_gaussians_2dgs(
+    means2d: Tensor,  # [..., N, 2]
+    ray_transforms: Tensor,  # [..., N, 3, 3]
+    opacities: Tensor,  # [..., N]
+    tile_offsets: Tensor,  # [..., tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+) -> Tuple[Tensor, Tensor]:
+    """``rasterize_num_contributing_gaussians`` for surfels: per pixel, the number of surfels
+    ``rasterize_to_pixels_2dgs`` composites and its accumulated alpha.  The decisions are the 2DGS compositing kernel's
+    own, so the alphas equal its ``render_alphas`` bit for bit.  Returns (counts int32 [..., H, W], alphas float32
+    [..., H, W])."""
+    checked = _contrib_dense(_CONTRIB_2DGS, means2d, ray_transforms, opacities, tile_offsets, flatten_ids, image_width,
+                             image_height, tile_size)
+    return _contrib_count("rasterize_num_contributing_gaussians_2dgs", checked)
+
+
+@torch.no_grad()
+def rasterize_num_contributing_gaussians_2dgs_sparse(
+    means2d: Tensor,  # [..., N, 2]
+    ray_transforms: Tensor,  # [..., N, 3, 3]
+    opacities: Tensor,  # [..., N]
+    active_tiles: Tensor,  # [AT]
+    tile_offsets: Tensor,  # [AT + 1]
+    flatten_ids: Tensor,  # [n_isects]
+    tile_pixel_mask: Tensor,  # [AT, 4]
+    tile_pixel_cumsum: Tensor,  # [AT]
+    pixel_map: Tensor,  # [P]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+) -> Tuple[Tensor, Tensor]:
+    """``rasterize_num_contributing_gaussians_2dgs`` at the pixels of a build_sparse_tile_layout layout, with the lists
+    of isect_tiles_sparse (conics=None) on the surfel rows.  Returns (counts int32 [P], alphas float32 [P]) in the
+    original pixel order."""
+    checked = _contrib_sparse(_CONTRIB_2DGS, means2d, ray_transforms, opacities, active_tiles, tile_offsets, flatten_ids,
+                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
+                              tile_width, tile_height)
+    return _contrib_count("rasterize_num_contributing_gaussians_2dgs_sparse", checked)
+
+
+@torch.no_grad()
+def rasterize_contributing_gaussian_ids_2dgs(
+    means2d: Tensor,  # [..., N, 2]
+    ray_transforms: Tensor,  # [..., N, 3, 3]
+    opacities: Tensor,  # [..., N]
+    tile_offsets: Tensor,  # [..., tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    num_contributing_gaussians: Tensor,  # [..., image_height, image_width]
+) -> Tuple[Tensor, Tensor]:
+    """Every surfel each pixel composites, front to back, with its weight ``alpha * T`` (T before it).  Returns
+    (ids int32, weights float32) [..., H, W, K] with K = ``num_contributing_gaussians.max()`` (read back to the host
+    once): a pixel's first K pairs (later ones are dropped), then -1 / 0.  Ids index N."""
+    checked = _contrib_dense(_CONTRIB_2DGS, means2d, ray_transforms, opacities, tile_offsets, flatten_ids, image_width,
+                             image_height, tile_size, num_contributing_gaussians)
+    return _contrib_ids("rasterize_contributing_gaussian_ids_2dgs", checked, num_contributing_gaussians)
+
+
+@torch.no_grad()
+def rasterize_contributing_gaussian_ids_2dgs_sparse(
+    means2d: Tensor,  # [..., N, 2]
+    ray_transforms: Tensor,  # [..., N, 3, 3]
+    opacities: Tensor,  # [..., N]
+    active_tiles: Tensor,  # [AT]
+    tile_offsets: Tensor,  # [AT + 1]
+    flatten_ids: Tensor,  # [n_isects]
+    tile_pixel_mask: Tensor,  # [AT, 4]
+    tile_pixel_cumsum: Tensor,  # [AT]
+    pixel_map: Tensor,  # [P]
+    num_contributing_gaussians: Tensor,  # [P] int32
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+) -> Tuple[Tensor, Tensor]:
+    """``rasterize_contributing_gaussian_ids_2dgs`` at the pixels of a sparse layout: (ids, weights) [P, K] in the
+    original pixel order."""
+    checked = _contrib_sparse(_CONTRIB_2DGS, means2d, ray_transforms, opacities, active_tiles, tile_offsets, flatten_ids,
+                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
+                              tile_width, tile_height, num_contributing_gaussians)
+    return _contrib_ids("rasterize_contributing_gaussian_ids_2dgs_sparse", checked, num_contributing_gaussians)
+
+
+@torch.no_grad()
+def rasterize_top_contributing_gaussian_ids_2dgs(
+    means2d: Tensor,  # [..., N, 2]
+    ray_transforms: Tensor,  # [..., N, 3, 3]
+    opacities: Tensor,  # [..., N]
+    tile_offsets: Tensor,  # [..., tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    num_depth_samples: int,
+) -> Tuple[Tensor, Tensor]:
+    """The ``num_depth_samples`` heaviest surfels of each pixel by ``alpha * T``, front to back: (ids int32, weights
+    float32) [..., H, W, K], -1 / 0 in unused slots, by the rule of ``rasterize_top_contributing_gaussian_ids``.  K must
+    lie in [1, the surfel walk's bound on the device] (71 on an H100); outside it a ValueError is raised before anything
+    runs."""
+    K = _depth_samples(num_depth_samples)
+    checked = _contrib_dense(_CONTRIB_2DGS, means2d, ray_transforms, opacities, tile_offsets, flatten_ids, image_width,
+                             image_height, tile_size)
+    return _contrib_top("rasterize_top_contributing_gaussian_ids_2dgs", checked, K)
+
+
+@torch.no_grad()
+def rasterize_top_contributing_gaussian_ids_2dgs_sparse(
+    means2d: Tensor,  # [..., N, 2]
+    ray_transforms: Tensor,  # [..., N, 3, 3]
+    opacities: Tensor,  # [..., N]
+    active_tiles: Tensor,  # [AT]
+    tile_offsets: Tensor,  # [AT + 1]
+    flatten_ids: Tensor,  # [n_isects]
+    tile_pixel_mask: Tensor,  # [AT, 4]
+    tile_pixel_cumsum: Tensor,  # [AT]
+    pixel_map: Tensor,  # [P]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+    num_depth_samples: int,
+) -> Tuple[Tensor, Tensor]:
+    """``rasterize_top_contributing_gaussian_ids_2dgs`` at the pixels of a sparse layout: (ids, weights) [P, K] in the
+    original pixel order."""
+    K = _depth_samples(num_depth_samples)
+    checked = _contrib_sparse(_CONTRIB_2DGS, means2d, ray_transforms, opacities, active_tiles, tile_offsets, flatten_ids,
+                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
+                              tile_width, tile_height)
+    return _contrib_top("rasterize_top_contributing_gaussian_ids_2dgs_sparse", checked, K)
 
 
 # --------------------------------------------------------------------------------------------

@@ -506,6 +506,37 @@ extern "C"
         int32_t *ids, float *weights, void *stream
     );
 
+    /* ---- 2DGS per-pixel contributor queries: rasterize_num_contributing_gaussians_2dgs,
+     * rasterize_contributing_gaussian_ids_2dgs, rasterize_top_contributing_gaussian_ids_2dgs and their _sparse forms (the
+     * reference has no 2DGS contributor queries).  The arguments, outputs, checks and return codes of gsb200_contrib_*,
+     * with ray_transforms [R,3,3] in place of conics; each pixel walks its tile's full list from T = 1 with the decisions
+     * of gsb200_surfel_indices (and so of gsb200_surfel_raster_fwd: count's alphas are its render_alphas).  Dense
+     * rows [I,N,*]; sparse lists from gsb200_isect_active_offsets on the surfel rows.
+     * gsb200_surfel_contrib_max_samples: the num_samples bound of gsb200_surfel_contrib_top, taken from the surfel walk's
+     * own staging arrays, or GSB200_E_CUDA without a device. */
+    int gsb200_surfel_contrib_max_samples(void);
+    int gsb200_surfel_contrib_count(
+        int64_t I, int64_t N, const float *means2d, const float *ray_transforms, const float *opacities,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int32_t *counts,
+        float *alphas, void *stream
+    );
+    int gsb200_surfel_contrib_ids(
+        int64_t I, int64_t N, const float *means2d, const float *ray_transforms, const float *opacities,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int max_samples,
+        int32_t *ids, float *weights, void *stream
+    );
+    int gsb200_surfel_contrib_top(
+        int64_t I, int64_t N, const float *means2d, const float *ray_transforms, const float *opacities,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int num_samples,
+        int32_t *ids, float *weights, void *stream
+    );
+
     /* ---- MCMC strategy ops ("next" row): relocation (ext.cpp `relocation`, gsplat/relocation.py:64,
      * csrc/RelocationCUDA.cu:36-80) and in-place position perturbation (csrc/MCMCPerturbCUDA.cu:28-60,
      * gsplat/strategy/ops.py).  ratios int32 [N] already clamped to [1, n_max]; binoms [n_max, n_max]. */

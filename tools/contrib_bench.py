@@ -3,7 +3,11 @@
 rasterize_top_contributing_gaussian_ids with K = 8 and 32, and the three _sparse forms on 4096 seeded pixels, with one
 rasterize_to_pixels forward on the same intersections for scale.
 
-    python tools/contrib_bench.py [--steps 20] [--warmup 5]
+With --2dgs the same scene is projected as surfels (fully_fused_projection_2dgs, the lists of isect_tiles_sorted and
+isect_tiles_sparse) and the six _2dgs queries are timed the same way, with one rasterize_to_pixels_2dgs forward (RGB +
+depth) for scale; the record also holds the surfel walk's top-K bound.
+
+    python tools/contrib_bench.py [--2dgs] [--steps 20] [--warmup 5]
 
 Each call is timed with CUDA events after `warmup` untimed calls; the ids query includes its host read of the largest
 count.  Projection, tile intersection and the sparse layout run once, outside the timed calls.  Prints one JSON line
@@ -34,6 +38,7 @@ def main() -> int:
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--2dgs", dest="surfels", action="store_true", help="the 2DGS queries on the scene's surfels")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("contrib_bench needs a GPU")
@@ -46,6 +51,8 @@ def main() -> int:
     colors = t(sc["colors"])[None].contiguous()
     rec = {"image": f"{W}x{H}", "n_gaussians": int(sc["means"].shape[0]), "sparse_pixels": N_SPARSE, "steps": args.steps}
     ms = lambda fn: timed(fn, args.steps, args.warmup)[0]  # noqa: E731
+    if args.surfels:
+        return main_2dgs(sc, t, vm, t(Ks), opac, colors, rec, ms, dev)
     with torch.no_grad():
         radii, m2, depths, conics, _ = gs.fully_fused_projection(t(sc["means"]), None, t(sc["quats"]), t(sc["scales"]), vm, t(Ks), W, H)
         _, ids, fl = gs.isect_tiles(m2, radii, depths, 16, TW, TH, conics=conics, opacities=opac)
@@ -61,11 +68,7 @@ def main() -> int:
         for k in (8, 32):
             rec[f"top{k}_ms"] = ms(lambda: gs.rasterize_top_contributing_gaussian_ids(*a, k))
 
-        rng = np.random.RandomState(42)
-        flat = rng.choice(W * H, N_SPARSE, replace=False)
-        pixels = t(np.stack([flat // W, flat % W], -1).astype(np.int32))
-        image_ids = torch.zeros(N_SPARSE, device=dev, dtype=torch.int32)
-        active, amask, words, cum, pmap = gs.build_sparse_tile_layout(pixels, image_ids, 1, 16, TW, TH)
+        active, amask, words, cum, pmap = _sparse_pixels(t, dev)
         s_off, s_fl = gs.isect_tiles_sparse(m2, radii, depths, amask, active, 1, 16, TW, TH)
         s = (m2, conics, opac, active, s_off, s_fl, words, cum, pmap)
         grid = (W, H, 16, TW, TH)
@@ -73,6 +76,50 @@ def main() -> int:
         rec["sparse_num_ms"] = ms(lambda: gs.rasterize_num_contributing_gaussians_sparse(*s, *grid))
         rec["sparse_ids_ms"] = ms(lambda: gs.rasterize_contributing_gaussian_ids_sparse(*s, s_counts, *grid))
         rec["sparse_top8_ms"] = ms(lambda: gs.rasterize_top_contributing_gaussian_ids_sparse(*s, *grid, 8))
+    rec.update(device_info())
+    print(json.dumps(rec), flush=True)
+    return 0
+
+
+def _sparse_pixels(t, dev):
+    """the 4096 seeded pixels of one image and their sparse layout"""
+    rng = np.random.RandomState(42)
+    flat = rng.choice(W * H, N_SPARSE, replace=False)
+    pixels = t(np.stack([flat // W, flat % W], -1).astype(np.int32))
+    image_ids = torch.zeros(N_SPARSE, device=dev, dtype=torch.int32)
+    return gs.build_sparse_tile_layout(pixels, image_ids, 1, 16, TW, TH)
+
+
+def main_2dgs(sc, t, vm, Ks, opac, colors, rec, ms, dev) -> int:
+    rec["pipeline"] = "2dgs"
+    with torch.no_grad():
+        radii, m2, depths, rt, nrm = gs.fully_fused_projection_2dgs(t(sc["means"]), t(sc["quats"]), t(sc["scales"]), vm, Ks,
+                                                                    W, H)
+        hits = gs.ops.isect_tiles_sorted(m2, radii, depths, 16, TW, TH)
+        off, fl = hits.isect_offsets.reshape(1, TH, TW), hits.flatten_ids
+        a = (m2, rt, opac, off, fl, W, H, 16)
+        counts, _ = gs.rasterize_num_contributing_gaussians_2dgs(*a)
+        rec["isects"] = int(fl.shape[0])
+        rec["pairs"] = int(counts.sum())
+        rec["max_count"] = int(counts.max())
+        rec["surfel_top_k_bound"] = gs.ops._max_depth_samples(torch.device(dev), "gsb200_surfel_contrib_max_samples")
+        rgbd = torch.cat([colors, depths[..., None]], -1).contiguous()
+        densify = torch.zeros_like(m2)
+        rec["raster_2dgs_fwd_ms"] = ms(lambda: gs.rasterize_to_pixels_2dgs(m2, rt, rgbd, opac, nrm, densify, W, H, 16, off, fl))
+        rec["num_ms"] = ms(lambda: gs.rasterize_num_contributing_gaussians_2dgs(*a))
+        rec["ids_ms"] = ms(lambda: gs.rasterize_contributing_gaussian_ids_2dgs(*a, counts))
+        for k in (8, 32):
+            rec[f"top{k}_ms"] = ms(lambda: gs.rasterize_top_contributing_gaussian_ids_2dgs(*a, k))
+
+        active, amask, words, cum, pmap = _sparse_pixels(t, dev)
+        s_off, s_fl = gs.isect_tiles_sparse(m2, radii, depths, amask, active, 1, 16, TW, TH)
+        s = (m2, rt, opac, active, s_off, s_fl, words, cum, pmap)
+        grid = (W, H, 16, TW, TH)
+        s_counts, _ = gs.rasterize_num_contributing_gaussians_2dgs_sparse(*s, *grid)
+        rec["sparse_num_ms"] = ms(lambda: gs.rasterize_num_contributing_gaussians_2dgs_sparse(*s, *grid))
+        rec["sparse_ids_ms"] = ms(lambda: gs.rasterize_contributing_gaussian_ids_2dgs_sparse(*s, s_counts, *grid))
+        for k in (8, 32):
+            rec[f"sparse_top{k}_ms"] = ms(lambda: gs.rasterize_top_contributing_gaussian_ids_2dgs_sparse(*s, *grid, k))
     rec.update(device_info())
     print(json.dumps(rec), flush=True)
     return 0
