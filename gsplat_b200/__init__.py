@@ -22,6 +22,7 @@ from .ops import (  # noqa: F401
     mcmc_perturb_positions,
     fully_fused_projection,
     fully_fused_projection_2dgs,
+    fully_fused_projection_with_ut,
     fused_project_sh,
     isect_offset_encode,
     isect_tiles,
@@ -40,6 +41,7 @@ from .ops import (  # noqa: F401
     rasterize_to_pixels,
     rasterize_to_pixels_2dgs,
     rasterize_to_pixels_2dgs_sparse,
+    rasterize_to_pixels_eval3d,
     rasterize_to_pixels_sparse,
     rasterize_top_contributing_gaussian_ids,
     rasterize_top_contributing_gaussian_ids_2dgs,
@@ -76,6 +78,9 @@ def has_2dgs() -> bool:
 
 
 def has_3dgut() -> bool:
+    """Reference: _wrapper.py has_3dgut -- False: ``rasterization(with_ut=True, with_eval3d=True)`` is not built.  The two
+    3DGUT operators, ``fully_fused_projection_with_ut`` and ``rasterize_to_pixels_eval3d``, are (pinhole and fisheye,
+    global shutter), and chain with ``isect_tiles`` / ``isect_offset_encode`` as in the reference's ``_rasterization``."""
     return False
 
 
@@ -91,6 +96,8 @@ def has_camera_wrappers() -> bool:
 __all__ = [
     "rasterization",
     "fully_fused_projection",
+    "fully_fused_projection_with_ut",
+    "rasterize_to_pixels_eval3d",
     "fused_project_sh",
     "spherical_harmonics",
     "isect_tiles",

@@ -28,8 +28,9 @@ UNITS = {
     "nvls.cu": [],
     "loss.cu": [],
     "surfel.cu": ["-fmad=false"],
+    "ut.cu": ["-fmad=false"],
 }
-HEADERS = ["common.cuh", "gaussmath.cuh", "indices.cuh", "isect.cuh", "pixels.cuh", "rowrec.cuh", os.path.join("..", "..", "include", "gsplat_b200.h")]
+HEADERS = ["camera.cuh", "common.cuh", "gaussmath.cuh", "indices.cuh", "isect.cuh", "pixels.cuh", "rowrec.cuh", os.path.join("..", "..", "include", "gsplat_b200.h")]
 
 
 def _nvcc() -> str:

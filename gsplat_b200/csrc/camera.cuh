@@ -1,0 +1,250 @@
+// camera.cuh -- the distorted camera models of the 3DGUT operators: OpenCV pinhole (radial 6 as a rational k1..k6,
+// tangential 2, thin prism 4) and OpenCV fisheye (odd polynomial theta + k1 theta^3 + .. + k4 theta^9), forward
+// projection of a camera-frame point and unprojection of an image point to a unit camera ray.
+//
+// Reference semantics: include/Cameras.cuh (PerfectPinholeCameraModel, OpenCVPinholeCameraModel with 5 Newton
+// undistortion steps, OpenCVFisheyeCameraModel with 20 Newton steps on the angle, the validity margin and the fisheye
+// maximum angle).  A pinhole camera given no coefficient group at all is the perfect pinhole: no radial validity test
+// and a closed-form ray.
+#pragma once
+#include <float.h>
+
+#include "common.cuh"
+
+namespace gsb
+{
+constexpr int kUtPinhole = 0;
+constexpr int kUtFisheye = 2; // ids as in ops._camera_model_id
+
+struct CamModel
+{
+    float fx, fy, cx, cy;
+    float k[6], p[2], s[4]; // fisheye: k[0..3]
+    uint32_t W, H;
+    int kind;
+    bool distorted;   // pinhole with any coefficient group given
+    float max_angle;  // fisheye
+    float inv_slope;  // fisheye: first guess of theta per unit normalised radius
+};
+
+// polynomials in theta^2 of the fisheye model: f(t) = t * P(t^2), f'(t) = Q(t^2)
+__device__ __forceinline__ float fe_f(const float *k, float t)
+{
+    const float t2 = t * t;
+    return t * (1.f + t2 * (k[0] + t2 * (k[1] + t2 * (k[2] + t2 * k[3]))));
+}
+__device__ __forceinline__ float fe_df(const float *k, float t)
+{
+    const float t2 = t * t;
+    return 1.f + t2 * (3.f * k[0] + t2 * (5.f * k[1] + t2 * (7.f * k[2] + t2 * (9.f * k[3]))));
+}
+
+__device__ __forceinline__ CamModel load_cam_model(
+    int kind, const float *K, const float *radial, const float *tangential, const float *thin, int64_t cam, uint32_t W,
+    uint32_t H
+)
+{
+    CamModel m;
+    m.kind = kind;
+    m.W = W, m.H = H;
+    m.fx = K[cam * 9 + 0], m.fy = K[cam * 9 + 4], m.cx = K[cam * 9 + 2], m.cy = K[cam * 9 + 5];
+#pragma unroll
+    for(int i = 0; i < 6; ++i)
+        m.k[i] = 0.f;
+#pragma unroll
+    for(int i = 0; i < 2; ++i)
+        m.p[i] = 0.f;
+#pragma unroll
+    for(int i = 0; i < 4; ++i)
+        m.s[i] = 0.f;
+    m.max_angle = FLT_MAX, m.inv_slope = 0.f;
+    m.distorted = false;
+    if(kind == kUtPinhole)
+    {
+        m.distorted = radial || tangential || thin;
+#pragma unroll
+        for(int i = 0; i < 6; ++i)
+            m.k[i] = radial ? radial[cam * 6 + i] : 0.f;
+#pragma unroll
+        for(int i = 0; i < 2; ++i)
+            m.p[i] = tangential ? tangential[cam * 2 + i] : 0.f;
+#pragma unroll
+        for(int i = 0; i < 4; ++i)
+            m.s[i] = thin ? thin[cam * 4 + i] : 0.f;
+        return m;
+    }
+#pragma unroll
+    for(int i = 0; i < 4; ++i)
+        m.k[i] = radial ? radial[cam * 4 + i] : 0.f;
+    // The model is trusted while the image radius grows with the angle: up to the first zero of f' or, past the
+    // image's far corner, the angle of that corner.  f' is sampled on [0, bound] and its first sign change bisected.
+    const float mdx = fmaxf((float)W - m.cx, m.cx), mdy = fmaxf((float)H - m.cy, m.cy);
+    const float max_r = sqrtf(mdx * mdx + mdy * mdy);
+    const float bound = fmaxf(max_r / m.fx, max_r / m.fy);
+    m.max_angle = bound;
+    constexpr int kSamples = 64;
+    float lo = 0.f;
+    for(int i = 1; i <= kSamples; ++i)
+    {
+        const float hi = bound * (float)i / (float)kSamples;
+        if(fe_df(m.k, hi) <= 0.f)
+        {
+            float a = lo, b = hi;
+            for(int it = 0; it < 32; ++it)
+            {
+                const float mid = 0.5f * (a + b);
+                if(fe_df(m.k, mid) > 0.f)
+                    a = mid;
+                else
+                    b = mid;
+            }
+            m.max_angle = a;
+            break;
+        }
+        lo = hi;
+    }
+    const float max_nd = fmaxf((float)W / 2.f / m.fx, (float)H / 2.f / m.fy);
+    m.inv_slope = m.max_angle / max_nd;
+    return m;
+}
+
+__device__ __forceinline__ bool in_margin(const CamModel &m, float u, float v, float margin)
+{
+    const float mx = (float)m.W * margin, my = (float)m.H * margin;
+    return -mx <= u && u < (float)m.W + mx && -my <= v && v < (float)m.H + my;
+}
+
+// OpenCV pinhole distortion at normalised (x, y): radial factor icD and the tangential + thin-prism offset
+__device__ __forceinline__ float pinhole_distort(const CamModel &m, float x, float y, float &dx, float &dy)
+{
+    const float x2 = x * x, y2 = y * y, r2 = x2 + y2;
+    const float num = 1.f + r2 * (m.k[0] + r2 * (m.k[1] + r2 * m.k[2]));
+    const float den = 1.f + r2 * (m.k[3] + r2 * (m.k[4] + r2 * m.k[5]));
+    const float a1 = 2.f * x * y;
+    dx = m.p[0] * a1 + m.p[1] * (r2 + 2.f * x2) + r2 * (m.s[0] + r2 * m.s[1]);
+    dy = m.p[0] * (r2 + 2.f * y2) + m.p[1] * a1 + r2 * (m.s[2] + r2 * m.s[3]);
+    return fabsf(den) > 1e-8f ? num / den : 0.f;
+}
+
+// The distortion map D(x, y) = icD (x, y) + offset and its Jacobian J (row-major d(Dx, Dy)/d(x, y)).  false: icD <= 0,
+// where the map folds the image over and has no inverse.
+__device__ __forceinline__ bool pinhole_distort_jacobian(const CamModel &m, float x, float y, float *D, float *J)
+{
+    const float r2  = x * x + y * y;
+    const float num = 1.f + r2 * (m.k[0] + r2 * (m.k[1] + r2 * m.k[2]));
+    const float den = 1.f + r2 * (m.k[3] + r2 * (m.k[4] + r2 * m.k[5]));
+    const float icd = num / den;
+    if(!(icd > 0.f))
+        return false;
+    // d icD / d r2, and the thin-prism slopes d(s0 r2 + s1 r2^2) / d r2
+    const float dnum = m.k[0] + r2 * (2.f * m.k[1] + 3.f * r2 * m.k[2]);
+    const float dden = m.k[3] + r2 * (2.f * m.k[4] + 3.f * r2 * m.k[5]);
+    const float dicd = (dnum - icd * dden) / den;
+    const float gx = m.s[0] + 2.f * m.s[1] * r2, gy = m.s[2] + 2.f * m.s[3] * r2;
+    const float p0 = m.p[0], p1 = m.p[1];
+    D[0] = icd * x + p0 * 2.f * x * y + p1 * (r2 + 2.f * x * x) + r2 * (m.s[0] + r2 * m.s[1]);
+    D[1] = icd * y + p0 * (r2 + 2.f * y * y) + p1 * 2.f * x * y + r2 * (m.s[2] + r2 * m.s[3]);
+    J[0] = icd + 2.f * x * x * dicd + 2.f * p0 * y + 6.f * p1 * x + 2.f * x * gx;
+    J[1] = 2.f * x * y * dicd + 2.f * p0 * x + 2.f * p1 * y + 2.f * y * gx;
+    J[2] = 2.f * x * y * dicd + 2.f * p0 * x + 2.f * p1 * y + 2.f * x * gy;
+    J[3] = icd + 2.f * y * y * dicd + 6.f * p0 * y + 2.f * p1 * x + 2.f * y * gy;
+    return true;
+}
+
+// Camera-frame point -> image point.  Returns validity; (u, v) is set also for an invalid point, as the unscented
+// transform averages every sigma point: (0, 0) behind the camera.
+__device__ __forceinline__ bool cam_project(const CamModel &m, const float *pc, float margin, float &u, float &v)
+{
+    u = 0.f, v = 0.f;
+    if(pc[2] <= 0.f)
+        return false;
+    if(m.kind == kUtPinhole)
+    {
+        const float x = pc[0] / pc[2], y = pc[1] / pc[2];
+        if(!m.distorted)
+        {
+            u = x * m.fx + m.cx, v = y * m.fy + m.cy;
+            return in_margin(m, u, v, margin);
+        }
+        float dx, dy;
+        const float icD = pinhole_distort(m, x, y, dx, dy);
+        u = (icD * x + dx) * m.fx + m.cx;
+        v = (icD * y + dy) * m.fy + m.cy;
+        return icD > 0.8f && in_margin(m, u, v, margin);
+    }
+    const float ax = fabsf(pc[0]), ay = fabsf(pc[1]);
+    const float lo = fminf(ax, ay), hi = fmaxf(ax, ay);
+    float rxy = 0.f;
+    if(hi > 0.f)
+    {
+        const float q = lo / hi;
+        rxy = hi * sqrtf(1.f + q * q);
+    }
+    if(rxy <= 0.f)
+        rxy = FLT_EPSILON;
+    const float th_full = atan2f(rxy, pc[2]);
+    const float th = th_full < m.max_angle ? th_full : m.max_angle;
+    const float delta = fe_f(m.k, th) / rxy;
+    if(delta <= 0.f)
+        return false;
+    u = m.fx * delta * pc[0] + m.cx;
+    v = m.fy * delta * pc[1] + m.cy;
+    return in_margin(m, u, v, margin) && th_full < m.max_angle;
+}
+
+// Image point -> unit camera ray.  false: the model cannot invert at this point (the Newton iteration did not converge
+// or left the valid range); such a pixel composites nothing.
+__device__ __forceinline__ bool cam_unproject(const CamModel &m, float u, float v, float *d)
+{
+    const float x0 = (u - m.cx) / m.fx, y0 = (v - m.cy) / m.fy;
+    if(m.kind == kUtPinhole)
+    {
+        float x = x0, y = y0;
+        bool ok = !m.distorted;
+        // Newton on D(x, y) = (x0, y0), D the distortion map, from the distorted point itself
+        for(int it = 0; it < 5 && m.distorted; ++it)
+        {
+            float D[2], J[4];
+            if(!pinhole_distort_jacobian(m, x, y, D, J))
+                break;
+            const float det = J[0] * J[3] - J[1] * J[2];
+            if(fabsf(det) < 1e-6f)
+                break;
+            const float ex = x0 - D[0], ey = y0 - D[1];
+            const float sx = (J[3] * ex - J[1] * ey) / det;
+            const float sy = (J[0] * ey - J[2] * ex) / det;
+            x += sx, y += sy;
+            if(fabsf(sx) < 1e-6f && fabsf(sy) < 1e-6f)
+            {
+                ok = true;
+                break;
+            }
+        }
+        const float inv = 1.f / sqrtf(x * x + y * y + 1.f);
+        d[0] = x * inv, d[1] = y * inv, d[2] = inv;
+        return ok;
+    }
+    const float delta = sqrtf(x0 * x0 + y0 * y0);
+    float t = m.inv_slope * delta;
+    bool conv = false;
+    for(int it = 0; it < 20; ++it)
+    {
+        const float dx = (fe_f(m.k, t) - delta) / fe_df(m.k, t);
+        t -= dx;
+        if(fabsf(dx) < 1e-6f)
+        {
+            conv = true;
+            break;
+        }
+    }
+    d[0] = 0.f, d[1] = 0.f, d[2] = 1.f;
+    if(t < 0.f || t >= m.max_angle || !conv)
+        return false;
+    if(delta >= 1e-6f)
+    {
+        const float sc = sinf(t) / delta;
+        d[0] = sc * x0, d[1] = sc * y0, d[2] = cosf(t);
+    }
+    return true;
+}
+} // namespace gsb

@@ -1,0 +1,677 @@
+// ut.cu -- 3DGUT: the unscented-transform projection through a distorted camera (fully_fused_projection_with_ut) and
+// the compositing that evaluates every gaussian in 3-D along each pixel's ray (rasterize_to_pixels_eval3d), with its
+// backward.  Compiled with -fmad=false: the forward and the backward evaluate each (pixel, gaussian) response with the
+// same individually rounded operations, so both passes take the same alpha and transmittance decisions.
+//
+// Reference semantics: csrc/ProjectionUT3DGSFused.cu and include/Cameras.cuh (sigma points, weights, the UT validity
+// rule, the culling tail), csrc/RasterizeToPixelsFromWorld3DGS.cuh (the maximum response of a gaussian along a ray and
+// the compositing thresholds).  The reference's backward gives no gradient to viewmats, and neither does this one.
+#include "camera.cuh"
+#include "gaussmath.cuh"
+
+namespace gsb
+{
+namespace
+{
+constexpr int kUtThreads = 256;
+
+struct UtParams
+{
+    float alpha, beta, kappa, margin;
+    int require_all;
+};
+
+// One thread per (b, c, n).  Culled rows get radii 0 and zero float outputs.
+__global__ void __launch_bounds__(kUtThreads) ut_project_kernel(
+    int64_t B, int64_t C, int64_t N, const float *__restrict__ means, const float *__restrict__ quats,
+    const float *__restrict__ scales, const float *__restrict__ opacities, const float *__restrict__ viewmats,
+    const float *__restrict__ Ks, int cam_kind, const float *__restrict__ radial, const float *__restrict__ tangential,
+    const float *__restrict__ thin, uint32_t W, uint32_t H, float eps2d, float near_plane, float far_plane,
+    float radius_clip, UtParams ut, int32_t *__restrict__ radii, float *__restrict__ means2d, float *__restrict__ depths,
+    float *__restrict__ conics, float *__restrict__ compensations
+)
+{
+    const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(idx >= B * C * N)
+        return;
+    const int64_t b = idx / (C * N), c = (idx / N) % C, n = idx % N;
+    const int64_t bn = b * N + n, bc = b * C + c;
+    const float mean[3] = {means[bn * 3], means[bn * 3 + 1], means[bn * 3 + 2]};
+    const float q[4]    = {quats[bn * 4], quats[bn * 4 + 1], quats[bn * 4 + 2], quats[bn * 4 + 3]};
+    const float s[3]    = {scales[bn * 3], scales[bn * 3 + 1], scales[bn * 3 + 2]};
+
+    int rx = 0, ry = 0;
+    float mx = 0.f, my = 0.f, depth = 0.f, ca = 0.f, cb = 0.f, cc = 0.f, comp = 0.f;
+    const float qn2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+    const Cam cam   = load_cam(viewmats + bc * 16, Ks + bc * 9);
+    float pc[3];
+#pragma unroll
+    for(int i = 0; i < 3; ++i)
+        pc[i] = cam.R.m[i * 3 + 0] * mean[0] + cam.R.m[i * 3 + 1] * mean[1] + cam.R.m[i * 3 + 2] * mean[2] + cam.t[i];
+    // a zero quaternion or a zero scale axis has no 3-D precision matrix to evaluate along a ray
+    const bool degenerate = fabsf(qn2) < FLT_EPSILON || fabsf(s[0]) < FLT_EPSILON || fabsf(s[1]) < FLT_EPSILON
+                         || fabsf(s[2]) < FLT_EPSILON;
+    if(!degenerate && !(pc[2] < near_plane || pc[2] > far_plane))
+    {
+        const CamModel cm = load_cam_model(cam_kind, Ks, radial, tangential, thin, bc, W, H);
+        const M3 Rq       = quat_to_rotmat(q);
+        const float lam   = ut.alpha * ut.alpha * (3.f + ut.kappa) - 3.f;
+        const float spread = sqrtf(3.f + lam);
+        const float w_mean0 = lam / (3.f + lam);
+        const float w_cov0  = w_mean0 + (1.f - ut.alpha * ut.alpha + ut.beta);
+        const float w_rest  = 1.f / (2.f * (3.f + lam));
+        float pu[7], pv[7];
+        bool any = false, all = true;
+        float m2x = 0.f, m2y = 0.f;
+#pragma unroll
+        for(int k = 0; k < 7; ++k)
+        {
+            // sigma point k: the mean, then mean +- spread * s_i * (column i of the rotation)
+            float x[3] = {mean[0], mean[1], mean[2]};
+            if(k > 0)
+            {
+                const int ax    = (k - 1) % 3;
+                const float sg  = k <= 3 ? 1.f : -1.f;
+                const float mag = spread * s[ax];
+#pragma unroll
+                for(int i = 0; i < 3; ++i)
+                    x[i] = sg > 0.f ? x[i] + mag * Rq.m[i * 3 + ax] : x[i] - mag * Rq.m[i * 3 + ax];
+            }
+            float xc[3];
+#pragma unroll
+            for(int i = 0; i < 3; ++i)
+                xc[i] = cam.R.m[i * 3 + 0] * x[0] + cam.R.m[i * 3 + 1] * x[1] + cam.R.m[i * 3 + 2] * x[2] + cam.t[i];
+            const bool ok = cam_project(cm, xc, ut.margin, pu[k], pv[k]);
+            any = any || ok;
+            all = all && ok;
+            // with every point required, the first invalid one ends the transform (the row is culled)
+            const float w = k == 0 ? w_mean0 : w_rest;
+            m2x = m2x + w * pu[k];
+            m2y = m2y + w * pv[k];
+        }
+        if(ut.require_all ? all : any)
+        {
+            float c00 = 0.f, c01 = 0.f, c11 = 0.f;
+#pragma unroll
+            for(int k = 0; k < 7; ++k)
+            {
+                const float w  = k == 0 ? w_cov0 : w_rest;
+                const float du = pu[k] - m2x, dv = pv[k] - m2y;
+                c00 = c00 + w * (du * du);
+                c01 = c01 + w * (du * dv);
+                c11 = c11 + w * (dv * dv);
+            }
+            const float det_orig = c00 * c11 - c01 * c01;
+            c00 += eps2d;
+            c11 += eps2d;
+            const float det      = c00 * c11 - c01 * c01;
+            const float ratio    = det_orig / det;
+            const float floor_   = kMinCompensation * kMinCompensation;
+            const float compensation = sqrtf(ratio > floor_ ? ratio : floor_);
+            // the centre covariance weight is negative, so the UT covariance need not be positive semi-definite
+            bool keep = det > 0.f && !(c00 < 0.f || c11 < 0.f);
+            float extend = kGaussianExtend;
+            if(keep && opacities != nullptr)
+            {
+                const float op = opacities[bn] * compensation;
+                keep = !(op < kAlphaThreshold);
+                if(keep)
+                {
+                    const float e2 = sqrtf(2.f * exact_log(op / kAlphaThreshold));
+                    extend = e2 < extend ? e2 : extend;
+                }
+            }
+            if(keep)
+            {
+                // tight box: the smaller of the axis extent and the larger eigenvalue's
+                const float hb  = 0.5f * (c00 + c11);
+                const float tmp = sqrtf(fmaxf(0.01f, hb * hb - det));
+                const float r1  = extend * sqrtf(hb + tmp);
+                const float fr_x = ceilf(fminf(extend * sqrtf(c00), r1));
+                const float fr_y = ceilf(fminf(extend * sqrtf(c11), r1));
+                const float ood  = 1.f / det;
+                const bool clipped = fr_x <= radius_clip && fr_y <= radius_clip;
+                const bool off = m2x + fr_x <= 0.f || m2x - fr_x >= (float)W || m2y + fr_y <= 0.f || m2y - fr_y >= (float)H;
+                const float k0 = c11 * ood, k1 = -c01 * ood, k2 = c00 * ood;
+                // finite inputs can overflow (a far sigma point through a strong distortion): a NaN row would pass every
+                // off-screen test, so it is culled
+                const bool finite = isfinite(m2x) && isfinite(m2y) && isfinite(k0) && isfinite(k1) && isfinite(k2)
+                                 && isfinite(fr_x) && isfinite(fr_y) && isfinite(pc[2]);
+                if(!clipped && !off && finite)
+                {
+                    rx = (int)fr_x, ry = (int)fr_y;
+                    mx = m2x, my = m2y, depth = pc[2];
+                    ca = k0, cb = k1, cc = k2;
+                    comp = compensation;
+                }
+            }
+        }
+    }
+    reinterpret_cast<int2 *>(radii)[idx]     = make_int2(rx, ry);
+    reinterpret_cast<float2 *>(means2d)[idx] = make_float2(mx, my);
+    depths[idx]         = depth;
+    conics[idx * 3 + 0] = ca;
+    conics[idx * 3 + 1] = cb;
+    conics[idx * 3 + 2] = cc;
+    if(compensations)
+        compensations[idx] = comp;
+}
+
+// ------------------------------------------------------------------ compositing
+// One staged gaussian of a tile: world mean, opacity of its (image, gaussian) row, the world-to-unit-sphere map
+// M = S^-1 R^T, its row id in [I * N] and its gaussian id in [B * N].
+struct EvalRec
+{
+    float mu[3], o;
+    float m[9];
+    int32_t id, bn;
+};
+
+__device__ __forceinline__ void stage(
+    EvalRec &r, int32_t g, int64_t C, int64_t N, const float *means, const float *quats, const float *scales,
+    const float *opacities
+)
+{
+    const int64_t bn = (g / (C * N)) * N + g % N;
+    r.id             = g;
+    r.bn             = (int32_t)bn;
+    r.o              = opacities[g];
+#pragma unroll
+    for(int k = 0; k < 3; ++k)
+        r.mu[k] = means[bn * 3 + k];
+    const float q[4] = {quats[bn * 4], quats[bn * 4 + 1], quats[bn * 4 + 2], quats[bn * 4 + 3]};
+    const M3 R       = quat_to_rotmat(q);
+#pragma unroll
+    for(int i = 0; i < 3; ++i)
+    {
+        const float inv = 1.f / scales[bn * 3 + i];
+#pragma unroll
+        for(int j = 0; j < 3; ++j)
+            r.m[i * 3 + j] = R.m[j * 3 + i] * inv;
+    }
+}
+
+// The world ray of pixel (i, j) of one camera: origin, unit direction.  false: the camera model cannot unproject it.
+__device__ __forceinline__ bool pixel_ray(
+    const float *vm, const CamModel &cm, uint32_t i, uint32_t j, float *ro, float *rd
+)
+{
+    float dc[3];
+    const bool ok = cam_unproject(cm, (float)j + 0.5f, (float)i + 0.5f, dc);
+    const float R[9] = {vm[0], vm[1], vm[2], vm[4], vm[5], vm[6], vm[8], vm[9], vm[10]};
+    const float t[3] = {vm[3], vm[7], vm[11]};
+#pragma unroll
+    for(int k = 0; k < 3; ++k)
+    {
+        ro[k] = -(R[0 * 3 + k] * t[0] + R[1 * 3 + k] * t[1] + R[2 * 3 + k] * t[2]);
+        rd[k] = R[0 * 3 + k] * dc[0] + R[1 * 3 + k] * dc[1] + R[2 * 3 + k] * dc[2];
+    }
+    return ok;
+}
+
+// Maximum response of one gaussian along a ray: a = M (o - mu), g = normalize(M d); the closest approach to the
+// gaussian's centre in its own frame is |g x a|.  ok = false: the approach lies behind the ray origin, or alpha < 1/255.
+struct EvalHit
+{
+    float w[3], a[3], b[3], bl, g[3], c[3], resp, alpha;
+    bool ok;
+};
+
+__device__ __forceinline__ EvalHit eval_hit(const EvalRec &r, const float *ro, const float *rd)
+{
+    EvalHit h;
+#pragma unroll
+    for(int k = 0; k < 3; ++k)
+        h.w[k] = ro[k] - r.mu[k];
+#pragma unroll
+    for(int i = 0; i < 3; ++i)
+    {
+        h.a[i] = r.m[i * 3 + 0] * h.w[0] + r.m[i * 3 + 1] * h.w[1] + r.m[i * 3 + 2] * h.w[2];
+        h.b[i] = r.m[i * 3 + 0] * rd[0] + r.m[i * 3 + 1] * rd[1] + r.m[i * 3 + 2] * rd[2];
+    }
+    const float l2 = h.b[0] * h.b[0] + h.b[1] * h.b[1] + h.b[2] * h.b[2];
+    h.bl           = sqrtf(l2);
+    const float inv = l2 > 0.f ? 1.f / h.bl : 1.f;
+#pragma unroll
+    for(int k = 0; k < 3; ++k)
+        h.g[k] = h.b[k] * inv;
+    const float hit_t = -(h.g[0] * h.a[0] + h.g[1] * h.a[1] + h.g[2] * h.a[2]);
+    h.c[0]  = h.g[1] * h.a[2] - h.g[2] * h.a[1];
+    h.c[1]  = h.g[2] * h.a[0] - h.g[0] * h.a[2];
+    h.c[2]  = h.g[0] * h.a[1] - h.g[1] * h.a[0];
+    const float dist = h.c[0] * h.c[0] + h.c[1] * h.c[1] + h.c[2] * h.c[2];
+    h.resp  = fast_exp(-0.5f * dist);
+    h.alpha = fminf(kMaxAlpha, r.o * h.resp);
+    h.ok    = !(hit_t < 0.f) && !(h.alpha < kAlphaThreshold) && l2 > 0.f;
+    return h;
+}
+
+struct EvalGeom
+{
+    uint32_t I, C, N, W, H, tw, th;
+    int cam_kind;
+    const float *viewmats, *Ks, *radial, *tangential, *thin;
+};
+
+// One CTA per 16x16 tile of the [I, th, tw] grid, one pixel per thread.  last_ids: the list index of the pixel's last
+// composited gaussian, -1 for none.
+template<int CDIM>
+__global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
+    EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
+    const float *__restrict__ colors, const float *__restrict__ opacities, const float *__restrict__ backgrounds,
+    const uint8_t *__restrict__ masks, const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids,
+    int64_t n_isects, float *__restrict__ render_colors, float *__restrict__ render_alphas, int32_t *__restrict__ last_ids
+)
+{
+    __shared__ EvalRec rec[kUtThreads];
+    const uint32_t tile = blockIdx.x;
+    const uint32_t img  = tile / (geo.tw * geo.th);
+    const uint32_t tin  = tile - img * geo.tw * geo.th;
+    const uint32_t tr   = threadIdx.x;
+    const uint32_t i    = (tin / geo.tw) * kTile + tr / kTile;
+    const uint32_t j    = (tin % geo.tw) * kTile + tr % kTile;
+    const bool inside   = i < geo.H && j < geo.W;
+    const int64_t pix   = (int64_t)img * geo.H * geo.W + (int64_t)i * geo.W + j;
+    const float *bg     = backgrounds ? backgrounds + (int64_t)img * CDIM : nullptr;
+    if(masks && !masks[tile])
+    {
+        if(inside)
+        {
+#pragma unroll
+            for(int k = 0; k < CDIM; ++k)
+                render_colors[pix * CDIM + k] = bg ? bg[k] : 0.f;
+            render_alphas[pix] = 0.f;
+            last_ids[pix]      = -1;
+        }
+        return;
+    }
+    const int64_t start = offsets[tile];
+    const int64_t end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
+    float ro[3] = {0.f, 0.f, 0.f}, rd[3] = {0.f, 0.f, 1.f};
+    bool done = !inside;
+    if(inside)
+    {
+        const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        done              = !pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
+    }
+    float T = 1.f, pix_out[CDIM];
+#pragma unroll
+    for(int k = 0; k < CDIM; ++k)
+        pix_out[k] = 0.f;
+    int32_t cur_idx = -1;
+    for(int64_t batch = start; batch < end; batch += kUtThreads)
+    {
+        if(__syncthreads_count(done) == kUtThreads)
+            break;
+        if(batch + tr < end)
+            stage(rec[tr], flatten_ids[batch + tr], geo.C, geo.N, means, quats, scales, opacities);
+        __syncthreads();
+        const int n_b = (int)min((int64_t)kUtThreads, end - batch);
+        for(int t = 0; t < n_b && !done; ++t)
+        {
+            const EvalRec &r = rec[t];
+            const EvalHit h  = eval_hit(r, ro, rd);
+            if(!h.ok)
+                continue;
+            const float next_T = T * (1.f - h.alpha);
+            if(next_T <= kTransmittanceThreshold)
+            { // exclusive: this gaussian does not contribute
+                done = true;
+                break;
+            }
+            const float vis = h.alpha * T;
+            const float *c  = colors + (int64_t)r.id * CDIM;
+#pragma unroll
+            for(int k = 0; k < CDIM; ++k)
+                pix_out[k] += c[k] * vis;
+            cur_idx = (int32_t)(batch + t);
+            T       = next_T;
+        }
+    }
+    if(!inside)
+        return;
+    render_alphas[pix] = 1.f - T;
+#pragma unroll
+    for(int k = 0; k < CDIM; ++k)
+        render_colors[pix * CDIM + k] = bg ? pix_out[k] + T * bg[k] : pix_out[k];
+    last_ids[pix] = cur_idx;
+}
+
+struct EvalGradDst
+{
+    float *colors, *opacities, *rec; // rec: [B * N, 12] = v_mean 3 | v_M 9
+};
+
+// Butterfly-reduces gv[OFF, OFF + 32) across the warp and adds each owned slot to its gradient row; recurses over the
+// remaining 32-value chunks.
+template<int OFF, int NV>
+__device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, const EvalRec &r, const EvalGradDst &dst, int CDIM)
+{
+    constexpr int M = (NV - OFF) < 32 ? (NV - OFF) : 32;
+    float v[M];
+#pragma unroll
+    for(int k = 0; k < M; ++k)
+        v[k] = gv[OFF + k];
+    Butterfly<M, 16>::run(v, lane);
+    const int s = butterfly_slot<M>(lane);
+    if(s >= 0 && v[0] != 0.f)
+    {
+        const int slot = OFF + s;
+        if(slot < CDIM)
+            atomicAdd(dst.colors + (int64_t)r.id * CDIM + slot, v[0]);
+        else if(slot == CDIM)
+            atomicAdd(dst.opacities + r.id, v[0]);
+        else
+            atomicAdd(dst.rec + (int64_t)r.bn * 12 + (slot - CDIM - 1), v[0]);
+    }
+    if constexpr(OFF + 32 < NV)
+        reduce_emit<OFF + 32, NV>(gv, lane, r, dst, CDIM);
+}
+
+// Back to front over each tile's list.  Per gaussian, the warp's per-pixel gradients (colours, opacity, mean, M) are
+// butterfly-reduced and added with one atomic per value.
+template<int CDIM>
+__global__ void __launch_bounds__(kUtThreads, 1) eval3d_bwd_kernel(
+    EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
+    const float *__restrict__ colors, const float *__restrict__ opacities, const float *__restrict__ backgrounds,
+    const uint8_t *__restrict__ masks, const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids,
+    int64_t n_isects, const float *__restrict__ render_alphas, const int32_t *__restrict__ last_ids,
+    const float *__restrict__ v_render_colors, const float *__restrict__ v_render_alphas, EvalGradDst dst
+)
+{
+    constexpr int NV = CDIM + 13; // colours | opacity 1 | mean 3 | M 9
+    __shared__ EvalRec rec[kUtThreads];
+    __shared__ float s_col[kUtThreads * CDIM];
+    const uint32_t tile = blockIdx.x;
+    if(masks && !masks[tile])
+        return;
+    const uint32_t img  = tile / (geo.tw * geo.th);
+    const uint32_t tin  = tile - img * geo.tw * geo.th;
+    const uint32_t tr   = threadIdx.x;
+    const unsigned lane = tr & 31;
+    const uint32_t i    = (tin / geo.tw) * kTile + tr / kTile;
+    const uint32_t j    = (tin % geo.tw) * kTile + tr % kTile;
+    // a pixel outside the image reads the image's first pixel and adds nothing
+    bool inside       = i < geo.H && j < geo.W;
+    const int64_t pix = inside ? (int64_t)img * geo.H * geo.W + (int64_t)i * geo.W + j : (int64_t)img * geo.H * geo.W;
+    const float *bg   = backgrounds ? backgrounds + (int64_t)img * CDIM : nullptr;
+    const int64_t start = offsets[tile];
+    const int64_t end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
+    float ro[3] = {0.f, 0.f, 0.f}, rd[3] = {0.f, 0.f, 1.f};
+    if(inside)
+    {
+        const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        inside            = pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
+    }
+
+    const float T_final = 1.f - render_alphas[pix];
+    float T             = T_final;
+    float buf[CDIM], v_rc[CDIM];
+#pragma unroll
+    for(int k = 0; k < CDIM; ++k)
+    {
+        buf[k]  = 0.f;
+        v_rc[k] = v_render_colors[pix * CDIM + k];
+    }
+    const float v_ra = v_render_alphas ? v_render_alphas[pix] : 0.f;
+    float bg_dot     = 0.f;
+    if(bg)
+    {
+#pragma unroll
+        for(int k = 0; k < CDIM; ++k)
+            bg_dot += bg[k] * v_rc[k];
+    }
+    const int64_t bin_final = inside ? last_ids[pix] : -1;
+    int64_t warp_bin_final  = bin_final;
+#pragma unroll
+    for(int off = 16; off >= 1; off >>= 1)
+        warp_bin_final = max(warp_bin_final, (int64_t)__shfl_xor_sync(0xffffffffu, (long long)warp_bin_final, off));
+
+    for(int64_t batch_end = end - 1; batch_end >= start; batch_end -= kUtThreads)
+    {
+        __syncthreads();
+        const int64_t idx = batch_end - tr;
+        if(idx >= start)
+        {
+            const int32_t g = flatten_ids[idx];
+            stage(rec[tr], g, geo.C, geo.N, means, quats, scales, opacities);
+#pragma unroll
+            for(int k = 0; k < CDIM; ++k)
+                s_col[tr * CDIM + k] = colors[(int64_t)g * CDIM + k];
+        }
+        __syncthreads();
+        const int n_b = (int)min((int64_t)kUtThreads, batch_end + 1 - start);
+        const int t0  = (int)max((int64_t)0, batch_end - warp_bin_final);
+        for(int t = t0; t < n_b; ++t)
+        {
+            const EvalRec &r = rec[t];
+            const int64_t gi = batch_end - t;
+            bool valid       = inside && gi <= bin_final;
+            EvalHit h;
+            if(valid)
+            {
+                h     = eval_hit(r, ro, rd);
+                valid = h.ok;
+            }
+            if(!__any_sync(0xffffffffu, valid))
+                continue;
+            float gv[NV];
+#pragma unroll
+            for(int k = 0; k < NV; ++k)
+                gv[k] = 0.f;
+            if(valid)
+            {
+                const float *c  = s_col + t * CDIM;
+                const float ra  = 1.f / fmaxf(kMinOneMinusAlpha, 1.f - h.alpha);
+                T               = T * ra;
+                const float fac = h.alpha * T;
+                float v_alpha   = 0.f;
+#pragma unroll
+                for(int k = 0; k < CDIM; ++k)
+                {
+                    gv[k] = fac * v_rc[k];
+                    v_alpha += (c[k] * T - buf[k] * ra) * v_rc[k];
+                }
+                v_alpha += T_final * ra * v_ra;
+                v_alpha += -T_final * ra * bg_dot;
+                if(r.o * h.resp <= kMaxAlpha)
+                {
+                    gv[CDIM] = h.resp * v_alpha;
+                    // d resp / d dist = -resp / 2, dist = |c|^2, c = g x a
+                    const float v_dist = -0.5f * h.resp * (r.o * v_alpha);
+                    float vc[3];
+#pragma unroll
+                    for(int k = 0; k < 3; ++k)
+                        vc[k] = 2.f * v_dist * h.c[k];
+                    // c = g x a:  v_g = a x vc,  v_a = vc x g
+                    const float vg[3] = {h.a[1] * vc[2] - h.a[2] * vc[1], h.a[2] * vc[0] - h.a[0] * vc[2], h.a[0] * vc[1] - h.a[1] * vc[0]};
+                    const float va[3] = {vc[1] * h.g[2] - vc[2] * h.g[1], vc[2] * h.g[0] - vc[0] * h.g[2], vc[0] * h.g[1] - vc[1] * h.g[0]};
+                    // g = b / |b|
+                    const float gd = h.g[0] * vg[0] + h.g[1] * vg[1] + h.g[2] * vg[2];
+                    float vb[3];
+#pragma unroll
+                    for(int k = 0; k < 3; ++k)
+                        vb[k] = (vg[k] - h.g[k] * gd) / h.bl;
+                    // a = M (o - mu), b = M d
+#pragma unroll
+                    for(int k = 0; k < 3; ++k)
+                        gv[CDIM + 1 + k] = -(r.m[0 * 3 + k] * va[0] + r.m[1 * 3 + k] * va[1] + r.m[2 * 3 + k] * va[2]);
+#pragma unroll
+                    for(int p = 0; p < 3; ++p)
+#pragma unroll
+                        for(int q = 0; q < 3; ++q)
+                            gv[CDIM + 4 + p * 3 + q] = va[p] * h.w[q] + vb[p] * rd[q];
+                }
+#pragma unroll
+                for(int k = 0; k < CDIM; ++k)
+                    buf[k] += c[k] * fac;
+            }
+            reduce_emit<0, NV>(gv, lane, r, dst, CDIM);
+        }
+    }
+}
+
+// Per gaussian: the accumulated record (v_mean, v_M) to v_means, v_quats, v_scales through M = S^-1 R^T.
+__global__ void __launch_bounds__(kUtThreads) eval3d_finish_kernel(
+    int64_t BN, const float *__restrict__ quats, const float *__restrict__ scales, const float *__restrict__ rec,
+    float *__restrict__ v_means, float *__restrict__ v_quats, float *__restrict__ v_scales
+)
+{
+    const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(g >= BN)
+        return;
+    const float *rg = rec + g * 12;
+#pragma unroll
+    for(int k = 0; k < 3; ++k)
+        v_means[g * 3 + k] = rg[k];
+    const float q[4] = {quats[g * 4], quats[g * 4 + 1], quats[g * 4 + 2], quats[g * 4 + 3]};
+    const M3 R       = quat_to_rotmat(q);
+    M3 vR;
+#pragma unroll
+    for(int i = 0; i < 3; ++i)
+    {
+        const float s   = scales[g * 3 + i];
+        const float inv = 1.f / s;
+        float acc       = 0.f;
+#pragma unroll
+        for(int j = 0; j < 3; ++j)
+        {
+            const float vm     = rg[3 + i * 3 + j];
+            vR.m[j * 3 + i]    = vm * inv;
+            acc               += vm * R.m[j * 3 + i];
+        }
+        v_scales[g * 3 + i] = -acc * inv * inv;
+    }
+    float vq[4] = {0.f, 0.f, 0.f, 0.f};
+    if(rg[3] != 0.f || rg[4] != 0.f || rg[5] != 0.f || rg[6] != 0.f || rg[7] != 0.f || rg[8] != 0.f || rg[9] != 0.f
+       || rg[10] != 0.f || rg[11] != 0.f)
+        quat_to_rotmat_vjp(q, vR, vq);
+#pragma unroll
+    for(int k = 0; k < 4; ++k)
+        v_quats[g * 4 + k] = vq[k];
+}
+
+int eval3d_checks(
+    int64_t B, int64_t C, int64_t N, int cam_kind, uint32_t W, uint32_t H, uint32_t tile_size, uint32_t tw, uint32_t th
+)
+{
+    if(B < 0 || C < 0 || N < 0)
+        return GSB200_E_INVALID;
+    if(cam_kind != kUtPinhole && cam_kind != kUtFisheye)
+        return GSB200_E_UNSUPPORTED;
+    if(tile_size != (uint32_t)kTile)
+        return GSB200_E_UNSUPPORTED;
+    if(B * C > 0 && W > 0 && H > 0 && !tile_grid_covers(tw, th, W, H))
+        return GSB200_E_INVALID;
+    if((double)B * C * N >= 2147483648.0 || (double)B * C * tw * th >= 2147483648.0)
+        return GSB200_E_UNSUPPORTED;
+    return GSB200_OK;
+}
+} // namespace
+} // namespace gsb
+
+// ---------------------------------------------------------------------------------------------
+// C ABI
+extern "C" int gsb200_ut_projection_fwd(
+    int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
+    const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+    const float *thin_prism_coeffs, uint32_t image_width, uint32_t image_height, float eps2d, float near_plane,
+    float far_plane, float radius_clip, float ut_alpha, float ut_beta, float ut_kappa, float ut_in_image_margin_factor,
+    int ut_require_all_sigma_points_valid, int32_t *radii, float *means2d, float *depths, float *conics,
+    float *compensations, void *stream
+)
+{
+    if(B < 0 || C < 0 || N < 0)
+        return GSB200_E_INVALID;
+    if(camera_model != gsb::kUtPinhole && camera_model != gsb::kUtFisheye)
+        return GSB200_E_UNSUPPORTED;
+    if(camera_model == gsb::kUtFisheye && (tangential_coeffs || thin_prism_coeffs))
+        return GSB200_E_INVALID;
+    if(!(ut_alpha * ut_alpha * (3.f + ut_kappa) > 0.f))
+        return GSB200_E_INVALID;
+    const int64_t n = B * C * N;
+    if(n == 0)
+        return GSB200_OK;
+    if(!means || !quats || !scales || !viewmats || !Ks || !radii || !means2d || !depths || !conics)
+        return GSB200_E_INVALID;
+    const gsb::UtParams ut{ut_alpha, ut_beta, ut_kappa, ut_in_image_margin_factor, ut_require_all_sigma_points_valid};
+    gsb::ut_project_kernel<<<gsb::grid_for(n, gsb::kUtThreads), gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
+        B, C, N, means, quats, scales, opacities, viewmats, Ks, camera_model, radial_coeffs, tangential_coeffs,
+        thin_prism_coeffs, image_width, image_height, eps2d, near_plane, far_plane, radius_clip, ut, radii, means2d, depths,
+        conics, compensations
+    );
+    return gsb::check_launch();
+}
+
+extern "C" int gsb200_eval3d_fwd(
+    int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
+    const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
+    const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+    const float *thin_prism_coeffs, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
+    uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, float *render_colors,
+    float *render_alphas, int32_t *last_ids, void *stream
+)
+{
+    if(n_isects < 0)
+        return GSB200_E_INVALID;
+    if(int rc = gsb::eval3d_checks(B, C, N, camera_model, image_width, image_height, tile_size, tile_width, tile_height))
+        return rc;
+    if(B * C == 0 || image_width == 0 || image_height == 0)
+        return GSB200_OK;
+    if(!viewmats || !Ks || !offsets || !render_colors || !render_alphas || !last_ids)
+        return GSB200_E_INVALID;
+    if(n_isects > 0 && (!means || !quats || !scales || !colors || !opacities || !flatten_ids))
+        return GSB200_E_INVALID;
+    const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height,
+                            camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
+    return gsb::with_channels(D, [&](auto CH) {
+        gsb::eval3d_fwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
+            geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects, render_colors,
+            render_alphas, last_ids
+        );
+        return gsb::check_launch();
+    });
+}
+
+extern "C" int gsb200_eval3d_bwd(
+    int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
+    const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
+    const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+    const float *thin_prism_coeffs, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
+    uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, const float *render_alphas,
+    const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, float *grad_records,
+    float *v_colors, float *v_opacities, float *v_means, float *v_quats, float *v_scales, void *stream
+)
+{
+    if(n_isects < 0)
+        return GSB200_E_INVALID;
+    if(int rc = gsb::eval3d_checks(B, C, N, camera_model, image_width, image_height, tile_size, tile_width, tile_height))
+        return rc;
+    if(B * N == 0)
+        return GSB200_OK;
+    if(!quats || !scales || !grad_records || !v_means || !v_quats || !v_scales)
+        return GSB200_E_INVALID;
+    cudaStream_t st = (cudaStream_t)stream;
+    if(n_isects > 0 && B * C > 0 && image_width > 0 && image_height > 0)
+    {
+        if(!means || !colors || !opacities || !viewmats || !Ks || !offsets || !flatten_ids || !render_alphas || !last_ids
+           || !v_render_colors || !v_colors || !v_opacities)
+            return GSB200_E_INVALID;
+        const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width,
+                                tile_height, camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
+        const gsb::EvalGradDst dst{v_colors, v_opacities, grad_records};
+        const int rc = gsb::with_channels(D, [&](auto CH) {
+            gsb::eval3d_bwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, st>>>(
+                geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
+                render_alphas, last_ids, v_render_colors, v_render_alphas, dst
+            );
+            return gsb::check_launch();
+        });
+        if(rc)
+            return rc;
+    }
+    gsb::eval3d_finish_kernel<<<gsb::grid_for(B * N, gsb::kUtThreads), gsb::kUtThreads, 0, st>>>(
+        B * N, quats, scales, grad_records, v_means, v_quats, v_scales
+    );
+    return gsb::check_launch();
+}

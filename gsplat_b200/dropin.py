@@ -63,6 +63,10 @@ _OPS_CONTRIB = (
     "rasterize_top_contributing_gaussian_ids_sparse",
 )
 
+# 3DGUT, likewise: a call with an argument the b200 kernels do not take (ftheta, lidar, rolling shutter, ...) raises
+# NotImplementedError on the b200 path and runs the package's own op
+_OPS_3DGUT = ("fully_fused_projection_with_ut", "rasterize_to_pixels_eval3d")
+
 _saved: List[Tuple[object, str, object]] = []
 
 # per rebound name: how many calls ran on the b200 kernels, how many were handed to the package's own implementation
@@ -121,7 +125,7 @@ def apply(losses: bool = True, ops: bool = True) -> Dict[str, object]:
 def _apply_ops(B, G) -> None:
     W = importlib.import_module("gsplat.cuda._wrapper")
     R = importlib.import_module("gsplat.rendering")
-    for name in _OPS + tuple(n for n in _OPS_2DGS + _OPS_INDICES + _OPS_CONTRIB if hasattr(W, n)):
+    for name in _OPS + tuple(n for n in _OPS_2DGS + _OPS_INDICES + _OPS_CONTRIB + _OPS_3DGUT if hasattr(W, n)):
         fn = _delegating(name, getattr(B, name), getattr(W, name))
         _set(W, name, fn)
         if hasattr(G, name):

@@ -2545,3 +2545,297 @@ def adam(
             ),
             "adam",
         )
+
+
+# --------------------------------------------------------------------------------------------
+# 3DGUT (reference wrappers gsplat/cuda/_wrapper.py: fully_fused_projection_with_ut, rasterize_to_pixels_eval3d): the
+# unscented-transform projection through a distorted pinhole or fisheye camera and the compositing that evaluates
+# each gaussian in 3-D along the pixel's ray.  Global shutter, dense rows, RendererConfig_MixedBatch.
+
+_UT_DEFAULTS = {"alpha": 0.1, "beta": 2.0, "kappa": 0.0, "in_image_margin_factor": 0.1, "require_all_sigma_points_valid": False}
+_UT_CAMERAS = {"pinhole": 0, "fisheye": 2}
+
+
+def _ut_params(ut_params) -> tuple:
+    """(alpha, beta, kappa, in_image_margin_factor, require_all_sigma_points_valid) of any object with the reference's
+    UnscentedTransformParameters fields (a missing field takes its default), or the defaults for None."""
+    v = {k: (d if ut_params is None else getattr(ut_params, k, d)) for k, d in _UT_DEFAULTS.items()}
+    alpha, kappa = float(v["alpha"]), float(v["kappa"])
+    if not alpha * alpha * (3.0 + kappa) > 0.0:
+        raise ValueError(f"ut_params: alpha^2 * (3 + kappa) must be > 0 (alpha={alpha}, kappa={kappa})")
+    return alpha, float(v["beta"]), kappa, float(v["in_image_margin_factor"]), bool(v["require_all_sigma_points_valid"])
+
+
+def _ut_camera(what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
+               external_distortion_coeffs, rolling_shutter, viewmats_rs, cams: tuple):
+    """Rejects what the 3DGUT kernels are not built for (NotImplementedError, naming the argument) and checks the
+    distortion coefficients.  Returns the camera model id and the coefficient tensors as [..., C, k] float32."""
+    for name, v in (("ftheta_coeffs", ftheta_coeffs), ("lidar_coeffs", lidar_coeffs),
+                    ("external_distortion_coeffs", external_distortion_coeffs), ("viewmats_rs", viewmats_rs)):
+        if v is not None:
+            raise NotImplementedError(f"{what}: {name} is not supported (global-shutter pinhole / fisheye only)")
+    if int(rolling_shutter) != 4:
+        raise NotImplementedError(f"{what}: rolling_shutter={rolling_shutter!r} is not supported (GLOBAL only)")
+    if camera_model not in _UT_CAMERAS:
+        if camera_model in ("ortho", "ftheta", "lidar"):
+            raise NotImplementedError(f"{what}: camera_model={camera_model!r} is not supported (pinhole / fisheye only)")
+        raise ValueError(f"{what}: unknown camera_model {camera_model!r}")
+    if camera_model == "fisheye":
+        for name, v in (("tangential_coeffs", tangential_coeffs), ("thin_prism_coeffs", thin_prism_coeffs)):
+            if v is not None:
+                raise ValueError(f"{what}: {name} applies to the pinhole camera only")
+    widths = (("radial_coeffs", radial_coeffs, 6 if camera_model == "pinhole" else 4),
+              ("tangential_coeffs", tangential_coeffs, 2), ("thin_prism_coeffs", thin_prism_coeffs, 4))
+    out = []
+    for name, v, k in widths:
+        if v is not None:
+            _check_shape(v, cams + (k,), name)
+            v = f32c(v, name)
+        out.append(v)
+    return (_UT_CAMERAS[camera_model], *out)
+
+
+def _ut_geometry(what, means, quats, scales, viewmats, Ks) -> tuple:
+    if means.dim() < 2 or means.shape[-1] != 3:
+        raise ValueError(f"{what}: means must be [..., N, 3], got {tuple(means.shape)}")
+    batch, N = tuple(means.shape[:-2]), means.shape[-2]
+    _check_shape(quats, batch + (N, 4), "quats")
+    _check_shape(scales, batch + (N, 3), "scales")
+    if viewmats.dim() != len(batch) + 3:
+        raise ValueError(f"{what}: viewmats must be [..., C, 4, 4], got {tuple(viewmats.shape)}")
+    C = viewmats.shape[-3]
+    _check_shape(viewmats, batch + (C, 4, 4), "viewmats")
+    _check_shape(Ks, batch + (C, 3, 3), "Ks")
+    for name, t in (("means", means), ("quats", quats), ("scales", scales), ("viewmats", viewmats), ("Ks", Ks)):
+        if t.dtype != torch.float32:
+            raise TypeError(f"{what}: {name} must be float32, got {t.dtype}")
+    return batch, C, N
+
+
+@torch.no_grad()
+def fully_fused_projection_with_ut(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    opacities: Optional[Tensor],  # [..., N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    width: int,
+    height: int,
+    eps2d: float = 0.3,
+    near_plane: float = 0.01,
+    far_plane: float = 1e10,
+    radius_clip: float = 0.0,
+    calc_compensations: bool = False,
+    camera_model: str = "pinhole",
+    ut_params=None,
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    lidar_coeffs=None,
+    external_distortion_coeffs=None,
+    rolling_shutter: int = 4,
+    viewmats_rs: Optional[Tensor] = None,
+    global_z_order: bool = True,
+) -> Tuple[Tensor, Tensor, Tensor, Tensor, Optional[Tensor]]:
+    """Projects 3D Gaussians through a distorted pinhole or fisheye camera with the unscented transform: 7 sigma points
+    per Gaussian are projected through the camera model and reduced to a 2-D mean and covariance, then blurred by
+    ``eps2d`` and culled as in ``fully_fused_projection``.  Returns (radii int32 [..., C, N, 2], means2d [..., C, N, 2],
+    depths [..., C, N], conics [..., C, N, 3], compensations [..., C, N] or None); culled rows have radii 0 and zero
+    floats.  Not differentiable, as in the reference.  ``ut_params``: any object with the fields of the reference's
+    UnscentedTransformParameters, or None for their defaults.  Global shutter, ``global_z_order=True`` only."""
+    what = "fully_fused_projection_with_ut"
+    if not global_z_order:
+        raise NotImplementedError(f"{what}: global_z_order=False is not supported")
+    batch, C, N = _ut_geometry(what, means, quats, scales, viewmats, Ks)
+    cam, radial, tangential, thin = _ut_camera(
+        what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
+        external_distortion_coeffs, rolling_shutter, viewmats_rs, batch + (C,),
+    )
+    if opacities is not None:
+        _check_shape(opacities, batch + (N,), "opacities")
+        opacities = f32c(opacities, "opacities")
+    alpha, beta, kappa, margin, require_all = _ut_params(ut_params)
+    dev = require_cuda(means, quats, scales, viewmats, Ks, opacities, radial, tangential, thin)
+    means, quats, scales, viewmats, Ks = (t.contiguous() for t in (means, quats, scales, viewmats, Ks))
+    B = _prod(batch)
+    o = dict(device=dev, dtype=torch.float32)
+    radii = torch.empty(batch + (C, N, 2), device=dev, dtype=torch.int32)
+    means2d = torch.empty(batch + (C, N, 2), **o)
+    depths = torch.empty(batch + (C, N), **o)
+    conics = torch.empty(batch + (C, N, 3), **o)
+    comps = torch.empty(batch + (C, N), **o) if calc_compensations else None
+    with _Ctx(dev) as st:
+        check(
+            lib().gsb200_ut_projection_fwd(
+                B, C, N, ptr(means), ptr(quats), ptr(scales), ptr(opacities), ptr(viewmats), ptr(Ks), cam, ptr(radial),
+                ptr(tangential), ptr(thin), int(width), int(height), float(eps2d), float(near_plane), float(far_plane),
+                float(radius_clip), alpha, beta, kappa, margin, int(require_all), ptr(radii), ptr(means2d), ptr(depths),
+                ptr(conics), ptr(comps), st,
+            ),
+            what,
+        )
+    return radii, means2d, depths, conics, comps
+
+
+class _RasterizeToPixelsEval3D(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, radial, tangential,
+                thin, width, height, isect_offsets, flatten_ids):
+        dev = require_cuda(means, quats, scales, colors, opacities, viewmats, Ks)
+        means, quats, scales = means.contiguous(), quats.contiguous(), scales.contiguous()
+        colors, opacities = f32c(colors, "colors"), f32c(opacities, "opacities")
+        backgrounds, viewmats, Ks = f32c(backgrounds, "backgrounds"), viewmats.contiguous(), Ks.contiguous()
+        batch, N = tuple(means.shape[:-2]), means.shape[-2]
+        B, C, D = _prod(batch), viewmats.shape[-3], colors.shape[-1]
+        image_dims = batch + (C,)
+        th, tw = isect_offsets.shape[-2:]
+        m8 = _mask_u8(masks)
+        offsets, fl = isect_offsets.contiguous(), flatten_ids.contiguous()
+        S = fl.shape[0]
+        o = dict(device=dev, dtype=torch.float32)
+        pix = image_dims + (height, width)
+        if S == 0:
+            # nothing intersects a tile: the background alone, no kernel launch
+            if backgrounds is not None:
+                render_colors = torch.broadcast_to(backgrounds[..., None, None, :], pix + (D,)).contiguous()
+            else:
+                render_colors = torch.zeros(pix + (D,), **o)
+            render_alphas = torch.zeros(pix + (1,), **o)
+            last_ids = torch.full(pix, -1, device=dev, dtype=torch.int32)
+        else:
+            render_colors = torch.empty(pix + (D,), **o)
+            render_alphas = torch.empty(pix + (1,), **o)
+            last_ids = torch.empty(pix, device=dev, dtype=torch.int32)
+            with _Ctx(dev) as st:
+                check(
+                    lib().gsb200_eval3d_fwd(
+                        B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds),
+                        ptr(m8), ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), width, height, 16,
+                        tw, th, ptr(offsets), ptr(fl), S, ptr(render_colors), ptr(render_alphas), ptr(last_ids), st,
+                    ),
+                    "rasterize_to_pixels_eval3d",
+                )
+        ctx.save_for_backward(means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, radial, tangential, thin,
+                              offsets, fl, render_alphas, last_ids)
+        ctx.set_materialize_grads(False)
+        ctx.meta = (B, C, N, D, cam, width, height, tw, th, S)
+        ctx.mark_non_differentiable(last_ids)
+        return render_colors, render_alphas
+
+    @staticmethod
+    def backward(ctx, v_render_colors, v_render_alphas):
+        (means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, radial, tangential, thin, offsets, fl,
+         render_alphas, last_ids) = ctx.saved_tensors
+        B, C, N, D, cam, width, height, tw, th, S = ctx.meta
+        dev = render_alphas.device
+        if v_render_colors is None:
+            v_render_colors = torch.zeros(render_alphas.shape[:-1] + (D,), device=dev, dtype=torch.float32)
+        v_render_colors = v_render_colors.float().contiguous()
+        v_render_alphas = None if v_render_alphas is None else v_render_alphas.float().contiguous()
+        v_colors, v_opacities = torch.zeros_like(colors), torch.zeros_like(opacities)
+        v_means, v_quats, v_scales = torch.empty_like(means), torch.empty_like(quats), torch.empty_like(scales)
+        records = torch.zeros((B * N, 12), device=dev, dtype=torch.float32)
+        with _Ctx(dev) as st:
+            check(
+                lib().gsb200_eval3d_bwd(
+                    B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds), ptr(m8),
+                    ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), width, height, 16, tw, th,
+                    ptr(offsets), ptr(fl), S, ptr(render_alphas), ptr(last_ids), ptr(v_render_colors), ptr(v_render_alphas),
+                    ptr(records), ptr(v_colors), ptr(v_opacities), ptr(v_means), ptr(v_quats), ptr(v_scales), st,
+                ),
+                "rasterize_to_pixels_eval3d_bwd",
+            )
+        v_backgrounds = None
+        if backgrounds is not None and ctx.needs_input_grad[5]:
+            v_backgrounds = (v_render_colors * (1.0 - render_alphas)).sum(dim=(-3, -2))
+        # viewmats, Ks and the camera coefficients get no gradient, as in the reference's backward
+        return (v_means, v_quats, v_scales, v_colors, v_opacities, v_backgrounds) + (None,) * 11
+
+
+def rasterize_to_pixels_eval3d(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    colors: Tensor,  # [..., C, N, channels]
+    opacities: Tensor,  # [..., C, N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    isect_offsets: Tensor,  # [..., C, tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+    backgrounds: Optional[Tensor] = None,  # [..., C, channels]
+    masks: Optional[Tensor] = None,  # [..., C, tile_height, tile_width]
+    camera_model: str = "pinhole",
+    ut_params=None,
+    rays: Optional[Tensor] = None,
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    lidar_coeffs=None,
+    external_distortion_coeffs=None,
+    rolling_shutter: int = 4,
+    viewmats_rs: Optional[Tensor] = None,
+    use_hit_distance: bool = False,
+    return_normals: bool = False,
+    renderer_config=None,
+) -> Tuple[Tensor, Tensor]:
+    """Composites depth-sorted Gaussians front to back per 16x16 tile, evaluating each in 3-D along the pixel's
+    world-space ray (from the camera model, the distortion inverted by Newton iteration) instead of as a 2-D conic: the
+    maximum response along the ray times the opacity is the alpha (min 0.99, skipped below 1/255, stop at T <= 1e-4).
+    Returns (render_colors [..., C, H, W, channels], render_alphas [..., C, H, W, 1]).  Differentiable in means, quats,
+    scales, colors, opacities and backgrounds; viewmats get no gradient, as in the reference.  ``ut_params`` is accepted
+    for the reference's signature and does not enter the compositing.  Dense rows, global shutter, the MixedBatch
+    renderer only."""
+    what = "rasterize_to_pixels_eval3d"
+    for name, v in (("rays", rays),):
+        if v is not None:
+            raise NotImplementedError(f"{what}: {name} is not supported")
+    if use_hit_distance:
+        raise NotImplementedError(f"{what}: use_hit_distance=True is not supported")
+    if return_normals:
+        raise NotImplementedError(f"{what}: return_normals=True is not supported")
+    if renderer_config is not None and type(renderer_config).__name__ != "RendererConfig_MixedBatch":
+        raise NotImplementedError(f"{what}: renderer_config={renderer_config!r} is not supported (RendererConfig_MixedBatch only)")
+    if colors.dim() == 2 or opacities.dim() == 1:
+        raise NotImplementedError(f"{what}: packed [nnz, channels] rows are not supported")
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    batch, C, N = _ut_geometry(what, means, quats, scales, viewmats, Ks)
+    image_dims = batch + (C,)
+    cam, radial, tangential, thin = _ut_camera(
+        what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
+        external_distortion_coeffs, rolling_shutter, viewmats_rs, image_dims,
+    )
+    _ut_params(ut_params)
+    if colors.dim() != len(image_dims) + 2:
+        raise ValueError(f"{what}: colors must be [..., C, N, channels], got {tuple(colors.shape)}")
+    D = colors.shape[-1]
+    _check_shape(colors, image_dims + (N, D), "colors")
+    _check_shape(opacities, image_dims + (N,), "opacities")
+    if isect_offsets.dim() != len(image_dims) + 2 or tuple(isect_offsets.shape[:-2]) != image_dims:
+        raise ValueError(f"isect_offsets must be {image_dims + ('tile_height', 'tile_width')}, got {tuple(isect_offsets.shape)}")
+    th, tw = isect_offsets.shape[-2:]
+    if th * 16 < image_height or tw * 16 < image_width:
+        raise ValueError(f"isect_offsets tile grid {tw}x{th} does not cover a {image_width}x{image_height} image")
+    if backgrounds is not None:
+        _check_shape(backgrounds, image_dims + (D,), "backgrounds")
+    if masks is not None:
+        _check_shape(masks, image_dims + (th, tw), "masks")
+    if isect_offsets.dtype != torch.int32 or flatten_ids.dtype != torch.int32 or flatten_ids.dim() != 1:
+        raise ValueError("isect_offsets and flatten_ids must be int32, flatten_ids one-dimensional")
+    for name, t in (("colors", colors), ("opacities", opacities), ("backgrounds", backgrounds)):
+        if t is not None and t.dtype != torch.float32:
+            raise TypeError(f"{what}: {name} must be float32, got {t.dtype}")
+    if D not in _SUPPORTED_CHANNELS:
+        raise NotImplementedError(f"{what}: {D} channels; the eval3d kernels are built for {_SUPPORTED_CHANNELS}")
+    require_cuda(means, quats, scales, colors, opacities, viewmats, Ks, backgrounds, masks, isect_offsets, flatten_ids,
+                 radial, tangential, thin)
+    return _RasterizeToPixelsEval3D.apply(
+        means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, radial, tangential, thin,
+        int(image_width), int(image_height), isect_offsets, flatten_ids,
+    )

@@ -1,0 +1,80 @@
+#!/usr/bin/env python
+"""Times one 3DGUT step (fully_fused_projection_with_ut + isect_tiles + isect_offset_encode + rasterize_to_pixels_eval3d
+forward and backward) next to the EWA step (fully_fused_projection + the same lists + rasterize_to_pixels forward and
+backward) on bench.py's scene (1M Gaussians, one 1920x1080 view) with a pinhole camera.  Median of --steps timed steps after --warmup, CUDA events; prints
+the device name and power limit with the numbers, as one JSON line.
+
+    python tools/bench_ut.py [--steps 20] [--warmup 5] [--distorted]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import gsplat_b200 as gs  # noqa: E402
+from tests import scene  # noqa: E402
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--distorted", action="store_true", help="pinhole with radial and tangential coefficients")
+    a = ap.parse_args()
+    assert torch.cuda.is_available(), "bench_ut needs a GPU"
+    dev = "cuda"
+    # bench.py's scene: the garden crop tiled 3x3 (about 1M Gaussians), one 1920x1080 view; colours instead of SH
+    sc = scene.make_scene(scene_grid=3, sh_degree=0)
+    W, H = 1920, 1080
+    t = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)  # noqa: E731
+    means, quats, scales = (t(sc[k]).requires_grad_(True) for k in ("means", "quats", "scales"))
+    opac = t(sc["opacities"])[None].contiguous().requires_grad_(True)
+    colors = t(sc["colors"])[None].contiguous().requires_grad_(True)
+    vm, K = t(sc["viewmats"][:1]), t(scene.rescale_K(sc["Ks"], sc["width"], sc["height"], W, H)[:1])
+    co = dict(radial_coeffs=t(np.float32([[0.05, -0.02, 0.0, 0.0, 0.0, 0.0]])), tangential_coeffs=t(np.float32([[0.001, -0.001]]))) if a.distorted else {}
+    tw, th = (W + 15) // 16, (H + 15) // 16
+
+    def ut_step():
+        r, m2, d, _, _ = gs.fully_fused_projection_with_ut(means.detach(), quats.detach(), scales.detach(), opac.detach()[0], vm, K, W, H, **co)
+        _, ii, fl = gs.isect_tiles(m2, r, d, 16, tw, th)
+        offs = gs.isect_offset_encode(ii, 1, tw, th)
+        rc, ra = gs.rasterize_to_pixels_eval3d(means, quats, scales, colors, opac, vm, K, W, H, 16, offs, fl, **co)
+        (rc.sum() + ra.sum()).backward()
+        return fl.numel()
+
+    def ewa_step():
+        r, m2, d, con, _ = gs.fully_fused_projection(means, None, quats, scales, vm, K, W, H)
+        _, ii, fl = gs.isect_tiles(m2, r, d, 16, tw, th)
+        offs = gs.isect_offset_encode(ii, 1, tw, th)
+        rc, ra = gs.rasterize_to_pixels(m2, con, colors, opac, W, H, 16, offs, fl)
+        (rc.sum() + ra.sum()).backward()
+        return fl.numel()
+
+    res = {}
+    for name, fn in (("ewa", ewa_step), ("ut", ut_step)):
+        for _ in range(a.warmup):
+            n = fn()
+        times = []
+        for _ in range(a.steps):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            fn()
+            e1.record()
+            torch.cuda.synchronize()
+            times.append(e0.elapsed_time(e1))
+        res[name] = {"median_ms": float(np.median(times)), "n_isects": int(n)}
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    res.update(device=torch.cuda.get_device_name(0), power_limit=q.stdout.strip(), gaussians=int(means.shape[0]), width=W,
+               height=H, distorted=a.distorted, steps=a.steps)
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
