@@ -78,9 +78,11 @@ def has_2dgs() -> bool:
 
 
 def has_3dgut() -> bool:
-    """Reference: _wrapper.py has_3dgut -- False: ``rasterization(with_ut=True, with_eval3d=True)`` is not built.  The two
-    3DGUT operators, ``fully_fused_projection_with_ut`` and ``rasterize_to_pixels_eval3d``, are (pinhole and fisheye,
-    global shutter), and chain with ``isect_tiles`` / ``isect_offset_encode`` as in the reference's ``_rasterization``."""
+    """Reference: _wrapper.py has_3dgut -- False.  In the reference this flag gates 3DGUT tests that need ftheta and lidar
+    cameras, rolling shutter, hit-distance modes and tile_size 8, none of which is built here.  What is built:
+    ``rasterization(with_ut=True, with_eval3d=True)`` with dense rows, and the two 3DGUT operators it runs on,
+    ``fully_fused_projection_with_ut`` and ``rasterize_to_pixels_eval3d`` (distorted pinhole and fisheye cameras, global
+    shutter), which also chain with ``isect_tiles`` / ``isect_offset_encode`` as in the reference's ``_rasterization``."""
     return False
 
 

@@ -7,8 +7,13 @@ mirrors (csrc/Rendering.cpp:745-1481); every kernel is ours (gsplat_b200.ops).
 Scope: the 3DGS EWA path named by BASELINE.json (pinhole / orthographic / fisheye cameras, dense or
 ``packed=True`` rows with optional ``sparse_grad``, classic / antialiased, RGB / D / ED / RGB+D / RGB+ED,
 backgrounds, masks, absgrad, SH or post-activation colours, ``distributed=True`` Gaussian sharding).
-3DGUT (with_ut / with_eval3d), lidar, distortion, rolling shutter, extra signals and normals are out of scope
-and raise NotImplementedError.
+
+3DGUT (``with_ut=True, with_eval3d=True`` together): the unscented-transform projection and the eval3d compositing
+through a distorted pinhole (radial / tangential / thin-prism coefficients) or fisheye (radial) camera, dense rows,
+global shutter, classic mode, RGB / D / ED / RGB+D / RGB+ED, following the reference's orchestrator
+(csrc/Rendering.cpp:890-934, 1307-1308, 1353-1410).  ``tile_size=None`` resolves to 16 here; the reference resolves it
+to 8 below 1080p.  with_ut or with_eval3d alone, ftheta / lidar cameras, external distortion, rolling shutter,
+hit-distance modes, normals, extra signals and packed 3DGUT rows raise NotImplementedError.
 
 rasterization_2dgs(): surfel splatting (2DGS) on the dense layout, following the reference's orchestrator
 (csrc/Rendering.cpp:1705-1958): ray-transform projection -> radius-box tile intersection -> compositing of colours,
@@ -23,13 +28,17 @@ import torch
 from torch import Tensor
 
 from .ops import (
+    _SUPPORTED_CHANNELS,
+    _ut_params,
     RowSideOutputs,
     fully_fused_projection,
     fully_fused_projection_2dgs,
+    fully_fused_projection_with_ut,
     fused_project_sh,
     isect_tiles_sorted,
     rasterize_to_pixels,
     rasterize_to_pixels_2dgs,
+    rasterize_to_pixels_eval3d,
     rasterize_to_pixels_rows,
     spherical_harmonics,
     spherical_harmonics_rows,
@@ -126,6 +135,20 @@ def _color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N)
     return torch.clamp_min(feat + 0.5, 0.0)
 
 
+def _with_depth_channel(feat, depths, backgrounds, has_color, has_depth, batch_dims, C):
+    """[colour | depth] features and backgrounds: D / ED / RGB+D / RGB+ED append the depths as the last channel and a
+    zero channel to the backgrounds (a depth-only mode renders the depths alone)."""
+    if has_color and has_depth:
+        feat = torch.cat((feat, depths[..., None]), dim=-1)
+        if backgrounds is not None:
+            backgrounds = torch.cat([backgrounds, torch.zeros(batch_dims + (C, 1), device=backgrounds.device)], dim=-1)
+    elif not has_color:
+        feat = depths[..., None]
+        if backgrounds is not None:
+            backgrounds = torch.zeros(batch_dims + (C, 1), device=backgrounds.device)
+    return feat, backgrounds
+
+
 def _normalize_expected_depth(render_colors, render_alphas, render_mode):
     """ED / RGB+ED: the last channel is the accumulated depth; divide it by the alpha."""
     if render_mode not in _EXPECTED_MODES:
@@ -208,10 +231,28 @@ def rasterization(
     renderer_config=None,
 ) -> Tuple[Tensor, Tensor, Dict]:
     """Rasterize N 3D Gaussians to C image planes.  Returns (render_colors [..., C, H, W, X],
-    render_alphas [..., C, H, W, 1], meta) with the reference's meta keys."""
+    render_alphas [..., C, H, W, 1], meta) with the reference's meta keys.
+
+    ``with_ut=True, with_eval3d=True`` renders 3DGUT: the unscented-transform projection through a distorted pinhole
+    (``radial_coeffs`` [..., C, 6], ``tangential_coeffs`` [..., C, 2], ``thin_prism_coeffs`` [..., C, 4]) or fisheye
+    (``radial_coeffs`` [..., C, 4]) camera, radius-box tile lists, and compositing that evaluates each Gaussian in 3-D
+    along the pixel's ray.  Dense rows only: pass ``packed=False``.  Gradients reach means, quats, scales, colours or SH
+    coefficients, opacities and backgrounds, and viewmats through the SH view directions only; ``meta["means2d"]``
+    carries none and ``absgrad`` is accepted and does nothing, as in the reference.  ``tile_size=None`` means 16; the
+    reference picks 8 below 1080p, which changes ``meta["tile_size"]`` and the tile grid, and can change pixels where a
+    Gaussian's 3-D response reaches outside its radius box (a 16-pixel tile list keeps pairs an 8-pixel one drops)."""
+    # ---- 3DGUT: the unscented-transform projection + eval3d compositing, only as the pair
+    if with_ut and with_eval3d:
+        return _rasterization_3dgut(
+            means, quats, scales, opacities, colors, viewmats, Ks, width, height, near_plane, far_plane, radius_clip,
+            eps2d, sh_degree, packed, tile_size, backgrounds, render_mode, sparse_grad, rasterize_mode, channel_chunk,
+            distributed, camera_model, covars, return_normals, global_z_order, rays, radial_coeffs, tangential_coeffs,
+            thin_prism_coeffs, ftheta_coeffs, lidar_coeffs, external_distortion_coeffs, rolling_shutter, viewmats_rs,
+            ut_params, extra_signals, renderer_config,
+        )
     # ---- features outside the path
     if with_ut or with_eval3d:
-        _unsupported("with_ut/with_eval3d", "3DGUT is a different algorithm (SURVEY.md section 2.1 #16)")
+        _unsupported("with_ut/with_eval3d", "3DGUT is built for with_ut=True and with_eval3d=True together")
     for name, val in (
         ("rays", rays), ("radial_coeffs", radial_coeffs), ("tangential_coeffs", tangential_coeffs),
         ("thin_prism_coeffs", thin_prism_coeffs), ("ftheta_coeffs", ftheta_coeffs), ("lidar_coeffs", lidar_coeffs),
@@ -411,14 +452,7 @@ def rasterization(
     isect_offsets = isect_offsets.reshape(batch_dims + (C, tile_height, tile_width))
 
     # ---- assemble channels: [colour | depth]
-    if has_color and has_depth:
-        feat = torch.cat((feat, depths[..., None]), dim=-1)
-        if backgrounds is not None:
-            backgrounds = torch.cat([backgrounds, torch.zeros(batch_dims + (C, 1), device=backgrounds.device)], dim=-1)
-    elif not has_color:
-        feat = depths[..., None]
-        if backgrounds is not None:
-            backgrounds = torch.zeros(batch_dims + (C, 1), device=backgrounds.device)
+    feat, backgrounds = _with_depth_channel(feat, depths, backgrounds, has_color, has_depth, batch_dims, C)
 
     # ---- compositing (chunked over channels, reference Rendering.cpp:1353-1447)
     n_ch = feat.shape[-1]
@@ -455,6 +489,175 @@ def rasterization(
         "tile_height": tile_height,
         "tiles_per_gauss": tiles_per_gauss,
         "isect_ids": isect_ids,
+        "flatten_ids": flatten_ids,
+        "isect_offsets": isect_offsets,
+        "width": width,
+        "height": height,
+        "tile_size": tile_size,
+        "n_batches": B,
+        "n_cameras": C,
+    })
+    return render_colors, render_alphas, meta
+
+
+def _global_shutter(rolling_shutter) -> bool:
+    """None, the reference's RollingShutterType.GLOBAL, or its value 4."""
+    if rolling_shutter is None or rolling_shutter in ("GLOBAL", "RollingShutterType.GLOBAL"):
+        return True
+    name = getattr(rolling_shutter, "name", None)
+    if name is not None:
+        return name == "GLOBAL"
+    return isinstance(rolling_shutter, int) and rolling_shutter == 4
+
+
+def _rasterization_3dgut(
+    means, quats, scales, opacities, colors, viewmats, Ks, width, height, near_plane, far_plane, radius_clip, eps2d,
+    sh_degree, packed, tile_size, backgrounds, render_mode, sparse_grad, rasterize_mode, channel_chunk, distributed,
+    camera_model, covars, return_normals, global_z_order, rays, radial_coeffs, tangential_coeffs, thin_prism_coeffs,
+    ftheta_coeffs, lidar_coeffs, external_distortion_coeffs, rolling_shutter, viewmats_rs, ut_params, extra_signals,
+    renderer_config,
+):
+    """rasterization(with_ut=True, with_eval3d=True), after the reference's orchestrator (csrc/Rendering.cpp
+    rasterization_3dgs under with_ut / with_eval3d): UT projection (no gradient) -> colours or SH -> [colour | depth]
+    -> radius-box tile lists -> eval3d compositing per channel chunk -> expected depth.  Every scope check runs before
+    anything touches the device."""
+    # ---- the reference's own rejections of 3DGUT arguments (rendering.py:164-175, Rendering.cpp:190-357), same wording
+    if distributed:
+        raise ValueError("distributed=True does not support with_ut=True")
+    if rasterize_mode not in ("classic", "antialiased"):
+        raise ValueError(f"unknown rasterize_mode {rasterize_mode!r}")
+    if rasterize_mode != "classic":
+        raise ValueError(
+            "3DGUT rendering only supports rasterize_mode='classic'. "
+            f"Got rasterize_mode='{rasterize_mode}' with with_ut=True and with_eval3d=True."
+        )
+    if covars is not None:
+        raise ValueError("UT and Eval3D rasterization require quats and scales, not covars")
+    if quats is None or scales is None:
+        raise ValueError("UT rasterization requires quats and scales")
+    if packed:
+        raise ValueError("Packed mode is not supported with UT")
+    if sparse_grad:
+        raise ValueError("Sparse grad is not supported with UT")
+    if channel_chunk <= 0:
+        raise ValueError("channel_chunk must be > 0")
+    if tile_size is None:
+        tile_size = 16
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    if render_mode not in _ALL_MODES:
+        raise ValueError(f"unknown render_mode {render_mode!r}")
+
+    # ---- what the 3DGUT kernels are not built for: NotImplementedError, naming the argument
+    if render_mode in _HIT_DISTANCE_MODES:
+        _unsupported(f"render_mode={render_mode!r}", "hit-distance modes are not built for 3DGUT")
+    if return_normals:
+        _unsupported("return_normals", "normals are not built for 3DGUT")
+    for name, val in (
+        ("rays", rays), ("ftheta_coeffs", ftheta_coeffs), ("lidar_coeffs", lidar_coeffs),
+        ("external_distortion_coeffs", external_distortion_coeffs), ("viewmats_rs", viewmats_rs),
+        ("extra_signals", extra_signals),
+    ):
+        if val is not None:
+            _unsupported(name, "not built for 3DGUT (global-shutter pinhole / fisheye cameras, colour and depth channels)")
+    if not _global_shutter(rolling_shutter):
+        _unsupported(f"rolling_shutter={rolling_shutter!r}", "3DGUT is built for the global shutter only")
+    if camera_model not in ("pinhole", "fisheye"):
+        if camera_model in ("ortho", "ftheta", "lidar"):
+            _unsupported(f"camera_model={camera_model!r}", "3DGUT is built for pinhole / fisheye cameras")
+        raise ValueError(f"unknown camera_model {camera_model!r}")
+    if not global_z_order:
+        _unsupported("global_z_order=False", "3DGUT is built for the global depth order only")
+    if renderer_config is not None and type(renderer_config).__name__ != "RendererConfig_MixedBatch":
+        _unsupported(f"renderer_config={type(renderer_config).__name__}", "3DGUT is built for RendererConfig_MixedBatch only")
+
+    # ---- shapes and dtypes
+    has_color = render_mode in _COLOR_MODES
+    has_depth = render_mode in _DEPTH_MODES
+    if means.dim() < 2 or means.shape[-1] != 3:
+        raise ValueError(f"means must be [..., N, 3], got {tuple(means.shape)}")
+    batch_dims = tuple(means.shape[:-2])
+    B = math.prod(batch_dims) if batch_dims else 1
+    N = means.shape[-2]
+    if viewmats.dim() != len(batch_dims) + 3:
+        raise ValueError(f"viewmats must be [..., C, 4, 4], got {tuple(viewmats.shape)}")
+    C = viewmats.shape[-3]
+    if tuple(quats.shape) != batch_dims + (N, 4) or tuple(scales.shape) != batch_dims + (N, 3):
+        raise ValueError(f"quats/scales shape mismatch: {tuple(quats.shape)}, {tuple(scales.shape)}")
+    if tuple(opacities.shape) != batch_dims + (N,):
+        raise ValueError(f"opacities must be [..., N], got {tuple(opacities.shape)}")
+    if tuple(viewmats.shape) != batch_dims + (C, 4, 4) or tuple(Ks.shape) != batch_dims + (C, 3, 3):
+        raise ValueError(f"viewmats/Ks shape mismatch: {tuple(viewmats.shape)}, {tuple(Ks.shape)}")
+    n_ch = int(has_depth)
+    if has_color:
+        if colors is None:
+            raise ValueError(f"render_mode={render_mode!r} needs colors")
+        _check_colors(colors, sh_degree, batch_dims, C, N)
+        if sh_degree is not None and colors.dtype in (torch.float16, torch.bfloat16):
+            colors = colors.float()  # half-precision SH storage, evaluated in fp32 as on the EWA path
+        if colors.dtype != torch.float32:
+            raise TypeError(f"colors must be float32, got {colors.dtype}")
+        if backgrounds is not None and tuple(backgrounds.shape) != batch_dims + (C, colors.shape[-1]):
+            raise ValueError(f"backgrounds must be {batch_dims + (C, colors.shape[-1])}, got {tuple(backgrounds.shape)}")
+        n_ch += colors.shape[-1]
+    if min(channel_chunk, n_ch) > _SUPPORTED_CHANNELS[-1]:
+        raise ValueError(
+            f"channel_chunk={channel_chunk}: the eval3d kernels composite up to {_SUPPORTED_CHANNELS[-1]} channels per pass"
+        )
+    _ut_params(ut_params)
+    cams = dict(camera_model=camera_model, radial_coeffs=radial_coeffs, tangential_coeffs=tangential_coeffs,
+                thin_prism_coeffs=thin_prism_coeffs)
+
+    # ---- projection through the camera model (no gradient, as in the reference)
+    radii, means2d, depths, conics, _ = fully_fused_projection_with_ut(
+        means, quats, scales, opacities, viewmats, Ks, width, height, eps2d=eps2d, near_plane=near_plane,
+        far_plane=far_plane, radius_clip=radius_clip, calc_compensations=False, ut_params=ut_params, **cams,
+    )
+    feat = _color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N) if has_color else None
+    feat, backgrounds = _with_depth_channel(feat, depths, backgrounds, has_color, has_depth, batch_dims, C)
+    opac = torch.broadcast_to(opacities[..., None, :], batch_dims + (C, N))
+
+    # ---- tile lists from the radius box alone: the eval3d response is not the 2-D conic, so a conic / opacity cull
+    # could drop pairs the compositing uses (the reference passes no conics here under with_ut)
+    tile_width = math.ceil(width / float(tile_size))
+    tile_height = math.ceil(height / float(tile_size))
+    hits = isect_tiles_sorted(means2d, radii, depths, tile_size, tile_width, tile_height)
+    flatten_ids = hits.flatten_ids
+    isect_offsets = hits.isect_offsets.reshape(batch_dims + (C, tile_height, tile_width))
+
+    # ---- compositing, chunked over channels; a chunk width the kernels are not built for is zero-padded
+    outs, render_alphas = [], None
+    for lo in range(0, feat.shape[-1], channel_chunk):
+        f = feat[..., lo : lo + channel_chunk]
+        bg = backgrounds[..., lo : lo + channel_chunk] if backgrounds is not None else None
+        D = f.shape[-1]
+        pad = next(c for c in _SUPPORTED_CHANNELS if c >= D) - D
+        if pad:
+            f = torch.nn.functional.pad(f, (0, pad))
+            bg = torch.nn.functional.pad(bg, (0, pad)) if bg is not None else None
+        rc, ra = rasterize_to_pixels_eval3d(
+            means, quats, scales, f, opac, viewmats, Ks, width, height, tile_size, isect_offsets, flatten_ids,
+            backgrounds=bg, ut_params=ut_params, **cams,
+        )
+        outs.append(rc[..., :D] if pad else rc)
+        if render_alphas is None:
+            render_alphas = ra
+    render_colors = outs[0] if len(outs) == 1 else torch.cat(outs, dim=-1)
+    render_colors = _normalize_expected_depth(render_colors, render_alphas, render_mode)
+
+    meta = _Meta({
+        "batch_ids": None,
+        "camera_ids": None,
+        "gaussian_ids": None,
+        "radii": radii,
+        "means2d": means2d,
+        "depths": depths,
+        "conics": conics,
+        "opacities": opac,
+        "tile_width": tile_width,
+        "tile_height": tile_height,
+        "tiles_per_gauss": hits.tiles_per_gauss,
+        "isect_ids": _Lazy(hits.isect_ids),
         "flatten_ids": flatten_ids,
         "isect_offsets": isect_offsets,
         "width": width,

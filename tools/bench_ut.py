@@ -4,7 +4,11 @@ forward and backward) next to the EWA step (fully_fused_projection + the same li
 backward) on bench.py's scene (1M Gaussians, one 1920x1080 view) with a pinhole camera.  Median of --steps timed steps after --warmup, CUDA events; prints
 the device name and power limit with the numbers, as one JSON line.
 
-    python tools/bench_ut.py [--steps 20] [--warmup 5] [--distorted]
+    python tools/bench_ut.py [--steps 20] [--warmup 5] [--distorted] [--rasterization]
+
+--rasterization times the public call instead: rasterization(with_ut=True, with_eval3d=True, sh_degree=3,
+packed=False) forward and backward on the same scene with SH degree 3, next to the same operators chained by hand, and
+reports the difference as the public call's overhead.
 """
 import argparse
 import json
@@ -27,8 +31,12 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--distorted", action="store_true", help="pinhole with radial and tangential coefficients")
+    ap.add_argument("--rasterization", action="store_true",
+                    help="time rasterization(with_ut=True, with_eval3d=True, sh_degree=3) next to the hand-chained operators")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_ut needs a GPU"
+    if a.rasterization:
+        return bench_rasterization(a)
     dev = "cuda"
     # bench.py's scene: the garden crop tiled 3x3 (about 1M Gaussians), one 1920x1080 view; colours instead of SH
     sc = scene.make_scene(scene_grid=3, sh_degree=0)
@@ -73,6 +81,63 @@ def main():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
     res.update(device=torch.cuda.get_device_name(0), power_limit=q.stdout.strip(), gaussians=int(means.shape[0]), width=W,
                height=H, distorted=a.distorted, steps=a.steps)
+    print(json.dumps(res))
+
+
+def _device_info():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return dict(device=torch.cuda.get_device_name(0), power_limit=q.stdout.strip())
+
+
+def bench_rasterization(a):
+    """rasterization(with_ut=True, with_eval3d=True, sh_degree=3, packed=False) forward + backward against the same
+    work chained by hand (UT projection, SH + clamp, isect_tiles + isect_offset_encode, eval3d compositing), alternated
+    step by step so that both see the same machine state."""
+    dev = "cuda"
+    sc = scene.make_scene(scene_grid=3, sh_degree=3)
+    W, H = 1920, 1080
+    t = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)  # noqa: E731
+    means, quats, scales, opac, sh = (t(sc[k]).requires_grad_(True) for k in ("means", "quats", "scales", "opacities", "sh"))
+    vm, K = t(sc["viewmats"][:1]), t(scene.rescale_K(sc["Ks"], sc["width"], sc["height"], W, H)[:1])
+    co = dict(radial_coeffs=t(np.float32([[0.05, -0.02, 0.0, 0.0, 0.0, 0.0]])), tangential_coeffs=t(np.float32([[0.001, -0.001]]))) if a.distorted else {}
+    tw, th = (W + 15) // 16, (H + 15) // 16
+    N = means.shape[0]
+
+    def public():
+        rc, ra, meta = gs.rasterization(means, quats, scales, opac, sh, vm, K, W, H, sh_degree=3, packed=False, with_ut=True,
+                                        with_eval3d=True, **co)
+        (rc.sum() + ra.sum()).backward()
+        return meta["flatten_ids"].numel()
+
+    def chain():
+        r, m2, d, _, _ = gs.fully_fused_projection_with_ut(means.detach(), quats.detach(), scales.detach(), opac.detach(), vm, K,
+                                                          W, H, **co)
+        feat = torch.clamp_min(gs.spherical_harmonics(3, means, vm, sh, masks=(r > 0).all(-1)) + 0.5, 0.0)
+        _, ii, fl = gs.isect_tiles(m2, r, d, 16, tw, th)
+        offs = gs.isect_offset_encode(ii, 1, tw, th)
+        o = torch.broadcast_to(opac[None], (1, N))
+        rc, ra = gs.rasterize_to_pixels_eval3d(means, quats, scales, feat, o, vm, K, W, H, 16, offs, fl, **co)
+        (rc.sum() + ra.sum()).backward()
+        return fl.numel()
+
+    fns = {"rasterization": public, "hand_chain": chain}
+    for fn in fns.values():
+        for _ in range(a.warmup):
+            fn()
+    torch.cuda.synchronize()
+    times = {k: [] for k in fns}
+    n = {}
+    for _ in range(a.steps):
+        for name, fn in fns.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            n[name] = fn()
+            e1.record()
+            torch.cuda.synchronize()
+            times[name].append(e0.elapsed_time(e1))
+    res = {name: {"median_ms": float(np.median(v)), "min_ms": float(np.min(v)), "n_isects": int(n[name])} for name, v in times.items()}
+    res["overhead_ms"] = res["rasterization"]["median_ms"] - res["hand_chain"]["median_ms"]
+    res.update(_device_info(), gaussians=int(N), width=W, height=H, sh_degree=3, distorted=a.distorted, steps=a.steps)
     print(json.dumps(res))
 
 

@@ -27,6 +27,10 @@ the trainable splats start from perturbed values (trainer-style init: init_opa, 
 runs on an accelerated schedule (``--refine-start/--refine-every``; defaults of the reference are 500 / 100) so that
 the 1M -> 3M growth of cfg5 happens within a bench-sized run; both backends get the same schedule and seeds.
 
+``--with-ut`` (with ``--strategy mcmc``, the only densification the reference supports for 3DGUT) trains 3DGUT:
+rasterization(with_ut=True, with_eval3d=True) through the plain pinhole; the ground truth stays the EWA render.  Both
+backends need the reference package in baseline/_ref; without it the tool prints a "not_run" line.
+
 Prints ONE JSON line.  Test / bench infrastructure: it imports oracle/refcuda.py to locate the reference.
 """
 from __future__ import annotations
@@ -35,6 +39,7 @@ import argparse
 import json
 import math
 import os
+import subprocess
 import sys
 import time
 
@@ -82,7 +87,11 @@ def main():
     ap.add_argument("--breakdown", action="store_true", help="CUDA-event phase times of a few steady steps (after the run)")
     ap.add_argument("--warm", type=int, default=20, help="untimed first steps (allocator / cuDNN autotune / lazy init)")
     ap.add_argument("--grad-stats", action="store_true", help="default strategy: print quantiles of the densification statistic")
+    ap.add_argument("--with-ut", action="store_true",
+                    help="train 3DGUT: rasterization(with_ut=True, with_eval3d=True), MCMC only (as in the reference)")
     args = ap.parse_args()
+    if args.with_ut and args.strategy != "mcmc":
+        ap.error("--with-ut trains with the MCMC strategy only (the reference densifies 3DGUT with MCMC alone)")
 
     from oracle import refcuda
     from tests import scene
@@ -90,6 +99,11 @@ def main():
     assert torch.cuda.is_available()
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
+    if not refcuda.package_available():
+        # the reference package (baseline/_ref) drives both backends: strategies, losses and the ground truth
+        print(json.dumps({"tool": "trainer_bench", "backend": args.backend, "strategy": args.strategy,
+                          "with_ut": args.with_ut, "not_run": "the reference package is not installed in baseline/_ref"}))
+        return
     gsplat = refcuda.import_package()
     from gsplat.strategy import DefaultStrategy, MCMCStrategy
     import gsplat.losses as glosses
@@ -183,7 +197,7 @@ def main():
             means=means, quats=quats, scales=scales, opacities=opacities, colors=colors,
             viewmats=torch.linalg.inv_ex(camtoworlds).inverse, Ks=Ks, width=W_IMG, height=H_IMG, packed=False,
             absgrad=(strategy.absgrad if isinstance(strategy, DefaultStrategy) else False), sparse_grad=False,
-            rasterize_mode="classic", distributed=False, camera_model="pinhole", with_ut=False, with_eval3d=False,
+            rasterize_mode="classic", distributed=False, camera_model="pinhole", with_ut=args.with_ut, with_eval3d=args.with_ut,
             sh_degree=sh_degree_to_use, near_plane=0.01, far_plane=1e10, render_mode="RGB",
         )
         colors_r = renders
@@ -250,7 +264,7 @@ def main():
         t_first_refine, steps_1m = t1, timed_steps
 
     out = {
-        "tool": "trainer_bench", "backend": args.backend, "strategy": args.strategy, "steps": args.steps,
+        "tool": "trainer_bench", "backend": args.backend, "strategy": args.strategy, "with_ut": args.with_ut, "steps": args.steps,
         "it_per_s_total": timed_steps / (t1 - t0),
         "steps_at_1M": steps_1m,
         "it_per_s_at_1M": (steps_1m / (t_first_refine - t0)) if steps_1m > 0 else None,
@@ -264,6 +278,9 @@ def main():
         "schedule": {"refine_start": args.refine_start, "refine_every": args.refine_every, "cap": args.cap,
                      "grow_grad2d": args.grow_grad2d, "views": args.views, "gt_scale": args.gt_scale},
         "max_mem_gb": torch.cuda.max_memory_allocated() / 2**30,
+        "device": torch.cuda.get_device_name(0),
+        "power_limit": subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
+                                      text=True).stdout.strip(),
     }
     if args.breakdown:
         # freeze the structure (no refinement) and time the phases of 10 steady steps with CUDA events
