@@ -16,6 +16,7 @@ their alphas equal its render_alphas bit for bit).  Importing the package does n
 operator does (and needs gsplat_b200/libgsplat_b200.so, built by ``python -m gsplat_b200.build``).
 """
 from .ops import (  # noqa: F401
+    RollingShutterType,
     adam,
     build_sparse_tile_layout,
     compute_relocation,
@@ -79,10 +80,11 @@ def has_2dgs() -> bool:
 
 def has_3dgut() -> bool:
     """Reference: _wrapper.py has_3dgut -- False.  In the reference this flag gates 3DGUT tests that need ftheta and lidar
-    cameras, rolling shutter, hit-distance modes and tile_size 8, none of which is built here.  What is built:
+    cameras, hit-distance modes and tile_size 8, none of which is built here.  What is built:
     ``rasterization(with_ut=True, with_eval3d=True)`` with dense rows, and the two 3DGUT operators it runs on,
     ``fully_fused_projection_with_ut`` and ``rasterize_to_pixels_eval3d`` (distorted pinhole and fisheye cameras, global
-    shutter), which also chain with ``isect_tiles`` / ``isect_offset_encode`` as in the reference's ``_rasterization``."""
+    or rolling shutter: ``rolling_shutter`` with the end-of-frame poses ``viewmats_rs``), which also chain with
+    ``isect_tiles`` / ``isect_offset_encode`` as in the reference's ``_rasterization``."""
     return False
 
 
@@ -102,6 +104,7 @@ __all__ = [
     "rasterize_to_pixels_eval3d",
     "fused_project_sh",
     "spherical_harmonics",
+    "RollingShutterType",
     "isect_tiles",
     "isect_offset_encode",
     "rasterize_to_pixels",

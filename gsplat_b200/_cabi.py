@@ -211,18 +211,19 @@ _SIGNATURES = {
     ),
     "gsb200_ut_projection_fwd": (
         c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32,
-         c_f32, c_f32, c_f32, c_f32, c_f32, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_u32, c_u32, c_f32,
+         c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     ),
     "gsb200_eval3d_fwd": (
         c_int,
-        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_u32,
-         c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp],
+        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
+         c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp],
     ),
     "gsb200_eval3d_bwd": (
         c_int,
-        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_u32,
-         c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
+         c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+         c_vp, c_vp],
     ),
 }
 

@@ -10,6 +10,7 @@
 #include <float.h>
 
 #include "common.cuh"
+#include "gaussmath.cuh"
 
 namespace gsb
 {
@@ -246,5 +247,160 @@ __device__ __forceinline__ bool cam_unproject(const CamModel &m, float u, float 
         d[0] = sc * x0, d[1] = sc * y0, d[2] = cosf(t);
     }
     return true;
+}
+
+// ------------------------------------------------------------------ rolling shutter
+// Reference semantics: include/Cameras.cuh (RollingShutterParameters, interpolate_shutter_pose,
+// shutter_relative_frame_time, world_point_to_image_point_shutter_pose).  Each image row or column is exposed at its
+// own pose, interpolated between the start pose (viewmats) and the end pose (viewmats_rs) at the frame time of that row
+// or column.  Ids as the reference's RollingShutterType.
+constexpr int kShutterTopToBottom = 0;
+constexpr int kShutterLeftToRight = 1;
+constexpr int kShutterBottomToTop = 2;
+constexpr int kShutterRightToLeft = 3;
+constexpr int kShutterGlobal      = 4;
+constexpr int kShutterIterations  = 10;
+
+// Kernel policies: the global shutter takes the pose of viewmats; the rolling one interpolates each camera's two poses.
+struct GlobalShutter
+{
+    static constexpr bool kRolling = false;
+};
+struct RollingShutter
+{
+    static constexpr bool kRolling = true;
+    const float *viewmats_rs;
+    int type;
+};
+
+// The two poses of one camera, rotations as quaternions (w, x, y, z) with q1 on q0's short arc, and the slerp's
+// constant angle between them (0: near-parallel, interpolated component-wise).
+struct RsPoses
+{
+    float q0[4], q1[4], t0[3], t1[3], angle, sin_angle;
+};
+
+// Unit quaternion of the rotation block of a row-major 4x4 pose, from its largest component (as glm::quat_cast).
+__device__ __forceinline__ void quat_from_pose(const float *vm, float *q)
+{
+    const float r00 = vm[0], r01 = vm[1], r02 = vm[2];
+    const float r10 = vm[4], r11 = vm[5], r12 = vm[6];
+    const float r20 = vm[8], r21 = vm[9], r22 = vm[10];
+    const float f[4] = {r00 + r11 + r22, r00 - r11 - r22, r11 - r00 - r22, r22 - r00 - r11}; // 4 c^2 - 1, c = w, x, y, z
+    int big = 0;
+#pragma unroll
+    for(int k = 1; k < 4; ++k)
+        big = f[k] > f[big] ? k : big;
+    const float v    = sqrtf(f[big] + 1.f) * 0.5f;
+    const float mult = 0.25f / v;
+    const float a = (r21 - r12) * mult, b = (r02 - r20) * mult, c = (r10 - r01) * mult; // w x, w y, w z
+    const float d = (r10 + r01) * mult, e = (r02 + r20) * mult, g = (r21 + r12) * mult; // x y, x z, y z
+    switch(big)
+    {
+    case 0: q[0] = v, q[1] = a, q[2] = b, q[3] = c; break;
+    case 1: q[0] = a, q[1] = v, q[2] = d, q[3] = e; break;
+    case 2: q[0] = b, q[1] = d, q[2] = v, q[3] = g; break;
+    default: q[0] = c, q[1] = e, q[2] = g, q[3] = v; break;
+    }
+}
+
+__device__ __forceinline__ RsPoses load_rs_poses(const float *vm0, const float *vm1)
+{
+    RsPoses P;
+    quat_from_pose(vm0, P.q0);
+    quat_from_pose(vm1, P.q1);
+    P.t0[0] = vm0[3], P.t0[1] = vm0[7], P.t0[2] = vm0[11];
+    P.t1[0] = vm1[3], P.t1[1] = vm1[7], P.t1[2] = vm1[11];
+    float c = P.q0[0] * P.q1[0] + P.q0[1] * P.q1[1] + P.q0[2] * P.q1[2] + P.q0[3] * P.q1[3];
+    if(c < 0.f)
+    {
+#pragma unroll
+        for(int k = 0; k < 4; ++k)
+            P.q1[k] = -P.q1[k];
+        c = -c;
+    }
+    P.angle = 0.f, P.sin_angle = 0.f;
+    if(!(c > 1.f - FLT_EPSILON))
+    {
+        P.angle     = acosf(c);
+        P.sin_angle = sinf(P.angle);
+    }
+    return P;
+}
+
+// The pose at relative frame time a (not clamped: points in the margin have times outside [0, 1]): translation
+// (1 - a) t0 + a t1, rotation the normalised slerp of the two quaternions.
+__device__ __forceinline__ Cam pose_at(const RsPoses &P, float a)
+{
+    float q[4];
+    if(P.angle == 0.f)
+    {
+#pragma unroll
+        for(int k = 0; k < 4; ++k)
+            q[k] = P.q0[k] * (1.f - a) + P.q1[k] * a;
+    }
+    else
+    {
+        const float s0 = sinf((1.f - a) * P.angle), s1 = sinf(a * P.angle);
+#pragma unroll
+        for(int k = 0; k < 4; ++k)
+            q[k] = (s0 * P.q0[k] + s1 * P.q1[k]) / P.sin_angle;
+    }
+    Cam c;
+    c.R = quat_to_rotmat(q); // normalises q
+#pragma unroll
+    for(int k = 0; k < 3; ++k)
+        c.t[k] = (1.f - a) * P.t0[k] + a * P.t1[k];
+    c.fx = c.fy = c.cx = c.cy = 0.f;
+    return c;
+}
+
+// Relative frame time of image point (u, v): the exposure time of its row or column, 0 at the first, 1 at the last.
+// The caller guarantees H > 1 (rows) or W > 1 (columns).
+__device__ __forceinline__ float shutter_time(int type, uint32_t W, uint32_t H, float u, float v)
+{
+    switch(type)
+    {
+    case kShutterTopToBottom: return floorf(v) / (float)(H - 1);
+    case kShutterLeftToRight: return floorf(u) / (float)(W - 1);
+    case kShutterBottomToTop: return ((float)H - ceilf(v)) / (float)(H - 1);
+    default: return ((float)W - ceilf(u)) / (float)(W - 1);
+    }
+}
+
+__device__ __forceinline__ bool cam_project_at(const CamModel &m, const Cam &pose, const float *x, float margin, float &u, float &v)
+{
+    float xc[3];
+#pragma unroll
+    for(int i = 0; i < 3; ++i)
+        xc[i] = pose.R.m[i * 3 + 0] * x[0] + pose.R.m[i * 3 + 1] * x[1] + pose.R.m[i * 3 + 2] * x[2] + pose.t[i];
+    return cam_project(m, xc, margin, u, v);
+}
+
+// World point -> image point through a rolling shutter: start from the start pose's projection if it is valid, else
+// the end pose's (neither valid: the point is invalid, at the end pose's image point), then re-project at the frame
+// time of the current point until that time repeats, at most kShutterIterations times.  The point and its validity are
+// those of the last projection.
+__device__ __forceinline__ bool cam_project_rs(
+    const CamModel &m, const RsPoses &P, int type, const float *x, float margin, float &u, float &v
+)
+{
+    float u0, v0, u1, v1;
+    const bool ok0 = cam_project_at(m, pose_at(P, 0.f), x, margin, u0, v0);
+    const bool ok1 = cam_project_at(m, pose_at(P, 1.f), x, margin, u1, v1);
+    u = ok0 ? u0 : u1, v = ok0 ? v0 : v1;
+    if(!ok0 && !ok1)
+        return false;
+    bool ok = true;
+    float prev = -FLT_MAX;
+    for(int it = 0; it < kShutterIterations; ++it)
+    {
+        const float a = shutter_time(type, m.W, m.H, u, v);
+        if(a == prev)
+            break;
+        prev = a;
+        ok   = cam_project_at(m, pose_at(P, a), x, margin, u, v);
+    }
+    return ok;
 }
 } // namespace gsb

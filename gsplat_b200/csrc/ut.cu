@@ -21,17 +21,40 @@ struct UtParams
     int require_all;
 };
 
-// One thread per (b, c, n).  Culled rows get radii 0 and zero float outputs.
+// Each camera's two poses for the threads of one projection CTA: the images its rows fall in, one thread per image.
+// Called by every thread of the CTA.
+__device__ __forceinline__ RsPoses cta_rs_poses(RsPoses *s_poses, int64_t total, int64_t N, const float *viewmats, const float *viewmats_rs)
+{
+    const int64_t lo    = (int64_t)blockIdx.x * kUtThreads;
+    const int64_t first = lo / N, last = (min(lo + kUtThreads, total) - 1) / N;
+    for(int64_t img = first + threadIdx.x; img <= last; img += kUtThreads)
+        s_poses[img - first] = load_rs_poses(viewmats + img * 16, viewmats_rs + img * 16);
+    __syncthreads();
+    const int64_t idx = lo + threadIdx.x;
+    return s_poses[(idx < total ? idx / N : first) - first];
+}
+
+// One thread per (b, c, n).  Culled rows get radii 0 and zero float outputs.  Rolling shutter: each sigma point is
+// projected at the pose of the row or column it lands in (cam_project_rs); the depth and the near / far cull take the
+// mid-frame pose.
+template<class Shutter>
 __global__ void __launch_bounds__(kUtThreads) ut_project_kernel(
     int64_t B, int64_t C, int64_t N, const float *__restrict__ means, const float *__restrict__ quats,
     const float *__restrict__ scales, const float *__restrict__ opacities, const float *__restrict__ viewmats,
     const float *__restrict__ Ks, int cam_kind, const float *__restrict__ radial, const float *__restrict__ tangential,
     const float *__restrict__ thin, uint32_t W, uint32_t H, float eps2d, float near_plane, float far_plane,
     float radius_clip, UtParams ut, int32_t *__restrict__ radii, float *__restrict__ means2d, float *__restrict__ depths,
-    float *__restrict__ conics, float *__restrict__ compensations
+    float *__restrict__ conics, float *__restrict__ compensations, Shutter shutter
 )
 {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    [[maybe_unused]] RsPoses poses;
+    if constexpr(Shutter::kRolling)
+    {
+        // at most one image per row of the CTA, plus the one its first row starts in
+        __shared__ RsPoses s_poses[kUtThreads + 1];
+        poses = cta_rs_poses(s_poses, B * C * N, N, viewmats, shutter.viewmats_rs);
+    }
     if(idx >= B * C * N)
         return;
     const int64_t b = idx / (C * N), c = (idx / N) % C, n = idx % N;
@@ -43,7 +66,7 @@ __global__ void __launch_bounds__(kUtThreads) ut_project_kernel(
     int rx = 0, ry = 0;
     float mx = 0.f, my = 0.f, depth = 0.f, ca = 0.f, cb = 0.f, cc = 0.f, comp = 0.f;
     const float qn2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-    const Cam cam   = load_cam(viewmats + bc * 16, Ks + bc * 9);
+    const Cam cam   = Shutter::kRolling ? pose_at(poses, 0.5f) : load_cam(viewmats + bc * 16, Ks + bc * 9);
     float pc[3];
 #pragma unroll
     for(int i = 0; i < 3; ++i)
@@ -77,11 +100,17 @@ __global__ void __launch_bounds__(kUtThreads) ut_project_kernel(
                 for(int i = 0; i < 3; ++i)
                     x[i] = sg > 0.f ? x[i] + mag * Rq.m[i * 3 + ax] : x[i] - mag * Rq.m[i * 3 + ax];
             }
-            float xc[3];
+            bool ok;
+            if constexpr(Shutter::kRolling)
+                ok = cam_project_rs(cm, poses, shutter.type, x, ut.margin, pu[k], pv[k]);
+            else
+            {
+                float xc[3];
 #pragma unroll
-            for(int i = 0; i < 3; ++i)
-                xc[i] = cam.R.m[i * 3 + 0] * x[0] + cam.R.m[i * 3 + 1] * x[1] + cam.R.m[i * 3 + 2] * x[2] + cam.t[i];
-            const bool ok = cam_project(cm, xc, ut.margin, pu[k], pv[k]);
+                for(int i = 0; i < 3; ++i)
+                    xc[i] = cam.R.m[i * 3 + 0] * x[0] + cam.R.m[i * 3 + 1] * x[1] + cam.R.m[i * 3 + 2] * x[2] + cam.t[i];
+                ok = cam_project(cm, xc, ut.margin, pu[k], pv[k]);
+            }
             any = any || ok;
             all = all && ok;
             // with every point required, the first invalid one ends the transform (the row is culled)
@@ -209,6 +238,41 @@ __device__ __forceinline__ bool pixel_ray(
     return ok;
 }
 
+// Rolling shutter: the same ray, carried to the world by the pose at the frame time of the pixel centre's row or column.
+// The forward and the backward build it alike, so both take the same alpha and transmittance decisions.
+__device__ __forceinline__ bool pixel_ray(
+    const RsPoses &P, int type, const CamModel &cm, uint32_t i, uint32_t j, float *ro, float *rd
+)
+{
+    float dc[3];
+    const float u = (float)j + 0.5f, v = (float)i + 0.5f;
+    const bool ok   = cam_unproject(cm, u, v, dc);
+    const Cam pose  = pose_at(P, shutter_time(type, cm.W, cm.H, u, v));
+    const float *R  = pose.R.m;
+#pragma unroll
+    for(int k = 0; k < 3; ++k)
+    {
+        ro[k] = -(R[0 * 3 + k] * pose.t[0] + R[1 * 3 + k] * pose.t[1] + R[2 * 3 + k] * pose.t[2]);
+        rd[k] = R[0 * 3 + k] * dc[0] + R[1 * 3 + k] * dc[1] + R[2 * 3 + k] * dc[2];
+    }
+    return ok;
+}
+
+// The pixel's ray under either shutter.  Rolling: the image's two poses are loaded once per CTA (one image per CTA);
+// every thread of the CTA calls this.
+template<class Shutter>
+__device__ __forceinline__ bool shutter_pixel_ray(
+    const Shutter &shutter, const float *viewmats, uint32_t img, bool inside, const CamModel &cm, uint32_t i, uint32_t j,
+    float *ro, float *rd
+)
+{
+    __shared__ RsPoses s_poses;
+    if(threadIdx.x == 0)
+        s_poses = load_rs_poses(viewmats + (int64_t)img * 16, shutter.viewmats_rs + (int64_t)img * 16);
+    __syncthreads();
+    return inside && pixel_ray(s_poses, shutter.type, cm, i, j, ro, rd);
+}
+
 // Maximum response of one gaussian along a ray: a = M (o - mu), g = normalize(M d); the closest approach to the
 // gaussian's centre in its own frame is |g x a|.  ok = false: the approach lies behind the ray origin, or alpha < 1/255.
 struct EvalHit
@@ -255,12 +319,13 @@ struct EvalGeom
 
 // One CTA per 16x16 tile of the [I, th, tw] grid, one pixel per thread.  last_ids: the list index of the pixel's last
 // composited gaussian, -1 for none.
-template<int CDIM>
+template<int CDIM, class Shutter>
 __global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
     EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
     const float *__restrict__ colors, const float *__restrict__ opacities, const float *__restrict__ backgrounds,
     const uint8_t *__restrict__ masks, const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids,
-    int64_t n_isects, float *__restrict__ render_colors, float *__restrict__ render_alphas, int32_t *__restrict__ last_ids
+    int64_t n_isects, float *__restrict__ render_colors, float *__restrict__ render_alphas, int32_t *__restrict__ last_ids,
+    Shutter shutter
 )
 {
     __shared__ EvalRec rec[kUtThreads];
@@ -289,7 +354,12 @@ __global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
     const int64_t end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
     float ro[3] = {0.f, 0.f, 0.f}, rd[3] = {0.f, 0.f, 1.f};
     bool done = !inside;
-    if(inside)
+    if constexpr(Shutter::kRolling)
+    {
+        const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        done              = !shutter_pixel_ray(shutter, geo.viewmats, img, inside, cm, i, j, ro, rd);
+    }
+    else if(inside)
     {
         const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
         done              = !pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
@@ -370,13 +440,13 @@ __device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, cons
 
 // Back to front over each tile's list.  Per gaussian, the warp's per-pixel gradients (colours, opacity, mean, M) are
 // butterfly-reduced and added with one atomic per value.
-template<int CDIM>
+template<int CDIM, class Shutter>
 __global__ void __launch_bounds__(kUtThreads, 1) eval3d_bwd_kernel(
     EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
     const float *__restrict__ colors, const float *__restrict__ opacities, const float *__restrict__ backgrounds,
     const uint8_t *__restrict__ masks, const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids,
     int64_t n_isects, const float *__restrict__ render_alphas, const int32_t *__restrict__ last_ids,
-    const float *__restrict__ v_render_colors, const float *__restrict__ v_render_alphas, EvalGradDst dst
+    const float *__restrict__ v_render_colors, const float *__restrict__ v_render_alphas, EvalGradDst dst, Shutter shutter
 )
 {
     constexpr int NV = CDIM + 13; // colours | opacity 1 | mean 3 | M 9
@@ -398,7 +468,12 @@ __global__ void __launch_bounds__(kUtThreads, 1) eval3d_bwd_kernel(
     const int64_t start = offsets[tile];
     const int64_t end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
     float ro[3] = {0.f, 0.f, 0.f}, rd[3] = {0.f, 0.f, 1.f};
-    if(inside)
+    if constexpr(Shutter::kRolling)
+    {
+        const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        inside            = shutter_pixel_ray(shutter, geo.viewmats, img, inside, cm, i, j, ro, rd);
+    }
+    else if(inside)
     {
         const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
         inside            = pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
@@ -567,6 +642,29 @@ int eval3d_checks(
         return GSB200_E_UNSUPPORTED;
     return GSB200_OK;
 }
+
+// A rolling shutter takes an end pose, the global shutter none; the frame time divides by the rows (or columns) - 1.
+int shutter_checks(const float *viewmats_rs, int rolling_shutter, uint32_t W, uint32_t H)
+{
+    if(rolling_shutter < 0 || rolling_shutter > kShutterGlobal)
+        return GSB200_E_INVALID;
+    if((viewmats_rs != nullptr) != (rolling_shutter != kShutterGlobal))
+        return GSB200_E_INVALID;
+    const bool rows = rolling_shutter == kShutterTopToBottom || rolling_shutter == kShutterBottomToTop;
+    const bool cols = rolling_shutter == kShutterLeftToRight || rolling_shutter == kShutterRightToLeft;
+    if((rows && H < 2) || (cols && W < 2))
+        return GSB200_E_INVALID;
+    return GSB200_OK;
+}
+
+// Runs f with the kernels' shutter policy: the global shutter for no end pose.
+template<class F>
+int with_shutter(const float *viewmats_rs, int rolling_shutter, F &&f)
+{
+    if(viewmats_rs)
+        return f(RollingShutter{viewmats_rs, rolling_shutter});
+    return f(GlobalShutter{});
+}
 } // namespace
 } // namespace gsb
 
@@ -575,14 +673,16 @@ int eval3d_checks(
 extern "C" int gsb200_ut_projection_fwd(
     int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
     const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-    const float *thin_prism_coeffs, uint32_t image_width, uint32_t image_height, float eps2d, float near_plane,
-    float far_plane, float radius_clip, float ut_alpha, float ut_beta, float ut_kappa, float ut_in_image_margin_factor,
-    int ut_require_all_sigma_points_valid, int32_t *radii, float *means2d, float *depths, float *conics,
-    float *compensations, void *stream
+    const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
+    uint32_t image_height, float eps2d, float near_plane, float far_plane, float radius_clip, float ut_alpha, float ut_beta,
+    float ut_kappa, float ut_in_image_margin_factor, int ut_require_all_sigma_points_valid, int32_t *radii,
+    float *means2d, float *depths, float *conics, float *compensations, void *stream
 )
 {
     if(B < 0 || C < 0 || N < 0)
         return GSB200_E_INVALID;
+    if(int rc = gsb::shutter_checks(viewmats_rs, rolling_shutter, image_width, image_height))
+        return rc;
     if(camera_model != gsb::kUtPinhole && camera_model != gsb::kUtFisheye)
         return GSB200_E_UNSUPPORTED;
     if(camera_model == gsb::kUtFisheye && (tangential_coeffs || thin_prism_coeffs))
@@ -595,26 +695,31 @@ extern "C" int gsb200_ut_projection_fwd(
     if(!means || !quats || !scales || !viewmats || !Ks || !radii || !means2d || !depths || !conics)
         return GSB200_E_INVALID;
     const gsb::UtParams ut{ut_alpha, ut_beta, ut_kappa, ut_in_image_margin_factor, ut_require_all_sigma_points_valid};
-    gsb::ut_project_kernel<<<gsb::grid_for(n, gsb::kUtThreads), gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
-        B, C, N, means, quats, scales, opacities, viewmats, Ks, camera_model, radial_coeffs, tangential_coeffs,
-        thin_prism_coeffs, image_width, image_height, eps2d, near_plane, far_plane, radius_clip, ut, radii, means2d, depths,
-        conics, compensations
-    );
-    return gsb::check_launch();
+    return gsb::with_shutter(viewmats_rs, rolling_shutter, [&](auto shutter) {
+        gsb::ut_project_kernel<<<gsb::grid_for(n, gsb::kUtThreads), gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
+            B, C, N, means, quats, scales, opacities, viewmats, Ks, camera_model, radial_coeffs, tangential_coeffs,
+            thin_prism_coeffs, image_width, image_height, eps2d, near_plane, far_plane, radius_clip, ut, radii, means2d,
+            depths, conics, compensations, shutter
+        );
+        return gsb::check_launch();
+    });
 }
 
 extern "C" int gsb200_eval3d_fwd(
     int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
     const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
     const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-    const float *thin_prism_coeffs, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
-    uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, float *render_colors,
-    float *render_alphas, int32_t *last_ids, void *stream
+    const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
+    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+    const int32_t *flatten_ids, int64_t n_isects, float *render_colors, float *render_alphas, int32_t *last_ids,
+    void *stream
 )
 {
     if(n_isects < 0)
         return GSB200_E_INVALID;
     if(int rc = gsb::eval3d_checks(B, C, N, camera_model, image_width, image_height, tile_size, tile_width, tile_height))
+        return rc;
+    if(int rc = gsb::shutter_checks(viewmats_rs, rolling_shutter, image_width, image_height))
         return rc;
     if(B * C == 0 || image_width == 0 || image_height == 0)
         return GSB200_OK;
@@ -624,12 +729,14 @@ extern "C" int gsb200_eval3d_fwd(
         return GSB200_E_INVALID;
     const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height,
                             camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
-    return gsb::with_channels(D, [&](auto CH) {
-        gsb::eval3d_fwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
-            geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects, render_colors,
-            render_alphas, last_ids
-        );
-        return gsb::check_launch();
+    return gsb::with_shutter(viewmats_rs, rolling_shutter, [&](auto shutter) {
+        return gsb::with_channels(D, [&](auto CH) {
+            gsb::eval3d_fwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
+                geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
+                render_colors, render_alphas, last_ids, shutter
+            );
+            return gsb::check_launch();
+        });
     });
 }
 
@@ -637,15 +744,18 @@ extern "C" int gsb200_eval3d_bwd(
     int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
     const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
     const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-    const float *thin_prism_coeffs, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
-    uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, const float *render_alphas,
-    const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, float *grad_records,
-    float *v_colors, float *v_opacities, float *v_means, float *v_quats, float *v_scales, void *stream
+    const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
+    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+    const int32_t *flatten_ids, int64_t n_isects, const float *render_alphas, const int32_t *last_ids,
+    const float *v_render_colors, const float *v_render_alphas, float *grad_records, float *v_colors, float *v_opacities,
+    float *v_means, float *v_quats, float *v_scales, void *stream
 )
 {
     if(n_isects < 0)
         return GSB200_E_INVALID;
     if(int rc = gsb::eval3d_checks(B, C, N, camera_model, image_width, image_height, tile_size, tile_width, tile_height))
+        return rc;
+    if(int rc = gsb::shutter_checks(viewmats_rs, rolling_shutter, image_width, image_height))
         return rc;
     if(B * N == 0)
         return GSB200_OK;
@@ -660,12 +770,14 @@ extern "C" int gsb200_eval3d_bwd(
         const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width,
                                 tile_height, camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
         const gsb::EvalGradDst dst{v_colors, v_opacities, grad_records};
-        const int rc = gsb::with_channels(D, [&](auto CH) {
-            gsb::eval3d_bwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, st>>>(
-                geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
-                render_alphas, last_ids, v_render_colors, v_render_alphas, dst
-            );
-            return gsb::check_launch();
+        const int rc = gsb::with_shutter(viewmats_rs, rolling_shutter, [&](auto shutter) {
+            return gsb::with_channels(D, [&](auto CH) {
+                gsb::eval3d_bwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, st>>>(
+                    geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
+                    render_alphas, last_ids, v_render_colors, v_render_alphas, dst, shutter
+                );
+                return gsb::check_launch();
+            });
         });
         if(rc)
             return rc;

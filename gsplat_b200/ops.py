@@ -12,6 +12,7 @@ hand-written sm_90a kernels.
 """
 from __future__ import annotations
 
+import enum
 import math
 import operator
 from typing import NamedTuple, Optional, Tuple
@@ -469,6 +470,18 @@ class _SphericalHarmonicsRows(torch.autograd.Function):
         return None, v_means, v_viewmats, v_coeffs, None, None, None
 
 
+def _mid_position_viewmats(viewmats: Tensor, viewmats_rs: Tensor) -> Tensor:
+    """View matrices [I | -c] whose camera position -R^T t is c, the mean of the positions of the two poses
+    (differentiable in both): the SH view direction of a rolling-shutter camera."""
+    def position(vm):
+        return -torch.einsum("...ji,...j->...i", vm[..., :3, :3], vm[..., :3, 3])
+
+    c = 0.5 * (position(viewmats) + position(viewmats_rs))
+    eye = torch.eye(3, device=viewmats.device, dtype=viewmats.dtype).expand(viewmats.shape[:-2] + (3, 3))
+    top = torch.cat([eye, -c[..., None]], dim=-1)
+    return torch.cat([top, viewmats[..., 3:, :].detach()], dim=-2)
+
+
 def spherical_harmonics_rows(
     degrees_to_use: int, means: Tensor, viewmats: Tensor, coeffs: Tensor, batch_ids: Tensor, camera_ids: Tensor,
     gaussian_ids: Tensor,
@@ -491,12 +504,15 @@ def spherical_harmonics(
     batch_ids: Optional[Tensor] = None,
     camera_ids: Optional[Tensor] = None,
     gaussian_ids: Optional[Tensor] = None,
-    viewmats_rs: Optional[Tensor] = None,
+    viewmats_rs: Optional[Tensor] = None,  # [..., C, 4, 4]
 ) -> Tensor:
     """Evaluates SH colours for view directions ``mean - camera_position`` (camera position recovered as
-    ``-R^T t``).  Returns [..., C, N, D]; masked-off rows are 0."""
+    ``-R^T t``).  Returns [..., C, N, D]; masked-off rows are 0.  With ``viewmats_rs`` (a rolling shutter's end-of-frame
+    poses) the camera position is the mean of the two poses' positions, and each pose gets half of its gradient."""
     if viewmats_rs is not None:
-        raise NotImplementedError("rolling-shutter view matrices are out of scope")
+        if tuple(viewmats_rs.shape) != tuple(viewmats.shape):
+            raise ValueError(f"viewmats_rs must be shaped like viewmats {tuple(viewmats.shape)}, got {tuple(viewmats_rs.shape)}")
+        viewmats = _mid_position_viewmats(viewmats, viewmats_rs)
     # the reference rejects these with TORCH_CHECK (RuntimeError), csrc/SphericalHarmonics.cpp
     if not (0 <= degrees_to_use <= 4):
         raise RuntimeError(f"degrees_to_use must be between 0 and 4, got {degrees_to_use}")
@@ -2550,7 +2566,7 @@ def adam(
 # --------------------------------------------------------------------------------------------
 # 3DGUT (reference wrappers gsplat/cuda/_wrapper.py: fully_fused_projection_with_ut, rasterize_to_pixels_eval3d): the
 # unscented-transform projection through a distorted pinhole or fisheye camera and the compositing that evaluates
-# each gaussian in 3-D along the pixel's ray.  Global shutter, dense rows, RendererConfig_MixedBatch.
+# each gaussian in 3-D along the pixel's ray.  Global or rolling shutter, dense rows, RendererConfig_MixedBatch.
 
 _UT_DEFAULTS = {"alpha": 0.1, "beta": 2.0, "kappa": 0.0, "in_image_margin_factor": 0.1, "require_all_sigma_points_valid": False}
 _UT_CAMERAS = {"pinhole": 0, "fisheye": 2}
@@ -2566,16 +2582,62 @@ def _ut_params(ut_params) -> tuple:
     return alpha, float(v["beta"]), kappa, float(v["in_image_margin_factor"]), bool(v["require_all_sigma_points_valid"])
 
 
+class RollingShutterType(enum.IntEnum):
+    """How a camera's sensor is exposed (the reference's RollingShutterType): row by row or column by column in the
+    given direction, each row or column at its own pose between ``viewmats`` and ``viewmats_rs``, or all at once."""
+
+    ROLLING_TOP_TO_BOTTOM = 0
+    ROLLING_LEFT_TO_RIGHT = 1
+    ROLLING_BOTTOM_TO_TOP = 2
+    ROLLING_RIGHT_TO_LEFT = 3
+    GLOBAL = 4
+
+
+def _shutter_type(rolling_shutter) -> RollingShutterType:
+    """The RollingShutterType of None (GLOBAL), of an int value, of any enum or object whose ``.name`` is a member's
+    name (this package's, the reference's), or of such a name as a string ("GLOBAL", "RollingShutterType.GLOBAL")."""
+    if rolling_shutter is None:
+        return RollingShutterType.GLOBAL
+    name = getattr(rolling_shutter, "name", None)
+    if name is None and isinstance(rolling_shutter, str):
+        name = rolling_shutter.rsplit(".", 1)[-1]
+    if name is not None:
+        if name in RollingShutterType.__members__:
+            return RollingShutterType[name]
+    elif isinstance(rolling_shutter, int) and rolling_shutter in set(RollingShutterType):
+        return RollingShutterType(rolling_shutter)
+    raise ValueError(f"unknown rolling_shutter {rolling_shutter!r}")
+
+
+def _ut_shutter(what, rolling_shutter, viewmats_rs, viewmats: Tensor, width: int, height: int):
+    """Checks the shutter arguments of the 3DGUT operators.  A rolling shutter needs ``viewmats_rs`` and the global one
+    takes none (NotImplementedError, naming the argument); a rolling shutter over a single row or column has no frame
+    time (ValueError).  Returns (shutter type id, viewmats_rs contiguous or None)."""
+    shutter = _shutter_type(rolling_shutter)
+    if shutter == RollingShutterType.GLOBAL:
+        if viewmats_rs is not None:
+            raise NotImplementedError(f"{what}: viewmats_rs is not supported with the global shutter (rolling_shutter=GLOBAL)")
+        return int(shutter), None
+    if viewmats_rs is None:
+        raise NotImplementedError(f"{what}: rolling_shutter={rolling_shutter!r} requires viewmats_rs, the end-of-frame poses")
+    _check_shape(viewmats_rs, tuple(viewmats.shape), "viewmats_rs")
+    if viewmats_rs.dtype != torch.float32:
+        raise TypeError(f"{what}: viewmats_rs must be float32, got {viewmats_rs.dtype}")
+    rows = shutter in (RollingShutterType.ROLLING_TOP_TO_BOTTOM, RollingShutterType.ROLLING_BOTTOM_TO_TOP)
+    if (height if rows else width) < 2:
+        raise ValueError(f"{what}: rolling_shutter={shutter.name} needs at least two image {'rows' if rows else 'columns'}, "
+                         f"got {width}x{height}")
+    return int(shutter), viewmats_rs.contiguous()
+
+
 def _ut_camera(what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
-               external_distortion_coeffs, rolling_shutter, viewmats_rs, cams: tuple):
+               external_distortion_coeffs, cams: tuple):
     """Rejects what the 3DGUT kernels are not built for (NotImplementedError, naming the argument) and checks the
     distortion coefficients.  Returns the camera model id and the coefficient tensors as [..., C, k] float32."""
     for name, v in (("ftheta_coeffs", ftheta_coeffs), ("lidar_coeffs", lidar_coeffs),
-                    ("external_distortion_coeffs", external_distortion_coeffs), ("viewmats_rs", viewmats_rs)):
+                    ("external_distortion_coeffs", external_distortion_coeffs)):
         if v is not None:
-            raise NotImplementedError(f"{what}: {name} is not supported (global-shutter pinhole / fisheye only)")
-    if int(rolling_shutter) != 4:
-        raise NotImplementedError(f"{what}: rolling_shutter={rolling_shutter!r} is not supported (GLOBAL only)")
+            raise NotImplementedError(f"{what}: {name} is not supported (pinhole / fisheye only)")
     if camera_model not in _UT_CAMERAS:
         if camera_model in ("ortho", "ftheta", "lidar"):
             raise NotImplementedError(f"{what}: camera_model={camera_model!r} is not supported (pinhole / fisheye only)")
@@ -2644,20 +2706,26 @@ def fully_fused_projection_with_ut(
     ``eps2d`` and culled as in ``fully_fused_projection``.  Returns (radii int32 [..., C, N, 2], means2d [..., C, N, 2],
     depths [..., C, N], conics [..., C, N, 3], compensations [..., C, N] or None); culled rows have radii 0 and zero
     floats.  Not differentiable, as in the reference.  ``ut_params``: any object with the fields of the reference's
-    UnscentedTransformParameters, or None for their defaults.  Global shutter, ``global_z_order=True`` only."""
+    UnscentedTransformParameters, or None for their defaults.  ``global_z_order=True`` only.
+
+    Rolling shutter: ``rolling_shutter`` (a RollingShutterType or its value) other than GLOBAL with ``viewmats_rs``
+    [..., C, 4, 4], the end-of-frame poses.  Each sigma point is projected at the pose of the image row or column it
+    lands in (translation lerp and rotation slerp between the two poses at that row's or column's frame time, iterated
+    up to 10 times from the start pose's projection); the depths and the near / far cull take the mid-frame pose."""
     what = "fully_fused_projection_with_ut"
     if not global_z_order:
         raise NotImplementedError(f"{what}: global_z_order=False is not supported")
     batch, C, N = _ut_geometry(what, means, quats, scales, viewmats, Ks)
     cam, radial, tangential, thin = _ut_camera(
         what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
-        external_distortion_coeffs, rolling_shutter, viewmats_rs, batch + (C,),
+        external_distortion_coeffs, batch + (C,),
     )
+    shutter, viewmats_rs = _ut_shutter(what, rolling_shutter, viewmats_rs, viewmats, width, height)
     if opacities is not None:
         _check_shape(opacities, batch + (N,), "opacities")
         opacities = f32c(opacities, "opacities")
     alpha, beta, kappa, margin, require_all = _ut_params(ut_params)
-    dev = require_cuda(means, quats, scales, viewmats, Ks, opacities, radial, tangential, thin)
+    dev = require_cuda(means, quats, scales, viewmats, Ks, opacities, radial, tangential, thin, viewmats_rs)
     means, quats, scales, viewmats, Ks = (t.contiguous() for t in (means, quats, scales, viewmats, Ks))
     B = _prod(batch)
     o = dict(device=dev, dtype=torch.float32)
@@ -2670,7 +2738,8 @@ def fully_fused_projection_with_ut(
         check(
             lib().gsb200_ut_projection_fwd(
                 B, C, N, ptr(means), ptr(quats), ptr(scales), ptr(opacities), ptr(viewmats), ptr(Ks), cam, ptr(radial),
-                ptr(tangential), ptr(thin), int(width), int(height), float(eps2d), float(near_plane), float(far_plane),
+                ptr(tangential), ptr(thin), ptr(viewmats_rs), shutter, int(width), int(height), float(eps2d),
+                float(near_plane), float(far_plane),
                 float(radius_clip), alpha, beta, kappa, margin, int(require_all), ptr(radii), ptr(means2d), ptr(depths),
                 ptr(conics), ptr(comps), st,
             ),
@@ -2682,7 +2751,7 @@ def fully_fused_projection_with_ut(
 class _RasterizeToPixelsEval3D(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, radial, tangential,
-                thin, width, height, isect_offsets, flatten_ids):
+                thin, viewmats_rs, shutter, width, height, isect_offsets, flatten_ids):
         dev = require_cuda(means, quats, scales, colors, opacities, viewmats, Ks)
         means, quats, scales = means.contiguous(), quats.contiguous(), scales.contiguous()
         colors, opacities = f32c(colors, "colors"), f32c(opacities, "opacities")
@@ -2712,23 +2781,24 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
                 check(
                     lib().gsb200_eval3d_fwd(
                         B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds),
-                        ptr(m8), ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), width, height, 16,
-                        tw, th, ptr(offsets), ptr(fl), S, ptr(render_colors), ptr(render_alphas), ptr(last_ids), st,
+                        ptr(m8), ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), ptr(viewmats_rs),
+                        shutter, width, height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_colors),
+                        ptr(render_alphas), ptr(last_ids), st,
                     ),
                     "rasterize_to_pixels_eval3d",
                 )
         ctx.save_for_backward(means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, radial, tangential, thin,
-                              offsets, fl, render_alphas, last_ids)
+                              viewmats_rs, offsets, fl, render_alphas, last_ids)
         ctx.set_materialize_grads(False)
-        ctx.meta = (B, C, N, D, cam, width, height, tw, th, S)
+        ctx.meta = (B, C, N, D, cam, shutter, width, height, tw, th, S)
         ctx.mark_non_differentiable(last_ids)
         return render_colors, render_alphas
 
     @staticmethod
     def backward(ctx, v_render_colors, v_render_alphas):
-        (means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, radial, tangential, thin, offsets, fl,
-         render_alphas, last_ids) = ctx.saved_tensors
-        B, C, N, D, cam, width, height, tw, th, S = ctx.meta
+        (means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, radial, tangential, thin, viewmats_rs,
+         offsets, fl, render_alphas, last_ids) = ctx.saved_tensors
+        B, C, N, D, cam, shutter, width, height, tw, th, S = ctx.meta
         dev = render_alphas.device
         if v_render_colors is None:
             v_render_colors = torch.zeros(render_alphas.shape[:-1] + (D,), device=dev, dtype=torch.float32)
@@ -2741,8 +2811,9 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
             check(
                 lib().gsb200_eval3d_bwd(
                     B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds), ptr(m8),
-                    ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), width, height, 16, tw, th,
-                    ptr(offsets), ptr(fl), S, ptr(render_alphas), ptr(last_ids), ptr(v_render_colors), ptr(v_render_alphas),
+                    ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), ptr(viewmats_rs), shutter, width,
+                    height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_alphas), ptr(last_ids), ptr(v_render_colors),
+                    ptr(v_render_alphas),
                     ptr(records), ptr(v_colors), ptr(v_opacities), ptr(v_means), ptr(v_quats), ptr(v_scales), st,
                 ),
                 "rasterize_to_pixels_eval3d_bwd",
@@ -2750,8 +2821,8 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
         v_backgrounds = None
         if backgrounds is not None and ctx.needs_input_grad[5]:
             v_backgrounds = (v_render_colors * (1.0 - render_alphas)).sum(dim=(-3, -2))
-        # viewmats, Ks and the camera coefficients get no gradient, as in the reference's backward
-        return (v_means, v_quats, v_scales, v_colors, v_opacities, v_backgrounds) + (None,) * 11
+        # viewmats, viewmats_rs, Ks and the camera coefficients get no gradient, as in the reference's backward
+        return (v_means, v_quats, v_scales, v_colors, v_opacities, v_backgrounds) + (None,) * 13
 
 
 def rasterize_to_pixels_eval3d(
@@ -2789,8 +2860,11 @@ def rasterize_to_pixels_eval3d(
     maximum response along the ray times the opacity is the alpha (min 0.99, skipped below 1/255, stop at T <= 1e-4).
     Returns (render_colors [..., C, H, W, channels], render_alphas [..., C, H, W, 1]).  Differentiable in means, quats,
     scales, colors, opacities and backgrounds; viewmats get no gradient, as in the reference.  ``ut_params`` is accepted
-    for the reference's signature and does not enter the compositing.  Dense rows, global shutter, the MixedBatch
-    renderer only."""
+    for the reference's signature and does not enter the compositing.  Dense rows, the MixedBatch renderer only.
+
+    Rolling shutter (``rolling_shutter`` other than GLOBAL with the end-of-frame poses ``viewmats_rs``): the ray of each
+    pixel leaves the camera at the pose of the pixel's row or column (translation lerp and rotation slerp between
+    ``viewmats`` and ``viewmats_rs`` at its frame time).  viewmats_rs gets no gradient either."""
     what = "rasterize_to_pixels_eval3d"
     for name, v in (("rays", rays),):
         if v is not None:
@@ -2809,8 +2883,9 @@ def rasterize_to_pixels_eval3d(
     image_dims = batch + (C,)
     cam, radial, tangential, thin = _ut_camera(
         what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
-        external_distortion_coeffs, rolling_shutter, viewmats_rs, image_dims,
+        external_distortion_coeffs, image_dims,
     )
+    shutter, viewmats_rs = _ut_shutter(what, rolling_shutter, viewmats_rs, viewmats, image_width, image_height)
     _ut_params(ut_params)
     if colors.dim() != len(image_dims) + 2:
         raise ValueError(f"{what}: colors must be [..., C, N, channels], got {tuple(colors.shape)}")
@@ -2834,8 +2909,8 @@ def rasterize_to_pixels_eval3d(
     if D not in _SUPPORTED_CHANNELS:
         raise NotImplementedError(f"{what}: {D} channels; the eval3d kernels are built for {_SUPPORTED_CHANNELS}")
     require_cuda(means, quats, scales, colors, opacities, viewmats, Ks, backgrounds, masks, isect_offsets, flatten_ids,
-                 radial, tangential, thin)
+                 radial, tangential, thin, viewmats_rs)
     return _RasterizeToPixelsEval3D.apply(
         means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, radial, tangential, thin,
-        int(image_width), int(image_height), isect_offsets, flatten_ids,
+        viewmats_rs, shutter, int(image_width), int(image_height), isect_offsets, flatten_ids,
     )

@@ -29,7 +29,9 @@ from torch import Tensor
 
 from .ops import (
     _SUPPORTED_CHANNELS,
+    _shutter_type,
     _ut_params,
+    RollingShutterType,
     RowSideOutputs,
     fully_fused_projection,
     fully_fused_projection_2dgs,
@@ -123,15 +125,15 @@ def _check_colors(colors, sh_degree, batch_dims, C, N):
             raise ValueError(f"sh_degree={sh_degree} needs K >= {(sh_degree + 1) ** 2}, got {colors.shape[-2]}")
 
 
-def _color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N):
+def _color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N, viewmats_rs=None):
     """[..., C, N, D] features of the dense rows: the post-activation colours broadcast over the cameras, or the SH
-    colours evaluated for every visible row."""
+    colours evaluated for every visible row (seen from the mean of the two poses' positions with ``viewmats_rs``)."""
     if sh_degree is None:
         if colors.dim() == len(batch_dims) + 2:
             return torch.broadcast_to(colors[..., None, :, :], batch_dims + (C, N, colors.shape[-1]))
         return colors
     valid = (radii > 0).all(dim=-1)
-    feat = spherical_harmonics(sh_degree, means, viewmats, colors, masks=valid)
+    feat = spherical_harmonics(sh_degree, means, viewmats, colors, masks=valid, viewmats_rs=viewmats_rs)
     return torch.clamp_min(feat + 0.5, 0.0)
 
 
@@ -267,8 +269,8 @@ def rasterization(
         _unsupported(f"renderer_config={type(renderer_config).__name__}", "eval3d renderer variants are out of scope")
     if return_normals:
         _unsupported("return_normals")
-    if rolling_shutter is not None and getattr(rolling_shutter, "name", str(rolling_shutter)) not in ("GLOBAL", "RollingShutterType.GLOBAL"):
-        _unsupported("rolling_shutter")
+    if _shutter_type(rolling_shutter) != RollingShutterType.GLOBAL:
+        _unsupported("rolling_shutter", "a rolling shutter is built for 3DGUT (with_ut=True, with_eval3d=True)")
     if camera_model not in ("pinhole", "ortho", "fisheye"):
         _unsupported(f"camera_model={camera_model!r}", "the EWA projection is built for pinhole / ortho / fisheye")
     if render_mode not in _ALL_MODES:
@@ -500,16 +502,6 @@ def rasterization(
     return render_colors, render_alphas, meta
 
 
-def _global_shutter(rolling_shutter) -> bool:
-    """None, the reference's RollingShutterType.GLOBAL, or its value 4."""
-    if rolling_shutter is None or rolling_shutter in ("GLOBAL", "RollingShutterType.GLOBAL"):
-        return True
-    name = getattr(rolling_shutter, "name", None)
-    if name is not None:
-        return name == "GLOBAL"
-    return isinstance(rolling_shutter, int) and rolling_shutter == 4
-
-
 def _rasterization_3dgut(
     means, quats, scales, opacities, colors, viewmats, Ks, width, height, near_plane, far_plane, radius_clip, eps2d,
     sh_degree, packed, tile_size, backgrounds, render_mode, sparse_grad, rasterize_mode, channel_chunk, distributed,
@@ -555,13 +547,15 @@ def _rasterization_3dgut(
         _unsupported("return_normals", "normals are not built for 3DGUT")
     for name, val in (
         ("rays", rays), ("ftheta_coeffs", ftheta_coeffs), ("lidar_coeffs", lidar_coeffs),
-        ("external_distortion_coeffs", external_distortion_coeffs), ("viewmats_rs", viewmats_rs),
-        ("extra_signals", extra_signals),
+        ("external_distortion_coeffs", external_distortion_coeffs), ("extra_signals", extra_signals),
     ):
         if val is not None:
-            _unsupported(name, "not built for 3DGUT (global-shutter pinhole / fisheye cameras, colour and depth channels)")
-    if not _global_shutter(rolling_shutter):
-        _unsupported(f"rolling_shutter={rolling_shutter!r}", "3DGUT is built for the global shutter only")
+            _unsupported(name, "not built for 3DGUT (pinhole / fisheye cameras, colour and depth channels)")
+    shutter = _shutter_type(rolling_shutter)
+    if shutter == RollingShutterType.GLOBAL and viewmats_rs is not None:
+        _unsupported("viewmats_rs", "the end-of-frame poses belong to a rolling shutter (rolling_shutter=GLOBAL)")
+    if shutter != RollingShutterType.GLOBAL and viewmats_rs is None:
+        _unsupported(f"rolling_shutter={rolling_shutter!r}", "a rolling shutter requires viewmats_rs, the end-of-frame poses")
     if camera_model not in ("pinhole", "fisheye"):
         if camera_model in ("ortho", "ftheta", "lidar"):
             _unsupported(f"camera_model={camera_model!r}", "3DGUT is built for pinhole / fisheye cameras")
@@ -588,6 +582,12 @@ def _rasterization_3dgut(
         raise ValueError(f"opacities must be [..., N], got {tuple(opacities.shape)}")
     if tuple(viewmats.shape) != batch_dims + (C, 4, 4) or tuple(Ks.shape) != batch_dims + (C, 3, 3):
         raise ValueError(f"viewmats/Ks shape mismatch: {tuple(viewmats.shape)}, {tuple(Ks.shape)}")
+    if viewmats_rs is not None and tuple(viewmats_rs.shape) != tuple(viewmats.shape):
+        raise ValueError(f"viewmats_rs must be {tuple(viewmats.shape)}, got {tuple(viewmats_rs.shape)}")
+    rows = shutter in (RollingShutterType.ROLLING_TOP_TO_BOTTOM, RollingShutterType.ROLLING_BOTTOM_TO_TOP)
+    if shutter != RollingShutterType.GLOBAL and (height if rows else width) < 2:
+        raise ValueError(f"rolling_shutter={shutter.name} needs at least two image {'rows' if rows else 'columns'}, "
+                         f"got {width}x{height}")
     n_ch = int(has_depth)
     if has_color:
         if colors is None:
@@ -606,14 +606,17 @@ def _rasterization_3dgut(
         )
     _ut_params(ut_params)
     cams = dict(camera_model=camera_model, radial_coeffs=radial_coeffs, tangential_coeffs=tangential_coeffs,
-                thin_prism_coeffs=thin_prism_coeffs)
+                thin_prism_coeffs=thin_prism_coeffs, rolling_shutter=int(shutter),
+                viewmats_rs=None if viewmats_rs is None else viewmats_rs.detach())
 
     # ---- projection through the camera model (no gradient, as in the reference)
     radii, means2d, depths, conics, _ = fully_fused_projection_with_ut(
         means, quats, scales, opacities, viewmats, Ks, width, height, eps2d=eps2d, near_plane=near_plane,
         far_plane=far_plane, radius_clip=radius_clip, calc_compensations=False, ut_params=ut_params, **cams,
     )
-    feat = _color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N) if has_color else None
+    # the SH view directions are the only path by which viewmats (and viewmats_rs) get a gradient
+    feat = (_color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N, viewmats_rs=viewmats_rs)
+            if has_color else None)
     feat, backgrounds = _with_depth_channel(feat, depths, backgrounds, has_color, has_depth, batch_dims, C)
     opac = torch.broadcast_to(opacities[..., None, :], batch_dims + (C, N))
 

@@ -539,16 +539,21 @@ extern "C"
 
     /* ---- 3DGUT (csrc/ut.cu): camera_model 0 pinhole (OpenCV: radial [B*C, 6], tangential [B*C, 2], thin prism
      * [B*C, 4], each optional; none at all is the perfect pinhole) or 2 fisheye (OpenCV: radial [B*C, 4] optional, the
-     * other two must be NULL); any other model is GSB200_E_UNSUPPORTED.  Global shutter.
+     * other two must be NULL); any other model is GSB200_E_UNSUPPORTED.
+     * Shutter: viewmats_rs NULL with rolling_shutter 4 is the global shutter (the pose of viewmats).  viewmats_rs
+     * [B*C, 4, 4] (the end-of-frame pose) with rolling_shutter 0 top to bottom, 1 left to right, 2 bottom to top or 3
+     * right to left exposes each image row or column at the pose interpolated between the two (translation lerp,
+     * rotation slerp) at its relative frame time.  Any other pairing, or a rolling shutter over a single row / column,
+     * is GSB200_E_INVALID.  The projection takes the mid-frame pose for the depths and the near / far cull.
      * UT projection: the rows of gsb200_projection_fwd (radii int32 [B,C,N,2], means2d, depths, conics, compensations or
      * NULL), culled rows radii 0 and zero floats; opacities [B,N] or NULL.  alpha^2 * (3 + kappa) must be > 0. */
     int gsb200_ut_projection_fwd(
         int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
         const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-        const float *thin_prism_coeffs, uint32_t image_width, uint32_t image_height, float eps2d, float near_plane,
-        float far_plane, float radius_clip, float ut_alpha, float ut_beta, float ut_kappa, float ut_in_image_margin_factor,
-        int ut_require_all_sigma_points_valid, int32_t *radii, float *means2d, float *depths, float *conics,
-        float *compensations, void *stream
+        const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
+        uint32_t image_height, float eps2d, float near_plane, float far_plane, float radius_clip, float ut_alpha, float ut_beta,
+        float ut_kappa, float ut_in_image_margin_factor, int ut_require_all_sigma_points_valid, int32_t *radii,
+        float *means2d, float *depths, float *conics, float *compensations, void *stream
     );
     /* Compositing with each gaussian evaluated in 3-D along the pixel's world ray: means/quats/scales [B,N,*], colors
      * [B*C, N, D], opacities [B*C, N], backgrounds [B*C, D] or NULL, masks [B*C, th, tw] or NULL, the lists of
@@ -559,18 +564,20 @@ extern "C"
         int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
         const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
         const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-        const float *thin_prism_coeffs, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
-        uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, float *render_colors,
-        float *render_alphas, int32_t *last_ids, void *stream
+        const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
+        uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+        const int32_t *flatten_ids, int64_t n_isects, float *render_colors, float *render_alphas, int32_t *last_ids,
+        void *stream
     );
     int gsb200_eval3d_bwd(
         int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
         const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
         const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-        const float *thin_prism_coeffs, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
-        uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, const float *render_alphas,
-        const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas, float *grad_records,
-        float *v_colors, float *v_opacities, float *v_means, float *v_quats, float *v_scales, void *stream
+        const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
+        uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
+        const int32_t *flatten_ids, int64_t n_isects, const float *render_alphas, const int32_t *last_ids,
+        const float *v_render_colors, const float *v_render_alphas, float *grad_records, float *v_colors, float *v_opacities,
+        float *v_means, float *v_quats, float *v_scales, void *stream
     );
 
     /* ---- MCMC strategy ops ("next" row): relocation (ext.cpp `relocation`, gsplat/relocation.py:64,

@@ -4,11 +4,16 @@ forward and backward) next to the EWA step (fully_fused_projection + the same li
 backward) on bench.py's scene (1M Gaussians, one 1920x1080 view) with a pinhole camera.  Median of --steps timed steps after --warmup, CUDA events; prints
 the device name and power limit with the numbers, as one JSON line.
 
-    python tools/bench_ut.py [--steps 20] [--warmup 5] [--distorted] [--rasterization]
+    python tools/bench_ut.py [--steps 20] [--warmup 5] [--distorted] [--rasterization] [--rolling-shutter]
 
 --rasterization times the public call instead: rasterization(with_ut=True, with_eval3d=True, sh_degree=3,
 packed=False) forward and backward on the same scene with SH degree 3, next to the same operators chained by hand, and
 reports the difference as the public call's overhead.
+
+--rolling-shutter times the rolling-shutter step (top to bottom; the end pose is the start pose turned by 2 degrees and
+moved by 0.03) next to the global-shutter step on the same scene, alternated step by step: the operator chain, or with
+--rasterization the public call.  It also times the UT projection alone under both shutters and reports its share of
+each step.
 """
 import argparse
 import json
@@ -33,8 +38,12 @@ def main():
     ap.add_argument("--distorted", action="store_true", help="pinhole with radial and tangential coefficients")
     ap.add_argument("--rasterization", action="store_true",
                     help="time rasterization(with_ut=True, with_eval3d=True, sh_degree=3) next to the hand-chained operators")
+    ap.add_argument("--rolling-shutter", action="store_true",
+                    help="time the rolling-shutter step next to the global-shutter step")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_ut needs a GPU"
+    if a.rolling_shutter:
+        return bench_rolling_shutter(a)
     if a.rasterization:
         return bench_rasterization(a)
     dev = "cuda"
@@ -138,6 +147,84 @@ def bench_rasterization(a):
     res = {name: {"median_ms": float(np.median(v)), "min_ms": float(np.min(v)), "n_isects": int(n[name])} for name, v in times.items()}
     res["overhead_ms"] = res["rasterization"]["median_ms"] - res["hand_chain"]["median_ms"]
     res.update(_device_info(), gaussians=int(N), width=W, height=H, sh_degree=3, distorted=a.distorted, steps=a.steps)
+    print(json.dumps(res))
+
+
+def _end_pose(vm: torch.Tensor, degrees=2.0, shift=0.03) -> torch.Tensor:
+    """vm [C, 4, 4] turned by `degrees` about a fixed axis and moved by `shift` in the camera frame."""
+    axis = torch.tensor([0.3, 0.8, -0.5], dtype=torch.float64)
+    axis = axis / axis.norm()
+    k = torch.tensor([[0, -axis[2], axis[1]], [axis[2], 0, -axis[0]], [-axis[1], axis[0], 0]], dtype=torch.float64)
+    th = torch.tensor(degrees, dtype=torch.float64).deg2rad()
+    delta = torch.eye(4, dtype=torch.float64)
+    delta[:3, :3] = torch.eye(3, dtype=torch.float64) + torch.sin(th) * k + (1 - torch.cos(th)) * (k @ k)
+    delta[:3, 3] = shift * axis
+    return (delta.to(vm.device) @ vm.double()).float().contiguous()
+
+
+def _time(fns, steps, warmup):
+    """Median and min ms of each fn, alternated step by step; its last return value."""
+    for fn in fns.values():
+        for _ in range(warmup):
+            fn()
+    torch.cuda.synchronize()
+    times, n = {k: [] for k in fns}, {}
+    for _ in range(steps):
+        for name, fn in fns.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            n[name] = fn()
+            e1.record()
+            torch.cuda.synchronize()
+            times[name].append(e0.elapsed_time(e1))
+    return {name: {"median_ms": float(np.median(v)), "min_ms": float(np.min(v)), "out": n[name]} for name, v in times.items()}
+
+
+def bench_rolling_shutter(a):
+    dev = "cuda"
+    sc = scene.make_scene(scene_grid=3, sh_degree=3 if a.rasterization else 0)
+    W, H = 1920, 1080
+    t = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)  # noqa: E731
+    means, quats, scales = (t(sc[k]).requires_grad_(True) for k in ("means", "quats", "scales"))
+    opac = t(sc["opacities"]).requires_grad_(True)
+    colors = t(sc["sh"] if a.rasterization else sc["colors"][None]).requires_grad_(True)
+    vm, K = t(sc["viewmats"][:1]), t(scene.rescale_K(sc["Ks"], sc["width"], sc["height"], W, H)[:1])
+    vm_rs = _end_pose(vm)
+    co = dict(radial_coeffs=t(np.float32([[0.05, -0.02, 0.0, 0.0, 0.0, 0.0]])), tangential_coeffs=t(np.float32([[0.001, -0.001]]))) if a.distorted else {}
+    shutters = {"global": {}, "rolling": dict(rolling_shutter=gs.RollingShutterType.ROLLING_TOP_TO_BOTTOM, viewmats_rs=vm_rs)}
+    tw, th = (W + 15) // 16, (H + 15) // 16
+    N = means.shape[0]
+
+    def step(rs):
+        if a.rasterization:
+            rc, ra, meta = gs.rasterization(means, quats, scales, opac, colors, vm, K, W, H, sh_degree=3, packed=False,
+                                            with_ut=True, with_eval3d=True, **co, **rs)
+            fl = meta["flatten_ids"]
+        else:
+            r, m2, d, _, _ = gs.fully_fused_projection_with_ut(means.detach(), quats.detach(), scales.detach(), opac.detach(), vm,
+                                                              K, W, H, **co, **rs)
+            _, ii, fl = gs.isect_tiles(m2, r, d, 16, tw, th)
+            offs = gs.isect_offset_encode(ii, 1, tw, th)
+            o = torch.broadcast_to(opac[None], (1, N))
+            rc, ra = gs.rasterize_to_pixels_eval3d(means, quats, scales, colors, o, vm, K, W, H, 16, offs, fl, **co, **rs)
+        (rc.sum() + ra.sum()).backward()
+        return fl.numel()
+
+    def projection(rs):
+        gs.fully_fused_projection_with_ut(means.detach(), quats.detach(), scales.detach(), opac.detach(), vm, K, W, H, **co, **rs)
+        return 0
+
+    fns = {f"{k}_step": (lambda rs=rs: step(rs)) for k, rs in shutters.items()}
+    fns.update({f"{k}_projection": (lambda rs=rs: projection(rs)) for k, rs in shutters.items()})
+    r = _time(fns, a.steps, a.warmup)
+    res = {}
+    for k in shutters:
+        s, p = r[f"{k}_step"], r[f"{k}_projection"]
+        res[k] = {"step_median_ms": s["median_ms"], "step_min_ms": s["min_ms"], "n_isects": int(s["out"]),
+                  "projection_median_ms": p["median_ms"], "projection_share": p["median_ms"] / s["median_ms"]}
+    res["rolling_over_global"] = res["rolling"]["step_median_ms"] / res["global"]["step_median_ms"]
+    res.update(_device_info(), gaussians=int(N), width=W, height=H, rasterization=a.rasterization, distorted=a.distorted,
+               shutter="ROLLING_TOP_TO_BOTTOM", steps=a.steps)
     print(json.dumps(res))
 
 
