@@ -16,6 +16,8 @@ their alphas equal its render_alphas bit for bit).  Importing the package does n
 operator does (and needs gsplat_b200/libgsplat_b200.so, built by ``python -m gsplat_b200.build``).
 """
 from .ops import (  # noqa: F401
+    FThetaCameraDistortionParameters,
+    FThetaPolynomialType,
     RollingShutterType,
     adam,
     build_sparse_tile_layout,
@@ -79,11 +81,12 @@ def has_2dgs() -> bool:
 
 
 def has_3dgut() -> bool:
-    """Reference: _wrapper.py has_3dgut -- False.  In the reference this flag gates 3DGUT tests that need ftheta and lidar
-    cameras, hit-distance modes and tile_size 8, none of which is built here.  What is built:
+    """Reference: _wrapper.py has_3dgut -- False.  In the reference this flag gates 3DGUT tests that need lidar cameras,
+    hit-distance modes and tile_size 8, none of which is built here.  What is built:
     ``rasterization(with_ut=True, with_eval3d=True)`` with dense rows, and the two 3DGUT operators it runs on,
-    ``fully_fused_projection_with_ut`` and ``rasterize_to_pixels_eval3d`` (distorted pinhole and fisheye cameras, global
-    or rolling shutter: ``rolling_shutter`` with the end-of-frame poses ``viewmats_rs``), which also chain with
+    ``fully_fused_projection_with_ut`` and ``rasterize_to_pixels_eval3d`` (distorted pinhole, fisheye and FTheta cameras,
+    the FTheta ones also in the Euclidean depth order ``global_z_order=False``; global or rolling shutter:
+    ``rolling_shutter`` with the end-of-frame poses ``viewmats_rs``), which also chain with
     ``isect_tiles`` / ``isect_offset_encode`` as in the reference's ``_rasterization``."""
     return False
 
@@ -105,6 +108,8 @@ __all__ = [
     "fused_project_sh",
     "spherical_harmonics",
     "RollingShutterType",
+    "FThetaPolynomialType",
+    "FThetaCameraDistortionParameters",
     "isect_tiles",
     "isect_offset_encode",
     "rasterize_to_pixels",

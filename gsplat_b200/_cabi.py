@@ -25,6 +25,18 @@ c_i64, c_u32, c_int, c_f32, c_vp, c_sz = (
     ctypes.c_size_t,
 )
 
+class FThetaParams(ctypes.Structure):
+    """gsb200_ftheta_params of include/gsplat_b200.h: the FTheta camera parameters of the 3DGUT entry points."""
+
+    _fields_ = [
+        ("reference_poly", ctypes.c_int),
+        ("pixeldist_to_angle_poly", ctypes.c_float * 6),
+        ("angle_to_pixeldist_poly", ctypes.c_float * 6),
+        ("max_angle", ctypes.c_float),
+        ("linear_cde", ctypes.c_float * 3),
+    ]
+
+
 # name -> (restype, argtypes) ; mirrors include/gsplat_b200.h one to one
 _SIGNATURES = {
     "gsb200_version": (ctypes.c_char_p, []),
@@ -211,18 +223,18 @@ _SIGNATURES = {
     ),
     "gsb200_ut_projection_fwd": (
         c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_u32, c_u32, c_f32,
-         c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_u32,
+         c_u32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     ),
     "gsb200_eval3d_fwd": (
         c_int,
         [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
-         c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp],
+         c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp],
     ),
     "gsb200_eval3d_bwd": (
         c_int,
         [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
-         c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+         c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
          c_vp, c_vp],
     ),
 }

@@ -109,7 +109,8 @@ __device__ __forceinline__ CamModel load_cam_model(
     return m;
 }
 
-__device__ __forceinline__ bool in_margin(const CamModel &m, float u, float v, float margin)
+template<class Model>
+__device__ __forceinline__ bool in_margin(const Model &m, float u, float v, float margin)
 {
     const float mx = (float)m.W * margin, my = (float)m.H * margin;
     return -mx <= u && u < (float)m.W + mx && -my <= v && v < (float)m.H + my;
@@ -249,6 +250,151 @@ __device__ __forceinline__ bool cam_unproject(const CamModel &m, float u, float 
     return true;
 }
 
+// ------------------------------------------------------------------ FTheta
+// Reference semantics: include/Cameras.cuh (FThetaCameraModel with 3 Newton steps).  The image radius delta of a ray at
+// angle theta from the optical axis is given by two polynomials of degree 5 calibrated together: the forward one
+// (angle to pixel distance) and the backward one (pixel distance to angle).  The reference polynomial is evaluated
+// directly, the other direction inverts it by Newton steps that start from the other polynomial.  A linear map
+// [[c, d], [e, 1]] takes the radial offset to the image, about the principal point Ks (cx, cy) + 0.5: FTheta's image
+// origin is the centre of the first pixel.  The parameters are shared by every camera of a call.
+constexpr int kUtFTheta           = 3;
+constexpr int kFThetaPixelToAngle = 0; // reference_poly: the backward polynomial is the reference
+constexpr int kFThetaAngleToPixel = 1; // the forward one is
+constexpr int kFThetaNewtonSteps  = 3;
+
+struct FThetaModel
+{
+    float bw[6], fw[6]; // backward (pixel distance -> angle), forward (angle -> pixel distance)
+    float dref[5];      // derivative of the reference polynomial
+    float max_angle, c, d, e, cx, cy;
+    uint32_t W, H;
+    int reference_poly;
+};
+
+__device__ __forceinline__ float poly6(const float *k, float x)
+{
+    return k[0] + x * (k[1] + x * (k[2] + x * (k[3] + x * (k[4] + x * k[5]))));
+}
+__device__ __forceinline__ float poly5(const float *k, float x)
+{
+    return k[0] + x * (k[1] + x * (k[2] + x * (k[3] + x * k[4])));
+}
+
+// x with ref(x) = y: kFThetaNewtonSteps Newton steps on the reference polynomial from approx(y), stopping early once a
+// step is below 1e-6 (converged).
+__device__ __forceinline__ float ftheta_newton(const float *ref, const float *dref, const float *approx, float y, bool &converged)
+{
+    float x   = poly6(approx, y);
+    converged = false;
+#pragma unroll
+    for(int it = 0; it < kFThetaNewtonSteps; ++it)
+    {
+        const float dx = (poly6(ref, x) - y) / poly5(dref, x);
+        x -= dx;
+        if(fabsf(dx) < 1e-6f)
+        {
+            converged = true;
+            break;
+        }
+    }
+    return x;
+}
+
+// Camera-frame point -> image point.  No z <= 0 guard: a calibration with max_angle > pi/2 images points behind the
+// camera plane.  Beyond max_angle the angle is clamped and the point is invalid; its image point is still set.  The
+// forward direction ignores the Newton convergence flag: float32 rounding keeps the last step near 1e-5 pixel for
+// typical calibrations, while delta is accurate.
+__device__ __forceinline__ bool cam_project(const FThetaModel &m, const float *pc, float margin, float &u, float &v)
+{
+    const float ax = fabsf(pc[0]), ay = fabsf(pc[1]);
+    const float lo = fminf(ax, ay), hi = fmaxf(ax, ay);
+    float rxy = 0.f;
+    if(hi > 0.f)
+    {
+        const float q = lo / hi;
+        rxy = hi * sqrtf(1.f + q * q);
+    }
+    if(rxy <= 0.f)
+        rxy = FLT_EPSILON;
+    const float th_full = atan2f(rxy, pc[2]);
+    const float th      = th_full < m.max_angle ? th_full : m.max_angle;
+    bool converged;
+    const float delta = m.reference_poly == kFThetaAngleToPixel ? poly6(m.fw, th) : ftheta_newton(m.bw, m.dref, m.fw, th, converged);
+    const float ix = delta * (pc[0] / rxy), iy = delta * (pc[1] / rxy);
+    u = m.c * ix + m.d * iy + m.cx;
+    v = m.e * ix + iy + m.cy;
+    return in_margin(m, u, v, margin) && th_full < m.max_angle;
+}
+
+// Image point -> unit camera ray.  false: the linear map is singular, or the Newton inversion of the forward polynomial
+// did not converge; such a pixel composites nothing.
+__device__ __forceinline__ bool cam_unproject(const FThetaModel &m, float u, float v, float *dir)
+{
+    dir[0] = 0.f, dir[1] = 0.f, dir[2] = 1.f;
+    const float x = u - m.cx, y = v - m.cy;
+    const float det = m.c - m.e * m.d;
+    if(fabsf(det) < 1e-8f)
+        return false;
+    const float ux = (x - m.d * y) / det, uy = (-m.e * x + m.c * y) / det;
+    const float delta = sqrtf(ux * ux + uy * uy);
+    float theta;
+    if(m.reference_poly == kFThetaPixelToAngle)
+        theta = poly6(m.bw, delta);
+    else
+    {
+        bool converged;
+        theta = ftheta_newton(m.fw, m.dref, m.bw, delta, converged);
+        if(!converged)
+            return false;
+    }
+    if(delta >= 1e-6f)
+    {
+        const float sc = sinf(theta) / delta;
+        dir[0] = sc * ux, dir[1] = sc * uy, dir[2] = cosf(theta);
+    }
+    return true;
+}
+
+// ------------------------------------------------------------------ lens policies
+// The kernels' camera model is a compile-time policy: CamLens is the runtime OpenCV pinhole / fisheye CamModel (loaded
+// from the per-camera coefficient arrays), FThetaLens carries the shared FTheta parameters by value.
+struct CamLens
+{
+    static constexpr bool kFTheta = false;
+    __device__ __forceinline__ CamModel model(
+        int kind, const float *K, const float *radial, const float *tangential, const float *thin, int64_t cam, uint32_t W,
+        uint32_t H
+    ) const
+    {
+        return load_cam_model(kind, K, radial, tangential, thin, cam, W, H);
+    }
+};
+struct FThetaLens
+{
+    static constexpr bool kFTheta = true;
+    gsb200_ftheta_params p;
+    int global_z_order; // 0: the projection culls and orders on the distance |mean_c|, not on z
+    __device__ __forceinline__ FThetaModel model(
+        int, const float *K, const float *, const float *, const float *, int64_t cam, uint32_t W, uint32_t H
+    ) const
+    {
+        FThetaModel m;
+#pragma unroll
+        for(int i = 0; i < 6; ++i)
+            m.bw[i] = p.pixeldist_to_angle_poly[i], m.fw[i] = p.angle_to_pixeldist_poly[i];
+        const bool bw_ref = p.reference_poly == kFThetaPixelToAngle;
+#pragma unroll
+        for(int i = 0; i < 5; ++i)
+            m.dref[i] = (float)(i + 1) * (bw_ref ? m.bw[i + 1] : m.fw[i + 1]);
+        m.max_angle = p.max_angle;
+        m.c = p.linear_cde[0], m.d = p.linear_cde[1], m.e = p.linear_cde[2];
+        m.cx = K[cam * 9 + 2] + 0.5f, m.cy = K[cam * 9 + 5] + 0.5f;
+        m.W = W, m.H = H;
+        m.reference_poly = p.reference_poly;
+        return m;
+    }
+};
+
 // ------------------------------------------------------------------ rolling shutter
 // Reference semantics: include/Cameras.cuh (RollingShutterParameters, interpolate_shutter_pose,
 // shutter_relative_frame_time, world_point_to_image_point_shutter_pose).  Each image row or column is exposed at its
@@ -368,7 +514,8 @@ __device__ __forceinline__ float shutter_time(int type, uint32_t W, uint32_t H, 
     }
 }
 
-__device__ __forceinline__ bool cam_project_at(const CamModel &m, const Cam &pose, const float *x, float margin, float &u, float &v)
+template<class Model>
+__device__ __forceinline__ bool cam_project_at(const Model &m, const Cam &pose, const float *x, float margin, float &u, float &v)
 {
     float xc[3];
 #pragma unroll
@@ -381,8 +528,9 @@ __device__ __forceinline__ bool cam_project_at(const CamModel &m, const Cam &pos
 // the end pose's (neither valid: the point is invalid, at the end pose's image point), then re-project at the frame
 // time of the current point until that time repeats, at most kShutterIterations times.  The point and its validity are
 // those of the last projection.
+template<class Model>
 __device__ __forceinline__ bool cam_project_rs(
-    const CamModel &m, const RsPoses &P, int type, const float *x, float margin, float &u, float &v
+    const Model &m, const RsPoses &P, int type, const float *x, float margin, float &u, float &v
 )
 {
     float u0, v0, u1, v1;

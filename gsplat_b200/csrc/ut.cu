@@ -36,15 +36,16 @@ __device__ __forceinline__ RsPoses cta_rs_poses(RsPoses *s_poses, int64_t total,
 
 // One thread per (b, c, n).  Culled rows get radii 0 and zero float outputs.  Rolling shutter: each sigma point is
 // projected at the pose of the row or column it lands in (cam_project_rs); the depth and the near / far cull take the
-// mid-frame pose.
-template<class Shutter>
+// mid-frame pose.  FTheta without the global z order: the near / far cull and the depth take the distance |mean_c|
+// from the camera centre, as the lens images points behind the camera plane.
+template<class Shutter, class Lens>
 __global__ void __launch_bounds__(kUtThreads) ut_project_kernel(
     int64_t B, int64_t C, int64_t N, const float *__restrict__ means, const float *__restrict__ quats,
     const float *__restrict__ scales, const float *__restrict__ opacities, const float *__restrict__ viewmats,
     const float *__restrict__ Ks, int cam_kind, const float *__restrict__ radial, const float *__restrict__ tangential,
     const float *__restrict__ thin, uint32_t W, uint32_t H, float eps2d, float near_plane, float far_plane,
     float radius_clip, UtParams ut, int32_t *__restrict__ radii, float *__restrict__ means2d, float *__restrict__ depths,
-    float *__restrict__ conics, float *__restrict__ compensations, Shutter shutter
+    float *__restrict__ conics, float *__restrict__ compensations, Shutter shutter, Lens lens
 )
 {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -74,9 +75,15 @@ __global__ void __launch_bounds__(kUtThreads) ut_project_kernel(
     // a zero quaternion or a zero scale axis has no 3-D precision matrix to evaluate along a ray
     const bool degenerate = fabsf(qn2) < FLT_EPSILON || fabsf(s[0]) < FLT_EPSILON || fabsf(s[1]) < FLT_EPSILON
                          || fabsf(s[2]) < FLT_EPSILON;
-    if(!degenerate && !(pc[2] < near_plane || pc[2] > far_plane))
+    float zc = pc[2];
+    if constexpr(Lens::kFTheta)
     {
-        const CamModel cm = load_cam_model(cam_kind, Ks, radial, tangential, thin, bc, W, H);
+        if(!lens.global_z_order)
+            zc = sqrtf(pc[0] * pc[0] + pc[1] * pc[1] + pc[2] * pc[2]);
+    }
+    if(!degenerate && !(zc < near_plane || zc > far_plane))
+    {
+        const auto cm = lens.model(cam_kind, Ks, radial, tangential, thin, bc, W, H);
         const M3 Rq       = quat_to_rotmat(q);
         const float lam   = ut.alpha * ut.alpha * (3.f + ut.kappa) - 3.f;
         const float spread = sqrtf(3.f + lam);
@@ -165,11 +172,11 @@ __global__ void __launch_bounds__(kUtThreads) ut_project_kernel(
                 // finite inputs can overflow (a far sigma point through a strong distortion): a NaN row would pass every
                 // off-screen test, so it is culled
                 const bool finite = isfinite(m2x) && isfinite(m2y) && isfinite(k0) && isfinite(k1) && isfinite(k2)
-                                 && isfinite(fr_x) && isfinite(fr_y) && isfinite(pc[2]);
+                                 && isfinite(fr_x) && isfinite(fr_y) && isfinite(zc);
                 if(!clipped && !off && finite)
                 {
                     rx = (int)fr_x, ry = (int)fr_y;
-                    mx = m2x, my = m2y, depth = pc[2];
+                    mx = m2x, my = m2y, depth = zc;
                     ca = k0, cb = k1, cc = k2;
                     comp = compensation;
                 }
@@ -221,9 +228,8 @@ __device__ __forceinline__ void stage(
 }
 
 // The world ray of pixel (i, j) of one camera: origin, unit direction.  false: the camera model cannot unproject it.
-__device__ __forceinline__ bool pixel_ray(
-    const float *vm, const CamModel &cm, uint32_t i, uint32_t j, float *ro, float *rd
-)
+template<class Model>
+__device__ __forceinline__ bool pixel_ray(const float *vm, const Model &cm, uint32_t i, uint32_t j, float *ro, float *rd)
 {
     float dc[3];
     const bool ok = cam_unproject(cm, (float)j + 0.5f, (float)i + 0.5f, dc);
@@ -240,8 +246,9 @@ __device__ __forceinline__ bool pixel_ray(
 
 // Rolling shutter: the same ray, carried to the world by the pose at the frame time of the pixel centre's row or column.
 // The forward and the backward build it alike, so both take the same alpha and transmittance decisions.
+template<class Model>
 __device__ __forceinline__ bool pixel_ray(
-    const RsPoses &P, int type, const CamModel &cm, uint32_t i, uint32_t j, float *ro, float *rd
+    const RsPoses &P, int type, const Model &cm, uint32_t i, uint32_t j, float *ro, float *rd
 )
 {
     float dc[3];
@@ -260,9 +267,9 @@ __device__ __forceinline__ bool pixel_ray(
 
 // The pixel's ray under either shutter.  Rolling: the image's two poses are loaded once per CTA (one image per CTA);
 // every thread of the CTA calls this.
-template<class Shutter>
+template<class Shutter, class Model>
 __device__ __forceinline__ bool shutter_pixel_ray(
-    const Shutter &shutter, const float *viewmats, uint32_t img, bool inside, const CamModel &cm, uint32_t i, uint32_t j,
+    const Shutter &shutter, const float *viewmats, uint32_t img, bool inside, const Model &cm, uint32_t i, uint32_t j,
     float *ro, float *rd
 )
 {
@@ -319,13 +326,13 @@ struct EvalGeom
 
 // One CTA per 16x16 tile of the [I, th, tw] grid, one pixel per thread.  last_ids: the list index of the pixel's last
 // composited gaussian, -1 for none.
-template<int CDIM, class Shutter>
+template<int CDIM, class Shutter, class Lens>
 __global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
     EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
     const float *__restrict__ colors, const float *__restrict__ opacities, const float *__restrict__ backgrounds,
     const uint8_t *__restrict__ masks, const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids,
     int64_t n_isects, float *__restrict__ render_colors, float *__restrict__ render_alphas, int32_t *__restrict__ last_ids,
-    Shutter shutter
+    Shutter shutter, Lens lens
 )
 {
     __shared__ EvalRec rec[kUtThreads];
@@ -356,13 +363,13 @@ __global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
     bool done = !inside;
     if constexpr(Shutter::kRolling)
     {
-        const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
-        done              = !shutter_pixel_ray(shutter, geo.viewmats, img, inside, cm, i, j, ro, rd);
+        const auto cm = lens.model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        done          = !shutter_pixel_ray(shutter, geo.viewmats, img, inside, cm, i, j, ro, rd);
     }
     else if(inside)
     {
-        const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
-        done              = !pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
+        const auto cm = lens.model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        done          = !pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
     }
     float T = 1.f, pix_out[CDIM];
 #pragma unroll
@@ -440,13 +447,14 @@ __device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, cons
 
 // Back to front over each tile's list.  Per gaussian, the warp's per-pixel gradients (colours, opacity, mean, M) are
 // butterfly-reduced and added with one atomic per value.
-template<int CDIM, class Shutter>
+template<int CDIM, class Shutter, class Lens>
 __global__ void __launch_bounds__(kUtThreads, 1) eval3d_bwd_kernel(
     EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
     const float *__restrict__ colors, const float *__restrict__ opacities, const float *__restrict__ backgrounds,
     const uint8_t *__restrict__ masks, const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids,
     int64_t n_isects, const float *__restrict__ render_alphas, const int32_t *__restrict__ last_ids,
-    const float *__restrict__ v_render_colors, const float *__restrict__ v_render_alphas, EvalGradDst dst, Shutter shutter
+    const float *__restrict__ v_render_colors, const float *__restrict__ v_render_alphas, EvalGradDst dst, Shutter shutter,
+    Lens lens
 )
 {
     constexpr int NV = CDIM + 13; // colours | opacity 1 | mean 3 | M 9
@@ -470,13 +478,13 @@ __global__ void __launch_bounds__(kUtThreads, 1) eval3d_bwd_kernel(
     float ro[3] = {0.f, 0.f, 0.f}, rd[3] = {0.f, 0.f, 1.f};
     if constexpr(Shutter::kRolling)
     {
-        const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
-        inside            = shutter_pixel_ray(shutter, geo.viewmats, img, inside, cm, i, j, ro, rd);
+        const auto cm = lens.model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        inside        = shutter_pixel_ray(shutter, geo.viewmats, img, inside, cm, i, j, ro, rd);
     }
     else if(inside)
     {
-        const CamModel cm = load_cam_model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
-        inside            = pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
+        const auto cm = lens.model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        inside        = pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
     }
 
     const float T_final = 1.f - render_alphas[pix];
@@ -626,14 +634,37 @@ __global__ void __launch_bounds__(kUtThreads) eval3d_finish_kernel(
         v_quats[g * 4 + k] = vq[k];
 }
 
+// The camera model and its coefficients: pinhole / fisheye take the per-camera arrays, FTheta the shared parameters
+// alone (reference_poly 0 or 1, finite values).
+int camera_checks(int cam_kind, const float *radial, const float *tangential, const float *thin, const gsb200_ftheta_params *ft)
+{
+    if(cam_kind != kUtPinhole && cam_kind != kUtFisheye && cam_kind != kUtFTheta)
+        return GSB200_E_UNSUPPORTED;
+    if((cam_kind == kUtFTheta) != (ft != nullptr))
+        return GSB200_E_INVALID;
+    if(cam_kind == kUtFTheta)
+    {
+        if(radial || tangential || thin)
+            return GSB200_E_INVALID;
+        if(ft->reference_poly != kFThetaPixelToAngle && ft->reference_poly != kFThetaAngleToPixel)
+            return GSB200_E_INVALID;
+        bool finite = isfinite(ft->max_angle);
+        for(int i = 0; i < 6; ++i)
+            finite = finite && isfinite(ft->pixeldist_to_angle_poly[i]) && isfinite(ft->angle_to_pixeldist_poly[i]);
+        for(int i = 0; i < 3; ++i)
+            finite = finite && isfinite(ft->linear_cde[i]);
+        if(!finite)
+            return GSB200_E_INVALID;
+    }
+    return GSB200_OK;
+}
+
 int eval3d_checks(
-    int64_t B, int64_t C, int64_t N, int cam_kind, uint32_t W, uint32_t H, uint32_t tile_size, uint32_t tw, uint32_t th
+    int64_t B, int64_t C, int64_t N, uint32_t W, uint32_t H, uint32_t tile_size, uint32_t tw, uint32_t th
 )
 {
     if(B < 0 || C < 0 || N < 0)
         return GSB200_E_INVALID;
-    if(cam_kind != kUtPinhole && cam_kind != kUtFisheye)
-        return GSB200_E_UNSUPPORTED;
     if(tile_size != (uint32_t)kTile)
         return GSB200_E_UNSUPPORTED;
     if(B * C > 0 && W > 0 && H > 0 && !tile_grid_covers(tw, th, W, H))
@@ -665,6 +696,18 @@ int with_shutter(const float *viewmats_rs, int rolling_shutter, F &&f)
         return f(RollingShutter{viewmats_rs, rolling_shutter});
     return f(GlobalShutter{});
 }
+
+// Runs f with the kernels' shutter and lens policies: FThetaLens, its parameters copied by value, for FTheta parameters;
+// CamLens (the runtime pinhole / fisheye model) otherwise.
+template<class F>
+int with_policies(const float *viewmats_rs, int rolling_shutter, const gsb200_ftheta_params *ft, int global_z_order, F &&f)
+{
+    return with_shutter(viewmats_rs, rolling_shutter, [&](auto shutter) {
+        if(ft)
+            return f(shutter, FThetaLens{*ft, global_z_order});
+        return f(shutter, CamLens{});
+    });
+}
 } // namespace
 } // namespace gsb
 
@@ -673,20 +716,23 @@ int with_shutter(const float *viewmats_rs, int rolling_shutter, F &&f)
 extern "C" int gsb200_ut_projection_fwd(
     int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
     const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-    const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
-    uint32_t image_height, float eps2d, float near_plane, float far_plane, float radius_clip, float ut_alpha, float ut_beta,
-    float ut_kappa, float ut_in_image_margin_factor, int ut_require_all_sigma_points_valid, int32_t *radii,
-    float *means2d, float *depths, float *conics, float *compensations, void *stream
+    const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+    int global_z_order, uint32_t image_width, uint32_t image_height, float eps2d, float near_plane, float far_plane,
+    float radius_clip, float ut_alpha, float ut_beta, float ut_kappa, float ut_in_image_margin_factor,
+    int ut_require_all_sigma_points_valid, int32_t *radii, float *means2d, float *depths, float *conics,
+    float *compensations, void *stream
 )
 {
     if(B < 0 || C < 0 || N < 0)
         return GSB200_E_INVALID;
     if(int rc = gsb::shutter_checks(viewmats_rs, rolling_shutter, image_width, image_height))
         return rc;
-    if(camera_model != gsb::kUtPinhole && camera_model != gsb::kUtFisheye)
-        return GSB200_E_UNSUPPORTED;
+    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta))
+        return rc;
     if(camera_model == gsb::kUtFisheye && (tangential_coeffs || thin_prism_coeffs))
         return GSB200_E_INVALID;
+    if(!global_z_order && camera_model != gsb::kUtFTheta)
+        return GSB200_E_UNSUPPORTED;
     if(!(ut_alpha * ut_alpha * (3.f + ut_kappa) > 0.f))
         return GSB200_E_INVALID;
     const int64_t n = B * C * N;
@@ -695,11 +741,11 @@ extern "C" int gsb200_ut_projection_fwd(
     if(!means || !quats || !scales || !viewmats || !Ks || !radii || !means2d || !depths || !conics)
         return GSB200_E_INVALID;
     const gsb::UtParams ut{ut_alpha, ut_beta, ut_kappa, ut_in_image_margin_factor, ut_require_all_sigma_points_valid};
-    return gsb::with_shutter(viewmats_rs, rolling_shutter, [&](auto shutter) {
+    return gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, global_z_order, [&](auto shutter, auto lens) {
         gsb::ut_project_kernel<<<gsb::grid_for(n, gsb::kUtThreads), gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
             B, C, N, means, quats, scales, opacities, viewmats, Ks, camera_model, radial_coeffs, tangential_coeffs,
             thin_prism_coeffs, image_width, image_height, eps2d, near_plane, far_plane, radius_clip, ut, radii, means2d,
-            depths, conics, compensations, shutter
+            depths, conics, compensations, shutter, lens
         );
         return gsb::check_launch();
     });
@@ -709,15 +755,17 @@ extern "C" int gsb200_eval3d_fwd(
     int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
     const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
     const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-    const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
-    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
-    const int32_t *flatten_ids, int64_t n_isects, float *render_colors, float *render_alphas, int32_t *last_ids,
+    const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+    const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, float *render_colors, float *render_alphas, int32_t *last_ids,
     void *stream
 )
 {
     if(n_isects < 0)
         return GSB200_E_INVALID;
-    if(int rc = gsb::eval3d_checks(B, C, N, camera_model, image_width, image_height, tile_size, tile_width, tile_height))
+    if(int rc = gsb::eval3d_checks(B, C, N, image_width, image_height, tile_size, tile_width, tile_height))
+        return rc;
+    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta))
         return rc;
     if(int rc = gsb::shutter_checks(viewmats_rs, rolling_shutter, image_width, image_height))
         return rc;
@@ -729,11 +777,11 @@ extern "C" int gsb200_eval3d_fwd(
         return GSB200_E_INVALID;
     const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height,
                             camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
-    return gsb::with_shutter(viewmats_rs, rolling_shutter, [&](auto shutter) {
+    return gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
         return gsb::with_channels(D, [&](auto CH) {
             gsb::eval3d_fwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
                 geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
-                render_colors, render_alphas, last_ids, shutter
+                render_colors, render_alphas, last_ids, shutter, lens
             );
             return gsb::check_launch();
         });
@@ -744,16 +792,18 @@ extern "C" int gsb200_eval3d_bwd(
     int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
     const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
     const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-    const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
-    uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
-    const int32_t *flatten_ids, int64_t n_isects, const float *render_alphas, const int32_t *last_ids,
+    const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+    const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, const float *render_alphas, const int32_t *last_ids,
     const float *v_render_colors, const float *v_render_alphas, float *grad_records, float *v_colors, float *v_opacities,
     float *v_means, float *v_quats, float *v_scales, void *stream
 )
 {
     if(n_isects < 0)
         return GSB200_E_INVALID;
-    if(int rc = gsb::eval3d_checks(B, C, N, camera_model, image_width, image_height, tile_size, tile_width, tile_height))
+    if(int rc = gsb::eval3d_checks(B, C, N, image_width, image_height, tile_size, tile_width, tile_height))
+        return rc;
+    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta))
         return rc;
     if(int rc = gsb::shutter_checks(viewmats_rs, rolling_shutter, image_width, image_height))
         return rc;
@@ -770,11 +820,11 @@ extern "C" int gsb200_eval3d_bwd(
         const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width,
                                 tile_height, camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
         const gsb::EvalGradDst dst{v_colors, v_opacities, grad_records};
-        const int rc = gsb::with_shutter(viewmats_rs, rolling_shutter, [&](auto shutter) {
+        const int rc = gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
             return gsb::with_channels(D, [&](auto CH) {
                 gsb::eval3d_bwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, st>>>(
                     geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
-                    render_alphas, last_ids, v_render_colors, v_render_alphas, dst, shutter
+                    render_alphas, last_ids, v_render_colors, v_render_alphas, dst, shutter, lens
                 );
                 return gsb::check_launch();
             });

@@ -19,9 +19,10 @@ executable form).  ``apply()`` rebinds, in place, the names the reference's call
   gsplat.optimizers.SelectiveAdam                                            (optimizers/selective_adam.py)
   gsplat.losses.ssim_loss when ``losses=True``                               (losses.py:154)
 
-3DGUT training steps (``rasterization(..., with_ut=True, with_eval3d=True)`` with dense rows through a distorted pinhole
-or fisheye camera, global or rolling shutter) run on the b200 kernels.  Calls the b200 path does not implement (with_ut
-or with_eval3d alone, ftheta / lidar cameras, hit distance, extra signals, float64 inputs, tile_size != 16, ...) and calls
+3DGUT training steps (``rasterization(..., with_ut=True, with_eval3d=True)`` with dense rows through a distorted pinhole,
+fisheye or FTheta camera -- the FTheta ones with their ``ftheta_coeffs``, in either depth order -- global or rolling
+shutter) run on the b200 kernels.  Calls the b200 path does not implement (with_ut or with_eval3d alone, lidar cameras,
+an ftheta camera without ``ftheta_coeffs``, hit distance, extra signals, float64 inputs, tile_size != 16, ...) and calls
 with invalid arguments are handed to the package's own implementation -- gsplat_b200 raises
 NotImplementedError / ValueError / TypeError before launching anything -- so upstream behaviour and error messages are
 preserved; ``stats`` counts per name how many calls ran on the b200 kernels and how many were handed over (and why).
@@ -65,14 +66,14 @@ _OPS_CONTRIB = (
     "rasterize_top_contributing_gaussian_ids_sparse",
 )
 
-# 3DGUT, likewise: a call with an argument the b200 kernels do not take (ftheta, lidar, hit distance, ...) raises
+# 3DGUT, likewise: a call with an argument the b200 kernels do not take (lidar, hit distance, ...) raises
 # NotImplementedError on the b200 path and runs the package's own op
 _OPS_3DGUT = ("fully_fused_projection_with_ut", "rasterize_to_pixels_eval3d")
 
 _saved: List[Tuple[object, str, object]] = []
 
 # per rebound name: how many calls ran on the b200 kernels, how many were handed to the package's own implementation
-# (and why).  The policy of the drop-in: anything the b200 path does not implement -- ftheta / lidar 3DGUT, hit
+# (and why).  The policy of the drop-in: anything the b200 path does not implement -- lidar 3DGUT, hit
 # distance, extra signals, float64 inputs, tile_size != 16, ... -- and every argument error is the STOCK implementation's business
 # (same results, same messages as upstream); gsplat_b200 declines BEFORE launching anything, so the hand-over is clean.
 stats: Dict[str, Dict[str, object]] = {}

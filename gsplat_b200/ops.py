@@ -2566,10 +2566,11 @@ def adam(
 # --------------------------------------------------------------------------------------------
 # 3DGUT (reference wrappers gsplat/cuda/_wrapper.py: fully_fused_projection_with_ut, rasterize_to_pixels_eval3d): the
 # unscented-transform projection through a distorted pinhole or fisheye camera and the compositing that evaluates
-# each gaussian in 3-D along the pixel's ray.  Global or rolling shutter, dense rows, RendererConfig_MixedBatch.
+# each gaussian in 3-D along the pixel's ray.  Pinhole, fisheye or FTheta cameras, global or rolling shutter, dense rows,
+# RendererConfig_MixedBatch.
 
 _UT_DEFAULTS = {"alpha": 0.1, "beta": 2.0, "kappa": 0.0, "in_image_margin_factor": 0.1, "require_all_sigma_points_valid": False}
-_UT_CAMERAS = {"pinhole": 0, "fisheye": 2}
+_UT_CAMERAS = {"pinhole": 0, "fisheye": 2, "ftheta": 3}
 
 
 def _ut_params(ut_params) -> tuple:
@@ -2609,6 +2610,76 @@ def _shutter_type(rolling_shutter) -> RollingShutterType:
     raise ValueError(f"unknown rolling_shutter {rolling_shutter!r}")
 
 
+class FThetaPolynomialType(enum.IntEnum):
+    """Which of an FTheta calibration's two polynomials is the reference (the reference's FThetaPolynomialType): the
+    other direction inverts it by Newton steps."""
+
+    PIXELDIST_TO_ANGLE = 0
+    ANGLE_TO_PIXELDIST = 1
+
+
+class FThetaCameraDistortionParameters:
+    """The parameters of an FTheta camera, shared by every camera of a call (the reference's
+    FThetaCameraDistortionParameters, same keywords and defaults).  ``pixeldist_to_angle_poly`` (backward) and
+    ``angle_to_pixeldist_poly`` (forward) are the coefficients c0 .. c5 of two degree-5 polynomials between the angle
+    of a ray from the optical axis and its distance in pixels from the principal point; ``reference_poly`` names the one
+    evaluated directly; ``max_angle`` bounds the field of view (radians, beyond pi / 2 for lenses that see behind the
+    camera plane); ``linear_cde`` = (c, d, e) maps the radial offset to the image by [[c, d], [e, 1]].  The principal
+    point is each camera's ``Ks`` (cx, cy) + 0.5, FTheta's image origin being the centre of the first pixel; fx and fy
+    are unused.  The operators accept any object with these five attributes."""
+
+    def __init__(self, reference_poly=0, pixeldist_to_angle_poly=(0.0,) * 6, angle_to_pixeldist_poly=(0.0,) * 6,
+                 max_angle=0.0, linear_cde=(0.0,) * 3):
+        self.reference_poly = reference_poly
+        self.pixeldist_to_angle_poly = list(pixeldist_to_angle_poly)
+        self.angle_to_pixeldist_poly = list(angle_to_pixeldist_poly)
+        self.max_angle = max_angle
+        self.linear_cde = list(linear_cde)
+
+    def __repr__(self):
+        return (f"FThetaCameraDistortionParameters(reference_poly={int(self.reference_poly)}, "
+                f"pixeldist_to_angle_poly={self.pixeldist_to_angle_poly}, angle_to_pixeldist_poly={self.angle_to_pixeldist_poly}, "
+                f"max_angle={self.max_angle}, linear_cde={self.linear_cde})")
+
+
+def _ftheta_params(what, ftheta_coeffs) -> "_cabi.FThetaParams":
+    """The gsb200_ftheta_params of any object with the five attributes of FThetaCameraDistortionParameters (this
+    package's, the reference's torch class).  ValueError for a missing attribute, a wrong length, a reference_poly other
+    than 0 / 1 or a non-finite value."""
+    fields = {}
+    for name, n in (("reference_poly", None), ("pixeldist_to_angle_poly", 6), ("angle_to_pixeldist_poly", 6),
+                    ("max_angle", None), ("linear_cde", 3)):
+        if not hasattr(ftheta_coeffs, name):
+            raise ValueError(f"{what}: ftheta_coeffs has no {name} (expected FThetaCameraDistortionParameters)")
+        v = getattr(ftheta_coeffs, name)
+        try:
+            v = [float(x) for x in v] if n is not None else float(v)
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"{what}: ftheta_coeffs.{name} is not {'a sequence of ' if n else 'a '}number{'s' if n else ''}: {v!r}") from e
+        if n is not None and len(v) != n:
+            raise ValueError(f"{what}: ftheta_coeffs.{name} must have {n} values, got {len(v)}")
+        if not all(math.isfinite(x) for x in (v if n is not None else [v])):
+            raise ValueError(f"{what}: ftheta_coeffs.{name} must be finite, got {v}")
+        fields[name] = v
+    if fields["reference_poly"] not in (0.0, 1.0):
+        raise ValueError(f"{what}: ftheta_coeffs.reference_poly must be 0 (PIXELDIST_TO_ANGLE) or 1 (ANGLE_TO_PIXELDIST), "
+                         f"got {ftheta_coeffs.reference_poly!r}")
+    p = _cabi.FThetaParams()
+    p.reference_poly = int(fields["reference_poly"])
+    p.pixeldist_to_angle_poly[:] = fields["pixeldist_to_angle_poly"]
+    p.angle_to_pixeldist_poly[:] = fields["angle_to_pixeldist_poly"]
+    p.max_angle = fields["max_angle"]
+    p.linear_cde[:] = fields["linear_cde"]
+    return p
+
+
+def _ftheta_ptr(params) -> int:
+    """Host address of a gsb200_ftheta_params (0 for None); the caller keeps ``params`` alive across the call."""
+    import ctypes
+
+    return 0 if params is None else ctypes.addressof(params)
+
+
 def _ut_shutter(what, rolling_shutter, viewmats_rs, viewmats: Tensor, width: int, height: int):
     """Checks the shutter arguments of the 3DGUT operators.  A rolling shutter needs ``viewmats_rs`` and the global one
     takes none (NotImplementedError, naming the argument); a rolling shutter over a single row or column has no frame
@@ -2631,17 +2702,31 @@ def _ut_shutter(what, rolling_shutter, viewmats_rs, viewmats: Tensor, width: int
 
 
 def _ut_camera(what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
-               external_distortion_coeffs, cams: tuple):
+               external_distortion_coeffs, cams: tuple, global_z_order: bool = True):
     """Rejects what the 3DGUT kernels are not built for (NotImplementedError, naming the argument) and checks the
-    distortion coefficients.  Returns the camera model id and the coefficient tensors as [..., C, k] float32."""
-    for name, v in (("ftheta_coeffs", ftheta_coeffs), ("lidar_coeffs", lidar_coeffs),
-                    ("external_distortion_coeffs", external_distortion_coeffs)):
+    camera parameters.  Returns the camera model id, the coefficient tensors as [..., C, k] float32 and the FTheta
+    parameters (a gsb200_ftheta_params, or None for the other models)."""
+    for name, v in (("lidar_coeffs", lidar_coeffs), ("external_distortion_coeffs", external_distortion_coeffs)):
         if v is not None:
-            raise NotImplementedError(f"{what}: {name} is not supported (pinhole / fisheye only)")
+            raise NotImplementedError(f"{what}: {name} is not supported (pinhole / fisheye / ftheta only)")
+    if ftheta_coeffs is not None and camera_model != "ftheta":
+        raise NotImplementedError(f"{what}: ftheta_coeffs is not supported with camera_model={camera_model!r} "
+                                  "(the FTheta parameters belong to camera_model='ftheta')")
     if camera_model not in _UT_CAMERAS:
-        if camera_model in ("ortho", "ftheta", "lidar"):
-            raise NotImplementedError(f"{what}: camera_model={camera_model!r} is not supported (pinhole / fisheye only)")
+        if camera_model in ("ortho", "lidar"):
+            raise NotImplementedError(f"{what}: camera_model={camera_model!r} is not supported (pinhole / fisheye / ftheta only)")
         raise ValueError(f"{what}: unknown camera_model {camera_model!r}")
+    if camera_model == "ftheta" and ftheta_coeffs is None:
+        raise NotImplementedError(f"{what}: camera_model='ftheta' requires ftheta_coeffs (FThetaCameraDistortionParameters)")
+    if not global_z_order and camera_model != "ftheta":
+        raise NotImplementedError(f"{what}: global_z_order=False is not supported with camera_model={camera_model!r} "
+                                  "(the Euclidean depth order is built for ftheta cameras)")
+    if camera_model == "ftheta":
+        for name, v in (("radial_coeffs", radial_coeffs), ("tangential_coeffs", tangential_coeffs),
+                        ("thin_prism_coeffs", thin_prism_coeffs)):
+            if v is not None:
+                raise ValueError(f"{what}: {name} does not apply to the ftheta camera (its distortion is ftheta_coeffs)")
+        return _UT_CAMERAS[camera_model], None, None, None, _ftheta_params(what, ftheta_coeffs)
     if camera_model == "fisheye":
         for name, v in (("tangential_coeffs", tangential_coeffs), ("thin_prism_coeffs", thin_prism_coeffs)):
             if v is not None:
@@ -2654,7 +2739,7 @@ def _ut_camera(what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_
             _check_shape(v, cams + (k,), name)
             v = f32c(v, name)
         out.append(v)
-    return (_UT_CAMERAS[camera_model], *out)
+    return (_UT_CAMERAS[camera_model], *out, None)
 
 
 def _ut_geometry(what, means, quats, scales, viewmats, Ks) -> tuple:
@@ -2701,24 +2786,28 @@ def fully_fused_projection_with_ut(
     viewmats_rs: Optional[Tensor] = None,
     global_z_order: bool = True,
 ) -> Tuple[Tensor, Tensor, Tensor, Tensor, Optional[Tensor]]:
-    """Projects 3D Gaussians through a distorted pinhole or fisheye camera with the unscented transform: 7 sigma points
+    """Projects 3D Gaussians through a distorted pinhole, fisheye or FTheta camera with the unscented transform: 7 sigma points
     per Gaussian are projected through the camera model and reduced to a 2-D mean and covariance, then blurred by
     ``eps2d`` and culled as in ``fully_fused_projection``.  Returns (radii int32 [..., C, N, 2], means2d [..., C, N, 2],
     depths [..., C, N], conics [..., C, N, 3], compensations [..., C, N] or None); culled rows have radii 0 and zero
     floats.  Not differentiable, as in the reference.  ``ut_params``: any object with the fields of the reference's
-    UnscentedTransformParameters, or None for their defaults.  ``global_z_order=True`` only.
+    UnscentedTransformParameters, or None for their defaults.
+
+    FTheta (``camera_model="ftheta"`` with ``ftheta_coeffs``, an FThetaCameraDistortionParameters shared by every
+    camera; the principal point is each camera's Ks (cx, cy) + 0.5): no z > 0 requirement, a sigma point is valid below
+    ``max_angle`` inside the image grown by the margin.  ``global_z_order=False`` (FTheta only) culls on and returns the
+    distance |mean_c| from the camera centre as the depth, so that tile lists sort by distance, as a lens beyond 180
+    degrees needs; True culls and orders on the camera-frame z.
 
     Rolling shutter: ``rolling_shutter`` (a RollingShutterType or its value) other than GLOBAL with ``viewmats_rs``
     [..., C, 4, 4], the end-of-frame poses.  Each sigma point is projected at the pose of the image row or column it
     lands in (translation lerp and rotation slerp between the two poses at that row's or column's frame time, iterated
     up to 10 times from the start pose's projection); the depths and the near / far cull take the mid-frame pose."""
     what = "fully_fused_projection_with_ut"
-    if not global_z_order:
-        raise NotImplementedError(f"{what}: global_z_order=False is not supported")
     batch, C, N = _ut_geometry(what, means, quats, scales, viewmats, Ks)
-    cam, radial, tangential, thin = _ut_camera(
+    cam, radial, tangential, thin, ftheta = _ut_camera(
         what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
-        external_distortion_coeffs, batch + (C,),
+        external_distortion_coeffs, batch + (C,), global_z_order,
     )
     shutter, viewmats_rs = _ut_shutter(what, rolling_shutter, viewmats_rs, viewmats, width, height)
     if opacities is not None:
@@ -2738,7 +2827,8 @@ def fully_fused_projection_with_ut(
         check(
             lib().gsb200_ut_projection_fwd(
                 B, C, N, ptr(means), ptr(quats), ptr(scales), ptr(opacities), ptr(viewmats), ptr(Ks), cam, ptr(radial),
-                ptr(tangential), ptr(thin), ptr(viewmats_rs), shutter, int(width), int(height), float(eps2d),
+                ptr(tangential), ptr(thin), _ftheta_ptr(ftheta), ptr(viewmats_rs), shutter, int(bool(global_z_order)),
+                int(width), int(height), float(eps2d),
                 float(near_plane), float(far_plane),
                 float(radius_clip), alpha, beta, kappa, margin, int(require_all), ptr(radii), ptr(means2d), ptr(depths),
                 ptr(conics), ptr(comps), st,
@@ -2751,7 +2841,7 @@ def fully_fused_projection_with_ut(
 class _RasterizeToPixelsEval3D(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, radial, tangential,
-                thin, viewmats_rs, shutter, width, height, isect_offsets, flatten_ids):
+                thin, ftheta, viewmats_rs, shutter, width, height, isect_offsets, flatten_ids):
         dev = require_cuda(means, quats, scales, colors, opacities, viewmats, Ks)
         means, quats, scales = means.contiguous(), quats.contiguous(), scales.contiguous()
         colors, opacities = f32c(colors, "colors"), f32c(opacities, "opacities")
@@ -2781,8 +2871,8 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
                 check(
                     lib().gsb200_eval3d_fwd(
                         B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds),
-                        ptr(m8), ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), ptr(viewmats_rs),
-                        shutter, width, height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_colors),
+                        ptr(m8), ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), _ftheta_ptr(ftheta),
+                        ptr(viewmats_rs), shutter, width, height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_colors),
                         ptr(render_alphas), ptr(last_ids), st,
                     ),
                     "rasterize_to_pixels_eval3d",
@@ -2790,7 +2880,7 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
         ctx.save_for_backward(means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, radial, tangential, thin,
                               viewmats_rs, offsets, fl, render_alphas, last_ids)
         ctx.set_materialize_grads(False)
-        ctx.meta = (B, C, N, D, cam, shutter, width, height, tw, th, S)
+        ctx.meta = (B, C, N, D, cam, ftheta, shutter, width, height, tw, th, S)
         ctx.mark_non_differentiable(last_ids)
         return render_colors, render_alphas
 
@@ -2798,7 +2888,7 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
     def backward(ctx, v_render_colors, v_render_alphas):
         (means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, radial, tangential, thin, viewmats_rs,
          offsets, fl, render_alphas, last_ids) = ctx.saved_tensors
-        B, C, N, D, cam, shutter, width, height, tw, th, S = ctx.meta
+        B, C, N, D, cam, ftheta, shutter, width, height, tw, th, S = ctx.meta
         dev = render_alphas.device
         if v_render_colors is None:
             v_render_colors = torch.zeros(render_alphas.shape[:-1] + (D,), device=dev, dtype=torch.float32)
@@ -2811,8 +2901,8 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
             check(
                 lib().gsb200_eval3d_bwd(
                     B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds), ptr(m8),
-                    ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), ptr(viewmats_rs), shutter, width,
-                    height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_alphas), ptr(last_ids), ptr(v_render_colors),
+                    ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), _ftheta_ptr(ftheta),
+                    ptr(viewmats_rs), shutter, width, height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_alphas), ptr(last_ids), ptr(v_render_colors),
                     ptr(v_render_alphas),
                     ptr(records), ptr(v_colors), ptr(v_opacities), ptr(v_means), ptr(v_quats), ptr(v_scales), st,
                 ),
@@ -2822,7 +2912,7 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
         if backgrounds is not None and ctx.needs_input_grad[5]:
             v_backgrounds = (v_render_colors * (1.0 - render_alphas)).sum(dim=(-3, -2))
         # viewmats, viewmats_rs, Ks and the camera coefficients get no gradient, as in the reference's backward
-        return (v_means, v_quats, v_scales, v_colors, v_opacities, v_backgrounds) + (None,) * 13
+        return (v_means, v_quats, v_scales, v_colors, v_opacities, v_backgrounds) + (None,) * 14
 
 
 def rasterize_to_pixels_eval3d(
@@ -2864,7 +2954,11 @@ def rasterize_to_pixels_eval3d(
 
     Rolling shutter (``rolling_shutter`` other than GLOBAL with the end-of-frame poses ``viewmats_rs``): the ray of each
     pixel leaves the camera at the pose of the pixel's row or column (translation lerp and rotation slerp between
-    ``viewmats`` and ``viewmats_rs`` at its frame time).  viewmats_rs gets no gradient either."""
+    ``viewmats`` and ``viewmats_rs`` at its frame time).  viewmats_rs gets no gradient either.
+
+    FTheta (``camera_model="ftheta"`` with ``ftheta_coeffs``): each pixel centre is unprojected through the shared FTheta
+    parameters; with the forward polynomial as the reference, a pixel whose Newton inversion does not converge
+    composites nothing."""
     what = "rasterize_to_pixels_eval3d"
     for name, v in (("rays", rays),):
         if v is not None:
@@ -2881,7 +2975,7 @@ def rasterize_to_pixels_eval3d(
         raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
     batch, C, N = _ut_geometry(what, means, quats, scales, viewmats, Ks)
     image_dims = batch + (C,)
-    cam, radial, tangential, thin = _ut_camera(
+    cam, radial, tangential, thin, ftheta = _ut_camera(
         what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
         external_distortion_coeffs, image_dims,
     )
@@ -2911,6 +3005,6 @@ def rasterize_to_pixels_eval3d(
     require_cuda(means, quats, scales, colors, opacities, viewmats, Ks, backgrounds, masks, isect_offsets, flatten_ids,
                  radial, tangential, thin, viewmats_rs)
     return _RasterizeToPixelsEval3D.apply(
-        means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, radial, tangential, thin,
+        means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, radial, tangential, thin, ftheta,
         viewmats_rs, shutter, int(image_width), int(image_height), isect_offsets, flatten_ids,
     )

@@ -9,11 +9,13 @@ Scope: the 3DGS EWA path named by BASELINE.json (pinhole / orthographic / fishey
 backgrounds, masks, absgrad, SH or post-activation colours, ``distributed=True`` Gaussian sharding).
 
 3DGUT (``with_ut=True, with_eval3d=True`` together): the unscented-transform projection and the eval3d compositing
-through a distorted pinhole (radial / tangential / thin-prism coefficients) or fisheye (radial) camera, dense rows,
-global shutter, classic mode, RGB / D / ED / RGB+D / RGB+ED, following the reference's orchestrator
-(csrc/Rendering.cpp:890-934, 1307-1308, 1353-1410).  ``tile_size=None`` resolves to 16 here; the reference resolves it
-to 8 below 1080p.  with_ut or with_eval3d alone, ftheta / lidar cameras, external distortion, rolling shutter,
-hit-distance modes, normals, extra signals and packed 3DGUT rows raise NotImplementedError.
+through a distorted pinhole (radial / tangential / thin-prism coefficients), fisheye (radial) or FTheta
+(``ftheta_coeffs``) camera, dense rows, global or rolling shutter, classic mode, RGB / D / ED / RGB+D / RGB+ED,
+following the reference's orchestrator (csrc/Rendering.cpp:890-934, 1307-1308, 1353-1410).  FTheta cameras also take
+``global_z_order=False``: the depths, the tile order and the D / ED channels are then the distance from the camera
+centre.  ``tile_size=None`` resolves to 16 here; the reference resolves it to 8 below 1080p.  with_ut or with_eval3d
+alone, lidar cameras, external distortion, ``global_z_order=False`` for pinhole / fisheye, hit-distance modes, normals,
+extra signals and packed 3DGUT rows raise NotImplementedError.
 
 rasterization_2dgs(): surfel splatting (2DGS) on the dense layout, following the reference's orchestrator
 (csrc/Rendering.cpp:1705-1958): ray-transform projection -> radius-box tile intersection -> compositing of colours,
@@ -29,6 +31,7 @@ from torch import Tensor
 
 from .ops import (
     _SUPPORTED_CHANNELS,
+    _ftheta_params,
     _shutter_type,
     _ut_params,
     RollingShutterType,
@@ -237,8 +240,10 @@ def rasterization(
 
     ``with_ut=True, with_eval3d=True`` renders 3DGUT: the unscented-transform projection through a distorted pinhole
     (``radial_coeffs`` [..., C, 6], ``tangential_coeffs`` [..., C, 2], ``thin_prism_coeffs`` [..., C, 4]) or fisheye
-    (``radial_coeffs`` [..., C, 4]) camera, radius-box tile lists, and compositing that evaluates each Gaussian in 3-D
-    along the pixel's ray.  Dense rows only: pass ``packed=False``.  Gradients reach means, quats, scales, colours or SH
+    (``radial_coeffs`` [..., C, 4]) or FTheta (``camera_model="ftheta"`` with ``ftheta_coeffs``, one
+    FThetaCameraDistortionParameters shared by every camera) camera, radius-box tile lists, and compositing that
+    evaluates each Gaussian in 3-D along the pixel's ray.  With an FTheta camera, ``global_z_order=False`` orders the
+    tile lists by the distance from the camera centre and renders that distance in D / ED.  Dense rows only: pass ``packed=False``.  Gradients reach means, quats, scales, colours or SH
     coefficients, opacities and backgrounds, and viewmats through the SH view directions only; ``meta["means2d"]``
     carries none and ``absgrad`` is accepted and does nothing, as in the reference.  ``tile_size=None`` means 16; the
     reference picks 8 below 1080p, which changes ``meta["tile_size"]`` and the tile grid, and can change pixels where a
@@ -546,22 +551,26 @@ def _rasterization_3dgut(
     if return_normals:
         _unsupported("return_normals", "normals are not built for 3DGUT")
     for name, val in (
-        ("rays", rays), ("ftheta_coeffs", ftheta_coeffs), ("lidar_coeffs", lidar_coeffs),
-        ("external_distortion_coeffs", external_distortion_coeffs), ("extra_signals", extra_signals),
+        ("rays", rays), ("lidar_coeffs", lidar_coeffs), ("external_distortion_coeffs", external_distortion_coeffs),
+        ("extra_signals", extra_signals),
     ):
         if val is not None:
-            _unsupported(name, "not built for 3DGUT (pinhole / fisheye cameras, colour and depth channels)")
+            _unsupported(name, "not built for 3DGUT (pinhole / fisheye / ftheta cameras, colour and depth channels)")
     shutter = _shutter_type(rolling_shutter)
     if shutter == RollingShutterType.GLOBAL and viewmats_rs is not None:
         _unsupported("viewmats_rs", "the end-of-frame poses belong to a rolling shutter (rolling_shutter=GLOBAL)")
     if shutter != RollingShutterType.GLOBAL and viewmats_rs is None:
         _unsupported(f"rolling_shutter={rolling_shutter!r}", "a rolling shutter requires viewmats_rs, the end-of-frame poses")
-    if camera_model not in ("pinhole", "fisheye"):
-        if camera_model in ("ortho", "ftheta", "lidar"):
-            _unsupported(f"camera_model={camera_model!r}", "3DGUT is built for pinhole / fisheye cameras")
+    if ftheta_coeffs is not None and camera_model != "ftheta":
+        _unsupported("ftheta_coeffs", f"the FTheta parameters belong to camera_model='ftheta', not {camera_model!r}")
+    if camera_model not in ("pinhole", "fisheye", "ftheta"):
+        if camera_model in ("ortho", "lidar"):
+            _unsupported(f"camera_model={camera_model!r}", "3DGUT is built for pinhole / fisheye / ftheta cameras")
         raise ValueError(f"unknown camera_model {camera_model!r}")
-    if not global_z_order:
-        _unsupported("global_z_order=False", "3DGUT is built for the global depth order only")
+    if camera_model == "ftheta" and ftheta_coeffs is None:
+        _unsupported("camera_model='ftheta'", "an FTheta camera requires ftheta_coeffs (FThetaCameraDistortionParameters)")
+    if not global_z_order and camera_model != "ftheta":
+        _unsupported("global_z_order=False", "the Euclidean depth order is built for ftheta cameras only")
     if renderer_config is not None and type(renderer_config).__name__ != "RendererConfig_MixedBatch":
         _unsupported(f"renderer_config={type(renderer_config).__name__}", "3DGUT is built for RendererConfig_MixedBatch only")
 
@@ -605,14 +614,17 @@ def _rasterization_3dgut(
             f"channel_chunk={channel_chunk}: the eval3d kernels composite up to {_SUPPORTED_CHANNELS[-1]} channels per pass"
         )
     _ut_params(ut_params)
+    if ftheta_coeffs is not None:
+        _ftheta_params("rasterization", ftheta_coeffs)  # malformed parameters: ValueError before the device is touched
     cams = dict(camera_model=camera_model, radial_coeffs=radial_coeffs, tangential_coeffs=tangential_coeffs,
-                thin_prism_coeffs=thin_prism_coeffs, rolling_shutter=int(shutter),
+                thin_prism_coeffs=thin_prism_coeffs, ftheta_coeffs=ftheta_coeffs, rolling_shutter=int(shutter),
                 viewmats_rs=None if viewmats_rs is None else viewmats_rs.detach())
 
     # ---- projection through the camera model (no gradient, as in the reference)
     radii, means2d, depths, conics, _ = fully_fused_projection_with_ut(
         means, quats, scales, opacities, viewmats, Ks, width, height, eps2d=eps2d, near_plane=near_plane,
-        far_plane=far_plane, radius_clip=radius_clip, calc_compensations=False, ut_params=ut_params, **cams,
+        far_plane=far_plane, radius_clip=radius_clip, calc_compensations=False, ut_params=ut_params,
+        global_z_order=global_z_order, **cams,
     )
     # the SH view directions are the only path by which viewmats (and viewmats_rs) get a gradient
     feat = (_color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N, viewmats_rs=viewmats_rs)

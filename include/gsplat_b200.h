@@ -23,6 +23,16 @@
 #include <stddef.h>
 #include <stdint.h>
 
+/* FTheta camera parameters of the 3DGUT entry points (see gsb200_ut_projection_fwd). */
+typedef struct
+{
+    int reference_poly;                /* 0: pixel distance -> angle is the reference polynomial, 1: angle -> pixel distance */
+    float pixeldist_to_angle_poly[6];  /* backward polynomial, c0 .. c5 */
+    float angle_to_pixeldist_poly[6];  /* forward polynomial, c0 .. c5 */
+    float max_angle;                   /* radians from the optical axis */
+    float linear_cde[3];               /* c, d, e of the linear map [[c, d], [e, 1]] */
+} gsb200_ftheta_params;
+
 #ifdef __cplusplus
 extern "C"
 {
@@ -538,8 +548,17 @@ extern "C"
     );
 
     /* ---- 3DGUT (csrc/ut.cu): camera_model 0 pinhole (OpenCV: radial [B*C, 6], tangential [B*C, 2], thin prism
-     * [B*C, 4], each optional; none at all is the perfect pinhole) or 2 fisheye (OpenCV: radial [B*C, 4] optional, the
-     * other two must be NULL); any other model is GSB200_E_UNSUPPORTED.
+     * [B*C, 4], each optional; none at all is the perfect pinhole), 2 fisheye (OpenCV: radial [B*C, 4] optional, the
+     * other two must be NULL) or 3 FTheta (ftheta non-NULL, the three coefficient arrays NULL); any other model is
+     * GSB200_E_UNSUPPORTED.  ftheta is a host pointer, read when the call is made, and must be NULL for the other models.
+     * FTheta: the parameters are shared by every camera; each camera's principal point is Ks (cx, cy) + 0.5 (FTheta's
+     * image origin is the centre of the first pixel), fx and fy are unused.  reference_poly 0: the backward polynomial
+     * (pixel distance -> angle) is the reference and the forward direction inverts it by 3 Newton steps; 1: the
+     * forward polynomial (angle -> pixel distance) is, and the unprojection inverts it (a pixel whose last Newton step
+     * stays above 1e-6 composites nothing).  Polynomial coefficients are c0 + c1 x + .. + c5 x^5; the image offset is
+     * [[c, d], [e, 1]] times the radial offset.  Rays at max_angle or beyond are invalid.
+     * global_z_order (projection): 1 culls on and returns the camera-frame z as the depth; 0 (FTheta only, else
+     * GSB200_E_UNSUPPORTED) culls on and returns the distance |mean_c| from the camera centre.
      * Shutter: viewmats_rs NULL with rolling_shutter 4 is the global shutter (the pose of viewmats).  viewmats_rs
      * [B*C, 4, 4] (the end-of-frame pose) with rolling_shutter 0 top to bottom, 1 left to right, 2 bottom to top or 3
      * right to left exposes each image row or column at the pose interpolated between the two (translation lerp,
@@ -550,10 +569,11 @@ extern "C"
     int gsb200_ut_projection_fwd(
         int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
         const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-        const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
-        uint32_t image_height, float eps2d, float near_plane, float far_plane, float radius_clip, float ut_alpha, float ut_beta,
-        float ut_kappa, float ut_in_image_margin_factor, int ut_require_all_sigma_points_valid, int32_t *radii,
-        float *means2d, float *depths, float *conics, float *compensations, void *stream
+        const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+        int global_z_order, uint32_t image_width, uint32_t image_height, float eps2d, float near_plane, float far_plane,
+        float radius_clip, float ut_alpha, float ut_beta, float ut_kappa, float ut_in_image_margin_factor,
+        int ut_require_all_sigma_points_valid, int32_t *radii, float *means2d, float *depths, float *conics,
+        float *compensations, void *stream
     );
     /* Compositing with each gaussian evaluated in 3-D along the pixel's world ray: means/quats/scales [B,N,*], colors
      * [B*C, N, D], opacities [B*C, N], backgrounds [B*C, D] or NULL, masks [B*C, th, tw] or NULL, the lists of
@@ -564,18 +584,18 @@ extern "C"
         int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
         const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
         const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-        const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
-        uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
-        const int32_t *flatten_ids, int64_t n_isects, float *render_colors, float *render_alphas, int32_t *last_ids,
+        const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, float *render_colors, float *render_alphas, int32_t *last_ids,
         void *stream
     );
     int gsb200_eval3d_bwd(
         int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
         const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
         const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
-        const float *thin_prism_coeffs, const float *viewmats_rs, int rolling_shutter, uint32_t image_width,
-        uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height, const int32_t *offsets,
-        const int32_t *flatten_ids, int64_t n_isects, const float *render_alphas, const int32_t *last_ids,
+        const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, const float *render_alphas, const int32_t *last_ids,
         const float *v_render_colors, const float *v_render_alphas, float *grad_records, float *v_colors, float *v_opacities,
         float *v_means, float *v_quats, float *v_scales, void *stream
     );

@@ -5,6 +5,7 @@ backward) on bench.py's scene (1M Gaussians, one 1920x1080 view) with a pinhole 
 the device name and power limit with the numbers, as one JSON line.
 
     python tools/bench_ut.py [--steps 20] [--warmup 5] [--distorted] [--rasterization] [--rolling-shutter]
+                             [--camera ftheta]
 
 --rasterization times the public call instead: rasterization(with_ut=True, with_eval3d=True, sh_degree=3,
 packed=False) forward and backward on the same scene with SH degree 3, next to the same operators chained by hand, and
@@ -14,6 +15,11 @@ reports the difference as the public call's overhead.
 moved by 0.03) next to the global-shutter step on the same scene, alternated step by step: the operator chain, or with
 --rasterization the public call.  It also times the UT projection alone under both shutters and reports its share of
 each step.
+
+--camera ftheta times the operator step through an FTheta camera (the 120-degree cross-left calibration of
+tests/golden/ftheta_calibrations.json scaled to 1920 pixels wide) in the global z order and in the Euclidean order
+(global_z_order=False) next to the pinhole step on the same scene, alternated step by step, with the UT projection
+alone under each and its share of the step.
 """
 import argparse
 import json
@@ -40,8 +46,12 @@ def main():
                     help="time rasterization(with_ut=True, with_eval3d=True, sh_degree=3) next to the hand-chained operators")
     ap.add_argument("--rolling-shutter", action="store_true",
                     help="time the rolling-shutter step next to the global-shutter step")
+    ap.add_argument("--camera", choices=("pinhole", "ftheta"), default="pinhole",
+                    help="ftheta: time the FTheta step in both depth orders next to the pinhole step")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_ut needs a GPU"
+    if a.camera == "ftheta":
+        return bench_ftheta(a)
     if a.rolling_shutter:
         return bench_rolling_shutter(a)
     if a.rasterization:
@@ -225,6 +235,53 @@ def bench_rolling_shutter(a):
     res["rolling_over_global"] = res["rolling"]["step_median_ms"] / res["global"]["step_median_ms"]
     res.update(_device_info(), gaussians=int(N), width=W, height=H, rasterization=a.rasterization, distorted=a.distorted,
                shutter="ROLLING_TOP_TO_BOTTOM", steps=a.steps)
+    print(json.dumps(res))
+
+
+def bench_ftheta(a):
+    from tests import ut_ftheta_oracle as F
+
+    dev = "cuda"
+    sc = scene.make_scene(scene_grid=3, sh_degree=0)
+    W, H = 1920, 1080
+    t = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)  # noqa: E731
+    means, quats, scales = (t(sc[k]).requires_grad_(True) for k in ("means", "quats", "scales"))
+    opac = t(sc["opacities"]).requires_grad_(True)
+    colors = t(sc["colors"][None]).requires_grad_(True)
+    vm, K = t(sc["viewmats"][:1]), t(scene.rescale_K(sc["Ks"], sc["width"], sc["height"], W, H)[:1])
+    params, pp, size = F.scaled(F.calibrations()["cross_left_120fov"], W)
+    assert size == (W, H)
+    K_ft = t(np.float32([[[1, 0, pp[0]], [0, 1, pp[1]], [0, 0, 1]]]))
+    ft = gs.FThetaCameraDistortionParameters(reference_poly=0, **params)
+    cams = {"pinhole": (K, {}), "ftheta_z": (K_ft, dict(camera_model="ftheta", ftheta_coeffs=ft)),
+            "ftheta_dist": (K_ft, dict(camera_model="ftheta", ftheta_coeffs=ft, global_z_order=False))}
+    tw, th = (W + 15) // 16, (H + 15) // 16
+    N = means.shape[0]
+
+    def step(Kc, co):
+        ev = {k: v for k, v in co.items() if k != "global_z_order"}  # the compositing takes no depth order
+        r, m2, d, _, _ = gs.fully_fused_projection_with_ut(means.detach(), quats.detach(), scales.detach(), opac.detach(), vm,
+                                                          Kc, W, H, **co)
+        _, ii, fl = gs.isect_tiles(m2, r, d, 16, tw, th)
+        offs = gs.isect_offset_encode(ii, 1, tw, th)
+        o = torch.broadcast_to(opac[None], (1, N))
+        rc, ra = gs.rasterize_to_pixels_eval3d(means, quats, scales, colors, o, vm, Kc, W, H, 16, offs, fl, **ev)
+        (rc.sum() + ra.sum()).backward()
+        return fl.numel()
+
+    def projection(Kc, co):
+        gs.fully_fused_projection_with_ut(means.detach(), quats.detach(), scales.detach(), opac.detach(), vm, Kc, W, H, **co)
+        return 0
+
+    fns = {f"{k}_step": (lambda c=c: step(*c)) for k, c in cams.items()}
+    fns.update({f"{k}_projection": (lambda c=c: projection(*c)) for k, c in cams.items()})
+    r = _time(fns, a.steps, a.warmup)
+    res = {}
+    for k in cams:
+        s, p = r[f"{k}_step"], r[f"{k}_projection"]
+        res[k] = {"step_median_ms": s["median_ms"], "step_min_ms": s["min_ms"], "n_isects": int(s["out"]),
+                  "projection_median_ms": p["median_ms"], "projection_share": p["median_ms"] / s["median_ms"]}
+    res.update(_device_info(), gaussians=int(N), width=W, height=H, calibration="cross_left_120fov", steps=a.steps)
     print(json.dumps(res))
 
 

@@ -14,7 +14,8 @@ and the tile-mask parameters that came with it, and with the pair-query kernels 
 ``surfel_indices_kernel`` named by their sink without their parameter list (``<false / true>`` became the
 ``CountSink`` / ``PairSink`` instantiations when each walk took a sink), and with the 3DGUT kernels
 (``ut_project_kernel``, ``eval3d_fwd_kernel``, ``eval3d_bwd_kernel``) without their ``gsb::GlobalShutter`` policy, the
-template argument and the trailing empty parameter they gained with the rolling shutter.  Instructions and their encodings must be
+template argument and the trailing empty parameter they gained with the rolling shutter, and without their
+``gsb::CamLens`` policy, the template argument and trailing empty parameter they gained with the FTheta lens.  Instructions and their encodings must be
 identical; address and line-info comments are ignored.  A library kernel (CUB) that several units instantiate must be
 identical in all of them.  Kernels that only the new objects have are listed as new.  Exit status 1 on any difference.  Needs nvcc / cuobjdump / cu++filt (no GPU).
 """
@@ -97,6 +98,10 @@ def kernels(obj: str):
         m = COUNT_KERNEL.match(d)
         if m:
             d = f"gsb::isect_count_totals_kernel({m.group(2)}, unsigned long long *)" if m.group(1) == "1" else f"gsb::isect_count_kernel({m.group(2)})"
+        if "gsb::CamLens" in d:
+            # the 3DGUT kernels' lens policy (template argument and last parameter): CamLens, the runtime pinhole / fisheye
+            # model, is the kernel as it was before FTheta became the other policy
+            d = POLICY_PARAM.sub(")", d).replace(", gsb::CamLens>", ">")
         if "gsb::GlobalShutter" in d:
             # the 3DGUT kernels' shutter policy (template argument and last parameter): GlobalShutter is the kernel as it was
             # (a kernel with no other template argument was not a template, and demangles without its return type)
