@@ -635,8 +635,12 @@ __global__ void __launch_bounds__(kUtThreads) eval3d_finish_kernel(
 }
 
 // The camera model and its coefficients: pinhole / fisheye take the per-camera arrays, FTheta the shared parameters
-// alone (reference_poly 0 or 1, finite values).
-int camera_checks(int cam_kind, const float *radial, const float *tangential, const float *thin, const gsb200_ftheta_params *ft)
+// alone (reference_poly 0 or 1, finite values).  A rolling shutter takes an end pose, the global shutter none; the frame
+// time divides by the rows (or columns) - 1.
+int camera_checks(
+    int cam_kind, const float *radial, const float *tangential, const float *thin, const gsb200_ftheta_params *ft,
+    const float *viewmats_rs, int rolling_shutter, uint32_t W, uint32_t H
+)
 {
     if(cam_kind != kUtPinhole && cam_kind != kUtFisheye && cam_kind != kUtFTheta)
         return GSB200_E_UNSUPPORTED;
@@ -656,6 +660,14 @@ int camera_checks(int cam_kind, const float *radial, const float *tangential, co
         if(!finite)
             return GSB200_E_INVALID;
     }
+    if(rolling_shutter < 0 || rolling_shutter > kShutterGlobal)
+        return GSB200_E_INVALID;
+    if((viewmats_rs != nullptr) != (rolling_shutter != kShutterGlobal))
+        return GSB200_E_INVALID;
+    const bool rows = rolling_shutter == kShutterTopToBottom || rolling_shutter == kShutterBottomToTop;
+    const bool cols = rolling_shutter == kShutterLeftToRight || rolling_shutter == kShutterRightToLeft;
+    if((rows && H < 2) || (cols && W < 2))
+        return GSB200_E_INVALID;
     return GSB200_OK;
 }
 
@@ -671,20 +683,6 @@ int eval3d_checks(
         return GSB200_E_INVALID;
     if((double)B * C * N >= 2147483648.0 || (double)B * C * tw * th >= 2147483648.0)
         return GSB200_E_UNSUPPORTED;
-    return GSB200_OK;
-}
-
-// A rolling shutter takes an end pose, the global shutter none; the frame time divides by the rows (or columns) - 1.
-int shutter_checks(const float *viewmats_rs, int rolling_shutter, uint32_t W, uint32_t H)
-{
-    if(rolling_shutter < 0 || rolling_shutter > kShutterGlobal)
-        return GSB200_E_INVALID;
-    if((viewmats_rs != nullptr) != (rolling_shutter != kShutterGlobal))
-        return GSB200_E_INVALID;
-    const bool rows = rolling_shutter == kShutterTopToBottom || rolling_shutter == kShutterBottomToTop;
-    const bool cols = rolling_shutter == kShutterLeftToRight || rolling_shutter == kShutterRightToLeft;
-    if((rows && H < 2) || (cols && W < 2))
-        return GSB200_E_INVALID;
     return GSB200_OK;
 }
 
@@ -725,9 +723,8 @@ extern "C" int gsb200_ut_projection_fwd(
 {
     if(B < 0 || C < 0 || N < 0)
         return GSB200_E_INVALID;
-    if(int rc = gsb::shutter_checks(viewmats_rs, rolling_shutter, image_width, image_height))
-        return rc;
-    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta))
+    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta, viewmats_rs,
+                                   rolling_shutter, image_width, image_height))
         return rc;
     if(camera_model == gsb::kUtFisheye && (tangential_coeffs || thin_prism_coeffs))
         return GSB200_E_INVALID;
@@ -765,9 +762,8 @@ extern "C" int gsb200_eval3d_fwd(
         return GSB200_E_INVALID;
     if(int rc = gsb::eval3d_checks(B, C, N, image_width, image_height, tile_size, tile_width, tile_height))
         return rc;
-    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta))
-        return rc;
-    if(int rc = gsb::shutter_checks(viewmats_rs, rolling_shutter, image_width, image_height))
+    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta, viewmats_rs,
+                                   rolling_shutter, image_width, image_height))
         return rc;
     if(B * C == 0 || image_width == 0 || image_height == 0)
         return GSB200_OK;
@@ -803,9 +799,8 @@ extern "C" int gsb200_eval3d_bwd(
         return GSB200_E_INVALID;
     if(int rc = gsb::eval3d_checks(B, C, N, image_width, image_height, tile_size, tile_width, tile_height))
         return rc;
-    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta))
-        return rc;
-    if(int rc = gsb::shutter_checks(viewmats_rs, rolling_shutter, image_width, image_height))
+    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta, viewmats_rs,
+                                   rolling_shutter, image_width, image_height))
         return rc;
     if(B * N == 0)
         return GSB200_OK;

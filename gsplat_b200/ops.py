@@ -2680,32 +2680,30 @@ def _ftheta_ptr(params) -> int:
     return 0 if params is None else ctypes.addressof(params)
 
 
-def _ut_shutter(what, rolling_shutter, viewmats_rs, viewmats: Tensor, width: int, height: int):
-    """Checks the shutter arguments of the 3DGUT operators.  A rolling shutter needs ``viewmats_rs`` and the global one
-    takes none (NotImplementedError, naming the argument); a rolling shutter over a single row or column has no frame
-    time (ValueError).  Returns (shutter type id, viewmats_rs contiguous or None)."""
-    shutter = _shutter_type(rolling_shutter)
-    if shutter == RollingShutterType.GLOBAL:
-        if viewmats_rs is not None:
-            raise NotImplementedError(f"{what}: viewmats_rs is not supported with the global shutter (rolling_shutter=GLOBAL)")
-        return int(shutter), None
-    if viewmats_rs is None:
-        raise NotImplementedError(f"{what}: rolling_shutter={rolling_shutter!r} requires viewmats_rs, the end-of-frame poses")
-    _check_shape(viewmats_rs, tuple(viewmats.shape), "viewmats_rs")
-    if viewmats_rs.dtype != torch.float32:
-        raise TypeError(f"{what}: viewmats_rs must be float32, got {viewmats_rs.dtype}")
-    rows = shutter in (RollingShutterType.ROLLING_TOP_TO_BOTTOM, RollingShutterType.ROLLING_BOTTOM_TO_TOP)
-    if (height if rows else width) < 2:
-        raise ValueError(f"{what}: rolling_shutter={shutter.name} needs at least two image {'rows' if rows else 'columns'}, "
-                         f"got {width}x{height}")
-    return int(shutter), viewmats_rs.contiguous()
+class _UtCamera(NamedTuple):
+    """A checked 3DGUT camera, shared by the projection and the compositing: the camera model id, the coefficient
+    tensors [..., C, k] float32 (None where absent), the FTheta parameters (a gsb200_ftheta_params, or None for the other
+    models), the shutter type id, the end-of-frame poses (detached and contiguous, None under the global shutter) and
+    the depth order."""
+
+    model: int
+    radial: Optional[Tensor]
+    tangential: Optional[Tensor]
+    thin: Optional[Tensor]
+    ftheta: Optional["_cabi.FThetaParams"]
+    shutter: int
+    viewmats_rs: Optional[Tensor]
+    global_z_order: bool
 
 
-def _ut_camera(what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
-               external_distortion_coeffs, cams: tuple, global_z_order: bool = True):
-    """Rejects what the 3DGUT kernels are not built for (NotImplementedError, naming the argument) and checks the
-    camera parameters.  Returns the camera model id, the coefficient tensors as [..., C, k] float32 and the FTheta
-    parameters (a gsb200_ftheta_params, or None for the other models)."""
+def _ut_camera(what, viewmats: Tensor, width: int, height: int, camera_model, radial_coeffs, tangential_coeffs,
+               thin_prism_coeffs, ftheta_coeffs, lidar_coeffs, external_distortion_coeffs, rolling_shutter, viewmats_rs,
+               global_z_order: bool = True) -> _UtCamera:
+    """Checks the camera and shutter arguments of the 3DGUT path.  What the kernels are not built for raises
+    NotImplementedError, naming the argument: lidar and external distortion, the camera arguments of another model, a
+    rolling shutter without ``viewmats_rs`` or ``viewmats_rs`` under the global shutter.  Malformed values raise
+    ValueError (or TypeError for a dtype), among them a rolling shutter over a single row or column, which has no frame
+    time."""
     for name, v in (("lidar_coeffs", lidar_coeffs), ("external_distortion_coeffs", external_distortion_coeffs)):
         if v is not None:
             raise NotImplementedError(f"{what}: {name} is not supported (pinhole / fisheye / ftheta only)")
@@ -2721,25 +2719,41 @@ def _ut_camera(what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_
     if not global_z_order and camera_model != "ftheta":
         raise NotImplementedError(f"{what}: global_z_order=False is not supported with camera_model={camera_model!r} "
                                   "(the Euclidean depth order is built for ftheta cameras)")
+    coeffs, ftheta = [None, None, None], None
     if camera_model == "ftheta":
         for name, v in (("radial_coeffs", radial_coeffs), ("tangential_coeffs", tangential_coeffs),
                         ("thin_prism_coeffs", thin_prism_coeffs)):
             if v is not None:
                 raise ValueError(f"{what}: {name} does not apply to the ftheta camera (its distortion is ftheta_coeffs)")
-        return _UT_CAMERAS[camera_model], None, None, None, _ftheta_params(what, ftheta_coeffs)
-    if camera_model == "fisheye":
-        for name, v in (("tangential_coeffs", tangential_coeffs), ("thin_prism_coeffs", thin_prism_coeffs)):
+        ftheta = _ftheta_params(what, ftheta_coeffs)
+    else:
+        if camera_model == "fisheye":
+            for name, v in (("tangential_coeffs", tangential_coeffs), ("thin_prism_coeffs", thin_prism_coeffs)):
+                if v is not None:
+                    raise ValueError(f"{what}: {name} applies to the pinhole camera only")
+        widths = (("radial_coeffs", radial_coeffs, 6 if camera_model == "pinhole" else 4),
+                  ("tangential_coeffs", tangential_coeffs, 2), ("thin_prism_coeffs", thin_prism_coeffs, 4))
+        for i, (name, v, k) in enumerate(widths):
             if v is not None:
-                raise ValueError(f"{what}: {name} applies to the pinhole camera only")
-    widths = (("radial_coeffs", radial_coeffs, 6 if camera_model == "pinhole" else 4),
-              ("tangential_coeffs", tangential_coeffs, 2), ("thin_prism_coeffs", thin_prism_coeffs, 4))
-    out = []
-    for name, v, k in widths:
-        if v is not None:
-            _check_shape(v, cams + (k,), name)
-            v = f32c(v, name)
-        out.append(v)
-    return (_UT_CAMERAS[camera_model], *out, None)
+                _check_shape(v, tuple(viewmats.shape[:-2]) + (k,), name)
+                coeffs[i] = f32c(v, name)
+
+    shutter = _shutter_type(rolling_shutter)
+    if shutter == RollingShutterType.GLOBAL:
+        if viewmats_rs is not None:
+            raise NotImplementedError(f"{what}: viewmats_rs is not supported with the global shutter (rolling_shutter=GLOBAL)")
+    else:
+        if viewmats_rs is None:
+            raise NotImplementedError(f"{what}: rolling_shutter={rolling_shutter!r} requires viewmats_rs, the end-of-frame poses")
+        _check_shape(viewmats_rs, tuple(viewmats.shape), "viewmats_rs")
+        if viewmats_rs.dtype != torch.float32:
+            raise TypeError(f"{what}: viewmats_rs must be float32, got {viewmats_rs.dtype}")
+        rows = shutter in (RollingShutterType.ROLLING_TOP_TO_BOTTOM, RollingShutterType.ROLLING_BOTTOM_TO_TOP)
+        if (height if rows else width) < 2:
+            raise ValueError(f"{what}: rolling_shutter={shutter.name} needs at least two image {'rows' if rows else 'columns'}, "
+                             f"got {width}x{height}")
+        viewmats_rs = viewmats_rs.detach().contiguous()
+    return _UtCamera(_UT_CAMERAS[camera_model], *coeffs, ftheta, int(shutter), viewmats_rs, bool(global_z_order))
 
 
 def _ut_geometry(what, means, quats, scales, viewmats, Ks) -> tuple:
@@ -2759,7 +2773,6 @@ def _ut_geometry(what, means, quats, scales, viewmats, Ks) -> tuple:
     return batch, C, N
 
 
-@torch.no_grad()
 def fully_fused_projection_with_ut(
     means: Tensor,  # [..., N, 3]
     quats: Tensor,  # [..., N, 4]
@@ -2805,18 +2818,23 @@ def fully_fused_projection_with_ut(
     up to 10 times from the start pose's projection); the depths and the near / far cull take the mid-frame pose."""
     what = "fully_fused_projection_with_ut"
     batch, C, N = _ut_geometry(what, means, quats, scales, viewmats, Ks)
-    cam, radial, tangential, thin, ftheta = _ut_camera(
-        what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
-        external_distortion_coeffs, batch + (C,), global_z_order,
-    )
-    shutter, viewmats_rs = _ut_shutter(what, rolling_shutter, viewmats_rs, viewmats, width, height)
+    cam = _ut_camera(what, viewmats, width, height, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs,
+                     ftheta_coeffs, lidar_coeffs, external_distortion_coeffs, rolling_shutter, viewmats_rs, global_z_order)
     if opacities is not None:
         _check_shape(opacities, batch + (N,), "opacities")
-        opacities = f32c(opacities, "opacities")
-    alpha, beta, kappa, margin, require_all = _ut_params(ut_params)
-    dev = require_cuda(means, quats, scales, viewmats, Ks, opacities, radial, tangential, thin, viewmats_rs)
+    return _project_ut(means, quats, scales, opacities, viewmats, Ks, width, height, eps2d, near_plane, far_plane,
+                       radius_clip, calc_compensations, _ut_params(ut_params), cam)
+
+
+@torch.no_grad()
+def _project_ut(means, quats, scales, opacities, viewmats, Ks, width, height, eps2d, near_plane, far_plane, radius_clip,
+                calc_compensations, ut: tuple, cam: _UtCamera):
+    """fully_fused_projection_with_ut on checked arguments: ``ut`` from _ut_params, ``cam`` from _ut_camera."""
+    batch, C, N = tuple(means.shape[:-2]), viewmats.shape[-3], means.shape[-2]
+    alpha, beta, kappa, margin, require_all = ut
+    opacities = None if opacities is None else f32c(opacities, "opacities")
+    dev = require_cuda(means, quats, scales, viewmats, Ks, opacities, cam.radial, cam.tangential, cam.thin, cam.viewmats_rs)
     means, quats, scales, viewmats, Ks = (t.contiguous() for t in (means, quats, scales, viewmats, Ks))
-    B = _prod(batch)
     o = dict(device=dev, dtype=torch.float32)
     radii = torch.empty(batch + (C, N, 2), device=dev, dtype=torch.int32)
     means2d = torch.empty(batch + (C, N, 2), **o)
@@ -2826,22 +2844,21 @@ def fully_fused_projection_with_ut(
     with _Ctx(dev) as st:
         check(
             lib().gsb200_ut_projection_fwd(
-                B, C, N, ptr(means), ptr(quats), ptr(scales), ptr(opacities), ptr(viewmats), ptr(Ks), cam, ptr(radial),
-                ptr(tangential), ptr(thin), _ftheta_ptr(ftheta), ptr(viewmats_rs), shutter, int(bool(global_z_order)),
-                int(width), int(height), float(eps2d),
-                float(near_plane), float(far_plane),
-                float(radius_clip), alpha, beta, kappa, margin, int(require_all), ptr(radii), ptr(means2d), ptr(depths),
-                ptr(conics), ptr(comps), st,
+                _prod(batch), C, N, ptr(means), ptr(quats), ptr(scales), ptr(opacities), ptr(viewmats), ptr(Ks), cam.model,
+                ptr(cam.radial), ptr(cam.tangential), ptr(cam.thin), _ftheta_ptr(cam.ftheta), ptr(cam.viewmats_rs),
+                cam.shutter, int(cam.global_z_order), int(width), int(height), float(eps2d), float(near_plane),
+                float(far_plane), float(radius_clip), alpha, beta, kappa, margin, int(require_all), ptr(radii),
+                ptr(means2d), ptr(depths), ptr(conics), ptr(comps), st,
             ),
-            what,
+            "fully_fused_projection_with_ut",
         )
     return radii, means2d, depths, conics, comps
 
 
 class _RasterizeToPixelsEval3D(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, radial, tangential,
-                thin, ftheta, viewmats_rs, shutter, width, height, isect_offsets, flatten_ids):
+    def forward(ctx, means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam: _UtCamera, width, height,
+                isect_offsets, flatten_ids):
         dev = require_cuda(means, quats, scales, colors, opacities, viewmats, Ks)
         means, quats, scales = means.contiguous(), quats.contiguous(), scales.contiguous()
         colors, opacities = f32c(colors, "colors"), f32c(opacities, "opacities")
@@ -2871,24 +2888,24 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
                 check(
                     lib().gsb200_eval3d_fwd(
                         B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds),
-                        ptr(m8), ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), _ftheta_ptr(ftheta),
-                        ptr(viewmats_rs), shutter, width, height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_colors),
+                        ptr(m8), ptr(viewmats), ptr(Ks), cam.model, ptr(cam.radial), ptr(cam.tangential), ptr(cam.thin),
+                        _ftheta_ptr(cam.ftheta), ptr(cam.viewmats_rs), cam.shutter, width, height, 16, tw, th, ptr(offsets),
+                        ptr(fl), S, ptr(render_colors),
                         ptr(render_alphas), ptr(last_ids), st,
                     ),
                     "rasterize_to_pixels_eval3d",
                 )
-        ctx.save_for_backward(means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, radial, tangential, thin,
-                              viewmats_rs, offsets, fl, render_alphas, last_ids)
+        ctx.save_for_backward(means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, offsets, fl,
+                              render_alphas, last_ids)
         ctx.set_materialize_grads(False)
-        ctx.meta = (B, C, N, D, cam, ftheta, shutter, width, height, tw, th, S)
+        ctx.meta = (B, C, N, D, cam, width, height, tw, th, S)
         ctx.mark_non_differentiable(last_ids)
         return render_colors, render_alphas
 
     @staticmethod
     def backward(ctx, v_render_colors, v_render_alphas):
-        (means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, radial, tangential, thin, viewmats_rs,
-         offsets, fl, render_alphas, last_ids) = ctx.saved_tensors
-        B, C, N, D, cam, ftheta, shutter, width, height, tw, th, S = ctx.meta
+        means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, offsets, fl, render_alphas, last_ids = ctx.saved_tensors
+        B, C, N, D, cam, width, height, tw, th, S = ctx.meta
         dev = render_alphas.device
         if v_render_colors is None:
             v_render_colors = torch.zeros(render_alphas.shape[:-1] + (D,), device=dev, dtype=torch.float32)
@@ -2901,9 +2918,9 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
             check(
                 lib().gsb200_eval3d_bwd(
                     B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds), ptr(m8),
-                    ptr(viewmats), ptr(Ks), cam, ptr(radial), ptr(tangential), ptr(thin), _ftheta_ptr(ftheta),
-                    ptr(viewmats_rs), shutter, width, height, 16, tw, th, ptr(offsets), ptr(fl), S, ptr(render_alphas), ptr(last_ids), ptr(v_render_colors),
-                    ptr(v_render_alphas),
+                    ptr(viewmats), ptr(Ks), cam.model, ptr(cam.radial), ptr(cam.tangential), ptr(cam.thin),
+                    _ftheta_ptr(cam.ftheta), ptr(cam.viewmats_rs), cam.shutter, width, height, 16, tw, th, ptr(offsets),
+                    ptr(fl), S, ptr(render_alphas), ptr(last_ids), ptr(v_render_colors), ptr(v_render_alphas),
                     ptr(records), ptr(v_colors), ptr(v_opacities), ptr(v_means), ptr(v_quats), ptr(v_scales), st,
                 ),
                 "rasterize_to_pixels_eval3d_bwd",
@@ -2911,8 +2928,8 @@ class _RasterizeToPixelsEval3D(torch.autograd.Function):
         v_backgrounds = None
         if backgrounds is not None and ctx.needs_input_grad[5]:
             v_backgrounds = (v_render_colors * (1.0 - render_alphas)).sum(dim=(-3, -2))
-        # viewmats, viewmats_rs, Ks and the camera coefficients get no gradient, as in the reference's backward
-        return (v_means, v_quats, v_scales, v_colors, v_opacities, v_backgrounds) + (None,) * 14
+        # viewmats, Ks and the camera (its coefficients, viewmats_rs) get no gradient, as in the reference's backward
+        return (v_means, v_quats, v_scales, v_colors, v_opacities, v_backgrounds) + (None,) * 8
 
 
 def rasterize_to_pixels_eval3d(
@@ -2975,11 +2992,8 @@ def rasterize_to_pixels_eval3d(
         raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
     batch, C, N = _ut_geometry(what, means, quats, scales, viewmats, Ks)
     image_dims = batch + (C,)
-    cam, radial, tangential, thin, ftheta = _ut_camera(
-        what, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, lidar_coeffs,
-        external_distortion_coeffs, image_dims,
-    )
-    shutter, viewmats_rs = _ut_shutter(what, rolling_shutter, viewmats_rs, viewmats, image_width, image_height)
+    cam = _ut_camera(what, viewmats, image_width, image_height, camera_model, radial_coeffs, tangential_coeffs,
+                     thin_prism_coeffs, ftheta_coeffs, lidar_coeffs, external_distortion_coeffs, rolling_shutter, viewmats_rs)
     _ut_params(ut_params)
     if colors.dim() != len(image_dims) + 2:
         raise ValueError(f"{what}: colors must be [..., C, N, channels], got {tuple(colors.shape)}")
@@ -3002,9 +3016,14 @@ def rasterize_to_pixels_eval3d(
             raise TypeError(f"{what}: {name} must be float32, got {t.dtype}")
     if D not in _SUPPORTED_CHANNELS:
         raise NotImplementedError(f"{what}: {D} channels; the eval3d kernels are built for {_SUPPORTED_CHANNELS}")
+    return _rasterize_eval3d(means, quats, scales, colors, opacities, viewmats, Ks, image_width, image_height,
+                             isect_offsets, flatten_ids, backgrounds, masks, cam)
+
+
+def _rasterize_eval3d(means, quats, scales, colors, opacities, viewmats, Ks, width, height, isect_offsets, flatten_ids,
+                      backgrounds, masks, cam: _UtCamera):
+    """rasterize_to_pixels_eval3d on checked arguments: ``cam`` from _ut_camera."""
     require_cuda(means, quats, scales, colors, opacities, viewmats, Ks, backgrounds, masks, isect_offsets, flatten_ids,
-                 radial, tangential, thin, viewmats_rs)
-    return _RasterizeToPixelsEval3D.apply(
-        means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, radial, tangential, thin, ftheta,
-        viewmats_rs, shutter, int(image_width), int(image_height), isect_offsets, flatten_ids,
-    )
+                 cam.radial, cam.tangential, cam.thin, cam.viewmats_rs)
+    return _RasterizeToPixelsEval3D.apply(means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam,
+                                          int(width), int(height), isect_offsets, flatten_ids)

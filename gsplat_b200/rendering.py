@@ -31,19 +31,20 @@ from torch import Tensor
 
 from .ops import (
     _SUPPORTED_CHANNELS,
-    _ftheta_params,
+    _project_ut,
+    _rasterize_eval3d,
     _shutter_type,
+    _ut_camera,
+    _ut_geometry,
     _ut_params,
     RollingShutterType,
     RowSideOutputs,
     fully_fused_projection,
     fully_fused_projection_2dgs,
-    fully_fused_projection_with_ut,
     fused_project_sh,
     isect_tiles_sorted,
     rasterize_to_pixels,
     rasterize_to_pixels_2dgs,
-    rasterize_to_pixels_eval3d,
     rasterize_to_pixels_rows,
     spherical_harmonics,
     spherical_harmonics_rows,
@@ -550,53 +551,19 @@ def _rasterization_3dgut(
         _unsupported(f"render_mode={render_mode!r}", "hit-distance modes are not built for 3DGUT")
     if return_normals:
         _unsupported("return_normals", "normals are not built for 3DGUT")
-    for name, val in (
-        ("rays", rays), ("lidar_coeffs", lidar_coeffs), ("external_distortion_coeffs", external_distortion_coeffs),
-        ("extra_signals", extra_signals),
-    ):
+    for name, val in (("rays", rays), ("extra_signals", extra_signals)):
         if val is not None:
             _unsupported(name, "not built for 3DGUT (pinhole / fisheye / ftheta cameras, colour and depth channels)")
-    shutter = _shutter_type(rolling_shutter)
-    if shutter == RollingShutterType.GLOBAL and viewmats_rs is not None:
-        _unsupported("viewmats_rs", "the end-of-frame poses belong to a rolling shutter (rolling_shutter=GLOBAL)")
-    if shutter != RollingShutterType.GLOBAL and viewmats_rs is None:
-        _unsupported(f"rolling_shutter={rolling_shutter!r}", "a rolling shutter requires viewmats_rs, the end-of-frame poses")
-    if ftheta_coeffs is not None and camera_model != "ftheta":
-        _unsupported("ftheta_coeffs", f"the FTheta parameters belong to camera_model='ftheta', not {camera_model!r}")
-    if camera_model not in ("pinhole", "fisheye", "ftheta"):
-        if camera_model in ("ortho", "lidar"):
-            _unsupported(f"camera_model={camera_model!r}", "3DGUT is built for pinhole / fisheye / ftheta cameras")
-        raise ValueError(f"unknown camera_model {camera_model!r}")
-    if camera_model == "ftheta" and ftheta_coeffs is None:
-        _unsupported("camera_model='ftheta'", "an FTheta camera requires ftheta_coeffs (FThetaCameraDistortionParameters)")
-    if not global_z_order and camera_model != "ftheta":
-        _unsupported("global_z_order=False", "the Euclidean depth order is built for ftheta cameras only")
     if renderer_config is not None and type(renderer_config).__name__ != "RendererConfig_MixedBatch":
         _unsupported(f"renderer_config={type(renderer_config).__name__}", "3DGUT is built for RendererConfig_MixedBatch only")
 
     # ---- shapes and dtypes
     has_color = render_mode in _COLOR_MODES
     has_depth = render_mode in _DEPTH_MODES
-    if means.dim() < 2 or means.shape[-1] != 3:
-        raise ValueError(f"means must be [..., N, 3], got {tuple(means.shape)}")
-    batch_dims = tuple(means.shape[:-2])
+    batch_dims, C, N = _ut_geometry("rasterization", means, quats, scales, viewmats, Ks)
     B = math.prod(batch_dims) if batch_dims else 1
-    N = means.shape[-2]
-    if viewmats.dim() != len(batch_dims) + 3:
-        raise ValueError(f"viewmats must be [..., C, 4, 4], got {tuple(viewmats.shape)}")
-    C = viewmats.shape[-3]
-    if tuple(quats.shape) != batch_dims + (N, 4) or tuple(scales.shape) != batch_dims + (N, 3):
-        raise ValueError(f"quats/scales shape mismatch: {tuple(quats.shape)}, {tuple(scales.shape)}")
     if tuple(opacities.shape) != batch_dims + (N,):
         raise ValueError(f"opacities must be [..., N], got {tuple(opacities.shape)}")
-    if tuple(viewmats.shape) != batch_dims + (C, 4, 4) or tuple(Ks.shape) != batch_dims + (C, 3, 3):
-        raise ValueError(f"viewmats/Ks shape mismatch: {tuple(viewmats.shape)}, {tuple(Ks.shape)}")
-    if viewmats_rs is not None and tuple(viewmats_rs.shape) != tuple(viewmats.shape):
-        raise ValueError(f"viewmats_rs must be {tuple(viewmats.shape)}, got {tuple(viewmats_rs.shape)}")
-    rows = shutter in (RollingShutterType.ROLLING_TOP_TO_BOTTOM, RollingShutterType.ROLLING_BOTTOM_TO_TOP)
-    if shutter != RollingShutterType.GLOBAL and (height if rows else width) < 2:
-        raise ValueError(f"rolling_shutter={shutter.name} needs at least two image {'rows' if rows else 'columns'}, "
-                         f"got {width}x{height}")
     n_ch = int(has_depth)
     if has_color:
         if colors is None:
@@ -613,19 +580,16 @@ def _rasterization_3dgut(
         raise ValueError(
             f"channel_chunk={channel_chunk}: the eval3d kernels composite up to {_SUPPORTED_CHANNELS[-1]} channels per pass"
         )
-    _ut_params(ut_params)
-    if ftheta_coeffs is not None:
-        _ftheta_params("rasterization", ftheta_coeffs)  # malformed parameters: ValueError before the device is touched
-    cams = dict(camera_model=camera_model, radial_coeffs=radial_coeffs, tangential_coeffs=tangential_coeffs,
-                thin_prism_coeffs=thin_prism_coeffs, ftheta_coeffs=ftheta_coeffs, rolling_shutter=int(shutter),
-                viewmats_rs=None if viewmats_rs is None else viewmats_rs.detach())
+
+    # ---- the camera, checked once for the projection and every channel chunk
+    cam = _ut_camera("rasterization", viewmats, width, height, camera_model, radial_coeffs, tangential_coeffs,
+                     thin_prism_coeffs, ftheta_coeffs, lidar_coeffs, external_distortion_coeffs, rolling_shutter,
+                     viewmats_rs, global_z_order)
+    ut = _ut_params(ut_params)
 
     # ---- projection through the camera model (no gradient, as in the reference)
-    radii, means2d, depths, conics, _ = fully_fused_projection_with_ut(
-        means, quats, scales, opacities, viewmats, Ks, width, height, eps2d=eps2d, near_plane=near_plane,
-        far_plane=far_plane, radius_clip=radius_clip, calc_compensations=False, ut_params=ut_params,
-        global_z_order=global_z_order, **cams,
-    )
+    radii, means2d, depths, conics, _ = _project_ut(means, quats, scales, opacities, viewmats, Ks, width, height, eps2d,
+                                                    near_plane, far_plane, radius_clip, False, ut, cam)
     # the SH view directions are the only path by which viewmats (and viewmats_rs) get a gradient
     feat = (_color_features(colors, sh_degree, means, viewmats, radii, batch_dims, C, N, viewmats_rs=viewmats_rs)
             if has_color else None)
@@ -650,10 +614,8 @@ def _rasterization_3dgut(
         if pad:
             f = torch.nn.functional.pad(f, (0, pad))
             bg = torch.nn.functional.pad(bg, (0, pad)) if bg is not None else None
-        rc, ra = rasterize_to_pixels_eval3d(
-            means, quats, scales, f, opac, viewmats, Ks, width, height, tile_size, isect_offsets, flatten_ids,
-            backgrounds=bg, ut_params=ut_params, **cams,
-        )
+        rc, ra = _rasterize_eval3d(means, quats, scales, f, opac, viewmats, Ks, width, height, isect_offsets, flatten_ids,
+                                   bg, None, cam)
         outs.append(rc[..., :D] if pad else rc)
         if render_alphas is None:
             render_alphas = ra

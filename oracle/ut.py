@@ -9,6 +9,25 @@ valid when it projects in front of the camera inside the image grown by the marg
 also radial factor > 0.8; fisheye: also below the model's maximum angle); the row is valid when any point is (all,
 with require_all_sigma_points_valid).  The ray response of a gaussian is exp(-|g x a|^2 / 2) with a = M (o - mu),
 g = M d / |M d|, M = S^-1 R^T, zero when the closest approach lies behind the origin.
+
+FTheta: a ray at angle theta from the optical axis lands at the pixel distance delta = fw(theta) from the principal
+point, fw the forward polynomial (angle -> pixel distance); bw, the backward polynomial (pixel distance -> angle), is
+calibrated together with it.  The reference polynomial (reference_poly 0: bw, 1: fw) is evaluated directly, the other
+direction inverts it by three Newton steps starting from the other polynomial, stopping early once a step is below
+1e-6.  The image offset is [[c, d], [e, 1]] times the radial offset delta * (x, y) / |(x, y)|, about the principal
+point Ks (cx, cy) + 0.5.  Projection: no z > 0 requirement; theta is clamped to max_angle and a point is valid below
+max_angle, inside the image grown by the margin; the Newton convergence flag is ignored.  Unprojection: invalid where
+the linear map is singular (|c - e d| < 1e-8) or, with the forward polynomial as the reference, where the last Newton
+step stays at or above 1e-6.  With global_z_order=False the near / far cull and the depth take the distance |mean_c|
+from the camera centre instead of z.
+
+Rolling shutter: every image row (or column) is exposed at its own pose, the start pose (viewmat) and the end pose
+(viewmat_rs) interpolated at the row's relative frame time, translation linearly and rotation by slerp of the poses'
+quaternions (taken from the rotation blocks from their largest component).  A sigma point is projected by a fixed-point
+iteration on its frame time, starting from the start pose's projection if it is valid, else the end pose's; a pixel's
+ray leaves at its row's pose; the depth and the near / far cull take the mid-frame pose; the SH view directions are
+taken from the mean of the two camera positions.  The projection, the rays and the compositing take either a view
+matrix (global shutter) or a ShutterPoses.
 """
 from __future__ import annotations
 
@@ -17,8 +36,15 @@ import math
 import torch
 
 F64 = torch.float64
+FLT_EPS = float(torch.finfo(torch.float32).eps)
 ALPHA_T, MAX_ALPHA, T_STOP, EXTEND, MIN_COMP = 1.0 / 255.0, 0.99, 1e-4, 3.33, 0.005
 UT_DEFAULTS = dict(alpha=0.1, beta=2.0, kappa=0.0, in_image_margin_factor=0.1, require_all_sigma_points_valid=False)
+# rolling shutter: ids as the reference's RollingShutterType
+TOP_TO_BOTTOM, LEFT_TO_RIGHT, BOTTOM_TO_TOP, RIGHT_TO_LEFT, GLOBAL = 0, 1, 2, 3, 4
+RS_ITERATIONS = 10
+# FTheta
+PIXELDIST_TO_ANGLE, ANGLE_TO_PIXELDIST = 0, 1
+NEWTON_STEPS, NEWTON_TOL = 3, 1e-6
 
 
 class Camera:
@@ -138,14 +164,201 @@ def quat_to_rotmat(q):
     ], -1).reshape(q.shape[:-1] + (3, 3))
 
 
-def ut_projection(means, quats, scales, opacities, viewmat, cam: Camera, eps2d=0.3, near_plane=0.01, far_plane=1e10,
-                  radius_clip=0.0, ut=None):
-    """One camera, N gaussians.  Returns dict of float64 radii [N, 2] (0: culled), means2d, depths, conics,
-    compensations, the unrounded radii and the margins of the decisions that cull a row (for threshold tests)."""
+def poly(c, x):
+    y = torch.zeros_like(x)
+    for k in reversed(c):
+        y = y * x + k
+    return y
+
+
+def dpoly(c):
+    return [k * c[k] for k in range(1, len(c))]
+
+
+def newton(ref, approx, y):
+    """x with ref(x) = y: three Newton steps from approx(y), each element stopping once its step is below 1e-6.
+    Returns (x, converged, |last step|)."""
+    d = dpoly(ref)
+    x = poly(approx, y)
+    live = torch.ones_like(x, dtype=torch.bool)
+    step = torch.full_like(x, math.inf)
+    for _ in range(NEWTON_STEPS):
+        dx = (poly(ref, x) - y) / poly(d, x)
+        x = torch.where(live, x - dx, x)
+        step = torch.where(live, dx.abs(), step)
+        live = live & ~(dx.abs() < NEWTON_TOL)
+    return x, ~live, step
+
+
+class FThetaCamera:
+    """One FTheta camera: the shared parameters (dict with the five fields of FThetaCameraDistortionParameters), its
+    principal point from K (cx, cy), the image size.  ``last_step`` after unproject: each pixel's last Newton step
+    (forward reference), for tests that exclude pixels at the 1e-6 convergence threshold."""
+
+    def __init__(self, params, K, W, H):
+        K = torch.as_tensor(K, dtype=F64)
+        self.W, self.H = int(W), int(H)
+        self.cx, self.cy = float(K[0, 2]) + 0.5, float(K[1, 2]) + 0.5
+        self.ref = int(params["reference_poly"])
+        self.bw = [float(x) for x in params["pixeldist_to_angle_poly"]]
+        self.fw = [float(x) for x in params["angle_to_pixeldist_poly"]]
+        self.max_angle = float(params["max_angle"])
+        self.c, self.d, self.e = (float(x) for x in params["linear_cde"])
+        self.last_step = None
+
+    def delta_of_angle(self, th):
+        if self.ref == ANGLE_TO_PIXELDIST:
+            return poly(self.fw, th)
+        return newton(self.bw, self.fw, th)[0]
+
+    def project(self, pc, margin):
+        """camera-frame points [..., 3] -> (uv [..., 2], valid [...]); an invalid point keeps its image point."""
+        x, y, z = pc[..., 0], pc[..., 1], pc[..., 2]
+        rxy = torch.sqrt(x * x + y * y)
+        rxy = torch.where(rxy <= 0, torch.full_like(rxy, FLT_EPS), rxy)
+        th_full = torch.atan2(rxy, z)
+        th = torch.minimum(th_full, torch.full_like(th_full, self.max_angle))
+        delta = self.delta_of_angle(th)
+        ix, iy = delta * (x / rxy), delta * (y / rxy)
+        u = self.c * ix + self.d * iy + self.cx
+        v = self.e * ix + iy + self.cy
+        mx, my = self.W * margin, self.H * margin
+        inb = (u >= -mx) & (u < self.W + mx) & (v >= -my) & (v < self.H + my)
+        return torch.stack([u, v], -1), inb & (th_full < self.max_angle)
+
+    def unproject(self, u, v):
+        """image points -> (unit camera rays [..., 3], valid)."""
+        u, v = torch.as_tensor(u, dtype=F64), torch.as_tensor(v, dtype=F64)
+        x, y = u - self.cx, v - self.cy
+        det = self.c - self.e * self.d
+        if abs(det) < 1e-8:
+            z = torch.zeros_like(x)
+            self.last_step = z
+            return torch.stack([z, z, torch.ones_like(x)], -1), torch.zeros_like(x, dtype=torch.bool)
+        ux, uy = (x - self.d * y) / det, (-self.e * x + self.c * y) / det
+        delta = torch.sqrt(ux * ux + uy * uy)
+        if self.ref == PIXELDIST_TO_ANGLE:
+            th, ok = poly(self.bw, delta), torch.ones_like(delta, dtype=torch.bool)
+            self.last_step = torch.zeros_like(delta)
+        else:
+            th, ok, self.last_step = newton(self.fw, self.bw, delta)
+        big = delta >= 1e-6
+        sc = torch.where(big, torch.sin(th) / torch.where(big, delta, torch.ones_like(delta)), torch.zeros_like(delta))
+        d = torch.stack([sc * ux, sc * uy, torch.where(big, torch.cos(th), torch.ones_like(th))], -1)
+        return d, ok
+
+
+def quat_from_rotmat(R):
+    """Unit quaternion (w, x, y, z) of a rotation matrix [3, 3], from its largest component."""
+    R = torch.as_tensor(R, dtype=F64)
+    f = torch.stack([R[0, 0] + R[1, 1] + R[2, 2], R[0, 0] - R[1, 1] - R[2, 2], R[1, 1] - R[0, 0] - R[2, 2],
+                     R[2, 2] - R[0, 0] - R[1, 1]])
+    big = int(torch.argmax(f))  # the first of equal maxima, as a strict > scan
+    v = torch.sqrt(f[big] + 1) * 0.5
+    m = 0.25 / v
+    wx, wy, wz = (R[2, 1] - R[1, 2]) * m, (R[0, 2] - R[2, 0]) * m, (R[1, 0] - R[0, 1]) * m
+    xy, xz, yz = (R[1, 0] + R[0, 1]) * m, (R[0, 2] + R[2, 0]) * m, (R[2, 1] + R[1, 2]) * m
+    return torch.stack([(v, wx, wy, wz), (wx, v, xy, xz), (wy, xy, v, yz), (wz, xz, yz, v)][big])
+
+
+def slerp(q0, q1, a):
+    """Normalised slerp of two unit quaternions at a (a tensor [P], not clamped) -> [P, 4]: the short arc, a
+    component-wise lerp when cos(theta) > 1 - FLT_EPSILON."""
+    a = torch.as_tensor(a, dtype=F64).reshape(-1, 1)
+    c = float((q0 * q1).sum())
+    if c < 0:
+        q1, c = -q1, -c
+    if c > 1 - FLT_EPS:
+        q = q0 * (1 - a) + q1 * a
+    else:
+        th = math.acos(c)
+        q = (torch.sin((1 - a) * th) * q0 + torch.sin(a * th) * q1) / math.sin(th)
+    return q / q.norm(dim=-1, keepdim=True)
+
+
+def frame_time(shutter, W, H, u, v):
+    """Relative frame time of image points (u, v): that of their row (or column)."""
+    u, v = torch.as_tensor(u, dtype=F64), torch.as_tensor(v, dtype=F64)
+    if shutter == TOP_TO_BOTTOM:
+        return torch.floor(v) / (H - 1)
+    if shutter == LEFT_TO_RIGHT:
+        return torch.floor(u) / (W - 1)
+    if shutter == BOTTOM_TO_TOP:
+        return (H - torch.ceil(v)) / (H - 1)
+    return (W - torch.ceil(u)) / (W - 1)
+
+
+class ShutterPoses:
+    """A rolling-shutter camera: its start and end poses (row-major 4x4 view matrices) as quaternions and translations,
+    and the shutter type; ``at(a)`` -> (R [P, 3, 3], t [P, 3]) at relative frame times a [P]: translation lerp,
+    rotation slerp."""
+
+    def __init__(self, viewmat, viewmat_rs, shutter):
+        vm0, vm1 = torch.as_tensor(viewmat, dtype=F64), torch.as_tensor(viewmat_rs, dtype=F64)
+        self.q0, self.q1 = quat_from_rotmat(vm0[:3, :3]), quat_from_rotmat(vm1[:3, :3])
+        self.t0, self.t1 = vm0[:3, 3], vm1[:3, 3]
+        self.shutter = shutter
+
+    def at(self, a):
+        a = torch.as_tensor(a, dtype=F64).reshape(-1)
+        t = (1 - a)[:, None] * self.t0 + a[:, None] * self.t1
+        return quat_to_rotmat(slerp(self.q0, self.q1, a)), t
+
+
+def rs_project(points, cam, poses: ShutterPoses, margin):
+    """World points [P, 3] -> (uv [P, 2], valid [P], edge [P]) through a rolling shutter: start from the start pose's
+    projection if valid, else the end pose's (neither: invalid, at the end pose's point); then re-project at the frame
+    time of the current point until that time repeats, at most 10 times.  ``edge``: a point whose row (or column)
+    coordinate came within 1e-3 pixel of a boundary on the way, where float32 may pick the neighbouring row's pose."""
+    P = points.shape[0]
+
+    def proj(a):
+        R, t = poses.at(a)
+        return cam.project(torch.einsum("pij,pj->pi", R, points) + t, margin)
+
+    uv0, ok0 = proj(torch.zeros(P, dtype=F64))
+    uv1, ok1 = proj(torch.ones(P, dtype=F64))
+    uv = torch.where(ok0[:, None], uv0, uv1)
+    valid = ok0 | ok1
+    live = valid.clone()
+    prev = torch.full((P,), -math.inf, dtype=F64)
+    coord = 1 if poses.shutter in (TOP_TO_BOTTOM, BOTTOM_TO_TOP) else 0
+    edge = torch.zeros(P, dtype=torch.bool)
+    for _ in range(RS_ITERATIONS):
+        a = frame_time(poses.shutter, cam.W, cam.H, uv[:, 0], uv[:, 1])
+        x = uv[:, coord]
+        edge = edge | (live & ((x - torch.round(x)).abs() < 1e-3))
+        live = live & (a != prev)
+        if not bool(live.any()):
+            break
+        prev = torch.where(live, a, prev)
+        uv_n, ok_n = proj(a)
+        uv = torch.where(live[:, None], uv_n, uv)
+        valid = torch.where(live, ok_n, valid)
+    return uv, valid, edge
+
+
+def rs_sh_viewmat(viewmat, viewmat_rs):
+    """[..., 4, 4] view matrices [I | -c] with c the mean of the two poses' positions -R^T t: the camera position the
+    SH view directions of a rolling-shutter camera are taken from."""
+    vm0, vm1 = torch.as_tensor(viewmat, dtype=F64), torch.as_tensor(viewmat_rs, dtype=F64)
+    pos = lambda vm: -torch.einsum("...ji,...j->...i", vm[..., :3, :3], vm[..., :3, 3])  # noqa: E731
+    out = torch.zeros(vm0.shape, dtype=F64)
+    out[..., :3, :3] = torch.eye(3, dtype=F64)
+    out[..., :3, 3] = -0.5 * (pos(vm0) + pos(vm1))
+    out[..., 3, 3] = 1
+    return out
+
+
+def ut_projection(means, quats, scales, opacities, pose, cam, eps2d=0.3, near_plane=0.01, far_plane=1e10,
+                  radius_clip=0.0, ut=None, global_z_order=True):
+    """One camera, N gaussians; ``pose`` a view matrix [4, 4] or a ShutterPoses.  Returns dict of float64 radii [N, 2]
+    (0: culled), means2d, depths, conics, compensations, the unrounded radii, the sigma points' validity and
+    ``rs_edge`` [N]: the rows with a sigma point near a row (column) boundary of a rolling shutter, where float32 may
+    take the neighbouring row's pose.  Under a rolling shutter the near / far cull and the depth take the mid-frame
+    pose; with global_z_order=False they take |mean_c| instead of z."""
     ut = dict(UT_DEFAULTS, **(ut or {}))
     means, quats, scales = (torch.as_tensor(t, dtype=F64) for t in (means, quats, scales))
-    vm = torch.as_tensor(viewmat, dtype=F64)
-    R, t = vm[:3, :3], vm[:3, 3]
     a, kap = ut["alpha"], ut["kappa"]
     lam = a * a * (3 + kap) - 3
     w_m = [lam / (3 + lam)] + [1 / (2 * (3 + lam))] * 6
@@ -153,14 +366,23 @@ def ut_projection(means, quats, scales, opacities, viewmat, cam: Camera, eps2d=0
     Rq = quat_to_rotmat(quats)
     delta = math.sqrt(3 + lam) * Rq * scales[:, None, :]  # column i = spread * s_i * R[:, i]
     pts = torch.stack([means] + [means + delta[..., i] for i in range(3)] + [means - delta[..., i] for i in range(3)], 1)
-    pc = pts @ R.T + t
-    uv, valid = cam.project(pc, ut["in_image_margin_factor"])
+    margin = ut["in_image_margin_factor"]
+    if isinstance(pose, ShutterPoses):
+        uv, valid, edge = rs_project(pts.reshape(-1, 3), cam, pose, margin)
+        uv, valid, rs_edge = uv.reshape(pts.shape[:-1] + (2,)), valid.reshape(pts.shape[:-1]), edge.reshape(pts.shape[:-1]).any(1)
+        Rs, ts = pose.at(torch.tensor([0.5], dtype=F64))
+        R, t = Rs[0], ts[0]
+    else:
+        vm = torch.as_tensor(pose, dtype=F64)
+        R, t = vm[:3, :3], vm[:3, 3]
+        uv, valid = cam.project(pts @ R.T + t, margin)
+        rs_edge = torch.zeros(len(means), dtype=torch.bool)
     wm, wc = torch.tensor(w_m, dtype=F64), torch.tensor(w_c, dtype=F64)
     mean2d = (wm[None, :, None] * uv).sum(1)
     du = uv - mean2d[:, None]
     cov = (wc[None, :, None, None] * du[..., :, None] * du[..., None, :]).sum(1)
     ok = valid.all(1) if ut["require_all_sigma_points_valid"] else valid.any(1)
-    zc = means @ R.T[:, 2] + t[2]
+    zc = means @ R.T[:, 2] + t[2] if global_z_order else (means @ R.T + t).norm(dim=-1)
     eps = torch.finfo(torch.float32).eps
     ok = ok & (zc >= near_plane) & (zc <= far_plane)
     ok = ok & ((quats * quats).sum(-1).abs() >= eps) & (scales.abs() >= eps).all(-1)
@@ -192,17 +414,22 @@ def ut_projection(means, quats, scales, opacities, viewmat, cam: Camera, eps2d=0
         "conics": torch.where(ok[:, None], conics, torch.zeros_like(conics)),
         "compensations": torch.where(ok, comp, z),
         "sigma_valid": valid,
+        "rs_edge": rs_edge,
     }
 
 
-def pixel_rays(viewmat, cam: Camera):
-    """World rays of every pixel centre: origins [H*W, 3], unit directions [H*W, 3], valid [H*W]."""
-    vm = torch.as_tensor(viewmat, dtype=F64)
-    R, t = vm[:3, :3], vm[:3, 3]
+def pixel_rays(pose, cam):
+    """World rays of every pixel centre: origins [H*W, 3], unit directions [H*W, 3], valid [H*W]; ``pose`` a view
+    matrix or a ShutterPoses, under which each pixel's ray leaves at the pose of its row (column)."""
     jj, ii = torch.meshgrid(torch.arange(cam.W, dtype=F64), torch.arange(cam.H, dtype=F64), indexing="xy")
-    d, ok = cam.unproject(jj.reshape(-1) + 0.5, ii.reshape(-1) + 0.5)
-    o = -(R.T @ t)
-    return o.expand(d.shape), d @ R, ok
+    u, v = jj.reshape(-1) + 0.5, ii.reshape(-1) + 0.5
+    d, ok = cam.unproject(u, v)
+    if isinstance(pose, ShutterPoses):
+        R, t = pose.at(frame_time(pose.shutter, cam.W, cam.H, u, v))
+        return -torch.einsum("pji,pj->pi", R, t), torch.einsum("pji,pj->pi", R, d), ok
+    vm = torch.as_tensor(pose, dtype=F64)
+    R, t = vm[:3, :3], vm[:3, 3]
+    return (-(R.T @ t)).expand(d.shape), d @ R, ok
 
 
 def eval3d_alpha(means, quats, scales, opacities, ro, rd):
@@ -220,9 +447,10 @@ def eval3d_alpha(means, quats, scales, opacities, ro, rd):
     return alpha, hit_t, raw
 
 
-def eval3d_render(means, quats, scales, colors, opacities, viewmat, cam: Camera, isect_offsets, flatten_ids, C, N,
-                  image_index, background=None, mask=None):
-    """Composites one image (index image_index of the [I] = [B*C] images) from its tile lists, front to back.  means /
+def eval3d_render(means, quats, scales, colors, opacities, pose, cam, isect_offsets, flatten_ids, C, N, image_index,
+                  background=None, mask=None):
+    """Composites one image (index image_index of the [I] = [B*C] images, seen from ``pose``, a view matrix or a
+    ShutterPoses) from its tile lists, front to back.  means /
     quats / scales [B*N, *], colors [I*N, D], opacities [I*N] (float64 tensors, autograd flows through).  Returns
     (render_colors [H, W, D], render_alphas [H, W, 1], margins [H, W]: the smallest distance of any decision taken at the
     pixel from its threshold, relative)."""
@@ -230,7 +458,7 @@ def eval3d_render(means, quats, scales, colors, opacities, viewmat, cam: Camera,
     th, tw = isect_offsets.shape[-2:]
     offs = isect_offsets.reshape(-1).tolist()
     n_isects = len(flatten_ids)
-    ro, rd, rok = pixel_rays(viewmat, cam)
+    ro, rd, rok = pixel_rays(pose, cam)
     out_c = [[None] * W for _ in range(H)]
     img = torch.zeros(H, W, D, dtype=F64)
     alp = torch.zeros(H, W, 1, dtype=F64)

@@ -5,7 +5,7 @@
 
 Writes tests/golden/ref_ut_ftheta.npz and tests/golden/ref_ut_ftheta_rasterization.npz on the seeded 96x64 garden
 crop of make_ref_ut_golden.py, through the calibrations of tests/golden/ftheta_calibrations.json scaled to 96 pixels
-wide (tests/ut_ftheta_oracle.scaled; each camera's Ks holds the scaled principal point, fx = fy = 1 unused).
+wide (tests/scene.scaled; each camera's Ks holds the scaled principal point, fx = fy = 1 unused).
 
 ref_ut_ftheta.npz: for every calibration, both reference polynomials (ptoa: pixel distance -> angle, atop: angle ->
 pixel distance) and both depth orders (z: global_z_order=True, dist: False), and for one top-to-bottom
@@ -52,7 +52,6 @@ def record():
     import gsplat_b200 as gs
     from oracle import refcuda
     from tests import scene
-    from tests import ut_ftheta_oracle as F
 
     ops = refcuda.load_ops()
     dev = "cuda"
@@ -71,8 +70,8 @@ def record():
             ref, params["pixeldist_to_angle_poly"], params["angle_to_pixeldist_poly"], params["max_angle"],
             params["linear_cde"])
 
-    for cname, cal in F.calibrations().items():
-        params, pp, _ = F.scaled(cal, W)
+    for cname, cal in scene.calibrations().items():
+        params, pp, _ = scene.scaled(cal, W)
         K = ftheta_K(pp)
         out[f"{cname}/Ks"] = K
         cases = [(p, o, 4) for p in POLYS for o in ORDERS] + [("ptoa", "dist", 0)]
@@ -108,7 +107,7 @@ def record():
     # ---- rasterization_3dgs: SH degree 3, RGB+ED, two cameras with distinct principal points, a background
     full = scene.make_scene(n_max=N_GAUSS, sh_degree=RASTER_SH_DEGREE, seed=0)
     C = RASTER_C
-    params, pp, _ = F.scaled(F.calibrations()[RASTER_CALIBRATION], W)
+    params, pp, _ = scene.scaled(scene.calibrations()[RASTER_CALIBRATION], W)
     inputs = dict(means=full["means"], quats=full["quats"], scales=(full["scales"] * SCALE).astype(np.float32),
                   opacities=full["opacities"], sh=full["sh"], viewmats=full["viewmats"][:C].astype(np.float32),
                   Ks=ftheta_K(pp, C, shift=(3.0, -2.0)))

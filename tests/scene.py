@@ -62,3 +62,24 @@ def rescale_K(Ks: np.ndarray, w0: int, h0: int, w: int, h: int) -> np.ndarray:
     Ks[..., 0, :] *= w / w0
     Ks[..., 1, :] *= h / h0
     return Ks
+
+
+def calibrations():
+    """{name: calibration dict} of tests/golden/ftheta_calibrations.json at native resolution."""
+    import json
+
+    with open(os.path.join(_GOLDEN, "ftheta_calibrations.json")) as f:
+        return {k: v for k, v in json.load(f).items() if not k.startswith("_")}
+
+
+def scaled(cal, width):
+    """The FTheta calibration for an image `width` pixels wide: principal point * s, forward coefficient k * s, backward
+    coefficient k * s^-k, s = width / native width.  Returns (params dict, principal point (cx, cy), (W, H))."""
+    W0, H0 = cal["resolution"]
+    s = width / W0
+    fw = [c * s for c in cal["angle_to_pixeldist_poly"]]
+    bw = [c * s ** (-k) for k, c in enumerate(cal["pixeldist_to_angle_poly"])]
+    pp = (cal["principal_point"][0] * s, cal["principal_point"][1] * s)
+    params = dict(pixeldist_to_angle_poly=bw, angle_to_pixeldist_poly=fw, max_angle=float(cal["max_angle"]),
+                  linear_cde=list(cal["linear_cde"]))
+    return params, pp, (int(width), int(round(H0 * s)))

@@ -11,7 +11,8 @@ import torch
 
 import gsplat_b200 as gs
 from gsplat_b200._cabi import GsplatB200Error
-from tests import ut_ftheta_oracle as F
+from oracle import ut as U
+from tests import scene
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_NPZ = os.path.join(ROOT, "tests", "golden", "ref_ut_ftheta.npz")
@@ -20,7 +21,7 @@ W, H = 96, 64
 
 
 def _params(ref=0, **kw):
-    params, _, _ = F.scaled(F.calibrations()["cross_left_120fov"], W)
+    params, _, _ = scene.scaled(scene.calibrations()["cross_left_120fov"], W)
     params = dict(params, reference_poly=ref)
     params.update(kw)
     return params
@@ -150,10 +151,10 @@ def test_coefficient_arrays_do_not_apply_to_ftheta():
 
 # ---- the oracle
 @pytest.mark.parametrize("ref", [0, 1])
-@pytest.mark.parametrize("cname", list(F.calibrations()))
+@pytest.mark.parametrize("cname", list(scene.calibrations()))
 def test_oracle_round_trip_at_pixel_centres(cname, ref):
-    params, pp, _ = F.scaled(F.calibrations()[cname], W)
-    cam = F.FThetaCamera(dict(params, reference_poly=ref), [[1, 0, pp[0]], [0, 1, pp[1]], [0, 0, 1]], W, H)
+    params, pp, _ = scene.scaled(scene.calibrations()[cname], W)
+    cam = U.FThetaCamera(dict(params, reference_poly=ref), [[1, 0, pp[0]], [0, 1, pp[1]], [0, 0, 1]], W, H)
     jj, ii = torch.meshgrid(torch.arange(W, dtype=torch.float64), torch.arange(H, dtype=torch.float64), indexing="xy")
     u, v = jj.reshape(-1) + 0.5, ii.reshape(-1) + 0.5
     d, ok = cam.unproject(u, v)
@@ -168,29 +169,29 @@ def test_oracle_round_trip_at_pixel_centres(cname, ref):
 
 @pytest.mark.parametrize("cname", ["cross_left_120fov", "front_tele_30fov"])
 def test_scaled_calibration_is_s_times_the_original(cname):
-    cal = F.calibrations()[cname]
-    params, pp, (w, h) = F.scaled(cal, W)
+    cal = scene.calibrations()[cname]
+    params, pp, (w, h) = scene.scaled(cal, W)
     s = W / cal["resolution"][0]
     assert (w, h) == (W, round(cal["resolution"][1] * s))
     np.testing.assert_allclose(pp, np.asarray(cal["principal_point"]) * s)
     th = torch.linspace(0.0, cal["max_angle"], 50, dtype=torch.float64)
-    np.testing.assert_allclose(F.poly(params["angle_to_pixeldist_poly"], th).numpy(),
-                               s * F.poly(cal["angle_to_pixeldist_poly"], th).numpy(), rtol=1e-12, atol=1e-12)
-    delta = F.poly(cal["angle_to_pixeldist_poly"], th)
-    np.testing.assert_allclose(F.poly(params["pixeldist_to_angle_poly"], s * delta).numpy(),
-                               F.poly(cal["pixeldist_to_angle_poly"], delta).numpy(), rtol=1e-9, atol=1e-12)
+    np.testing.assert_allclose(U.poly(params["angle_to_pixeldist_poly"], th).numpy(),
+                               s * U.poly(cal["angle_to_pixeldist_poly"], th).numpy(), rtol=1e-12, atol=1e-12)
+    delta = U.poly(cal["angle_to_pixeldist_poly"], th)
+    np.testing.assert_allclose(U.poly(params["pixeldist_to_angle_poly"], s * delta).numpy(),
+                               U.poly(cal["pixeldist_to_angle_poly"], delta).numpy(), rtol=1e-9, atol=1e-12)
 
 
 def test_synthetic_calibration_sees_beyond_180_degrees():
-    cal = F.calibrations()["synthetic_wide_190"]
+    cal = scene.calibrations()["synthetic_wide_190"]
     assert cal["max_angle"] > math.pi / 2 + 0.2 and cal["reference_poly"] == 0
-    cam = F.FThetaCamera(dict(F.scaled(cal, W)[0], reference_poly=0), [[1, 0, 47.3], [0, 1, 31.6], [0, 0, 1]], W, H)
+    cam = U.FThetaCamera(dict(scene.scaled(cal, W)[0], reference_poly=0), [[1, 0, 47.3], [0, 1, 31.6], [0, 0, 1]], W, H)
     pc = torch.tensor([[math.sin(1.75), 0.0, math.cos(1.75)]], dtype=torch.float64) * 2.0  # z < 0
     uv, valid = cam.project(pc, 0.1)
     assert bool(valid[0]) and 0 <= float(uv[0, 0]) < W
 
 
-@pytest.mark.parametrize("cname", list(F.calibrations()))
+@pytest.mark.parametrize("cname", list(scene.calibrations()))
 def test_oracle_reproduces_reference_records(cname):
     import sys
 
@@ -198,15 +199,15 @@ def test_oracle_reproduces_reference_records(cname):
     from make_ref_ut_ftheta_golden import ORDERS, POLYS
 
     z = np.load(REF_NPZ)
-    params, _, _ = F.scaled(F.calibrations()[cname], W)
+    params, _, _ = scene.scaled(scene.calibrations()[cname], W)
     K = z[f"{cname}/Ks"][0]
     for pname, ref in POLYS.items():
         for oname, gzo in ORDERS.items():
             for rolling in ((False, True) if (pname, oname) == ("ptoa", "dist") else (False,)):
                 name = f"{cname}/{pname}/{oname}" + ("/rs" if rolling else "")
-                cam = F.FThetaCamera(dict(params, reference_poly=ref), K, W, H)
-                o = F.ut_projection(z["means"], z["quats"], z["scales"], z["opacities"], z["viewmats"][0], cam,
-                                    global_z_order=gzo, viewmat_rs=z["viewmats_rs"][0], shutter=0 if rolling else 4)
+                cam = U.FThetaCamera(dict(params, reference_poly=ref), K, W, H)
+                pose = U.ShutterPoses(z["viewmats"][0], z["viewmats_rs"][0], 0) if rolling else z["viewmats"][0]
+                o = U.ut_projection(z["means"], z["quats"], z["scales"], z["opacities"], pose, cam, global_z_order=gzo)
                 r, rr = o["radii"].numpy(), z[f"{name}/radii"][0]
                 frac = o["radii_unrounded"].numpy()
                 loose = (np.abs(frac - np.round(frac)) < 1e-3).any(-1) | o["rs_edge"].numpy()

@@ -1,5 +1,5 @@
 """FTheta 3DGUT on the GPU: the UT projection and the eval3d compositing (forward and gradients) against the float64
-oracle (tests/ut_ftheta_oracle.py) and the reference's records (ref_ut_ftheta.npz, make_ref_ut_ftheta_golden.py), for
+oracle (oracle/ut.py) and the reference's records (ref_ut_ftheta.npz, make_ref_ut_ftheta_golden.py), for
 both reference polynomials and both depth orders; a lens beyond 180 degrees; rolling shutter; rasterization() against
 the hand chain; batch dims and cameras sharing one parameter set; the drop-in and a short fit."""
 import os
@@ -12,7 +12,7 @@ import torch
 
 import gsplat_b200 as gs
 from tests import scene
-from tests import ut_ftheta_oracle as F
+from oracle import ut as U
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -25,7 +25,7 @@ from make_ref_ut_rs_golden import cotangents, end_poses  # noqa: E402
 
 W, H = 96, 64
 TW, TH = (W + 15) // 16, (H + 15) // 16
-CALS = list(F.calibrations())
+CALS = list(scene.calibrations())
 
 
 def _t(a, grad=False):
@@ -33,7 +33,7 @@ def _t(a, grad=False):
 
 
 def _cal(name, ref):
-    params, pp, _ = F.scaled(F.calibrations()[name], W)
+    params, pp, _ = scene.scaled(scene.calibrations()[name], W)
     return dict(params, reference_poly=ref), pp
 
 
@@ -90,8 +90,8 @@ def test_projection_against_oracle(cname, ref, gzo):
     params, pp = _cal(cname, ref)
     K = ftheta_K(pp)
     out = _project(p, params, K, gzo)
-    cam = F.FThetaCamera(params, K[0], W, H)
-    o = F.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], p["viewmats"][0], cam, global_z_order=gzo)
+    cam = U.FThetaCamera(params, K[0], W, H)
+    o = U.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], p["viewmats"][0], cam, global_z_order=gzo)
     ok = _check_projection(out, o)
     if not gzo:
         # the depth is the distance from the camera centre
@@ -111,11 +111,11 @@ def _eval_case(p, params, K, offs, fl, bg, shutter=4):
 
 def _check_eval(p, params, K, offs, fl, bg, leaves, rc, ra, v_rc, v_ra, ref=None, shutter=4):
     N = len(p["means"])
-    cam = F.FThetaCamera(params, K[0], W, H)
+    cam = U.FThetaCamera(params, K[0], W, H)
     f8 = [torch.from_numpy(np.asarray(x, np.float64)).requires_grad_(True)
           for x in (p["means"], p["quats"], p["scales"], p["colors"], p["opacities"], bg[0])]
-    oc, oa, margin = F.eval3d_render(*f8[:5], p["viewmats"][0], cam, offs.cpu(), fl.cpu().tolist(), 1, N, 0,
-                                     background=f8[5], viewmat_rs=p["viewmats_rs"][0], shutter=shutter)
+    pose = p["viewmats"][0] if shutter == U.GLOBAL else U.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0], shutter)
+    oc, oa, margin = U.eval3d_render(*f8[:5], pose, cam, offs.cpu(), fl.cpu().tolist(), 1, N, 0, background=f8[5])
     ((oc * torch.from_numpy(v_rc[0].astype(np.float64))).sum() + (oa * torch.from_numpy(v_ra[0].astype(np.float64))).sum()).backward()
     # pixels whose Newton step sits near the 1e-6 convergence threshold may converge in one precision only
     step = cam.last_step.reshape(H, W).numpy()
@@ -163,9 +163,9 @@ def test_rolling_shutter_against_oracle(cname, gzo):
     params, pp = _cal(cname, 0)
     K = ftheta_K(pp)
     out = _project(p, params, K, gzo, shutter=0)
-    cam = F.FThetaCamera(params, K[0], W, H)
-    o = F.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], p["viewmats"][0], cam, global_z_order=gzo,
-                        viewmat_rs=p["viewmats_rs"][0], shutter=0)
+    cam = U.FThetaCamera(params, K[0], W, H)
+    o = U.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"],
+                        U.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0], 0), cam, global_z_order=gzo)
     _check_projection(out, o)
     offs, fl = _lists(*out[:3])
     rng = np.random.RandomState(2)
@@ -192,9 +192,9 @@ def test_kernels_against_reference(cname, pname, oname, rolling):
     K = z[f"{cname}/Ks"]
     gzo, shutter = ORDERS[oname], (0 if rolling else 4)
     out = _project(p, params, K, gzo, shutter)
-    cam = F.FThetaCamera(params, K[0], W, H)
-    o = F.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], p["viewmats"][0], cam, global_z_order=gzo,
-                        viewmat_rs=p["viewmats_rs"][0], shutter=shutter)
+    cam = U.FThetaCamera(params, K[0], W, H)
+    pose = p["viewmats"][0] if shutter == U.GLOBAL else U.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0], shutter)
+    o = U.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], pose, cam, global_z_order=gzo)
     rows = {k: z[f"{name}/{k}"][0] for k in ("radii", "means2d", "depths")}
     _check_projection(out, o, rows)
     # the oracle reproduces the reference's rows too
@@ -230,8 +230,8 @@ def test_beyond_180_degrees():
     assert seen.sum() > n // 2, seen.sum()
     np.testing.assert_allclose(d_far[0].cpu().numpy()[seen], np.linalg.norm(means, axis=-1)[seen], rtol=1e-5)
     assert (r_z[0] == 0).all()  # z < near_plane: culled in the global z order
-    cam = F.FThetaCamera(params, K[0], W, H)
-    o = F.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], p["viewmats"][0], cam, global_z_order=False)
+    cam = U.FThetaCamera(params, K[0], W, H)
+    o = U.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], p["viewmats"][0], cam, global_z_order=False)
     assert ((o["radii"].numpy() > 0).all(-1) == seen).mean() > 0.95
 
 

@@ -12,7 +12,6 @@ import torch
 import gsplat_b200 as gs
 from gsplat_b200._cabi import GsplatB200Error
 from oracle import ut as U
-from tests import ut_rs_oracle as R8
 from tests import scene
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -61,13 +60,13 @@ def test_frame_time_at_pixel_centres():
     W, H = 7, 5
     jj, ii = np.meshgrid(np.arange(W), np.arange(H), indexing="xy")
     u, v = torch.from_numpy(jj + 0.5), torch.from_numpy(ii + 0.5)
-    np.testing.assert_array_equal(R8.frame_time(0, W, H, u, v).numpy(), ii / (H - 1))
-    np.testing.assert_array_equal(R8.frame_time(1, W, H, u, v).numpy(), jj / (W - 1))
-    np.testing.assert_array_equal(R8.frame_time(2, W, H, u, v).numpy(), (H - 1 - ii) / (H - 1))
-    np.testing.assert_array_equal(R8.frame_time(3, W, H, u, v).numpy(), (W - 1 - jj) / (W - 1))
+    np.testing.assert_array_equal(U.frame_time(0, W, H, u, v).numpy(), ii / (H - 1))
+    np.testing.assert_array_equal(U.frame_time(1, W, H, u, v).numpy(), jj / (W - 1))
+    np.testing.assert_array_equal(U.frame_time(2, W, H, u, v).numpy(), (H - 1 - ii) / (H - 1))
+    np.testing.assert_array_equal(U.frame_time(3, W, H, u, v).numpy(), (W - 1 - jj) / (W - 1))
     # not clamped: a point in the margin has a time outside [0, 1]
-    assert float(R8.frame_time(0, W, H, torch.tensor(0.0), torch.tensor(-2.5))) < 0
-    assert float(R8.frame_time(1, W, H, torch.tensor(W + 3.5), torch.tensor(0.0))) > 1
+    assert float(U.frame_time(0, W, H, torch.tensor(0.0), torch.tensor(-2.5))) < 0
+    assert float(U.frame_time(1, W, H, torch.tensor(W + 3.5), torch.tensor(0.0))) > 1
 
 
 def _quat(axis, deg):
@@ -79,17 +78,17 @@ def _quat(axis, deg):
 def test_slerp_ends_and_branches():
     q0, q1 = _quat([0, 0, 1], 10.0), _quat([1, 2, 0], 35.0)
     a = torch.tensor([0.0, 1.0], dtype=torch.float64)
-    np.testing.assert_allclose(R8.slerp(q0, q1, a).numpy(), torch.stack([q0, q1]).numpy(), atol=1e-15)
+    np.testing.assert_allclose(U.slerp(q0, q1, a).numpy(), torch.stack([q0, q1]).numpy(), atol=1e-15)
     # the short arc: -q1 is the same rotation
-    np.testing.assert_allclose(R8.slerp(q0, -q1, a).numpy(), torch.stack([q0, q1]).numpy(), atol=1e-15)
+    np.testing.assert_allclose(U.slerp(q0, -q1, a).numpy(), torch.stack([q0, q1]).numpy(), atol=1e-15)
     # constant angular speed: halfway is half the angle
-    mid = R8.slerp(q0, q1, torch.tensor([0.5], dtype=torch.float64))[0]
+    mid = U.slerp(q0, q1, torch.tensor([0.5], dtype=torch.float64))[0]
     ang = lambda p, q: 2 * math.acos(min(1.0, abs(float((p * q).sum()))))  # noqa: E731
     assert abs(ang(q0, mid) - ang(mid, q1)) < 1e-12
     # near-parallel (cos > 1 - FLT_EPSILON): the normalised component-wise lerp
     q2 = _quat([1, 2, 0], 35.0 + 1e-3)
-    assert float((q1 * q2).sum()) > 1 - R8.FLT_EPS
-    s = R8.slerp(q1, q2, torch.tensor([0.25, 1.5], dtype=torch.float64))
+    assert float((q1 * q2).sum()) > 1 - U.FLT_EPS
+    s = U.slerp(q1, q2, torch.tensor([0.25, 1.5], dtype=torch.float64))
     lerp = torch.stack([0.75 * q1 + 0.25 * q2, -0.5 * q1 + 1.5 * q2])
     np.testing.assert_allclose(s.numpy(), (lerp / lerp.norm(dim=-1, keepdim=True)).numpy(), atol=1e-15)
 
@@ -97,7 +96,7 @@ def test_slerp_ends_and_branches():
 def test_quaternion_of_a_pose():
     for axis, deg in (([0, 0, 1], 10.0), ([1, -2, 3], 170.0), ([1, 0, 0], 179.0), ([0, 1, 0.1], -120.0)):
         q = _quat(axis, deg)
-        got = R8.quat_from_rotmat(U.quat_to_rotmat(q))
+        got = U.quat_from_rotmat(U.quat_to_rotmat(q))
         np.testing.assert_allclose((got * torch.sign((got * q).sum())).numpy(), q.numpy(), atol=1e-14)
 
 
@@ -116,15 +115,15 @@ def test_oracle_without_motion_is_global(shutter, kind, coeffs):
     sc, vm, K, W, H = _small()
     cam = U.Camera(kind, K, W, H, **coeffs)
     s = sc["scales"] * 4.0
-    g = R8.ut_projection(sc["means"], sc["quats"], s, sc["opacities"], vm, cam)
-    r = R8.ut_projection(sc["means"], sc["quats"], s, sc["opacities"], vm, cam, viewmat_rs=vm, shutter=shutter)
+    g = U.ut_projection(sc["means"], sc["quats"], s, sc["opacities"], vm, cam)
+    r = U.ut_projection(sc["means"], sc["quats"], s, sc["opacities"], U.ShutterPoses(vm, vm, shutter), cam)
     assert g["valid"].sum() > 20
     assert torch.equal(g["valid"], r["valid"])
     # the float32 view matrix is orthonormal to ~1e-7 only; its quaternion is the nearest rotation
     for k in ("means2d", "depths", "conics", "compensations"):
         np.testing.assert_allclose(r[k].numpy(), g[k].numpy(), rtol=1e-5, atol=1e-6)
-    o0, d0, ok0 = R8.pixel_rays(vm, cam)
-    o1, d1, ok1 = R8.pixel_rays(vm, cam, vm, shutter)
+    o0, d0, ok0 = U.pixel_rays(vm, cam)
+    o1, d1, ok1 = U.pixel_rays(U.ShutterPoses(vm, vm, shutter), cam)
     assert torch.equal(ok0, ok1)
     np.testing.assert_allclose(o1.numpy(), o0.numpy(), atol=1e-5)
     np.testing.assert_allclose(d1.numpy(), d0.numpy(), atol=1e-6)
@@ -136,7 +135,7 @@ def test_sh_camera_position_is_the_mean():
     vm1 = vm.astype(np.float64).copy()
     vm1[:3, :3] = R @ vm1[:3, :3]
     vm1[:3, 3] += [0.1, -0.2, 0.05]
-    avg = R8.rs_sh_viewmat(vm, vm1).numpy()
+    avg = U.rs_sh_viewmat(vm, vm1).numpy()
     pos = lambda m: -m[:3, :3].T @ m[:3, 3]  # noqa: E731
     np.testing.assert_allclose(pos(avg), 0.5 * (pos(vm.astype(np.float64)) + pos(vm1)), atol=1e-12)
 
@@ -155,8 +154,8 @@ def test_oracle_against_reference(cname, sname):
     W, H = int(z["width"]), int(z["height"])
     model, coeffs = ref_case(z, cname)
     cam = U.Camera(model, z["Ks"][0], W, H, **coeffs)
-    o = R8.ut_projection(z["means"], z["quats"], z["scales"], z["opacities"], z["viewmats"][0], cam,
-                        viewmat_rs=z["viewmats_rs"][0], shutter=SHUTTERS[sname])
+    o = U.ut_projection(z["means"], z["quats"], z["scales"], z["opacities"],
+                        U.ShutterPoses(z["viewmats"][0], z["viewmats_rs"][0], SHUTTERS[sname]), cam)
     name = f"{cname}/{sname}"
     rr = z[f"{name}/radii"][0]
     ro = o["radii"].numpy()

@@ -14,7 +14,6 @@ import torch
 import gsplat_b200 as gs
 from oracle import gso
 from oracle import ut as U
-from tests import ut_rs_oracle as R8
 from tests import scene
 from tests.test_ut_gpu import CAMS, KEYS, H, W
 
@@ -74,8 +73,8 @@ def test_projection_against_oracle(kind, coeffs, shutter):
     p = _small()
     r, m2, d, co, cp = _project(p, kind, _coeffs(coeffs), shutter)
     cam = U.Camera(kind, p["Ks"][0], W, H, **coeffs)
-    o = R8.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], p["viewmats"][0], cam,
-                        viewmat_rs=p["viewmats_rs"][0], shutter=shutter)
+    o = U.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"],
+                        U.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0], shutter), cam)
     r, ro = r[0].cpu().numpy(), o["radii"].numpy()
     frac = o["radii_unrounded"].numpy()
     edge = o["rs_edge"].numpy()
@@ -110,8 +109,8 @@ def _check_against_oracle(p, kind, coeffs, shutter, offs, fl, bg, leaves, rc, ra
     cam = U.Camera(kind, p["Ks"][0], W, H, **coeffs)
     f8 = [torch.from_numpy(np.asarray(x, np.float64)).requires_grad_(True)
           for x in (p["means"], p["quats"], p["scales"], p["colors"], p["opacities"], bg[0])]
-    oc, oa, margin = R8.eval3d_render(*f8[:5], p["viewmats"][0], cam, offs.cpu(), fl.cpu().tolist(), 1, N, 0, background=f8[5],
-                                     viewmat_rs=p["viewmats_rs"][0], shutter=shutter)
+    oc, oa, margin = U.eval3d_render(*f8[:5], U.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0], shutter), cam, offs.cpu(),
+                                     fl.cpu().tolist(), 1, N, 0, background=f8[5])
     ((oc * torch.from_numpy(v_rc[0].astype(np.float64))).sum() + (oa * torch.from_numpy(v_ra[0].astype(np.float64))).sum()).backward()
     clear = (margin > 1e-3).numpy()
     target_c = oc.detach().numpy() if ref is None else ref["render_colors"][0]
@@ -156,8 +155,8 @@ def test_kernels_against_reference(cname, sname):
     name, shutter = f"{cname}/{sname}", SNAMES[sname]
     r, m2, d, cn, cp = _project(p, model, _coeffs(coeffs), shutter)
     cam = U.Camera(model, p["Ks"][0], W, H, **coeffs)
-    o = R8.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], p["viewmats"][0], cam,
-                        viewmat_rs=p["viewmats_rs"][0], shutter=shutter)
+    o = U.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"],
+                        U.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0], shutter), cam)
     frac = o["radii_unrounded"].numpy()
     loose = o["rs_edge"].numpy() | (np.abs(frac - np.round(frac)) < 1e-3).any(-1)
     r, rr = r[0].cpu().numpy(), z[f"{name}/radii"][0]
@@ -190,7 +189,7 @@ def test_rows_and_columns_are_global_renders_at_their_pose(shutter):
     bg = _t(np.float32([[0.2, 0.4, 0.6]]))
     rc, ra = gs.rasterize_to_pixels_eval3d(*args, _t(p["viewmats"]), _t(p["Ks"]), W, H, 16, offs, fl, backgrounds=bg,
                                            camera_model=kind, rolling_shutter=shutter, viewmats_rs=_t(p["viewmats_rs"]), **co)
-    poses = R8.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0])
+    poses = U.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0], shutter)
     n = H if shutter == 0 else W
     R, tt = poses.at(torch.arange(n, dtype=torch.float64) / (n - 1))
     worst = 0.0
@@ -301,7 +300,7 @@ def test_sh_gradient_splits_between_the_poses():
     sh = _t(p["sh"])
     out = gs.spherical_harmonics(3, m, vm, sh, viewmats_rs=vm_rs)
     # the same as the global SH seen from the mean camera position
-    mid = R8.rs_sh_viewmat(p["viewmats"], p["viewmats_rs"]).float().to(DEV)
+    mid = U.rs_sh_viewmat(p["viewmats"], p["viewmats_rs"]).float().to(DEV)
     torch.testing.assert_close(out, gs.spherical_harmonics(3, m, mid, sh), rtol=1e-5, atol=1e-5)
     x = gso.spherical_harmonics(3, p["means"].astype(np.float64), mid.cpu().double().numpy(), p["sh"].astype(np.float64))
     np.testing.assert_allclose(out.detach().cpu().numpy(), x, rtol=1e-4, atol=1e-5)
@@ -384,14 +383,14 @@ def test_fit_to_a_rolling_shutter_target():
     N = len(p["means"])
     # the target: the float64 oracle's projection, its tile lists, and its compositing of the colours
     cam = U.Camera(kind, p["Ks"][0], W, H, **coeffs)
-    o = R8.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"], p["viewmats"][0], cam,
-                        viewmat_rs=p["viewmats_rs"][0], shutter=shutter)
+    o = U.ut_projection(p["means"], p["quats"], p["scales"], p["opacities"],
+                        U.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0], shutter), cam)
     offs, fl = _lists(_t(o["radii"].numpy().astype(np.int32)[None]), _t(o["means2d"].numpy().astype(np.float32)[None]),
                       _t(o["depths"].numpy().astype(np.float32)[None]))
     f8 = [torch.from_numpy(np.asarray(p[k], np.float64)) for k in ("means", "quats", "scales", "colors", "opacities")]
     with torch.no_grad():
-        gt, _, _ = R8.eval3d_render(*f8, p["viewmats"][0], cam, offs.cpu(), fl.cpu().tolist(), 1, N, 0,
-                                   viewmat_rs=p["viewmats_rs"][0], shutter=shutter)
+        gt, _, _ = U.eval3d_render(*f8, U.ShutterPoses(p["viewmats"][0], p["viewmats_rs"][0], shutter), cam, offs.cpu(),
+                                   fl.cpu().tolist(), 1, N, 0)
     gt = gt.float().to(DEV)[None]
     g = torch.Generator(device="cpu").manual_seed(13)
     params = {

@@ -239,7 +239,6 @@ def bench_rolling_shutter(a):
 
 
 def bench_ftheta(a):
-    from tests import ut_ftheta_oracle as F
 
     dev = "cuda"
     sc = scene.make_scene(scene_grid=3, sh_degree=0)
@@ -249,7 +248,7 @@ def bench_ftheta(a):
     opac = t(sc["opacities"]).requires_grad_(True)
     colors = t(sc["colors"][None]).requires_grad_(True)
     vm, K = t(sc["viewmats"][:1]), t(scene.rescale_K(sc["Ks"], sc["width"], sc["height"], W, H)[:1])
-    params, pp, size = F.scaled(F.calibrations()["cross_left_120fov"], W)
+    params, pp, size = scene.scaled(scene.calibrations()["cross_left_120fov"], W)
     assert size == (W, H)
     K_ft = t(np.float32([[[1, 0, pp[0]], [0, 1, pp[1]], [0, 0, 1]]]))
     ft = gs.FThetaCameraDistortionParameters(reference_poly=0, **params)
