@@ -5,7 +5,8 @@ rasterization, fully_fused_projection, spherical_harmonics, isect_tiles, isect_o
 rasterize_to_pixels, quat_scale_to_covar_preci, the sparse-pixel ops build_sparse_tile_layout,
 isect_tiles_sparse, rasterize_to_pixels_sparse, and 2DGS: rasterization_2dgs, fully_fused_projection_2dgs,
 rasterize_to_pixels_2dgs (dense layout) and its sparse-pixel form rasterize_to_pixels_2dgs_sparse (this library's own:
-the reference has no such op), the pair queries rasterize_to_indices_in_range /
+the reference has no such op), the sparse-pixel form of the 3DGUT compositing rasterize_to_pixels_eval3d_sparse (also
+this library's own), the pair queries rasterize_to_indices_in_range /
 rasterize_to_indices_in_range_2dgs, and the per-pixel contributor queries rasterize_num_contributing_gaussians,
 rasterize_contributing_gaussian_ids, rasterize_top_contributing_gaussian_ids and their _sparse forms (the pair query's
 walk with the compositing kernel's decisions: against the reference's ops they can differ only at pairs on the 1/255
@@ -45,6 +46,7 @@ from .ops import (  # noqa: F401
     rasterize_to_pixels_2dgs,
     rasterize_to_pixels_2dgs_sparse,
     rasterize_to_pixels_eval3d,
+    rasterize_to_pixels_eval3d_sparse,
     rasterize_to_pixels_sparse,
     rasterize_top_contributing_gaussian_ids,
     rasterize_top_contributing_gaussian_ids_2dgs,
@@ -105,6 +107,7 @@ __all__ = [
     "fully_fused_projection",
     "fully_fused_projection_with_ut",
     "rasterize_to_pixels_eval3d",
+    "rasterize_to_pixels_eval3d_sparse",
     "fused_project_sh",
     "spherical_harmonics",
     "RollingShutterType",

@@ -237,6 +237,18 @@ _SIGNATURES = {
          c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
          c_vp, c_vp],
     ),
+    "gsb200_eval3d_sparse_fwd": (
+        c_int,
+        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
+         c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+         c_vp],
+    ),
+    "gsb200_eval3d_sparse_bwd": (
+        c_int,
+        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
+         c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    ),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

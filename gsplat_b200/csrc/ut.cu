@@ -8,6 +8,7 @@
 // the compositing thresholds).  The reference's backward gives no gradient to viewmats, and neither does this one.
 #include "camera.cuh"
 #include "gaussmath.cuh"
+#include "pixels.cuh"
 
 namespace gsb
 {
@@ -324,30 +325,44 @@ struct EvalGeom
     const float *viewmats, *Ks, *radial, *tangential, *thin;
 };
 
-// One CTA per 16x16 tile of the [I, th, tw] grid, one pixel per thread.  last_ids: the list index of the pixel's last
-// composited gaussian, -1 for none.
-template<int CDIM, class Shutter, class Lens>
+// One CTA per 16x16 tile of the pixel policy (pixels.cuh), one pixel per thread: every tile of the [I, th, tw] grid
+// (DensePixels), or every active tile with its requested pixels only (SparsePixels).  A pixel is composited when it has
+// an output row (live) and lies inside the W x H image: its ray and its rolling-shutter frame time are defined there
+// only, so a live margin pixel of a partial sparse tile gets the background and alpha 0.  Every other thread stages
+// records and meets every barrier but composites nothing.  last_ids: the list index of the pixel's last composited
+// gaussian, -1 for none.
+template<int CDIM, class Shutter, class Lens, class Pix = DensePixels>
 __global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
     EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
     const float *__restrict__ colors, const float *__restrict__ opacities, const float *__restrict__ backgrounds,
     const uint8_t *__restrict__ masks, const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids,
     int64_t n_isects, float *__restrict__ render_colors, float *__restrict__ render_alphas, int32_t *__restrict__ last_ids,
-    Shutter shutter, Lens lens
+    Shutter shutter, Lens lens, const Pix pixmap = Pix{}
 )
 {
     __shared__ EvalRec rec[kUtThreads];
-    const uint32_t tile = blockIdx.x;
+    const uint32_t tile = pixmap.tile(blockIdx.x); // image * th * tw + tile row * tw + tile col
     const uint32_t img  = tile / (geo.tw * geo.th);
     const uint32_t tin  = tile - img * geo.tw * geo.th;
     const uint32_t tr   = threadIdx.x;
     const uint32_t i    = (tin / geo.tw) * kTile + tr / kTile;
     const uint32_t j    = (tin % geo.tw) * kTile + tr % kTile;
-    const bool inside   = i < geo.H && j < geo.W;
-    const int64_t pix   = (int64_t)img * geo.H * geo.W + (int64_t)i * geo.W + j;
+    bool live, inside = i < geo.H && j < geo.W;
+    int64_t pix;
+    if constexpr(Pix::kSparse)
+    {
+        pix    = pixmap.slot(blockIdx.x, (int)tr, live);
+        inside = inside && live;
+    }
+    else
+    {
+        live = inside;
+        pix  = (int64_t)img * geo.H * geo.W + (int64_t)i * geo.W + j;
+    }
     const float *bg     = backgrounds ? backgrounds + (int64_t)img * CDIM : nullptr;
     if(masks && !masks[tile])
     {
-        if(inside)
+        if(live)
         {
 #pragma unroll
             for(int k = 0; k < CDIM; ++k)
@@ -357,8 +372,17 @@ __global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
         }
         return;
     }
-    const int64_t start = offsets[tile];
-    const int64_t end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
+    int64_t start, end;
+    if constexpr(Pix::kSparse)
+    {
+        start = offsets[blockIdx.x];
+        end   = offsets[blockIdx.x + 1];
+    }
+    else
+    {
+        start = offsets[tile];
+        end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
+    }
     float ro[3] = {0.f, 0.f, 0.f}, rd[3] = {0.f, 0.f, 1.f};
     bool done = !inside;
     if constexpr(Shutter::kRolling)
@@ -405,7 +429,7 @@ __global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
             T       = next_T;
         }
     }
-    if(!inside)
+    if(!live)
         return;
     render_alphas[pix] = 1.f - T;
 #pragma unroll
@@ -446,21 +470,22 @@ __device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, cons
 }
 
 // Back to front over each tile's list.  Per gaussian, the warp's per-pixel gradients (colours, opacity, mean, M) are
-// butterfly-reduced and added with one atomic per value.
-template<int CDIM, class Shutter, class Lens>
+// butterfly-reduced and added with one atomic per value.  The tiles and the pixels that composite are the forward's
+// (eval3d_fwd_kernel, same pixel policy).
+template<int CDIM, class Shutter, class Lens, class Pix = DensePixels>
 __global__ void __launch_bounds__(kUtThreads, 1) eval3d_bwd_kernel(
     EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
     const float *__restrict__ colors, const float *__restrict__ opacities, const float *__restrict__ backgrounds,
     const uint8_t *__restrict__ masks, const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids,
     int64_t n_isects, const float *__restrict__ render_alphas, const int32_t *__restrict__ last_ids,
     const float *__restrict__ v_render_colors, const float *__restrict__ v_render_alphas, EvalGradDst dst, Shutter shutter,
-    Lens lens
+    Lens lens, const Pix pixmap = Pix{}
 )
 {
     constexpr int NV = CDIM + 13; // colours | opacity 1 | mean 3 | M 9
     __shared__ EvalRec rec[kUtThreads];
     __shared__ float s_col[kUtThreads * CDIM];
-    const uint32_t tile = blockIdx.x;
+    const uint32_t tile = pixmap.tile(blockIdx.x);
     if(masks && !masks[tile])
         return;
     const uint32_t img  = tile / (geo.tw * geo.th);
@@ -469,12 +494,30 @@ __global__ void __launch_bounds__(kUtThreads, 1) eval3d_bwd_kernel(
     const unsigned lane = tr & 31;
     const uint32_t i    = (tin / geo.tw) * kTile + tr / kTile;
     const uint32_t j    = (tin % geo.tw) * kTile + tr % kTile;
-    // a pixel outside the image reads the image's first pixel and adds nothing
-    bool inside       = i < geo.H && j < geo.W;
-    const int64_t pix = inside ? (int64_t)img * geo.H * geo.W + (int64_t)i * geo.W + j : (int64_t)img * geo.H * geo.W;
-    const float *bg   = backgrounds ? backgrounds + (int64_t)img * CDIM : nullptr;
-    const int64_t start = offsets[tile];
-    const int64_t end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
+    // a pixel that does not composite reads the row of a live one (the image's first pixel; sparse: its own row, or row
+    // 0 when it has none) and adds nothing
+    bool inside = i < geo.H && j < geo.W;
+    int64_t pix;
+    if constexpr(Pix::kSparse)
+    {
+        bool live;
+        pix    = pixmap.slot(blockIdx.x, (int)tr, live);
+        inside = inside && live;
+    }
+    else
+        pix = inside ? (int64_t)img * geo.H * geo.W + (int64_t)i * geo.W + j : (int64_t)img * geo.H * geo.W;
+    const float *bg = backgrounds ? backgrounds + (int64_t)img * CDIM : nullptr;
+    int64_t start, end;
+    if constexpr(Pix::kSparse)
+    {
+        start = offsets[blockIdx.x];
+        end   = offsets[blockIdx.x + 1];
+    }
+    else
+    {
+        start = offsets[tile];
+        end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
+    }
     float ro[3] = {0.f, 0.f, 0.f}, rd[3] = {0.f, 0.f, 1.f};
     if constexpr(Shutter::kRolling)
     {
@@ -821,6 +864,109 @@ extern "C" int gsb200_eval3d_bwd(
                     geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
                     render_alphas, last_ids, v_render_colors, v_render_alphas, dst, shutter, lens
                 );
+                return gsb::check_launch();
+            });
+        });
+        if(rc)
+            return rc;
+    }
+    gsb::eval3d_finish_kernel<<<gsb::grid_for(B * N, gsb::kUtThreads), gsb::kUtThreads, 0, st>>>(
+        B * N, quats, scales, grad_records, v_means, v_quats, v_scales
+    );
+    return gsb::check_launch();
+}
+
+// ---- sparse pixels (rasterize_to_pixels_eval3d_sparse): one CTA per active tile of the layout of gsb200_sparse_layout_*,
+// outputs [P, *] in the original pixel order.  Every check of the dense entries and of the sparse layout runs before
+// any launch.
+extern "C" int gsb200_eval3d_sparse_fwd(
+    int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
+    const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
+    const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+    const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+    int64_t n_active, const int32_t *active_tiles, const int32_t *tile_offsets, const int32_t *flatten_ids,
+    int64_t n_isects, const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map,
+    float *render_colors, float *render_alphas, int32_t *last_ids, void *stream
+)
+{
+    if(n_isects < 0)
+        return GSB200_E_INVALID;
+    if(int rc = gsb::eval3d_checks(B, C, N, image_width, image_height, tile_size, tile_width, tile_height))
+        return rc;
+    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta, viewmats_rs,
+                                   rolling_shutter, image_width, image_height))
+        return rc;
+    if(int rc = gsb::sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map,
+                                    image_width, image_height, tile_width, tile_height))
+        return rc;
+    if(n_active == 0)
+        return GSB200_OK;
+    if(B * C == 0 || !viewmats || !Ks || !render_colors || !render_alphas || !last_ids)
+        return GSB200_E_INVALID;
+    if(n_isects > 0 && (!means || !quats || !scales || !colors || !opacities || !flatten_ids))
+        return GSB200_E_INVALID;
+    const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height,
+                            camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
+    const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
+    return gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
+        return gsb::with_channels(D, [&](auto CH) {
+            gsb::eval3d_fwd_kernel<CH, decltype(shutter), decltype(lens), gsb::SparsePixels>
+                <<<(uint32_t)n_active, gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
+                    geo, means, quats, scales, colors, opacities, backgrounds, masks, tile_offsets, flatten_ids, n_isects,
+                    render_colors, render_alphas, last_ids, shutter, lens, pm
+                );
+            return gsb::check_launch();
+        });
+    });
+}
+
+extern "C" int gsb200_eval3d_sparse_bwd(
+    int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
+    const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
+    const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+    const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+    int64_t n_active, const int32_t *active_tiles, const int32_t *tile_offsets, const int32_t *flatten_ids,
+    int64_t n_isects, const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map,
+    const float *render_alphas, const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas,
+    float *grad_records, float *v_colors, float *v_opacities, float *v_means, float *v_quats, float *v_scales, void *stream
+)
+{
+    if(n_isects < 0)
+        return GSB200_E_INVALID;
+    if(int rc = gsb::eval3d_checks(B, C, N, image_width, image_height, tile_size, tile_width, tile_height))
+        return rc;
+    if(int rc = gsb::camera_checks(camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta, viewmats_rs,
+                                   rolling_shutter, image_width, image_height))
+        return rc;
+    if(int rc = gsb::sparse_args_ok(n_active, active_tiles, tile_offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map,
+                                    image_width, image_height, tile_width, tile_height))
+        return rc;
+    if(B * N == 0)
+        return GSB200_OK;
+    if(!quats || !scales || !grad_records || !v_means || !v_quats || !v_scales)
+        return GSB200_E_INVALID;
+    // the finish kernel runs without the compositing: an unsupported channel count is refused before either
+    if(gsb::with_channels(D, [](auto) { return GSB200_OK; }))
+        return GSB200_E_UNSUPPORTED;
+    cudaStream_t st = (cudaStream_t)stream;
+    if(n_isects > 0 && n_active > 0)
+    {
+        if(B * C == 0 || !means || !colors || !opacities || !viewmats || !Ks || !flatten_ids || !render_alphas || !last_ids
+           || !v_render_colors || !v_colors || !v_opacities)
+            return GSB200_E_INVALID;
+        const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width,
+                                tile_height, camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
+        const gsb::EvalGradDst dst{v_colors, v_opacities, grad_records};
+        const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
+        const int rc = gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
+            return gsb::with_channels(D, [&](auto CH) {
+                gsb::eval3d_bwd_kernel<CH, decltype(shutter), decltype(lens), gsb::SparsePixels>
+                    <<<(uint32_t)n_active, gsb::kUtThreads, 0, st>>>(
+                        geo, means, quats, scales, colors, opacities, backgrounds, masks, tile_offsets, flatten_ids,
+                        n_isects, render_alphas, last_ids, v_render_colors, v_render_alphas, dst, shutter, lens, pm
+                    );
                 return gsb::check_launch();
             });
         });

@@ -3027,3 +3027,172 @@ def _rasterize_eval3d(means, quats, scales, colors, opacities, viewmats, Ks, wid
                  cam.radial, cam.tangential, cam.thin, cam.viewmats_rs)
     return _RasterizeToPixelsEval3D.apply(means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam,
                                           int(width), int(height), isect_offsets, flatten_ids)
+
+
+class _RasterizeToPixelsEval3DSparse(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam: _UtCamera, width, height,
+                tile_width, tile_height, image_ids, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask,
+                tile_pixel_cumsum, pixel_map):
+        dev = require_cuda(means, quats, scales, colors, opacities, viewmats, Ks, active_tiles, tile_offsets, flatten_ids,
+                           pixel_map)
+        means, quats, scales = means.contiguous(), quats.contiguous(), scales.contiguous()
+        colors, opacities = f32c(colors, "colors"), f32c(opacities, "opacities")
+        backgrounds, viewmats, Ks = f32c(backgrounds, "backgrounds"), viewmats.contiguous(), Ks.contiguous()
+        B, C, N, D = _prod(means.shape[:-2]), viewmats.shape[-3], means.shape[-2], colors.shape[-1]
+        m8 = _mask_u8(masks)
+        active, offsets, fl = active_tiles.contiguous(), tile_offsets.contiguous(), flatten_ids.contiguous()
+        words, cumsum, pmap = tile_pixel_mask.contiguous(), tile_pixel_cumsum.contiguous(), pixel_map.contiguous()
+        AT, S, P = active.shape[0], fl.shape[0], pmap.shape[0]
+        o = dict(device=dev, dtype=torch.float32)
+        if P == 0 or S == 0 or AT == 0:
+            # no requested pixel, or nothing listed in any active tile: the background alone, no kernel launch
+            if backgrounds is not None and P > 0:
+                render_colors = backgrounds[image_ids.long()]
+            else:
+                render_colors = torch.zeros((P, D), **o)
+            render_alphas = torch.zeros((P, 1), **o)
+            last_ids = torch.full((P,), -1, device=dev, dtype=torch.int32)
+        else:
+            render_colors, render_alphas = torch.empty((P, D), **o), torch.empty((P, 1), **o)
+            last_ids = torch.empty(P, device=dev, dtype=torch.int32)
+            with _Ctx(dev) as st:
+                check(
+                    lib().gsb200_eval3d_sparse_fwd(
+                        B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds),
+                        ptr(m8), ptr(viewmats), ptr(Ks), cam.model, ptr(cam.radial), ptr(cam.tangential), ptr(cam.thin),
+                        _ftheta_ptr(cam.ftheta), ptr(cam.viewmats_rs), cam.shutter, width, height, 16, tile_width,
+                        tile_height, AT, ptr(active), ptr(offsets), ptr(fl), S, ptr(words), ptr(cumsum), ptr(pmap),
+                        ptr(render_colors), ptr(render_alphas), ptr(last_ids), st,
+                    ),
+                    "rasterize_to_pixels_eval3d_sparse",
+                )
+        ctx.save_for_backward(means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, image_ids, active,
+                              offsets, fl, words, cumsum, pmap, render_alphas, last_ids)
+        ctx.set_materialize_grads(False)
+        ctx.meta = (B, C, N, D, cam, width, height, tile_width, tile_height)
+        return render_colors, render_alphas
+
+    @staticmethod
+    def backward(ctx, v_render_colors, v_render_alphas):
+        (means, quats, scales, colors, opacities, backgrounds, m8, viewmats, Ks, image_ids, active, offsets, fl, words,
+         cumsum, pmap, render_alphas, last_ids) = ctx.saved_tensors
+        B, C, N, D, cam, width, height, tw, th = ctx.meta
+        dev = render_alphas.device
+        if v_render_colors is None:
+            v_render_colors = torch.zeros((pmap.shape[0], D), device=dev, dtype=torch.float32)
+        v_render_colors = v_render_colors.float().contiguous()
+        v_render_alphas = None if v_render_alphas is None else v_render_alphas.float().contiguous()
+        v_colors, v_opacities = torch.zeros_like(colors), torch.zeros_like(opacities)
+        if fl.shape[0] == 0 or pmap.shape[0] == 0 or active.shape[0] == 0:
+            # nothing was composited: zero gradients, no kernel launch
+            v_means, v_quats, v_scales = torch.zeros_like(means), torch.zeros_like(quats), torch.zeros_like(scales)
+        else:
+            v_means, v_quats, v_scales = torch.empty_like(means), torch.empty_like(quats), torch.empty_like(scales)
+            records = torch.zeros((B * N, 12), device=dev, dtype=torch.float32)
+            with _Ctx(dev) as st:
+                check(
+                    lib().gsb200_eval3d_sparse_bwd(
+                        B, C, N, D, ptr(means), ptr(quats), ptr(scales), ptr(colors), ptr(opacities), ptr(backgrounds),
+                        ptr(m8), ptr(viewmats), ptr(Ks), cam.model, ptr(cam.radial), ptr(cam.tangential), ptr(cam.thin),
+                        _ftheta_ptr(cam.ftheta), ptr(cam.viewmats_rs), cam.shutter, width, height, 16, tw, th,
+                        active.shape[0], ptr(active), ptr(offsets), ptr(fl), fl.shape[0], ptr(words), ptr(cumsum),
+                        ptr(pmap), ptr(render_alphas), ptr(last_ids), ptr(v_render_colors), ptr(v_render_alphas),
+                        ptr(records), ptr(v_colors), ptr(v_opacities), ptr(v_means), ptr(v_quats), ptr(v_scales), st,
+                    ),
+                    "rasterize_to_pixels_eval3d_sparse_bwd",
+                )
+        v_backgrounds = None
+        if backgrounds is not None and ctx.needs_input_grad[5]:
+            v_backgrounds = torch.zeros_like(backgrounds).index_add_(0, image_ids.long(), v_render_colors * (1.0 - render_alphas))
+        # viewmats, Ks and the camera (its coefficients, viewmats_rs) get no gradient, as in rasterize_to_pixels_eval3d
+        return (v_means, v_quats, v_scales, v_colors, v_opacities, v_backgrounds) + (None,) * 15
+
+
+def rasterize_to_pixels_eval3d_sparse(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    colors: Tensor,  # [..., C, N, channels]
+    opacities: Tensor,  # [..., C, N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    image_ids: Tensor,  # [P]
+    active_tiles: Tensor,  # [AT]
+    tile_offsets: Tensor,  # [AT + 1]
+    flatten_ids: Tensor,  # [n_isects]
+    tile_pixel_mask: Tensor,  # [AT, 4]
+    tile_pixel_cumsum: Tensor,  # [AT]
+    pixel_map: Tensor,  # [P]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+    backgrounds: Optional[Tensor] = None,  # [n_images, channels]
+    masks: Optional[Tensor] = None,  # [n_images, tile_height, tile_width]
+    camera_model: str = "pinhole",
+    ut_params=None,
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    rolling_shutter: int = RollingShutterType.GLOBAL,
+    viewmats_rs: Optional[Tensor] = None,  # [..., C, 4, 4]
+) -> Tuple[Tensor, Tensor]:
+    """rasterize_to_pixels_eval3d at the pixels of a build_sparse_tile_layout layout only, with the lists of
+    isect_tiles_sparse (conics=None) on the UT rows of fully_fused_projection_with_ut.  The geometry, colours,
+    opacities, cameras and camera arguments are those of rasterize_to_pixels_eval3d; the images are its (batch, camera)
+    images flattened: image ``i`` of the layout is camera ``i % C`` of batch ``i // C``.  ``backgrounds`` is
+    [n_images, channels] and ``masks`` [n_images, tile_height, tile_width], as in the other sparse ops.  Returns
+    (render_colors [P, channels], render_alphas [P, 1]) in the original pixel order.  Differentiable in means, quats,
+    scales, colors, opacities and backgrounds; viewmats, ``viewmats_rs`` and the camera coefficients get no gradient.
+
+    - A requested pixel inside the W x H image gets the value rasterize_to_pixels_eval3d gives it, bit for bit, for the
+      same rows, lists, camera and shutter.
+    - A requested pixel in the margin of a partial tile (inside the tile grid, outside the image) gets the background
+      (or 0) and alpha 0, and passes no gradient to the Gaussians; its colour cotangent goes to its background.
+      rasterize_to_pixels_sparse and rasterize_to_pixels_2dgs_sparse render such pixels, but an eval3d pixel's ray comes
+      from the camera model and its rolling-shutter frame time is defined on the W x H image, and the dense op has no
+      such pixel to agree with.
+    - An FTheta pixel whose unprojection does not converge composites nothing, as in the dense op.
+
+    ``ut_params`` is checked and does not enter the compositing.  With no requested pixel, or no Gaussian listed in any
+    active tile, nothing is launched: the background (or 0) with alpha 0, and zero gradients."""
+    what = "rasterize_to_pixels_eval3d_sparse"
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    _check_sparse_layout(
+        image_ids, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width,
+        image_height, tile_width, tile_height,
+    )
+    if flatten_ids.dim() != 1:
+        raise ValueError(f"flatten_ids must be one-dimensional, got {tuple(flatten_ids.shape)}")
+    batch, C, N = _ut_geometry(what, means, quats, scales, viewmats, Ks)
+    image_dims = batch + (C,)
+    n_images = _prod(image_dims)
+    cam = _ut_camera(what, viewmats, image_width, image_height, camera_model, radial_coeffs, tangential_coeffs,
+                     thin_prism_coeffs, ftheta_coeffs, None, None, rolling_shutter, viewmats_rs)
+    _ut_params(ut_params)
+    if colors.dim() != len(image_dims) + 2:
+        raise ValueError(f"{what}: colors must be [..., C, N, channels], got {tuple(colors.shape)}")
+    D = colors.shape[-1]
+    _check_shape(colors, image_dims + (N, D), "colors")
+    _check_shape(opacities, image_dims + (N,), "opacities")
+    if backgrounds is not None:
+        _check_shape(backgrounds, (n_images, D), "backgrounds")
+    if masks is not None:
+        _check_shape(masks, (n_images, tile_height, tile_width), "masks")
+    for name, t in (("colors", colors), ("opacities", opacities), ("backgrounds", backgrounds)):
+        if t is not None and t.dtype != torch.float32:
+            raise TypeError(f"{what}: {name} must be float32, got {t.dtype}")
+    if D not in _SUPPORTED_CHANNELS:
+        raise NotImplementedError(f"{what}: {D} channels; the eval3d kernels are built for {_SUPPORTED_CHANNELS}")
+    require_cuda(means, quats, scales, colors, opacities, viewmats, Ks, backgrounds, masks, image_ids, active_tiles,
+                 tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, cam.radial, cam.tangential,
+                 cam.thin, cam.viewmats_rs)
+    return _RasterizeToPixelsEval3DSparse.apply(
+        means, quats, scales, colors, opacities, backgrounds, masks, viewmats, Ks, cam, int(image_width),
+        int(image_height), int(tile_width), int(tile_height), image_ids, active_tiles, tile_offsets, flatten_ids,
+        tile_pixel_mask, tile_pixel_cumsum, pixel_map,
+    )

@@ -599,6 +599,38 @@ extern "C"
         const float *v_render_colors, const float *v_render_alphas, float *grad_records, float *v_colors, float *v_opacities,
         float *v_means, float *v_quats, float *v_scales, void *stream
     );
+    /* Eval3d compositing of the requested pixels only (rasterize_to_pixels_eval3d_sparse; no reference counterpart): one
+     * CTA per active tile, the layout of gsb200_sparse_layout_* and the per-active-tile lists [n_active + 1] of
+     * gsb200_isect_active_offsets on the UT rows.  The other arguments are those of gsb200_eval3d_fwd / _bwd, with
+     * backgrounds [B*C, D] and masks [B*C, th, tw] indexed by the layout's image (the flattened (b, c)).  A requested
+     * pixel inside the W x H image gets the dense forward's values there; one in the margin of a partial tile gets the
+     * background (or 0), alpha 0 and last id -1, and passes no gradient.  Outputs in the original pixel order:
+     * render_colors [P, D], render_alphas [P], last_ids int32 [P].  The backward reads render_alphas, last_ids,
+     * v_render_colors [P, D] and v_render_alphas [P] (or NULL) per requested pixel and accumulates and writes the
+     * gradients of gsb200_eval3d_bwd.  Every check runs before any launch; the return codes are those of the dense
+     * entries and of gsb200_raster_sparse_fwd / _bwd. */
+    int gsb200_eval3d_sparse_fwd(
+        int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
+        const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
+        const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+        const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        int64_t n_active, const int32_t *active_tiles, const int32_t *tile_offsets, const int32_t *flatten_ids,
+        int64_t n_isects, const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map,
+        float *render_colors, float *render_alphas, int32_t *last_ids, void *stream
+    );
+    int gsb200_eval3d_sparse_bwd(
+        int64_t B, int64_t C, int64_t N, int D, const float *means, const float *quats, const float *scales,
+        const float *colors, const float *opacities, const float *backgrounds, const uint8_t *masks, const float *viewmats,
+        const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+        const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        int64_t n_active, const int32_t *active_tiles, const int32_t *tile_offsets, const int32_t *flatten_ids,
+        int64_t n_isects, const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map,
+        const float *render_alphas, const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas,
+        float *grad_records, float *v_colors, float *v_opacities, float *v_means, float *v_quats, float *v_scales,
+        void *stream
+    );
 
     /* ---- MCMC strategy ops ("next" row): relocation (ext.cpp `relocation`, gsplat/relocation.py:64,
      * csrc/RelocationCUDA.cu:36-80) and in-place position perturbation (csrc/MCMCPerturbCUDA.cu:28-60,

@@ -1,6 +1,6 @@
 """Sparse-pixel rendering against the dense pipeline on bench.py's scene (1M Gaussians, one 1920x1080 view, seed 42).
 
-    python tools/sparse_bench.py [--2dgs] [--steps 20] [--warmup 5] [--out FILE]
+    python tools/sparse_bench.py [--2dgs | --3dgut [--rolling-shutter]] [--steps 20] [--warmup 5] [--out FILE]
 
 One step of each pipeline, timed on the host around a device synchronise (both pipelines read one count back to the
 host, so a step is not asynchronous anyway):
@@ -12,6 +12,13 @@ are the 2DGS ones:
   sparse: build_sparse_tile_layout + isect_tiles_sparse + rasterize_to_pixels_2dgs_sparse forward + backward;
   dense:  isect_tiles_sorted + rasterize_to_pixels_2dgs forward + backward over the whole image (the same lists), the
           loss on all five outputs at the requested pixels only.
+With --3dgut the same scene (colours, not SH) is projected by fully_fused_projection_with_ut through the distorted
+pinhole of tools/bench_ut.py, and the pipelines are the 3DGUT ones:
+  sparse: build_sparse_tile_layout + isect_tiles_sparse + rasterize_to_pixels_eval3d_sparse forward + backward;
+  dense:  isect_tiles_sorted + rasterize_to_pixels_eval3d forward + backward over the whole image (the same lists), the
+          loss on the requested pixels only.
+--rolling-shutter (with --3dgut) exposes the image top to bottom, the end pose being tools/bench_ut.py's (the start
+pose turned by 2 degrees and moved by 0.03).
 Workloads: (a) 4096 random pixels, (b) sixteen 64x64 patches, (c) every pixel.  The projection runs once, outside the
 timed steps.  Prints one JSON line per workload with the median step times, and the device name and power limit.
 """
@@ -68,7 +75,13 @@ def main() -> int:
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--out", help="also append the JSON lines to this file")
     ap.add_argument("--2dgs", dest="surfels", action="store_true", help="the 2DGS pipelines on the scene's surfels")
+    ap.add_argument("--3dgut", dest="ut", action="store_true", help="the 3DGUT pipelines through a distorted pinhole")
+    ap.add_argument("--rolling-shutter", action="store_true", help="with --3dgut: a top-to-bottom rolling shutter")
     args = ap.parse_args()
+    if args.rolling_shutter and not args.ut:
+        ap.error("--rolling-shutter needs --3dgut")
+    if args.surfels and args.ut:
+        ap.error("--2dgs and --3dgut are exclusive")
     if not torch.cuda.is_available():
         raise SystemExit("sparse_bench needs a GPU")
     dev = "cuda:0"
@@ -78,6 +91,8 @@ def main() -> int:
     N = sc["means"].shape[0]
     if args.surfels:
         return main_2dgs(args, sc, Ks, t, N, dev)
+    if args.ut:
+        return main_3dgut(args, sc, Ks, t, N, dev)
     with torch.no_grad():
         radii, m2, depths, conics, _ = gs.fully_fused_projection(
             t(sc["means"]), None, t(sc["quats"]), t(sc["scales"]), t(sc["viewmats"][:1]), t(Ks[:1]), W, H
@@ -191,6 +206,64 @@ def main_2dgs(args, sc, Ks, t, N, dev) -> int:
             pipeline="2dgs", workload=name, pixels=P, n_gaussians=N, image=f"{W}x{H}", channels=D, steps=args.steps,
             sparse_ms=round(sparse_ms, 3), sparse_min_ms=round(sparse_min, 3), dense_ms=round(dense_ms, 3),
             dense_min_ms=round(dense_min, 3), sparse_over_dense=round(sparse_ms / dense_ms, 3), **stats, **info,
+        )
+        line = json.dumps(rec)
+        print(line, flush=True)
+        lines.append(line)
+    _write(args, lines)
+    return 0
+
+
+def main_3dgut(args, sc, Ks, t, N, dev) -> int:
+    sys.path.insert(0, os.path.join(ROOT, "tools"))
+    from bench_ut import _end_pose
+
+    vm, K = t(sc["viewmats"][:1]), t(Ks[:1])
+    # the distorted pinhole of tools/bench_ut.py --distorted
+    cam = dict(radial_coeffs=t(np.float32([[0.05, -0.02, 0.0, 0.0, 0.0, 0.0]])), tangential_coeffs=t(np.float32([[0.001, -0.001]])))
+    if args.rolling_shutter:
+        cam.update(rolling_shutter=gs.RollingShutterType.ROLLING_TOP_TO_BOTTOM, viewmats_rs=_end_pose(vm))
+    means, quats, scales = t(sc["means"]), t(sc["quats"]), t(sc["scales"])
+    colors = t(sc["colors"])[None].contiguous()
+    opac = t(sc["opacities"])[None].contiguous()
+    with torch.no_grad():
+        radii, m2, depths, _, _ = gs.fully_fused_projection_with_ut(means, quats, scales, opac[0], vm, K, W, H, **cam)
+    params = [x.detach().clone().requires_grad_(True) for x in (means, quats, scales, colors, opac)]
+    info = device_info()
+    lines = []
+    for name, pix in workloads(np.random.RandomState(42)).items():
+        pixels = t(pix.astype(np.int32))
+        image_ids = torch.zeros(pixels.shape[0], device=dev, dtype=torch.int32)
+        P = pixels.shape[0]
+        v = torch.randn((P, 3), device=dev, generator=torch.Generator(device=dev).manual_seed(0))
+        v_img = torch.zeros((1, H, W, 3), device=dev)
+        v_img[0, pixels[:, 0].long(), pixels[:, 1].long()] = v
+        stats = {}
+
+        def sparse_step():
+            active, amask, words, cum, pmap = gs.build_sparse_tile_layout(pixels, image_ids, 1, 16, TW, TH)
+            toff, fl = gs.isect_tiles_sparse(m2, radii, depths, amask, active, 1, 16, TW, TH)
+            rc, _ = gs.rasterize_to_pixels_eval3d_sparse(
+                *params, vm, K, image_ids, active, toff, fl, words, cum, pmap, W, H, 16, TW, TH, **cam
+            )
+            (rc * v).sum().backward()
+            stats.update(n_active=int(active.shape[0]), n_isects=int(fl.shape[0]))
+
+        def dense_step():
+            hits = gs.ops.isect_tiles_sorted(m2, radii, depths, 16, TW, TH)
+            off = hits.isect_offsets.reshape(1, TH, TW)
+            rc, _ = gs.rasterize_to_pixels_eval3d(*params, vm, K, W, H, 16, off, hits.flatten_ids, **cam)
+            (rc * v_img).sum().backward()
+            stats.update(dense_isects=int(hits.flatten_ids.shape[0]))
+
+        sparse_ms, sparse_min = _timed(sparse_step, args.steps, args.warmup)
+        dense_ms, dense_min = _timed(dense_step, args.steps, args.warmup)
+        rec = dict(
+            pipeline="3dgut", camera="pinhole radial+tangential",
+            shutter="rolling top to bottom" if args.rolling_shutter else "global", workload=name, pixels=P,
+            n_gaussians=N, image=f"{W}x{H}", steps=args.steps, sparse_ms=round(sparse_ms, 3),
+            sparse_min_ms=round(sparse_min, 3), dense_ms=round(dense_ms, 3), dense_min_ms=round(dense_min, 3),
+            sparse_over_dense=round(sparse_ms / dense_ms, 3), **stats, **info,
         )
         line = json.dumps(rec)
         print(line, flush=True)
