@@ -13,8 +13,11 @@ walk with the compositing kernel's decisions: against the reference's ops they c
 and 1e-4 thresholds), and their 2DGS forms rasterize_num_contributing_gaussians_2dgs,
 rasterize_contributing_gaussian_ids_2dgs, rasterize_top_contributing_gaussian_ids_2dgs and their _2dgs_sparse forms
 (this library's own: the reference has no such ops; the surfel walk takes rasterize_to_pixels_2dgs's decisions, so
-their alphas equal its render_alphas bit for bit).  Importing the package does not need a GPU; calling an
-operator does (and needs gsplat_b200/libgsplat_b200.so, built by ``python -m gsplat_b200.build``).
+their alphas equal its render_alphas bit for bit), and for 3DGUT the pair query rasterize_to_indices_in_range_eval3d and
+the contributor queries rasterize_num_contributing_gaussians_eval3d, rasterize_contributing_gaussian_ids_eval3d,
+rasterize_top_contributing_gaussian_ids_eval3d and their _eval3d_sparse forms (this library's own as well; the eval3d
+walk takes rasterize_to_pixels_eval3d's decisions, so their alphas equal its render_alphas bit for bit).  Importing the
+package does not need a GPU; calling an operator does (and needs gsplat_b200/libgsplat_b200.so, built by ``python -m gsplat_b200.build``).
 """
 from .ops import (  # noqa: F401
     FThetaCameraDistortionParameters,
@@ -35,13 +38,18 @@ from .ops import (  # noqa: F401
     rasterize_contributing_gaussian_ids,
     rasterize_contributing_gaussian_ids_2dgs,
     rasterize_contributing_gaussian_ids_2dgs_sparse,
+    rasterize_contributing_gaussian_ids_eval3d,
+    rasterize_contributing_gaussian_ids_eval3d_sparse,
     rasterize_contributing_gaussian_ids_sparse,
     rasterize_num_contributing_gaussians,
     rasterize_num_contributing_gaussians_2dgs,
     rasterize_num_contributing_gaussians_2dgs_sparse,
+    rasterize_num_contributing_gaussians_eval3d,
+    rasterize_num_contributing_gaussians_eval3d_sparse,
     rasterize_num_contributing_gaussians_sparse,
     rasterize_to_indices_in_range,
     rasterize_to_indices_in_range_2dgs,
+    rasterize_to_indices_in_range_eval3d,
     rasterize_to_pixels,
     rasterize_to_pixels_2dgs,
     rasterize_to_pixels_2dgs_sparse,
@@ -51,6 +59,8 @@ from .ops import (  # noqa: F401
     rasterize_top_contributing_gaussian_ids,
     rasterize_top_contributing_gaussian_ids_2dgs,
     rasterize_top_contributing_gaussian_ids_2dgs_sparse,
+    rasterize_top_contributing_gaussian_ids_eval3d,
+    rasterize_top_contributing_gaussian_ids_eval3d_sparse,
     rasterize_top_contributing_gaussian_ids_sparse,
     spherical_harmonics,
 )
@@ -137,6 +147,13 @@ __all__ = [
     "rasterize_contributing_gaussian_ids_2dgs_sparse",
     "rasterize_top_contributing_gaussian_ids_2dgs",
     "rasterize_top_contributing_gaussian_ids_2dgs_sparse",
+    "rasterize_to_indices_in_range_eval3d",
+    "rasterize_num_contributing_gaussians_eval3d",
+    "rasterize_num_contributing_gaussians_eval3d_sparse",
+    "rasterize_contributing_gaussian_ids_eval3d",
+    "rasterize_contributing_gaussian_ids_eval3d_sparse",
+    "rasterize_top_contributing_gaussian_ids_eval3d",
+    "rasterize_top_contributing_gaussian_ids_eval3d_sparse",
     "quat_scale_to_covar_preci",
     "compute_relocation",
     "mcmc_perturb_positions",

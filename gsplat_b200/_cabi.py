@@ -249,6 +249,27 @@ _SIGNATURES = {
          c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
          c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     ),
+    "gsb200_eval3d_indices": (
+        c_int,
+        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_u32,
+         c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp],
+    ),
+    "gsb200_eval3d_contrib_max_samples": (c_int, []),
+    "gsb200_eval3d_contrib_count": (
+        c_int,
+        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_u32, c_u32,
+         c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    ),
+    "gsb200_eval3d_contrib_ids": (
+        c_int,
+        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_u32, c_u32,
+         c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp],
+    ),
+    "gsb200_eval3d_contrib_top": (
+        c_int,
+        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_u32, c_u32,
+         c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp],
+    ),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -1,6 +1,7 @@
-// indices.cuh -- sinks and host side of the index queries (gsb200_raster_indices, gsb200_surfel_indices): which
-// gaussians each pixel composites, walking only the batches [range_start, range_end) of kIndexBatch records of its list;
-// and of the per-pixel contributor queries of both walks (gsb200_contrib_*, gsb200_surfel_contrib_*).
+// indices.cuh -- sinks and host side of the index queries (gsb200_raster_indices, gsb200_surfel_indices,
+// gsb200_eval3d_indices): which gaussians each pixel composites, walking only the batches [range_start, range_end) of
+// kIndexBatch records of its list; and of the per-pixel contributor queries of the three walks (gsb200_contrib_*,
+// gsb200_surfel_contrib_*, gsb200_eval3d_contrib_*).
 //
 // Two passes over the same workspace: the count pass writes the pair count of every pixel and their exclusive int64
 // scan (sort.cu) and copies the total to the caller; the emit pass writes each pixel's pairs, front to back, at its
@@ -8,6 +9,7 @@
 #pragma once
 
 #include <algorithm>
+#include <initializer_list>
 
 #include "common.cuh"
 #include "pixels.cuh"
@@ -29,8 +31,8 @@ PixelCounts carve_pixel_counts(void *workspace, int64_t P);
 // exclusive scan of counts [P + 1] into starts, then total[0] = starts[P] (device to device)
 int scan_pixel_counts(const PixelCounts &pc, int64_t P, int64_t *total, cudaStream_t st);
 
-// What a pair-query walk (raster_indices_kernel of raster.cu, surfel_indices_kernel of surfel.cu) does with a pixel's
-// pairs is its Sink's (both walks run kIndexBatch threads per CTA, one pixel per thread):
+// What a pair-query walk (raster_indices_kernel of raster.cu, surfel_indices_kernel of surfel.cu, eval3d_indices_kernel
+// of ut.cu) does with a pixel's pairs is its Sink's (every walk runs kIndexBatch threads per CTA, one pixel per thread):
 //   begin(live, pix, pix_in, image_id)  once per thread (pix: the output row, pix_in: the row-major pixel in its image)
 //   pair(k, g, w)                        the pixel's k-th pair: flatten id g, weight w = alpha * T before the pair
 //   end(pix, count, T)                   once per live pixel, after the walk
@@ -218,12 +220,10 @@ int run_index_pass(
 // tiles of a sparse layout (active_tiles != null).  The checks run in run_index_pass's order with its return codes;
 // every pixel is written, also when there are no intersections.
 //
-// The arguments of the C entries of both walks: `rows` is conics [R, 3] (raster.cu) or ray_transforms [R, 3, 3]
-// (surfel.cu).
+// The arguments of the C entries that do not depend on what a walk composites; the walk (below) carries the rest.
 struct ContribArgs
 {
     int64_t I, N;
-    const float *means2d, *rows, *opacities;
     uint32_t W, H, tile_size, tw, th;
     const int32_t *offsets, *flatten_ids;
     int64_t n_isects, n_active;
@@ -232,18 +232,27 @@ struct ContribArgs
     const int64_t *tile_pixel_cumsum, *pixel_map;
 };
 
-// ContribArgs from the parameters of a contributor entry, named as gsb200_contrib_count's with `rows` for conics
-#define GSB200_CONTRIB_ARGS(rows)                                                                                       \
+// ContribArgs from the parameters of a contributor entry, named as gsb200_contrib_count's, over I images
+#define GSB200_CONTRIB_ARGS(I)                                                                                          \
     gsb::ContribArgs                                                                                                    \
     {                                                                                                                   \
-        I, N, means2d, rows, opacities, image_width, image_height, tile_size, tile_width, tile_height, offsets,         \
-            flatten_ids, n_isects, n_active, active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map                \
+        I, N, image_width, image_height, tile_size, tile_width, tile_height, offsets, flatten_ids, n_isects, n_active,   \
+            active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map                                                 \
     }
 
-// A Walk is one unit's pair-query kernel:
-//   Walk::launch(a, n_tiles, pixmap, sink, smem, st)  launches it over n_tiles CTAs from T = 1 through the whole lists
+// The rows of the 2-D walks (raster.cu, surfel.cu): means2d [R, 2], conics [R, 3] or ray_transforms [R, 3, 3],
+// opacities [R].  They are read only when there are intersections.
+struct PlanarRows
+{
+    const float *means2d, *rows, *opacities;
+    bool inputs_ok(int64_t n_isects) const { return n_isects == 0 || (means2d && rows && opacities); }
+};
+
+// A Walk is one unit's pair-query kernel with what it composites:
+//   walk.inputs_ok(n_isects)                        whether what it reads is given
+//   walk.launch(a, n_tiles, pixmap, sink, smem, st)  launches it over n_tiles CTAs from T = 1 through the whole lists
 //   Walk::max_samples()                             the largest K of its TopSink on the current device (top_max_samples)
-// launch_walk and top_max_samples are the steps both walks take.
+// launch_walk and top_max_samples are the steps every walk takes.
 template<class... Params, class... Args>
 int launch_walk(void (*kernel)(Params...), unsigned n_tiles, size_t smem, cudaStream_t st, const Args &...args)
 {
@@ -254,14 +263,14 @@ int launch_walk(void (*kernel)(Params...), unsigned n_tiles, size_t smem, cudaSt
 }
 
 // largest K of a top-K walk on the current device: its opt-in shared memory per block, less the static shared memory
-// (the staging arrays) of the larger of its two TopSink instantiations, over the K slots of every thread
-inline int top_max_samples(const void *dense_walk, const void *sparse_walk)
+// (the staging arrays) of the largest of its TopSink instantiations, over the K slots of every thread
+inline int top_max_samples(std::initializer_list<const void *> walks)
 {
     int dev = 0, optin = 0;
     GSB_CUDA_TRY(cudaGetDevice(&dev));
     GSB_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     size_t staging = 0;
-    for(const void *k : {dense_walk, sparse_walk})
+    for(const void *k : walks)
     {
         cudaFuncAttributes a;
         GSB_CUDA_TRY(cudaFuncGetAttributes(&a, k));
@@ -273,7 +282,7 @@ inline int top_max_samples(const void *dense_walk, const void *sparse_walk)
 }
 
 template<class Walk, class Sink>
-int run_contrib(const ContribArgs &a, bool outputs_ok, size_t smem, const Sink &sink, cudaStream_t st)
+int run_contrib(const Walk &walk, const ContribArgs &a, bool outputs_ok, size_t smem, const Sink &sink, cudaStream_t st)
 {
     const bool sparse = a.active_tiles != nullptr;
     if(a.I < 0 || a.N < 0 || a.n_isects < 0 || a.n_active < 0)
@@ -283,38 +292,38 @@ int run_contrib(const ContribArgs &a, bool outputs_ok, size_t smem, const Sink &
     const int64_t n_tiles = sparse ? a.n_active : a.I * (int64_t)a.tw * a.th;
     if(n_tiles == 0 || a.W == 0 || a.H == 0)
         return GSB200_OK; // no pixels
-    const bool inputs_ok = a.offsets && (a.n_isects == 0 || (a.means2d && a.rows && a.opacities && a.flatten_ids))
+    const bool inputs_ok = a.offsets && walk.inputs_ok(a.n_isects) && (a.n_isects == 0 || a.flatten_ids)
                         && (!sparse || (a.tile_pixel_mask && a.tile_pixel_cumsum && a.pixel_map));
     if(!inputs_ok || !outputs_ok || !tile_grid_covers(a.tw, a.th, a.W, a.H))
         return GSB200_E_INVALID;
     if(n_tiles >= 2147483648LL || a.n_isects >= 2147483648LL)
         return GSB200_E_UNSUPPORTED;
     if(sparse)
-        return Walk::launch(a, (unsigned)n_tiles, SparsePixels{a.active_tiles, a.tile_pixel_mask, a.tile_pixel_cumsum, a.pixel_map}, sink, smem, st);
-    return Walk::launch(a, (unsigned)n_tiles, DensePixels{}, sink, smem, st);
+        return walk.launch(a, (unsigned)n_tiles, SparsePixels{a.active_tiles, a.tile_pixel_mask, a.tile_pixel_cumsum, a.pixel_map}, sink, smem, st);
+    return walk.launch(a, (unsigned)n_tiles, DensePixels{}, sink, smem, st);
 }
 
 // count: CountSink
 template<class Walk>
-int contrib_count(const ContribArgs &a, int32_t *counts, float *alphas, cudaStream_t st)
+int contrib_count(const Walk &walk, const ContribArgs &a, int32_t *counts, float *alphas, cudaStream_t st)
 {
-    return run_contrib<Walk>(a, counts != nullptr, 0, CountSink{counts, alphas}, st);
+    return run_contrib(walk, a, counts != nullptr, 0, CountSink{counts, alphas}, st);
 }
 
 // ids: IdsSink; max_samples = 0 writes nothing
 template<class Walk>
-int contrib_ids(const ContribArgs &a, int max_samples, int32_t *ids, float *weights, cudaStream_t st)
+int contrib_ids(const Walk &walk, const ContribArgs &a, int max_samples, int32_t *ids, float *weights, cudaStream_t st)
 {
     if(max_samples < 0 || a.N > 0x7fffffffLL)
         return GSB200_E_INVALID;
     if(max_samples == 0)
         return GSB200_OK;
-    return run_contrib<Walk>(a, ids && weights, 0, IdsSink{(int32_t)a.N, max_samples, ids, weights, 0}, st);
+    return run_contrib(walk, a, ids && weights, 0, IdsSink{(int32_t)a.N, max_samples, ids, weights, 0}, st);
 }
 
 // top: TopSink, num_samples in [1, Walk::max_samples()]
 template<class Walk>
-int contrib_top(const ContribArgs &a, int num_samples, int32_t *ids, float *weights, cudaStream_t st)
+int contrib_top(const Walk &walk, const ContribArgs &a, int num_samples, int32_t *ids, float *weights, cudaStream_t st)
 {
     if(num_samples <= 0 || a.N > 0x7fffffffLL)
         return GSB200_E_INVALID;
@@ -325,6 +334,6 @@ int contrib_top(const ContribArgs &a, int num_samples, int32_t *ids, float *weig
         return GSB200_E_UNSUPPORTED;
     const TopSink sink{(int32_t)a.N, num_samples, ids, weights, 0, nullptr, nullptr, nullptr};
     const size_t smem = (size_t)num_samples * kIndexBatch * TopSink::kSlotBytes;
-    return run_contrib<Walk>(a, ids && weights, smem, sink, st);
+    return run_contrib(walk, a, ids && weights, smem, sink, st);
 }
 } // namespace gsb

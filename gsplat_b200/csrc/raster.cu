@@ -1402,21 +1402,21 @@ extern "C" int gsb200_raster_indices(
 // ---- per-pixel contributor queries over raster_indices_kernel (indices.cuh: run_contrib and its checks)
 namespace gsb
 {
-struct RasterWalk
+struct RasterWalk : PlanarRows
 {
     template<class Pix, class Sink>
-    static int launch(const ContribArgs &a, unsigned n_tiles, const Pix &pm, const Sink &sink, size_t smem, cudaStream_t st)
+    int launch(const ContribArgs &a, unsigned n_tiles, const Pix &pm, const Sink &sink, size_t smem, cudaStream_t st) const
     {
         return launch_walk(
-            raster_indices_kernel<Sink, Pix>, n_tiles, smem, st, (uint32_t)a.I, a.n_isects, a.means2d, a.rows, a.opacities,
+            raster_indices_kernel<Sink, Pix>, n_tiles, smem, st, (uint32_t)a.I, a.n_isects, means2d, rows, opacities,
             (const float *)nullptr, a.W, a.H, a.tw, a.th, a.offsets, a.flatten_ids, (int32_t)0, (int32_t)0x7fffffff, sink, pm
         );
     }
     static int max_samples()
     {
-        return top_max_samples(
+        return top_max_samples({
             (const void *)raster_indices_kernel<TopSink, DensePixels>, (const void *)raster_indices_kernel<TopSink, SparsePixels>
-        );
+        });
     }
 };
 } // namespace gsb
@@ -1434,7 +1434,9 @@ extern "C" int gsb200_contrib_count(
     float *alphas, void *stream
 )
 {
-    return gsb::contrib_count<gsb::RasterWalk>(GSB200_CONTRIB_ARGS(conics), counts, alphas, (cudaStream_t)stream);
+    return gsb::contrib_count(
+        gsb::RasterWalk{{means2d, conics, opacities}}, GSB200_CONTRIB_ARGS(I), counts, alphas, (cudaStream_t)stream
+    );
 }
 
 extern "C" int gsb200_contrib_ids(
@@ -1445,7 +1447,9 @@ extern "C" int gsb200_contrib_ids(
     int32_t *ids, float *weights, void *stream
 )
 {
-    return gsb::contrib_ids<gsb::RasterWalk>(GSB200_CONTRIB_ARGS(conics), max_samples, ids, weights, (cudaStream_t)stream);
+    return gsb::contrib_ids(
+        gsb::RasterWalk{{means2d, conics, opacities}}, GSB200_CONTRIB_ARGS(I), max_samples, ids, weights, (cudaStream_t)stream
+    );
 }
 
 extern "C" int gsb200_contrib_top(
@@ -1456,5 +1460,7 @@ extern "C" int gsb200_contrib_top(
     int32_t *ids, float *weights, void *stream
 )
 {
-    return gsb::contrib_top<gsb::RasterWalk>(GSB200_CONTRIB_ARGS(conics), num_samples, ids, weights, (cudaStream_t)stream);
+    return gsb::contrib_top(
+        gsb::RasterWalk{{means2d, conics, opacities}}, GSB200_CONTRIB_ARGS(I), num_samples, ids, weights, (cudaStream_t)stream
+    );
 }

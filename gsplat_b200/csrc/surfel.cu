@@ -1013,22 +1013,22 @@ extern "C" int gsb200_surfel_indices(
 // order and with the return codes of gsb200_contrib_*)
 namespace gsb
 {
-struct SurfelWalk
+struct SurfelWalk : PlanarRows
 {
     template<class Pix, class Sink>
-    static int launch(const ContribArgs &a, unsigned n_tiles, const Pix &pm, const Sink &sink, size_t smem, cudaStream_t st)
+    int launch(const ContribArgs &a, unsigned n_tiles, const Pix &pm, const Sink &sink, size_t smem, cudaStream_t st) const
     {
         return launch_walk(
-            surfel_indices_kernel<Sink, Pix>, n_tiles, smem, st, (uint32_t)a.I, a.means2d, a.rows, a.opacities,
+            surfel_indices_kernel<Sink, Pix>, n_tiles, smem, st, (uint32_t)a.I, means2d, rows, opacities,
             (const float *)nullptr, a.W, a.H, a.tw, a.th, a.offsets, a.flatten_ids, a.n_isects, (int32_t)0,
             (int32_t)0x7fffffff, sink, pm
         );
     }
     static int max_samples()
     {
-        return top_max_samples(
+        return top_max_samples({
             (const void *)surfel_indices_kernel<TopSink, DensePixels>, (const void *)surfel_indices_kernel<TopSink, SparsePixels>
-        );
+        });
     }
 };
 } // namespace gsb
@@ -1046,7 +1046,9 @@ extern "C" int gsb200_surfel_contrib_count(
     float *alphas, void *stream
 )
 {
-    return gsb::contrib_count<gsb::SurfelWalk>(GSB200_CONTRIB_ARGS(ray_transforms), counts, alphas, (cudaStream_t)stream);
+    return gsb::contrib_count(
+        gsb::SurfelWalk{{means2d, ray_transforms, opacities}}, GSB200_CONTRIB_ARGS(I), counts, alphas, (cudaStream_t)stream
+    );
 }
 
 extern "C" int gsb200_surfel_contrib_ids(
@@ -1057,7 +1059,9 @@ extern "C" int gsb200_surfel_contrib_ids(
     int32_t *ids, float *weights, void *stream
 )
 {
-    return gsb::contrib_ids<gsb::SurfelWalk>(GSB200_CONTRIB_ARGS(ray_transforms), max_samples, ids, weights, (cudaStream_t)stream);
+    return gsb::contrib_ids(
+        gsb::SurfelWalk{{means2d, ray_transforms, opacities}}, GSB200_CONTRIB_ARGS(I), max_samples, ids, weights, (cudaStream_t)stream
+    );
 }
 
 extern "C" int gsb200_surfel_contrib_top(
@@ -1068,5 +1072,7 @@ extern "C" int gsb200_surfel_contrib_top(
     int32_t *ids, float *weights, void *stream
 )
 {
-    return gsb::contrib_top<gsb::SurfelWalk>(GSB200_CONTRIB_ARGS(ray_transforms), num_samples, ids, weights, (cudaStream_t)stream);
+    return gsb::contrib_top(
+        gsb::SurfelWalk{{means2d, ray_transforms, opacities}}, GSB200_CONTRIB_ARGS(I), num_samples, ids, weights, (cudaStream_t)stream
+    );
 }

@@ -8,6 +8,7 @@
 // the compositing thresholds).  The reference's backward gives no gradient to viewmats, and neither does this one.
 #include "camera.cuh"
 #include "gaussmath.cuh"
+#include "indices.cuh"
 #include "pixels.cuh"
 
 namespace gsb
@@ -438,6 +439,92 @@ __global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
     last_ids[pix] = cur_idx;
 }
 
+// The pair-query walk of rasterize_to_indices_in_range_eval3d and the 3DGUT contributor queries: the (pixel, gaussian)
+// pairs eval3d_fwd_kernel composites, walking only the batches [b0, b1) of each tile's list from the pixel's given
+// transmittance (null: T = 1).  The tiles, the pixel mapping, the ray (camera model, rolling-shutter pose), staging,
+// eval_hit and the stop rule are the forward's, so the alphas are its render_alphas bit for bit.  As in the forward, a
+// pixel composites only when it has an output row (live) and lies inside the W x H image with a ray; a live pixel that
+// does not composite still gets begin and end (count 0, T as given).  Every thread stages records and meets every
+// barrier.  What the walk does with a pixel's pairs is the Sink's (indices.cuh).
+template<class Sink, class Shutter, class Lens, class Pix = DensePixels>
+__global__ void __launch_bounds__(kUtThreads, 1) eval3d_indices_kernel(
+    EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
+    const float *__restrict__ opacities, const float *__restrict__ transmittances, const int32_t *__restrict__ offsets,
+    const int32_t *__restrict__ flatten_ids, int64_t n_isects, int32_t b0, int32_t b1, Sink sink, Shutter shutter,
+    Lens lens, const Pix pixmap = Pix{}
+)
+{
+    static_assert(kUtThreads == kIndexBatch, "one record of a batch per thread");
+    __shared__ EvalRec rec[kUtThreads];
+    const uint32_t tile  = pixmap.tile(blockIdx.x); // image * th * tw + tile row * tw + tile col
+    const uint32_t img   = tile / (geo.tw * geo.th);
+    const uint32_t tin   = tile - img * geo.tw * geo.th;
+    const uint32_t tr    = threadIdx.x;
+    const uint32_t i     = (tin / geo.tw) * kTile + tr / kTile;
+    const uint32_t j     = (tin % geo.tw) * kTile + tr % kTile;
+    const int64_t pix_in = (int64_t)i * geo.W + j;
+    bool live, inside = i < geo.H && j < geo.W;
+    int64_t pix, start, end;
+    if constexpr(Pix::kSparse)
+    {
+        pix    = pixmap.slot(blockIdx.x, (int)tr, live);
+        inside = inside && live;
+        start  = offsets[blockIdx.x];
+        end    = offsets[blockIdx.x + 1];
+    }
+    else
+    {
+        live  = inside;
+        pix   = (int64_t)img * geo.H * geo.W + pix_in;
+        start = offsets[tile];
+        end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
+    }
+    const int64_t b_end = min((int64_t)b1, (end - start + kUtThreads - 1) / kUtThreads);
+    float ro[3] = {0.f, 0.f, 0.f}, rd[3] = {0.f, 0.f, 1.f};
+    bool done = !inside;
+    if constexpr(Shutter::kRolling)
+    {
+        const auto cm = lens.model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        done          = !shutter_pixel_ray(shutter, geo.viewmats, img, inside, cm, i, j, ro, rd);
+    }
+    else if(inside)
+    {
+        const auto cm = lens.model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
+        done          = !pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
+    }
+    float T     = (live && transmittances != nullptr) ? transmittances[pix] : 1.f;
+    int32_t cnt = 0;
+    sink.begin(live, pix, pix_in, img);
+    for(int64_t b = b0; b < b_end; ++b)
+    {
+        if(__syncthreads_count(done) == kUtThreads)
+            break;
+        const int64_t batch = start + b * kUtThreads;
+        if(batch + tr < end)
+            stage(rec[tr], flatten_ids[batch + tr], geo.C, geo.N, means, quats, scales, opacities);
+        __syncthreads();
+        const int n_b = (int)min((int64_t)kUtThreads, end - batch);
+        for(int t = 0; t < n_b && !done; ++t)
+        {
+            const EvalRec &r = rec[t];
+            const EvalHit h  = eval_hit(r, ro, rd);
+            if(!h.ok)
+                continue;
+            const float next_T = T * (1.f - h.alpha);
+            if(next_T <= kTransmittanceThreshold)
+            { // exclusive: this gaussian does not contribute
+                done = true;
+                break;
+            }
+            sink.pair(cnt, r.id, h.alpha * T);
+            ++cnt;
+            T = next_T;
+        }
+    }
+    if(live)
+        sink.end(pix, cnt, T);
+}
+
 struct EvalGradDst
 {
     float *colors, *opacities, *rec; // rec: [B * N, 12] = v_mean 3 | v_M 9
@@ -749,6 +836,66 @@ int with_policies(const float *viewmats_rs, int rolling_shutter, const gsb200_ft
         return f(shutter, CamLens{});
     });
 }
+
+// The contributor queries' walk (indices.cuh: run_contrib): eval3d_indices_kernel over the rows and the camera of
+// gsb200_eval3d_fwd, from T = 1 through the whole lists.  Its inputs are the camera (every pixel's ray reads it) and,
+// when there are intersections, the gaussians; a sparse layout needs at least one image for its tiles to lie in.
+struct Eval3dWalk
+{
+    EvalGeom geo;
+    const float *means, *quats, *scales, *opacities;
+    const gsb200_ftheta_params *ft;
+    const float *viewmats_rs;
+    int rolling_shutter;
+
+    bool inputs_ok(int64_t n_isects) const
+    {
+        return geo.I > 0 && geo.viewmats && geo.Ks && (n_isects == 0 || (means && quats && scales && opacities));
+    }
+    template<class Pix, class Sink>
+    int launch(const ContribArgs &a, unsigned n_tiles, const Pix &pm, const Sink &sink, size_t smem, cudaStream_t st) const
+    {
+        return with_policies(viewmats_rs, rolling_shutter, ft, 1, [&](auto shutter, auto lens) {
+            return launch_walk(
+                eval3d_indices_kernel<Sink, decltype(shutter), decltype(lens), Pix>, n_tiles, smem, st, geo, means, quats,
+                scales, opacities, (const float *)nullptr, a.offsets, a.flatten_ids, a.n_isects, (int32_t)0,
+                (int32_t)0x7fffffff, sink, shutter, lens, pm
+            );
+        });
+    }
+    // one bound for every camera and shutter: the largest staging of the eight top-K instantiations (the rolling ones
+    // also hold the image's two poses)
+    static int max_samples()
+    {
+        return top_max_samples({
+            (const void *)eval3d_indices_kernel<TopSink, GlobalShutter, CamLens, DensePixels>,
+            (const void *)eval3d_indices_kernel<TopSink, GlobalShutter, FThetaLens, DensePixels>,
+            (const void *)eval3d_indices_kernel<TopSink, RollingShutter, CamLens, DensePixels>,
+            (const void *)eval3d_indices_kernel<TopSink, RollingShutter, FThetaLens, DensePixels>,
+            (const void *)eval3d_indices_kernel<TopSink, GlobalShutter, CamLens, SparsePixels>,
+            (const void *)eval3d_indices_kernel<TopSink, GlobalShutter, FThetaLens, SparsePixels>,
+            (const void *)eval3d_indices_kernel<TopSink, RollingShutter, CamLens, SparsePixels>,
+            (const void *)eval3d_indices_kernel<TopSink, RollingShutter, FThetaLens, SparsePixels>,
+        });
+    }
+};
+
+// The checks of every 3DGUT query entry before its own: sizes, camera, and the sparse layout when there is one.
+int eval3d_query_checks(
+    int64_t B, int64_t C, int64_t N, int cam_kind, const float *radial, const float *tangential, const float *thin,
+    const gsb200_ftheta_params *ft, const float *viewmats_rs, int rolling_shutter, uint32_t W, uint32_t H,
+    uint32_t tile_size, uint32_t tw, uint32_t th, int64_t n_active, const int32_t *active_tiles, const int32_t *offsets,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map
+)
+{
+    if(int rc = eval3d_checks(B, C, N, W, H, tile_size, tw, th))
+        return rc;
+    if(int rc = camera_checks(cam_kind, radial, tangential, thin, ft, viewmats_rs, rolling_shutter, W, H))
+        return rc;
+    if(active_tiles != nullptr)
+        return sparse_args_ok(n_active, active_tiles, offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, W, H, tw, th);
+    return GSB200_OK;
+}
 } // namespace
 } // namespace gsb
 
@@ -977,4 +1124,106 @@ extern "C" int gsb200_eval3d_sparse_bwd(
         B * N, quats, scales, grad_records, v_means, v_quats, v_scales
     );
     return gsb::check_launch();
+}
+
+// ---- rasterize_to_indices_in_range_eval3d: count pass (emit = 0) and emit pass (emit = 1) over one workspace
+// (indices.cuh), after the size and camera checks of gsb200_eval3d_fwd
+extern "C" int gsb200_eval3d_indices(
+    int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
+    const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+    const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+    const float *transmittances, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
+    uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t range_start,
+    int64_t range_end, int emit, void *workspace, size_t workspace_bytes, int64_t *total, int64_t *gaussian_ids,
+    int64_t *pixel_ids, int64_t *image_ids, void *stream
+)
+{
+    if(int rc = gsb::eval3d_query_checks(B, C, N, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta,
+                                         viewmats_rs, rolling_shutter, image_width, image_height, tile_size, tile_width,
+                                         tile_height, 0, nullptr, nullptr, nullptr, nullptr, nullptr))
+        return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const bool inputs_ok  = means && quats && scales && opacities && viewmats && Ks && transmittances && offsets && flatten_ids;
+    const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height,
+                            camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
+    return gsb::run_index_pass(
+        B * C, N, image_width, image_height, tile_size, tile_width, tile_height, n_isects, range_start, range_end, inputs_ok,
+        emit, workspace, workspace_bytes, total, gaussian_ids, pixel_ids, image_ids, st,
+        [&](unsigned n_tiles, int32_t b0, int32_t b1, auto sink) {
+            return gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
+                gsb::eval3d_indices_kernel<<<n_tiles, gsb::kUtThreads, 0, st>>>(
+                    geo, means, quats, scales, opacities, transmittances, offsets, flatten_ids, n_isects, b0, b1, sink,
+                    shutter, lens
+                );
+                return gsb::check_launch();
+            });
+        }
+    );
+}
+
+// ---- 3DGUT per-pixel contributor queries over eval3d_indices_kernel: the size, camera and (sparse) layout checks of
+// gsb200_eval3d_sparse_fwd, then run_contrib's (indices.cuh), in the order and with the return codes of gsb200_contrib_*
+// the checks and the walk of a contributor entry, from its parameters (named as gsb200_eval3d_contrib_count's)
+#define GSB200_EVAL3D_QUERY_CHECKS                                                                                      \
+    gsb::eval3d_query_checks(                                                                                           \
+        B, C, N, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta, viewmats_rs, rolling_shutter, \
+        image_width, image_height, tile_size, tile_width, tile_height, n_active, active_tiles, offsets, tile_pixel_mask,  \
+        tile_pixel_cumsum, pixel_map                                                                                    \
+    )
+#define GSB200_EVAL3D_WALK                                                                                              \
+    gsb::Eval3dWalk                                                                                                     \
+    {                                                                                                                   \
+        {(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height, camera_model,  \
+         viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs},                                            \
+            means, quats, scales, opacities, ftheta, viewmats_rs, rolling_shutter                                       \
+    }
+
+extern "C" int gsb200_eval3d_contrib_max_samples(void)
+{
+    return gsb::Eval3dWalk::max_samples();
+}
+
+extern "C" int gsb200_eval3d_contrib_count(
+    int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
+    const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+    const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+    const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int32_t *counts,
+    float *alphas, void *stream
+)
+{
+    if(int rc = GSB200_EVAL3D_QUERY_CHECKS)
+        return rc;
+    return gsb::contrib_count(GSB200_EVAL3D_WALK, GSB200_CONTRIB_ARGS(B * C), counts, alphas, (cudaStream_t)stream);
+}
+
+extern "C" int gsb200_eval3d_contrib_ids(
+    int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
+    const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+    const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+    const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int max_samples,
+    int32_t *ids, float *weights, void *stream
+)
+{
+    if(int rc = GSB200_EVAL3D_QUERY_CHECKS)
+        return rc;
+    return gsb::contrib_ids(GSB200_EVAL3D_WALK, GSB200_CONTRIB_ARGS(B * C), max_samples, ids, weights, (cudaStream_t)stream);
+}
+
+extern "C" int gsb200_eval3d_contrib_top(
+    int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
+    const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+    const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+    const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int num_samples,
+    int32_t *ids, float *weights, void *stream
+)
+{
+    if(int rc = GSB200_EVAL3D_QUERY_CHECKS)
+        return rc;
+    return gsb::contrib_top(GSB200_EVAL3D_WALK, GSB200_CONTRIB_ARGS(B * C), num_samples, ids, weights, (cudaStream_t)stream);
 }

@@ -1515,6 +1515,13 @@ def _indices_in_range(
         return tuple(torch.empty(0, device=dev, dtype=torch.int64) for _ in range(3))
     tr, m2, rw, op = (t.contiguous() for t in (transmittances, means2d, rows, opacities))
     off, fl = isect_offsets.contiguous(), flatten_ids.contiguous()
+    args = (I, N, ptr(m2), ptr(rw), ptr(op), ptr(tr), W, H, 16, tw, th, ptr(off), ptr(fl), S, rs, re_)
+    return _index_passes(what, entry, args, P, dev)
+
+
+def _index_passes(what, entry, args, P, dev):
+    """The count and emit passes of a pair-query entry over P pixels: ``args`` are its arguments before ``emit`` (the
+    tensors they point into are kept alive by the caller)."""
     L = lib()
     ws = torch.empty(L.gsb200_indices_workspace_bytes(P), device=dev, dtype=torch.uint8)
     total = torch.empty(1, device=dev, dtype=torch.int64)
@@ -1522,11 +1529,7 @@ def _indices_in_range(
     with _Ctx(dev) as st:
 
         def run(emit, outs):
-            check(
-                fn(I, N, ptr(m2), ptr(rw), ptr(op), ptr(tr), W, H, 16, tw, th, ptr(off), ptr(fl), S, rs, re_, emit, ptr(ws),
-                   ws.numel(), ptr(total), *(ptr(o) for o in outs), st),
-                what,
-            )
+            check(fn(*args, emit, ptr(ws), ws.numel(), ptr(total), *(ptr(o) for o in outs), st), what)
 
         run(0, (None, None, None))
         M = int(total.item())  # the host sync between the two passes (reference: csrc/Rasterization.cpp:1050)
@@ -2022,8 +2025,8 @@ def rasterize_to_pixels_2dgs_sparse(
 class _ContribWalk(NamedTuple):
     """One pair-query walk of the contributor queries: its rows (tail and name) and its C entries."""
 
-    rows_tail: tuple  # (3,) conics or (3, 3) ray_transforms
-    rows_name: str
+    rows_tail: Optional[tuple]  # (3,) conics or (3, 3) ray_transforms; None for the 3-D rows of the eval3d walk
+    rows_name: Optional[str]
     packed: bool  # whether the dense form also takes packed [nnz, *] rows
     count: str
     ids: str
@@ -2035,6 +2038,8 @@ _CONTRIB_3DGS = _ContribWalk((3,), "conics", True, "gsb200_contrib_count", "gsb2
                              "gsb200_contrib_max_samples")
 _CONTRIB_2DGS = _ContribWalk((3, 3), "ray_transforms", False, "gsb200_surfel_contrib_count", "gsb200_surfel_contrib_ids",
                              "gsb200_surfel_contrib_top", "gsb200_surfel_contrib_max_samples")
+_CONTRIB_EVAL3D = _ContribWalk(None, None, False, "gsb200_eval3d_contrib_count", "gsb200_eval3d_contrib_ids",
+                               "gsb200_eval3d_contrib_top", "gsb200_eval3d_contrib_max_samples")
 
 _max_samples_cache = {}
 
@@ -2075,6 +2080,71 @@ def _contrib_rows(walk, means2d, rows, opacities, image_dims=None) -> int:
     return lead[-1]
 
 
+class _PlanarRows(NamedTuple):
+    """What the 3DGS and 2DGS walks composite: means2d, conics or ray_transforms, opacities."""
+
+    walk: _ContribWalk
+    means2d: Tensor
+    rows: Tensor
+    opacities: Tensor
+
+    def check(self, image_dims=None) -> int:
+        """The shapes, against the images of a dense layout if given; returns N."""
+        return _contrib_rows(self.walk, self.means2d, self.rows, self.opacities, image_dims)
+
+    def floats(self):
+        return (self.means2d, "means2d"), (self.rows, self.walk.rows_name), (self.opacities, "opacities")
+
+    def tensors(self):
+        return self.means2d, self.rows, self.opacities
+
+    def head(self, I, N):
+        """The C arguments before the image size, and the tensors they point into."""
+        keep = [t.contiguous() for t in self.tensors()]
+        return (I, N) + tuple(ptr(t) for t in keep), keep
+
+
+class _Eval3dRows:
+    """What the eval3d walk composites: the 3-D Gaussians, the (batch, camera) opacities and the cameras of
+    rasterize_to_pixels_eval3d, checked as it checks them."""
+
+    walk = _CONTRIB_EVAL3D
+
+    def __init__(self, what, means, quats, scales, opacities, viewmats, Ks, width, height, camera_model, radial_coeffs,
+                 tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, rolling_shutter, viewmats_rs):
+        self.what, self.means, self.quats, self.scales, self.opacities = what, means, quats, scales, opacities
+        self.viewmats, self.Ks, self.width, self.height = viewmats, Ks, int(width), int(height)
+        self.camera = (camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, rolling_shutter,
+                       viewmats_rs)
+        self.cam = None
+
+    def check(self, image_dims=None) -> int:
+        batch, C, N = _ut_geometry(self.what, self.means, self.quats, self.scales, self.viewmats, self.Ks)
+        if image_dims is not None and tuple(image_dims) != batch + (C,):
+            raise ValueError(f"{self.what}: tile_offsets must be {batch + (C, 'tile_height', 'tile_width')} to match the "
+                             f"cameras, got images {tuple(image_dims)}")
+        _check_shape(self.opacities, batch + (C, N), "opacities")
+        model, radial, tangential, thin, ftheta, shutter, viewmats_rs = self.camera
+        self.cam = _ut_camera(self.what, self.viewmats, self.width, self.height, model, radial, tangential, thin, ftheta,
+                              None, None, shutter, viewmats_rs)
+        self.B, self.C = _prod(batch), C
+        return N
+
+    def floats(self):
+        return ((self.opacities, "opacities"),)  # the geometry's dtypes are _ut_geometry's
+
+    def tensors(self):
+        c = self.cam
+        return (self.means, self.quats, self.scales, self.opacities, self.viewmats, self.Ks, c.radial, c.tangential, c.thin,
+                c.viewmats_rs)
+
+    def head(self, I, N):
+        c = self.cam
+        keep = [t.contiguous() for t in self.tensors()[:6]] + [c]  # c.ftheta is read through its host address
+        return (self.B, self.C, N, *(ptr(t) for t in keep[:6]), c.model, ptr(c.radial), ptr(c.tangential), ptr(c.thin),
+                _ftheta_ptr(c.ftheta), ptr(c.viewmats_rs), c.shutter), keep
+
+
 def _contrib_dtypes(floats, ints) -> None:
     for t, name in floats:
         if t.dtype != torch.float32:
@@ -2094,10 +2164,10 @@ def _check_counts(num_contributing_gaussians, dims) -> None:
         raise TypeError(f"num_contributing_gaussians must have dtype int32, got {nc.dtype}")
 
 
-def _contrib_dense(walk, means2d, rows, opacities, tile_offsets, flatten_ids, image_width, image_height, tile_size,
-                   counts=None):
-    """Checks the dense-layout arguments (and the per-pixel counts, if given); returns (the walk, the output dims
-    [..., H, W], (the C arguments before the outputs, the tensors they point into), the device)."""
+def _contrib_dense(rows, tile_offsets, flatten_ids, image_width, image_height, tile_size, counts=None):
+    """Checks the dense-layout arguments (and the per-pixel counts, if given) over the walk's rows (_PlanarRows or
+    _Eval3dRows); returns (the walk, the output dims [..., H, W], (the C arguments before the outputs, the tensors they
+    point into), the device)."""
     W, H = int(image_width), int(image_height)
     if tile_size != 16:
         raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
@@ -2105,29 +2175,27 @@ def _contrib_dense(walk, means2d, rows, opacities, tile_offsets, flatten_ids, im
         raise ValueError(f"tile_offsets must be [..., tile_height, tile_width], got {tuple(tile_offsets.shape)}")
     image_dims = tuple(tile_offsets.shape[:-2])
     th, tw = tile_offsets.shape[-2:]
-    N = _contrib_rows(walk, means2d, rows, opacities, image_dims)
+    N = rows.check(image_dims)
     if th * 16 < H or tw * 16 < W:
         raise ValueError(f"tile_offsets tile grid {tw}x{th} does not cover a {W}x{H} image")
     if flatten_ids.dim() != 1:
         raise ValueError(f"flatten_ids must be one-dimensional, got {tuple(flatten_ids.shape)}")
-    _contrib_dtypes(((means2d, "means2d"), (rows, walk.rows_name), (opacities, "opacities")),
-                    ((tile_offsets, "tile_offsets", torch.int32), (flatten_ids, "flatten_ids", torch.int32)))
+    _contrib_dtypes(rows.floats(), ((tile_offsets, "tile_offsets", torch.int32), (flatten_ids, "flatten_ids", torch.int32)))
     _check_counts(counts, image_dims + (H, W))
-    dev = require_cuda(means2d, rows, opacities, tile_offsets, flatten_ids, counts)
-    keep = [t.contiguous() for t in (means2d, rows, opacities, tile_offsets, flatten_ids)]
-    m2, rw, op, off, fl = keep
-    args = (_prod(image_dims), N, ptr(m2), ptr(rw), ptr(op), W, H, 16, tw, th, ptr(off), ptr(fl), fl.shape[0], 0, None, None,
-            None, None)
-    return walk, image_dims + (H, W), (args, keep), dev
+    dev = require_cuda(*rows.tensors(), tile_offsets, flatten_ids, counts)
+    head, keep = rows.head(_prod(image_dims), N)
+    off, fl = tile_offsets.contiguous(), flatten_ids.contiguous()
+    args = head + (W, H, 16, tw, th, ptr(off), ptr(fl), fl.shape[0], 0, None, None, None, None)
+    return rows.walk, image_dims + (H, W), (args, keep + [off, fl]), dev
 
 
-def _contrib_sparse(walk, means2d, rows, opacities, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask,
-                    tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size, tile_width, tile_height, counts=None):
+def _contrib_sparse(rows, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map,
+                    image_width, image_height, tile_size, tile_width, tile_height, counts=None):
     """_contrib_dense for a sparse layout: the output dims are [P]."""
     W, H, tw, th = int(image_width), int(image_height), int(tile_width), int(tile_height)
     if tile_size != 16:
         raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
-    N = _contrib_rows(walk, means2d, rows, opacities)
+    N = rows.check()
     if active_tiles.dim() != 1 or pixel_map.dim() != 1 or flatten_ids.dim() != 1:
         raise ValueError("active_tiles [AT], pixel_map [P] and flatten_ids [n_isects] must be one-dimensional")
     AT, P = active_tiles.shape[0], pixel_map.shape[0]
@@ -2141,19 +2209,19 @@ def _contrib_sparse(walk, means2d, rows, opacities, active_tiles, tile_offsets, 
         raise ValueError(f"a {tw} x {th} tile grid does not cover {W} x {H} pixels")
     if tile_pixel_mask.element_size() != 8 or tile_pixel_mask.is_floating_point():
         raise TypeError(f"tile_pixel_mask must be a 64-bit integer tensor, got {tile_pixel_mask.dtype}")
-    _contrib_dtypes(((means2d, "means2d"), (rows, walk.rows_name), (opacities, "opacities")),
+    _contrib_dtypes(rows.floats(),
                     ((active_tiles, "active_tiles", torch.int32), (tile_offsets, "tile_offsets", torch.int32),
                      (flatten_ids, "flatten_ids", torch.int32), (tile_pixel_cumsum, "tile_pixel_cumsum", torch.int64),
                      (pixel_map, "pixel_map", torch.int64)))
     _check_counts(counts, (P,))
-    dev = require_cuda(means2d, rows, opacities, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum,
+    dev = require_cuda(*rows.tensors(), active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum,
                        pixel_map, counts)
-    keep = [t.contiguous() for t in (means2d, rows, opacities, tile_offsets, flatten_ids, active_tiles, tile_pixel_mask,
-                                     tile_pixel_cumsum, pixel_map)]
-    m2, rw, op, off, fl, act, words, cum, pmap = keep
-    args = (1, N, ptr(m2), ptr(rw), ptr(op), W, H, 16, tw, th, ptr(off), ptr(fl), fl.shape[0], AT, ptr(act), ptr(words),
-            ptr(cum), ptr(pmap))
-    return walk, (P,), (args, keep), dev
+    head, keep = rows.head(1, N)
+    layout = [t.contiguous() for t in (tile_offsets, flatten_ids, active_tiles, tile_pixel_mask, tile_pixel_cumsum,
+                                       pixel_map)]
+    off, fl, act, words, cum, pmap = layout
+    args = head + (W, H, 16, tw, th, ptr(off), ptr(fl), fl.shape[0], AT, ptr(act), ptr(words), ptr(cum), ptr(pmap))
+    return rows.walk, (P,), (args, keep + layout), dev
 
 
 def _contrib_count(what, checked):
@@ -2209,8 +2277,8 @@ def rasterize_num_contributing_gaussians(
     """Per pixel, the number of Gaussians ``rasterize_to_pixels`` composites and its accumulated alpha.  The decisions
     are the compositing kernel's own, so the alphas equal ``render_alphas``.  Returns (counts int32 [..., H, W],
     alphas float32 [..., H, W])."""
-    checked = _contrib_dense(_CONTRIB_3DGS, means2d, conics, opacities, tile_offsets, flatten_ids, image_width,
-                             image_height, tile_size)
+    checked = _contrib_dense(_PlanarRows(_CONTRIB_3DGS, means2d, conics, opacities), tile_offsets, flatten_ids,
+                             image_width, image_height, tile_size)
     return _contrib_count("rasterize_num_contributing_gaussians", checked)
 
 
@@ -2233,9 +2301,9 @@ def rasterize_num_contributing_gaussians_sparse(
 ) -> Tuple[Tensor, Tensor]:
     """``rasterize_num_contributing_gaussians`` at the pixels of a build_sparse_tile_layout layout, with the lists of
     isect_tiles_sparse.  Returns (counts int32 [P], alphas float32 [P]) in the original pixel order."""
-    checked = _contrib_sparse(_CONTRIB_3DGS, means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids,
-                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
-                              tile_width, tile_height)
+    checked = _contrib_sparse(_PlanarRows(_CONTRIB_3DGS, means2d, conics, opacities), active_tiles, tile_offsets,
+                              flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height,
+                              tile_size, tile_width, tile_height)
     return _contrib_count("rasterize_num_contributing_gaussians_sparse", checked)
 
 
@@ -2254,8 +2322,8 @@ def rasterize_contributing_gaussian_ids(
     """Every Gaussian each pixel composites, front to back, with its weight ``alpha * T`` (T before it).  Returns
     (ids int32, weights float32) [..., H, W, K] with K = ``num_contributing_gaussians.max()`` (read back to the host
     once): a pixel's first K pairs (later ones are dropped), then -1 / 0.  Ids index N (dense rows) or nnz (packed)."""
-    checked = _contrib_dense(_CONTRIB_3DGS, means2d, conics, opacities, tile_offsets, flatten_ids, image_width,
-                             image_height, tile_size, num_contributing_gaussians)
+    checked = _contrib_dense(_PlanarRows(_CONTRIB_3DGS, means2d, conics, opacities), tile_offsets, flatten_ids,
+                             image_width, image_height, tile_size, num_contributing_gaussians)
     return _contrib_ids("rasterize_contributing_gaussian_ids", checked, num_contributing_gaussians)
 
 
@@ -2279,9 +2347,9 @@ def rasterize_contributing_gaussian_ids_sparse(
 ) -> Tuple[Tensor, Tensor]:
     """``rasterize_contributing_gaussian_ids`` at the pixels of a sparse layout: (ids, weights) [P, K] in the original
     pixel order."""
-    checked = _contrib_sparse(_CONTRIB_3DGS, means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids,
-                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
-                              tile_width, tile_height, num_contributing_gaussians)
+    checked = _contrib_sparse(_PlanarRows(_CONTRIB_3DGS, means2d, conics, opacities), active_tiles, tile_offsets,
+                              flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height,
+                              tile_size, tile_width, tile_height, num_contributing_gaussians)
     return _contrib_ids("rasterize_contributing_gaussian_ids_sparse", checked, num_contributing_gaussians)
 
 
@@ -2302,8 +2370,8 @@ def rasterize_top_contributing_gaussian_ids(
     strictly heavier, as in the reference.  K must lie in [1, the device's bound] (about 71 on an H100: K slots per pixel
     live in shared memory); outside it a ValueError is raised before anything runs."""
     K = _depth_samples(num_depth_samples)
-    checked = _contrib_dense(_CONTRIB_3DGS, means2d, conics, opacities, tile_offsets, flatten_ids, image_width,
-                             image_height, tile_size)
+    checked = _contrib_dense(_PlanarRows(_CONTRIB_3DGS, means2d, conics, opacities), tile_offsets, flatten_ids,
+                             image_width, image_height, tile_size)
     return _contrib_top("rasterize_top_contributing_gaussian_ids", checked, K)
 
 
@@ -2328,9 +2396,9 @@ def rasterize_top_contributing_gaussian_ids_sparse(
     """``rasterize_top_contributing_gaussian_ids`` at the pixels of a sparse layout: (ids, weights) [P, K] in the
     original pixel order."""
     K = _depth_samples(num_depth_samples)
-    checked = _contrib_sparse(_CONTRIB_3DGS, means2d, conics, opacities, active_tiles, tile_offsets, flatten_ids,
-                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
-                              tile_width, tile_height)
+    checked = _contrib_sparse(_PlanarRows(_CONTRIB_3DGS, means2d, conics, opacities), active_tiles, tile_offsets,
+                              flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height,
+                              tile_size, tile_width, tile_height)
     return _contrib_top("rasterize_top_contributing_gaussian_ids_sparse", checked, K)
 
 
@@ -2349,8 +2417,8 @@ def rasterize_num_contributing_gaussians_2dgs(
     ``rasterize_to_pixels_2dgs`` composites and its accumulated alpha.  The decisions are the 2DGS compositing kernel's
     own, so the alphas equal its ``render_alphas`` bit for bit.  Returns (counts int32 [..., H, W], alphas float32
     [..., H, W])."""
-    checked = _contrib_dense(_CONTRIB_2DGS, means2d, ray_transforms, opacities, tile_offsets, flatten_ids, image_width,
-                             image_height, tile_size)
+    checked = _contrib_dense(_PlanarRows(_CONTRIB_2DGS, means2d, ray_transforms, opacities), tile_offsets, flatten_ids,
+                             image_width, image_height, tile_size)
     return _contrib_count("rasterize_num_contributing_gaussians_2dgs", checked)
 
 
@@ -2374,9 +2442,9 @@ def rasterize_num_contributing_gaussians_2dgs_sparse(
     """``rasterize_num_contributing_gaussians_2dgs`` at the pixels of a build_sparse_tile_layout layout, with the lists
     of isect_tiles_sparse (conics=None) on the surfel rows.  Returns (counts int32 [P], alphas float32 [P]) in the
     original pixel order."""
-    checked = _contrib_sparse(_CONTRIB_2DGS, means2d, ray_transforms, opacities, active_tiles, tile_offsets, flatten_ids,
-                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
-                              tile_width, tile_height)
+    checked = _contrib_sparse(_PlanarRows(_CONTRIB_2DGS, means2d, ray_transforms, opacities), active_tiles,
+                              tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width,
+                              image_height, tile_size, tile_width, tile_height)
     return _contrib_count("rasterize_num_contributing_gaussians_2dgs_sparse", checked)
 
 
@@ -2395,8 +2463,8 @@ def rasterize_contributing_gaussian_ids_2dgs(
     """Every surfel each pixel composites, front to back, with its weight ``alpha * T`` (T before it).  Returns
     (ids int32, weights float32) [..., H, W, K] with K = ``num_contributing_gaussians.max()`` (read back to the host
     once): a pixel's first K pairs (later ones are dropped), then -1 / 0.  Ids index N."""
-    checked = _contrib_dense(_CONTRIB_2DGS, means2d, ray_transforms, opacities, tile_offsets, flatten_ids, image_width,
-                             image_height, tile_size, num_contributing_gaussians)
+    checked = _contrib_dense(_PlanarRows(_CONTRIB_2DGS, means2d, ray_transforms, opacities), tile_offsets, flatten_ids,
+                             image_width, image_height, tile_size, num_contributing_gaussians)
     return _contrib_ids("rasterize_contributing_gaussian_ids_2dgs", checked, num_contributing_gaussians)
 
 
@@ -2420,9 +2488,9 @@ def rasterize_contributing_gaussian_ids_2dgs_sparse(
 ) -> Tuple[Tensor, Tensor]:
     """``rasterize_contributing_gaussian_ids_2dgs`` at the pixels of a sparse layout: (ids, weights) [P, K] in the
     original pixel order."""
-    checked = _contrib_sparse(_CONTRIB_2DGS, means2d, ray_transforms, opacities, active_tiles, tile_offsets, flatten_ids,
-                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
-                              tile_width, tile_height, num_contributing_gaussians)
+    checked = _contrib_sparse(_PlanarRows(_CONTRIB_2DGS, means2d, ray_transforms, opacities), active_tiles,
+                              tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width,
+                              image_height, tile_size, tile_width, tile_height, num_contributing_gaussians)
     return _contrib_ids("rasterize_contributing_gaussian_ids_2dgs_sparse", checked, num_contributing_gaussians)
 
 
@@ -2443,8 +2511,8 @@ def rasterize_top_contributing_gaussian_ids_2dgs(
     lie in [1, the surfel walk's bound on the device] (71 on an H100); outside it a ValueError is raised before anything
     runs."""
     K = _depth_samples(num_depth_samples)
-    checked = _contrib_dense(_CONTRIB_2DGS, means2d, ray_transforms, opacities, tile_offsets, flatten_ids, image_width,
-                             image_height, tile_size)
+    checked = _contrib_dense(_PlanarRows(_CONTRIB_2DGS, means2d, ray_transforms, opacities), tile_offsets, flatten_ids,
+                             image_width, image_height, tile_size)
     return _contrib_top("rasterize_top_contributing_gaussian_ids_2dgs", checked, K)
 
 
@@ -2469,9 +2537,9 @@ def rasterize_top_contributing_gaussian_ids_2dgs_sparse(
     """``rasterize_top_contributing_gaussian_ids_2dgs`` at the pixels of a sparse layout: (ids, weights) [P, K] in the
     original pixel order."""
     K = _depth_samples(num_depth_samples)
-    checked = _contrib_sparse(_CONTRIB_2DGS, means2d, ray_transforms, opacities, active_tiles, tile_offsets, flatten_ids,
-                              tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width, image_height, tile_size,
-                              tile_width, tile_height)
+    checked = _contrib_sparse(_PlanarRows(_CONTRIB_2DGS, means2d, ray_transforms, opacities), active_tiles,
+                              tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum, pixel_map, image_width,
+                              image_height, tile_size, tile_width, tile_height)
     return _contrib_top("rasterize_top_contributing_gaussian_ids_2dgs_sparse", checked, K)
 
 
@@ -3196,3 +3264,289 @@ def rasterize_to_pixels_eval3d_sparse(
         int(image_height), int(tile_width), int(tile_height), image_ids, active_tiles, tile_offsets, flatten_ids,
         tile_pixel_mask, tile_pixel_cumsum, pixel_map,
     )
+
+
+# --------------------------------------------------------------------------------------------
+# 3DGUT pair query and per-pixel contributor queries (the reference has none): the pairs rasterize_to_pixels_eval3d
+# composites, from the walk of csrc/ut.cu (eval3d_indices_kernel) with the forward's rays, responses and stop rule.  The
+# contributor forms are those of the 3DGS / 2DGS queries over that walk, with the geometry and cameras of
+# rasterize_to_pixels_eval3d in place of 2-D rows.
+
+@torch.no_grad()
+def rasterize_to_indices_in_range_eval3d(
+    range_start: int,
+    range_end: int,
+    transmittances: Tensor,  # [..., C, image_height, image_width]
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    opacities: Tensor,  # [..., C, N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    isect_offsets: Tensor,  # [..., C, tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+    camera_model: str = "pinhole",
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    rolling_shutter: int = RollingShutterType.GLOBAL,
+    viewmats_rs: Optional[Tensor] = None,  # [..., C, 4, 4]
+) -> Tuple[Tensor, Tensor, Tensor]:
+    """``rasterize_to_indices_in_range`` for 3DGUT: the (gaussian, pixel) pairs ``rasterize_to_pixels_eval3d``
+    composites when every pixel starts from its transmittance and walks only the batches ``[range_start, range_end)``
+    of 256 Gaussians of its tile's list, with the forward's own decisions (the pixel's ray through the camera model and
+    shutter, the largest response along it, the stop at T <= 1e-4).  A pixel whose ray cannot be unprojected (an FTheta
+    pixel whose inversion does not converge) has no pairs.  Dense rows only.  Returns int64 ``(gaussian_ids, pixel_ids,
+    image_ids)`` [M], ordered as ``rasterize_to_indices_in_range``'s; ``image_ids`` index the flattened (batch,
+    camera) images."""
+    what = "rasterize_to_indices_in_range_eval3d"
+    rs, re_ = _batch_index(range_start, "range_start"), _batch_index(range_end, "range_end")
+    W, H = int(image_width), int(image_height)
+    if tile_size != 16:
+        raise ValueError(f"Unsupported tile_size {tile_size}; gsplat_b200 is built for tile_size 16")
+    rows = _Eval3dRows(what, means, quats, scales, opacities, viewmats, Ks, W, H, camera_model, radial_coeffs,
+                       tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, rolling_shutter, viewmats_rs)
+    if isect_offsets.dim() < 2:
+        raise ValueError(f"isect_offsets must be [..., C, tile_height, tile_width], got {tuple(isect_offsets.shape)}")
+    image_dims = tuple(isect_offsets.shape[:-2])
+    N = rows.check(image_dims)
+    _check_shape(transmittances, image_dims + (H, W), "transmittances")
+    th, tw = isect_offsets.shape[-2:]
+    if th * 16 < H or tw * 16 < W:
+        raise ValueError(f"isect_offsets tile grid {tw}x{th} does not cover a {W}x{H} image")
+    if flatten_ids.dim() != 1:
+        raise ValueError(f"flatten_ids must be one-dimensional, got {tuple(flatten_ids.shape)}")
+    if isect_offsets.dtype != torch.int32 or flatten_ids.dtype != torch.int32:
+        raise TypeError("isect_offsets and flatten_ids must be int32")
+    _contrib_dtypes(rows.floats() + ((transmittances, "transmittances"),), ())
+    dev = require_cuda(*rows.tensors(), transmittances, isect_offsets, flatten_ids)
+    S, P = flatten_ids.shape[0], _prod(image_dims) * H * W
+    if N == 0 or S == 0 or P == 0 or re_ <= rs:
+        return tuple(torch.empty(0, device=dev, dtype=torch.int64) for _ in range(3))
+    head, keep = rows.head(_prod(image_dims), N)
+    tr, off, fl = transmittances.contiguous(), isect_offsets.contiguous(), flatten_ids.contiguous()
+    args = head + (ptr(tr), W, H, 16, tw, th, ptr(off), ptr(fl), S, rs, re_)
+    return _index_passes(what, "gsb200_eval3d_indices", args, P, dev)
+
+
+@torch.no_grad()
+def rasterize_num_contributing_gaussians_eval3d(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    opacities: Tensor,  # [..., C, N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    tile_offsets: Tensor,  # [..., C, tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    camera_model: str = "pinhole",
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    rolling_shutter: int = RollingShutterType.GLOBAL,
+    viewmats_rs: Optional[Tensor] = None,  # [..., C, 4, 4]
+) -> Tuple[Tensor, Tensor]:
+    """``rasterize_num_contributing_gaussians`` for 3DGUT: per pixel, the number of Gaussians
+    ``rasterize_to_pixels_eval3d`` composites and its accumulated alpha, equal to its ``render_alphas`` bit for bit for
+    the same Gaussians, cameras and lists (after ``rasterization(..., with_ut=True, with_eval3d=True)``: its
+    ``meta["opacities"]``, ``meta["isect_offsets"]`` and ``meta["flatten_ids"]``).  A pixel that composites nothing
+    (an FTheta pixel whose unprojection does not converge) has count 0 and alpha 0.  Returns (counts int32 [..., C, H,
+    W], alphas float32 [..., C, H, W])."""
+    what = "rasterize_num_contributing_gaussians_eval3d"
+    rows = _Eval3dRows(what, means, quats, scales, opacities, viewmats, Ks, image_width, image_height, camera_model,
+                       radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, rolling_shutter, viewmats_rs)
+    checked = _contrib_dense(rows, tile_offsets, flatten_ids, image_width, image_height, tile_size)
+    return _contrib_count(what, checked)
+
+
+@torch.no_grad()
+def rasterize_num_contributing_gaussians_eval3d_sparse(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    opacities: Tensor,  # [..., C, N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    active_tiles: Tensor,  # [AT]
+    tile_offsets: Tensor,  # [AT + 1]
+    flatten_ids: Tensor,  # [n_isects]
+    tile_pixel_mask: Tensor,  # [AT, 4]
+    tile_pixel_cumsum: Tensor,  # [AT]
+    pixel_map: Tensor,  # [P]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+    camera_model: str = "pinhole",
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    rolling_shutter: int = RollingShutterType.GLOBAL,
+    viewmats_rs: Optional[Tensor] = None,  # [..., C, 4, 4]
+) -> Tuple[Tensor, Tensor]:
+    """``rasterize_num_contributing_gaussians_eval3d`` at the pixels of a build_sparse_tile_layout layout, with the lists
+    of isect_tiles_sparse (conics=None) on the UT rows, as rasterize_to_pixels_eval3d_sparse takes them.  A requested
+    pixel in the margin of a partial tile composites nothing (count 0, alpha 0), as in that op.  Returns (counts int32
+    [P], alphas float32 [P]) in the original pixel order."""
+    what = "rasterize_num_contributing_gaussians_eval3d_sparse"
+    rows = _Eval3dRows(what, means, quats, scales, opacities, viewmats, Ks, image_width, image_height, camera_model,
+                       radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, rolling_shutter, viewmats_rs)
+    checked = _contrib_sparse(rows, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum,
+                              pixel_map, image_width, image_height, tile_size, tile_width, tile_height)
+    return _contrib_count(what, checked)
+
+
+@torch.no_grad()
+def rasterize_contributing_gaussian_ids_eval3d(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    opacities: Tensor,  # [..., C, N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    tile_offsets: Tensor,  # [..., C, tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    num_contributing_gaussians: Tensor,  # [..., C, image_height, image_width] int32
+    camera_model: str = "pinhole",
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    rolling_shutter: int = RollingShutterType.GLOBAL,
+    viewmats_rs: Optional[Tensor] = None,  # [..., C, 4, 4]
+) -> Tuple[Tensor, Tensor]:
+    """Every Gaussian each pixel composites in ``rasterize_to_pixels_eval3d``, front to back, with its weight
+    ``alpha * T`` (T before it).  Returns (ids int32, weights float32) [..., C, H, W, K] with K =
+    ``num_contributing_gaussians.max()`` (read back to the host once): a pixel's first K pairs (later ones are
+    dropped), then -1 / 0.  Ids index N."""
+    what = "rasterize_contributing_gaussian_ids_eval3d"
+    rows = _Eval3dRows(what, means, quats, scales, opacities, viewmats, Ks, image_width, image_height, camera_model,
+                       radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, rolling_shutter, viewmats_rs)
+    checked = _contrib_dense(rows, tile_offsets, flatten_ids, image_width, image_height, tile_size,
+                             num_contributing_gaussians)
+    return _contrib_ids(what, checked, num_contributing_gaussians)
+
+
+@torch.no_grad()
+def rasterize_contributing_gaussian_ids_eval3d_sparse(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    opacities: Tensor,  # [..., C, N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    active_tiles: Tensor,  # [AT]
+    tile_offsets: Tensor,  # [AT + 1]
+    flatten_ids: Tensor,  # [n_isects]
+    tile_pixel_mask: Tensor,  # [AT, 4]
+    tile_pixel_cumsum: Tensor,  # [AT]
+    pixel_map: Tensor,  # [P]
+    num_contributing_gaussians: Tensor,  # [P] int32
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+    camera_model: str = "pinhole",
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    rolling_shutter: int = RollingShutterType.GLOBAL,
+    viewmats_rs: Optional[Tensor] = None,  # [..., C, 4, 4]
+) -> Tuple[Tensor, Tensor]:
+    """``rasterize_contributing_gaussian_ids_eval3d`` at the pixels of a sparse layout: (ids, weights) [P, K] in the
+    original pixel order."""
+    what = "rasterize_contributing_gaussian_ids_eval3d_sparse"
+    rows = _Eval3dRows(what, means, quats, scales, opacities, viewmats, Ks, image_width, image_height, camera_model,
+                       radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, rolling_shutter, viewmats_rs)
+    checked = _contrib_sparse(rows, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum,
+                              pixel_map, image_width, image_height, tile_size, tile_width, tile_height,
+                              num_contributing_gaussians)
+    return _contrib_ids(what, checked, num_contributing_gaussians)
+
+
+@torch.no_grad()
+def rasterize_top_contributing_gaussian_ids_eval3d(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    opacities: Tensor,  # [..., C, N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    tile_offsets: Tensor,  # [..., C, tile_height, tile_width]
+    flatten_ids: Tensor,  # [n_isects]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    num_depth_samples: int,
+    camera_model: str = "pinhole",
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    rolling_shutter: int = RollingShutterType.GLOBAL,
+    viewmats_rs: Optional[Tensor] = None,  # [..., C, 4, 4]
+) -> Tuple[Tensor, Tensor]:
+    """The ``num_depth_samples`` heaviest Gaussians of each pixel of ``rasterize_to_pixels_eval3d`` by ``alpha * T``,
+    front to back: (ids int32, weights float32) [..., C, H, W, K], -1 / 0 in unused slots, by the rule of
+    ``rasterize_top_contributing_gaussian_ids``.  K must lie in [1, the eval3d walk's bound on the device], one bound
+    for every camera and shutter; outside it a ValueError is raised before anything runs."""
+    what = "rasterize_top_contributing_gaussian_ids_eval3d"
+    K = _depth_samples(num_depth_samples)
+    rows = _Eval3dRows(what, means, quats, scales, opacities, viewmats, Ks, image_width, image_height, camera_model,
+                       radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, rolling_shutter, viewmats_rs)
+    checked = _contrib_dense(rows, tile_offsets, flatten_ids, image_width, image_height, tile_size)
+    return _contrib_top(what, checked, K)
+
+
+@torch.no_grad()
+def rasterize_top_contributing_gaussian_ids_eval3d_sparse(
+    means: Tensor,  # [..., N, 3]
+    quats: Tensor,  # [..., N, 4]
+    scales: Tensor,  # [..., N, 3]
+    opacities: Tensor,  # [..., C, N]
+    viewmats: Tensor,  # [..., C, 4, 4]
+    Ks: Tensor,  # [..., C, 3, 3]
+    active_tiles: Tensor,  # [AT]
+    tile_offsets: Tensor,  # [AT + 1]
+    flatten_ids: Tensor,  # [n_isects]
+    tile_pixel_mask: Tensor,  # [AT, 4]
+    tile_pixel_cumsum: Tensor,  # [AT]
+    pixel_map: Tensor,  # [P]
+    image_width: int,
+    image_height: int,
+    tile_size: int,
+    tile_width: int,
+    tile_height: int,
+    num_depth_samples: int,
+    camera_model: str = "pinhole",
+    radial_coeffs: Optional[Tensor] = None,  # [..., C, 6] pinhole or [..., C, 4] fisheye
+    tangential_coeffs: Optional[Tensor] = None,  # [..., C, 2]
+    thin_prism_coeffs: Optional[Tensor] = None,  # [..., C, 4]
+    ftheta_coeffs=None,
+    rolling_shutter: int = RollingShutterType.GLOBAL,
+    viewmats_rs: Optional[Tensor] = None,  # [..., C, 4, 4]
+) -> Tuple[Tensor, Tensor]:
+    """``rasterize_top_contributing_gaussian_ids_eval3d`` at the pixels of a sparse layout: (ids, weights) [P, K] in
+    the original pixel order."""
+    what = "rasterize_top_contributing_gaussian_ids_eval3d_sparse"
+    K = _depth_samples(num_depth_samples)
+    rows = _Eval3dRows(what, means, quats, scales, opacities, viewmats, Ks, image_width, image_height, camera_model,
+                       radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta_coeffs, rolling_shutter, viewmats_rs)
+    checked = _contrib_sparse(rows, active_tiles, tile_offsets, flatten_ids, tile_pixel_mask, tile_pixel_cumsum,
+                              pixel_map, image_width, image_height, tile_size, tile_width, tile_height)
+    return _contrib_top(what, checked, K)

@@ -632,6 +632,56 @@ extern "C"
         void *stream
     );
 
+    /* ---- 3DGUT pair query and per-pixel contributor queries (rasterize_to_indices_in_range_eval3d,
+     * rasterize_num_contributing_gaussians_eval3d, rasterize_contributing_gaussian_ids_eval3d,
+     * rasterize_top_contributing_gaussian_ids_eval3d and their _sparse forms; the reference has no 3DGUT queries).  Each
+     * pixel walks its tile's list with the decisions of gsb200_eval3d_fwd (its ray through the camera model and shutter,
+     * the maximum response along it, the stop rule), so count's alphas are its render_alphas.  The geometry and camera
+     * arguments are gsb200_eval3d_fwd's (images B*C, flatten ids over [B*C*N], ids = flatten id % N); the rest are those of
+     * gsb200_raster_indices / gsb200_contrib_*, with their outputs, sparse layouts and return codes.  A pixel that does
+     * not composite (outside the W x H image, or a ray that cannot be unprojected) has no pairs; with an output row it
+     * gets count 0 and ids -1 / weights 0.  Checks, all before any launch: the sizes of gsb200_eval3d_fwd, the camera,
+     * the sparse layout (active_tiles non-null), then the query's own.
+     * gsb200_eval3d_contrib_max_samples: the num_samples bound of gsb200_eval3d_contrib_top for every camera and shutter,
+     * or GSB200_E_CUDA without a device. */
+    int gsb200_eval3d_indices(
+        int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
+        const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+        const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+        const float *transmittances, uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width,
+        uint32_t tile_height, const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t range_start,
+        int64_t range_end, int emit, void *workspace, size_t workspace_bytes, int64_t *total, int64_t *gaussian_ids,
+        int64_t *pixel_ids, int64_t *image_ids, void *stream
+    );
+    int gsb200_eval3d_contrib_max_samples(void);
+    int gsb200_eval3d_contrib_count(
+        int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
+        const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+        const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int32_t *counts,
+        float *alphas, void *stream
+    );
+    int gsb200_eval3d_contrib_ids(
+        int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
+        const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+        const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int max_samples,
+        int32_t *ids, float *weights, void *stream
+    );
+    int gsb200_eval3d_contrib_top(
+        int64_t B, int64_t C, int64_t N, const float *means, const float *quats, const float *scales, const float *opacities,
+        const float *viewmats, const float *Ks, int camera_model, const float *radial_coeffs, const float *tangential_coeffs,
+        const float *thin_prism_coeffs, const gsb200_ftheta_params *ftheta, const float *viewmats_rs, int rolling_shutter,
+        uint32_t image_width, uint32_t image_height, uint32_t tile_size, uint32_t tile_width, uint32_t tile_height,
+        const int32_t *offsets, const int32_t *flatten_ids, int64_t n_isects, int64_t n_active, const int32_t *active_tiles,
+        const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map, int num_samples,
+        int32_t *ids, float *weights, void *stream
+    );
+
     /* ---- MCMC strategy ops ("next" row): relocation (ext.cpp `relocation`, gsplat/relocation.py:64,
      * csrc/RelocationCUDA.cu:36-80) and in-place position perturbation (csrc/MCMCPerturbCUDA.cu:28-60,
      * gsplat/strategy/ops.py).  ratios int32 [N] already clamped to [1, n_max]; binoms [n_max, n_max]. */
