@@ -1,29 +1,29 @@
 """ctypes binding of libgsplat_b200.so (the C ABI declared in include/gsplat_b200.h).
 
-The library is the only compute path: if it cannot be loaded this module raises -- there is no
-PyTorch / CPU fallback (tests would otherwise pass on a silent eager path).
+Every entry point's restype and argtypes are read from the header when this module is imported, so the prototypes
+the compiler checks against the definitions are the only copy of the signatures.  The library is the only compute
+path: if it cannot be loaded this module raises -- there is no PyTorch / CPU fallback (tests would otherwise pass on
+a silent eager path).
 """
 from __future__ import annotations
 
 import ctypes
 import os
+import re
 from typing import Optional
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgsplat_b200.so")
+HEADER_PATH = os.path.normpath(os.path.join(_HERE, os.pardir, "include", "gsplat_b200.h"))
 
 _lib = None
 
-c_i64, c_u32, c_int, c_f32, c_vp, c_sz = (
-    ctypes.c_int64,
-    ctypes.c_uint32,
-    ctypes.c_int,
-    ctypes.c_float,
-    ctypes.c_void_p,
-    ctypes.c_size_t,
-)
+
+class GsplatB200Error(RuntimeError):
+    pass
+
 
 class FThetaParams(ctypes.Structure):
     """gsb200_ftheta_params of include/gsplat_b200.h: the FTheta camera parameters of the 3DGUT entry points."""
@@ -37,246 +37,49 @@ class FThetaParams(ctypes.Structure):
     ]
 
 
-# name -> (restype, argtypes) ; mirrors include/gsplat_b200.h one to one
-_SIGNATURES = {
-    "gsb200_version": (ctypes.c_char_p, []),
-    "gsb200_source_hash": (ctypes.c_char_p, []),
-    "gsb200_error_string": (ctypes.c_char_p, [c_int]),
-    "gsb200_last_cuda_error": (ctypes.c_char_p, []),
-    "gsb200_bits_for_count": (c_u32, [c_i64]),
-    "gsb200_raster_supports_channels": (c_int, [c_int]),
-    "gsb200_quat_scale_to_covar_preci_fwd": (c_int, [c_i64, c_vp, c_vp, c_int, c_vp, c_vp, c_vp]),
-    "gsb200_quat_scale_to_covar_preci_bwd": (c_int, [c_i64, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_projection_fwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32, c_f32, c_int,
-         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_projection_bwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_int, c_vp, c_vp, c_vp,
-         c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_sh_fwd": (c_int, [c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_sh_bwd": (c_int, [c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_project_sh_fwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32, c_f32,
-         c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_project_sh_bwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_sh_rows_fwd": (c_int, [c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_sh_rows_bwd": (
-        c_int, [c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_projection_packed_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64]),
-    "gsb200_projection_packed_count": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32, c_f32, c_int, c_int,
-         c_vp, c_sz, c_vp, c_vp],
-    ),
-    "gsb200_projection_packed_emit": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32, c_f32, c_int,
-         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_projection_packed_bwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_int, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_isect_scan_workspace_bytes": (c_sz, [c_i64]),
-    "gsb200_isect_count": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp, c_sz, c_vp]),
-    "gsb200_isect_emit": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp]),
-    "gsb200_l1_loss_workspace_bytes": (c_sz, []),
-    "gsb200_l1_loss_fwd": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_l1_loss_bwd": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_ssim_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_i64]),
-    "gsb200_ssim_fwd": (c_int, [c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_ssim_bwd": (c_int, [c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_adam": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_f32, c_f32, c_f32, c_f32, c_vp]),
-    "gsb200_nvls_allreduce_f32": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp]),
-    "gsb200_p2p_allreduce_f32": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp]),
-    "gsb200_rows_allreduce_f32": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp, c_vp]),
-    "gsb200_isect_count_totals": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_vp]),
-    "gsb200_project_sh_fwd_rows": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32, c_f32, c_u32,
-         c_u32, c_u32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_raster_fwd_rows": (
-        c_int,
-        [c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_publish_totals": (c_int, [c_vp, c_vp, c_i64, c_vp]),
-    "gsb200_isect_sorted_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_i64, c_int, c_u32, c_u32]),
-    "gsb200_isect_sorted": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp,
-         c_vp, c_vp, c_vp, c_sz, c_vp],
-    ),
-    "gsb200_isect_ids_from_tilekeys": (c_int, [c_i64, c_int, c_vp, c_vp, c_vp, c_i64, c_u32, c_u32, c_vp, c_vp]),
-    "gsb200_isect_offsets": (c_int, [c_i64, c_vp, c_i64, c_u32, c_u32, c_vp, c_vp]),
-    "gsb200_relocation": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_f32, c_vp, c_vp, c_vp]),
-    "gsb200_mcmc_perturb_positions": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_f32, c_f32, c_f32, c_vp]),
-    "gsb200_raster_records_bytes": (c_sz, [c_i64, c_int, c_i64]),
-    "gsb200_raster_pack": (c_int, [c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp]),
-    "gsb200_raster_fwd": (
-        c_int,
-        [c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64,
-         c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_raster_bwd": (
-        c_int,
-        [c_i64, c_i64, c_int, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_int, c_vp, c_vp],
-    ),
-    "gsb200_sparse_layout_workspace_bytes": (c_sz, [c_i64, c_i64, c_u32, c_u32]),
-    "gsb200_sparse_layout_sort": (c_int, [c_i64, c_vp, c_vp, c_i64, c_u32, c_u32, c_u32, c_vp, c_sz, c_vp, c_vp]),
-    "gsb200_sparse_layout_finish": (c_int, [c_i64, c_i64, c_u32, c_u32, c_i64, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsb200_isect_active_offsets": (c_int, [c_i64, c_vp, c_i64, c_u32, c_u32, c_vp, c_i64, c_vp, c_vp]),
-    "gsb200_raster_sparse_fwd": (
-        c_int,
-        [c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp,
-         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_raster_sparse_bwd": (
-        c_int,
-        [c_i64, c_int, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp],
-    ),
-    "gsb200_surfel_projection_fwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_f32, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_surfel_projection_bwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_surfel_raster_fwd": (
-        c_int,
-        [c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64,
-         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_surfel_raster_bwd": (
-        c_int,
-        [c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64,
-         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_surfel_raster_sparse_fwd": (
-        c_int,
-        [c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp,
-         c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_surfel_raster_sparse_bwd": (
-        c_int,
-        [c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp,
-         c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_vp],
-    ),
-    "gsb200_indices_workspace_bytes": (c_sz, [c_i64]),
-    "gsb200_raster_indices": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp,
-         c_sz, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_surfel_indices": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp,
-         c_sz, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_contrib_max_samples": (c_int, []),
-    "gsb200_contrib_count": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_vp, c_vp],
-    ),
-    "gsb200_contrib_ids": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_int, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_contrib_top": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_int, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_surfel_contrib_max_samples": (c_int, []),
-    "gsb200_surfel_contrib_count": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_vp, c_vp],
-    ),
-    "gsb200_surfel_contrib_ids": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_int, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_surfel_contrib_top": (
-        c_int,
-        [c_i64, c_i64, c_vp, c_vp, c_vp, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp,
-         c_int, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_ut_projection_fwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_u32,
-         c_u32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_eval3d_fwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_eval3d_bwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_vp],
-    ),
-    "gsb200_eval3d_sparse_fwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-         c_vp],
-    ),
-    "gsb200_eval3d_sparse_bwd": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_int, c_u32, c_u32, c_u32, c_u32, c_u32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_eval3d_indices": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_u32,
-         c_u32, c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_eval3d_contrib_max_samples": (c_int, []),
-    "gsb200_eval3d_contrib_count": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_u32, c_u32,
-         c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_eval3d_contrib_ids": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_u32, c_u32,
-         c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp],
-    ),
-    "gsb200_eval3d_contrib_top": (
-        c_int,
-        [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_u32, c_u32,
-         c_u32, c_u32, c_u32, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp],
-    ),
+# The C types the header passes by value.  Any pointer is passed as c_void_p; any other type is refused, so that a
+# new one (a double, a uint16_t) cannot be bound as an integer of the wrong width.
+_BY_VALUE = {
+    "int64_t": ctypes.c_int64,
+    "uint32_t": ctypes.c_uint32,
+    "int": ctypes.c_int,
+    "float": ctypes.c_float,
+    "size_t": ctypes.c_size_t,
 }
+_PROTOTYPE = re.compile(r"^\s*((?:const\s+)?\w+\s*\*?)\s*(gsb200_\w+)\s*\(([^)]*)\)\s*;", re.M)
 
+
+def _parse_header(text: str) -> dict:
+    """{name: (restype, [argtypes])} of every gsb200_* prototype in the header text."""
+
+    def ctype(decl: str, fn: str, what: str):
+        if "*" in decl:
+            return ctypes.c_void_p
+        base = next((w for w in decl.split() if w != "const"), "")
+        if base not in _BY_VALUE:
+            raise GsplatB200Error(f"gsplat_b200.h: {fn}: {what} `{decl}` has a C type the binding does not map")
+        return _BY_VALUE[base]
+
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    out = {}
+    for m in _PROTOTYPE.finditer(text):
+        ret, name, params = m.group(1).strip(), m.group(2), m.group(3).strip()
+        plist = [] if params in ("", "void") else [p.strip() for p in params.split(",")]
+        res = ctypes.c_char_p if re.fullmatch(r"const\s+char\s*\*", ret) else ctype(ret, name, "return type")
+        out[name] = (res, [ctype(p, name, "parameter") for p in plist])
+    return out
+
+
+def _read_header() -> str:
+    try:
+        with open(HEADER_PATH) as f:
+            return f.read()
+    except OSError as e:
+        raise GsplatB200Error(f"{HEADER_PATH} cannot be read ({e.strerror}): the binding takes its signatures from it") from e
+
+
+_SIGNATURES = _parse_header(_read_header())
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
-
-
-class GsplatB200Error(RuntimeError):
-    pass
 
 
 def lib():

@@ -1,6 +1,6 @@
-"""CPU-side checks of the drop-in boundary: the C-ABI library loads, exports every symbol that
-include/gsplat_b200.h declares, the ctypes signatures in gsplat_b200/_cabi.py agree with the header
-parameter by parameter, and the product path refuses to run without a GPU (no CPU fallback)."""
+"""CPU-side checks of the drop-in boundary: the C-ABI library loads, the binding in gsplat_b200/_cabi.py reads every
+prototype of include/gsplat_b200.h with the right ctypes and the library exports each one, and the product path
+refuses to run without a GPU (no CPU fallback)."""
 import ctypes
 import os
 import re
@@ -9,52 +9,92 @@ import pytest
 import torch
 
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
+HEADER = os.path.join(ROOT, "include", "gsplat_b200.h")
 
-
-def _header_functions():
-    src = open(os.path.join(ROOT, "include", "gsplat_b200.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    out = {}
-    for m in re.finditer(r"\n\s*((?:const\s+)?[A-Za-z_0-9]+\s*\*?)\s*(gsb200_[a-z_0-9]+)\s*\((.*?)\)\s*;", src, flags=re.S):
-        ret, name, params = m.group(1).strip(), m.group(2), m.group(3).strip()
-        plist = [] if params in ("", "void") else [p.strip() for p in params.split(",")]
-        out[name] = (ret, plist)
-    return out
-
-
-def _ctype_of(decl: str):
-    from gsplat_b200 import _cabi as c
-
-    if "*" in decl:
-        return ctypes.c_char_p if decl.startswith("const char") and "(" in decl else c.c_vp
-    base = decl.replace("const", "").split()[0]
-    return {"int64_t": c.c_i64, "uint32_t": c.c_u32, "int": c.c_int, "float": c.c_f32, "size_t": c.c_sz}[base]
+I64, U32, INT, F32, SZ, VP = (
+    ctypes.c_int64, ctypes.c_uint32, ctypes.c_int, ctypes.c_float, ctypes.c_size_t, ctypes.c_void_p
+)
 
 
 def test_library_exports_every_declared_symbol():
     from gsplat_b200 import _cabi
 
-    funcs = _header_functions()
-    assert len(funcs) >= 20
-    assert set(funcs) == set(_cabi.EXPORTED_SYMBOLS), set(funcs) ^ set(_cabi.EXPORTED_SYMBOLS)
+    assert len(_cabi.EXPORTED_SYMBOLS) >= 80
     L = _cabi.lib()
-    for name in funcs:
+    for name in _cabi.EXPORTED_SYMBOLS:
         assert hasattr(L, name), f"{name} not exported by libgsplat_b200.so"
 
 
-def test_ctypes_signatures_match_header():
+def test_every_prototype_is_bound():
+    """A prototype the parser misses would still be callable through ctypes, with int conversions that truncate
+    pointers; so every gsb200_* name followed by '(' in the header, found without the parser's pattern, is bound."""
     from gsplat_b200 import _cabi
 
-    funcs = _header_functions()
-    for name, (ret, params) in funcs.items():
-        res, args = _cabi._SIGNATURES[name]
-        assert len(args) == len(params), f"{name}: header has {len(params)} params, binding has {len(args)}"
-        for i, (p, a) in enumerate(zip(params, args)):
-            assert _ctype_of(p) is a, f"{name} arg {i} ({p}): binding uses {a}"
-        if ret.startswith("const char"):
-            assert res is ctypes.c_char_p
-        else:
-            assert res is _ctype_of(ret + " x")
+    assert os.path.samefile(_cabi.HEADER_PATH, HEADER)
+    src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
+    declared = set(re.findall(r"\b(gsb200_\w+)\s*\(", src))
+    assert declared == set(_cabi.EXPORTED_SYMBOLS), declared ^ set(_cabi.EXPORTED_SYMBOLS)
+
+
+def test_ctypes_of_every_c_spelling():
+    """Known answers covering every return and parameter type the header spells."""
+    from gsplat_b200 import _cabi
+
+    expected = {
+        "gsb200_version": (ctypes.c_char_p, []),
+        "gsb200_error_string": (ctypes.c_char_p, [INT]),
+        "gsb200_bits_for_count": (U32, [I64]),
+        "gsb200_raster_records_bytes": (SZ, [I64, INT, I64]),
+        "gsb200_publish_totals": (INT, [VP, VP, I64, VP]),
+        "gsb200_quat_scale_to_covar_preci_fwd": (INT, [I64, VP, VP, INT, VP, VP, VP]),
+        "gsb200_projection_fwd": (INT, [I64] * 3 + [VP] * 7 + [U32] * 2 + [F32] * 4 + [INT] + [VP] * 6),
+        "gsb200_isect_count_totals": (INT, [I64] * 2 + [VP] * 6 + [U32] * 3 + [VP] * 3),
+        "gsb200_sparse_layout_finish": (INT, [I64, I64, U32, U32, I64, VP, SZ] + [VP] * 6),
+        "gsb200_raster_sparse_fwd": (INT, [INT] + [VP] * 6 + [U32] * 5 + [I64] + [VP] * 3 + [I64] + [VP] * 8),
+        "gsb200_project_sh_bwd": (
+            INT, [I64] * 3 + [INT] + [VP] * 6 + [U32] * 2 + [F32] + [VP] * 5 + [I64, VP] * 3 + [I64] + [VP] * 7,
+        ),
+        "gsb200_eval3d_fwd": (
+            INT, [I64] * 3 + [INT] + [VP] * 9 + [INT] + [VP] * 5 + [INT] + [U32] * 5 + [VP] * 2 + [I64] + [VP] * 4,
+        ),
+        "gsb200_nvls_allreduce_f32": (INT, [VP, I64, INT, INT, VP, I64, INT, VP]),
+    }
+    for name, sig in expected.items():
+        assert _cabi._SIGNATURES[name] == sig, name
+
+
+def test_functions_are_bound_as_parsed():
+    from gsplat_b200 import _cabi
+
+    L = _cabi.lib()
+    for name, (res, args) in _cabi._SIGNATURES.items():
+        fn = getattr(L, name)
+        assert fn.restype is res and list(fn.argtypes) == args, name
+
+
+def test_parse_header_refuses_unmapped_types():
+    from gsplat_b200._cabi import GsplatB200Error, _parse_header
+
+    for ctype in ("double", "uint16_t"):
+        with pytest.raises(GsplatB200Error, match=rf"gsb200_f: parameter `{ctype} scale`"):
+            _parse_header(f"int gsb200_f(int64_t n, {ctype} scale, void *stream);")
+    with pytest.raises(GsplatB200Error, match="gsb200_g: return type `double`"):
+        _parse_header("double gsb200_g(void);")
+
+
+def test_parse_header_prototype_forms():
+    from gsplat_b200._cabi import _parse_header
+
+    text = """
+    /* int gsb200_commented_out(int x); */
+    const char *gsb200_a(void);
+    size_t
+    gsb200_b(
+        int64_t n, const float *x,  /* comment */
+        void *const *pads, float eps
+    );
+    """
+    assert _parse_header(text) == {"gsb200_a": (ctypes.c_char_p, []), "gsb200_b": (SZ, [I64, VP, VP, F32])}
 
 
 def test_host_only_entry_points():
