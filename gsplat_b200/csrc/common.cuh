@@ -227,5 +227,23 @@ __device__ __forceinline__ int butterfly_slot(unsigned lane)
     }
     return (mr >= 1 && primary) ? slot : -1;
 }
+
+// The compositing backwards' gradient emit (surfel.cu, ut.cu): butterfly-reduces gv[OFF, OFF + 32) across the warp, adds
+// each owned nonzero slot of record r with dst.add(slot, r, sum, CDIM); recurses over the remaining 32-value chunks.
+template<int OFF, int NV, class Rec, class Dst>
+__device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, const Rec &r, const Dst &dst, int CDIM)
+{
+    constexpr int M = (NV - OFF) < 32 ? (NV - OFF) : 32;
+    float v[M];
+#pragma unroll
+    for(int k = 0; k < M; ++k)
+        v[k] = gv[OFF + k];
+    Butterfly<M, 16>::run(v, lane);
+    const int s = butterfly_slot<M>(lane);
+    if(s >= 0 && v[0] != 0.f)
+        dst.add(OFF + s, r, v[0], CDIM);
+    if constexpr(OFF + 32 < NV)
+        reduce_emit<OFF + 32, NV>(gv, lane, r, dst, CDIM);
+}
 #endif // __CUDACC__
 } // namespace gsb

@@ -31,8 +31,8 @@ PixelCounts carve_pixel_counts(void *workspace, int64_t P);
 // exclusive scan of counts [P + 1] into starts, then total[0] = starts[P] (device to device)
 int scan_pixel_counts(const PixelCounts &pc, int64_t P, int64_t *total, cudaStream_t st);
 
-// What a pair-query walk (raster_indices_kernel of raster.cu, surfel_indices_kernel of surfel.cu, eval3d_indices_kernel
-// of ut.cu) does with a pixel's pairs is its Sink's (every walk runs kIndexBatch threads per CTA, one pixel per thread):
+// What a pair-query walk (raster_indices_kernel of raster.cu, pair_walk_kernel below with the models of surfel.cu and
+// ut.cu) does with a pixel's pairs is its Sink's (every walk runs kIndexBatch threads per CTA, one pixel per thread):
 //   begin(live, pix, pix_in, image_id)  once per thread (pix: the output row, pix_in: the row-major pixel in its image)
 //   pair(k, g, w)                        the pixel's k-th pair: flatten id g, weight w = alpha * T before the pair
 //   end(pix, count, T)                   once per live pixel, after the walk
@@ -173,6 +173,82 @@ struct TopSink
         }
     }
 };
+
+// The pair-query walk of the 2DGS and 3DGUT queries: the (pixel, gaussian) pairs a family's compositing forward
+// composites, walking only the batches [b0, b1) of each tile's list from the pixel's given transmittance (null: T = 1).
+// One CTA per 16x16 tile of the pixel policy (DensePixels: every tile of the [I, th, tw] grid; SparsePixels: every
+// active tile), one pixel per thread; a pixel is live when it has an output row.  The Model (SurfelModel of surfel.cu,
+// Eval3dModel of ut.cu) is the forward's:
+//   I, W, H, tw, th                           the tile grid
+//   kMinBlocks                                the forward's minimum of resident CTAs (launch bounds; 0: none)
+//   Rec, stage(rec, g)                        the staged record of flatten id g (one per thread of a batch)
+//   Pixel, setup(img, i, j, live, px) -> bool  the pixel's state; whether it composites.  Called by every thread.
+//   hit(rec, px) -> {ok, alpha}               the forward's evaluation of one record at the pixel
+// A live pixel that does not composite still gets begin and end (count 0, T as given).  Every thread stages records and
+// meets every barrier.  The stop rule is the forward's, so the alphas are its render_alphas bit for bit.
+template<class Model, class Sink, class Pix = DensePixels>
+__global__ void __launch_bounds__(kIndexBatch, Model::kMinBlocks) pair_walk_kernel(
+    Model model, const float *__restrict__ transmittances, const int32_t *__restrict__ offsets,
+    const int32_t *__restrict__ flatten_ids, int64_t n_isects, int32_t b0, int32_t b1, Sink sink, const Pix pixmap = Pix{}
+)
+{
+    __shared__ typename Model::Rec rec[kIndexBatch];
+    const uint32_t tile  = pixmap.tile(blockIdx.x); // image * th * tw + tile row * tw + tile col
+    const uint32_t img   = tile / (model.tw * model.th);
+    const uint32_t tin   = tile - img * model.tw * model.th;
+    const uint32_t tr    = threadIdx.x;
+    const uint32_t i     = (tin / model.tw) * kTile + tr / kTile;
+    const uint32_t j     = (tin % model.tw) * kTile + tr % kTile;
+    const int64_t pix_in = (int64_t)i * model.W + j;
+    bool live;
+    int64_t pix, start, end;
+    if constexpr(Pix::kSparse)
+    {
+        pix   = pixmap.slot(blockIdx.x, (int)tr, live);
+        start = offsets[blockIdx.x];
+        end   = offsets[blockIdx.x + 1];
+    }
+    else
+    {
+        live  = i < model.H && j < model.W;
+        pix   = (int64_t)img * model.H * model.W + pix_in;
+        start = offsets[tile];
+        end   = (tile + 1 == model.I * model.tw * model.th) ? n_isects : offsets[tile + 1];
+    }
+    const int64_t b_end = min((int64_t)b1, (end - start + kIndexBatch - 1) / kIndexBatch);
+    typename Model::Pixel px;
+    bool done   = !model.setup(img, i, j, live, px);
+    float T     = (live && transmittances != nullptr) ? transmittances[pix] : 1.f;
+    int32_t cnt = 0;
+    sink.begin(live, pix, pix_in, img);
+    for(int64_t b = b0; b < b_end; ++b)
+    {
+        if(__syncthreads_count(done) == kIndexBatch)
+            break;
+        const int64_t batch = start + b * kIndexBatch;
+        if(batch + tr < end)
+            model.stage(rec[tr], flatten_ids[batch + tr]);
+        __syncthreads();
+        const int n_b = (int)min((int64_t)kIndexBatch, end - batch);
+        for(int t = 0; t < n_b && !done; ++t)
+        {
+            const auto h = model.hit(rec[t], px);
+            if(!h.ok)
+                continue;
+            const float next_T = T * (1.f - h.alpha);
+            if(next_T <= kTransmittanceThreshold)
+            { // exclusive: this gaussian does not contribute
+                done = true;
+                break;
+            }
+            sink.pair(cnt, rec[t].id, h.alpha * T);
+            ++cnt;
+            T = next_T;
+        }
+    }
+    if(live)
+        sink.end(pix, cnt, T);
+}
 
 // Argument checks and the pass sequence shared by both index queries.  `inputs_ok`: the gaussian rows, the
 // transmittances, offsets and flatten_ids are given.  launch(n_tiles, b0, b1, sink) launches the pass's kernel with its

@@ -472,122 +472,52 @@ __global__ void __launch_bounds__(kSurfThreads) surfel_raster_fwd_kernel(
     median_ids[pix]     = median_idx;
 }
 
-// The pair-query walk of rasterize_to_indices_in_range_2dgs and the 2DGS contributor queries: the (pixel, surfel) pairs
-// surfel_raster_fwd_kernel composites, walking only the batches [b0, b1) of each tile's list from the pixel's given
-// transmittance (null: T = 1).  One CTA per tile of the pixel policy (DensePixels: every tile of the [I, th, tw] grid;
-// SparsePixels: every active tile, its live pixels only); the pixel mapping, staging, surf_eval and the stop rule are
-// the forward's.  What the walk does with a pixel's pairs is the Sink's (indices.cuh).
-template<class Sink, class Pix = DensePixels>
-__global__ void __launch_bounds__(kSurfThreads) surfel_indices_kernel(
-    uint32_t I, const float *__restrict__ means2d, const float *__restrict__ rt, const float *__restrict__ opacities,
-    const float *__restrict__ transmittances, uint32_t W, uint32_t H, uint32_t tw, uint32_t th,
-    const int32_t *__restrict__ offsets, const int32_t *__restrict__ flatten_ids, int64_t n_isects, int32_t b0, int32_t b1,
-    Sink sink, const Pix pixmap = Pix{}
-)
+// The 2DGS model of pair_walk_kernel (indices.cuh), the pair query and contributor queries of
+// rasterize_to_indices_in_range_2dgs and rasterize_*_contributing_gaussian*_2dgs: surfel_raster_fwd_kernel's staging
+// and surf_eval at the pixel centre.  Every live pixel composites, margin pixels of a sparse tile included.
+struct SurfelModel
 {
-    static_assert(kSurfThreads == kIndexBatch, "one record of a batch per thread");
-    __shared__ SurfRec rec[kSurfThreads];
-    const uint32_t tile  = pixmap.tile(blockIdx.x); // image * th * tw + tile row * tw + tile col
-    const uint32_t img   = tile / (tw * th);
-    const uint32_t tin   = tile - img * tw * th;
-    const uint32_t tr    = threadIdx.x;
-    const uint32_t i     = (tin / tw) * kTile + tr / kTile;
-    const uint32_t j     = (tin % tw) * kTile + tr % kTile;
-    const int64_t pix_in = (int64_t)i * W + j;
-    bool inside;
-    int64_t pix, start, end;
-    if constexpr(Pix::kSparse)
+    uint32_t I, W, H, tw, th;
+    const float *means2d, *rt, *opacities;
+    static constexpr int kMinBlocks = 0; // the forward's launch bounds: no minimum
+    using Rec   = SurfRec;
+    using Pixel = float2; // the pixel centre
+    __device__ __forceinline__ void stage(SurfRec &r, int32_t g) const { gsb::stage(r, g, means2d, opacities, rt); }
+    __device__ __forceinline__ bool setup(uint32_t, uint32_t i, uint32_t j, bool live, float2 &p) const
     {
-        pix   = pixmap.slot(blockIdx.x, (int)tr, inside);
-        start = offsets[blockIdx.x];
-        end   = offsets[blockIdx.x + 1];
+        p = make_float2((float)j + 0.5f, (float)i + 0.5f);
+        return live;
     }
-    else
-    {
-        inside = i < H && j < W;
-        pix    = (int64_t)img * H * W + pix_in;
-        start  = offsets[tile];
-        end    = (tile + 1 == I * tw * th) ? n_isects : offsets[tile + 1];
-    }
-    const int64_t b_end = min((int64_t)b1, (end - start + kSurfThreads - 1) / kSurfThreads);
-    const float px = (float)j + 0.5f, py = (float)i + 0.5f;
-
-    float T     = (inside && transmittances != nullptr) ? transmittances[pix] : 1.f;
-    bool done   = !inside;
-    int32_t cnt = 0;
-    sink.begin(inside, pix, pix_in, img);
-    for(int64_t b = b0; b < b_end; ++b)
-    {
-        if(__syncthreads_count(done) == kSurfThreads)
-            break;
-        const int64_t batch = start + b * kSurfThreads;
-        if(batch + tr < end)
-            stage(rec[tr], flatten_ids[batch + tr], means2d, opacities, rt);
-        __syncthreads();
-        const int n_b = (int)min((int64_t)kSurfThreads, end - batch);
-        for(int t = 0; t < n_b && !done; ++t)
-        {
-            const SurfHit h = surf_eval(rec[t], px, py);
-            if(!h.ok)
-                continue;
-            const float next_T = T * (1.f - h.alpha);
-            if(next_T <= kTransmittanceThreshold)
-            { // exclusive: this surfel does not contribute
-                done = true;
-                break;
-            }
-            sink.pair(cnt, rec[t].id, h.alpha * T);
-            ++cnt;
-            T = next_T;
-        }
-    }
-    if(inside)
-        sink.end(pix, cnt, T);
-}
+    __device__ __forceinline__ SurfHit hit(const SurfRec &r, float2 p) const { return surf_eval(r, p.x, p.y); }
+};
 
 struct SurfGradDst
 {
     float *means2d, *rt, *colors, *opacities, *normals, *densify, *abs;
-};
 
-// Butterfly-reduces gv[OFF, OFF + 32) across the warp and adds each owned slot to its gradient row; recurses over the
-// remaining 32-value chunks (a lane owns at most one slot of a chunk).
-template<int OFF, int NV>
-__device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, const SurfRec &r, const SurfGradDst &dst, int CDIM)
-{
-    constexpr int M = (NV - OFF) < 32 ? (NV - OFF) : 32;
-    float v[M];
-#pragma unroll
-    for(int k = 0; k < M; ++k)
-        v[k] = gv[OFF + k];
-    Butterfly<M, 16>::run(v, lane);
-    const int s = butterfly_slot<M>(lane);
-    if(s >= 0 && v[0] != 0.f)
+    // reduce_emit's routing (common.cuh): slot of the gradient vector of surfel_raster_bwd_kernel to its row
+    __device__ __forceinline__ void add(int slot, const SurfRec &r, float val, int CDIM) const
     {
-        const int slot  = OFF + s;
         const int64_t g = r.id;
-        const float val = v[0];
         if(slot < CDIM)
-            atomicAdd(dst.colors + g * CDIM + slot, val);
+            atomicAdd(colors + g * CDIM + slot, val);
         else if(slot < CDIM + 3)
-            atomicAdd(dst.normals + g * 3 + (slot - CDIM), val);
+            atomicAdd(normals + g * 3 + (slot - CDIM), val);
         else if(slot < CDIM + 12)
         {
             const int e = slot - CDIM - 3;
-            atomicAdd(dst.rt + g * 9 + e, val);
+            atomicAdd(rt + g * 9 + e, val);
             if(e == 2 || e == 5)
-                atomicAdd(dst.densify + g * 2 + (e == 5), val * r.m[8]);
+                atomicAdd(densify + g * 2 + (e == 5), val * r.m[8]);
         }
         else if(slot < CDIM + 14)
-            atomicAdd(dst.means2d + g * 2 + (slot - CDIM - 12), val);
+            atomicAdd(means2d + g * 2 + (slot - CDIM - 12), val);
         else if(slot == CDIM + 14)
-            atomicAdd(dst.opacities + g, val);
-        else if(dst.abs)
-            atomicAdd(dst.abs + g * 2 + (slot - CDIM - 15), val);
+            atomicAdd(opacities + g, val);
+        else if(abs)
+            atomicAdd(abs + g * 2 + (slot - CDIM - 15), val);
     }
-    if constexpr(OFF + 32 < NV)
-        reduce_emit<OFF + 32, NV>(gv, lane, r, dst, CDIM);
-}
+};
 
 // Back to front over each tile's list.  Per gaussian, the warp's per-pixel gradients (colours, normals, ray transform,
 // screen mean, opacity, |screen mean|) are butterfly-reduced and added with one atomic per value; v_densify is the
@@ -793,6 +723,26 @@ int surfel_raster_limits(int64_t I, int64_t N, uint32_t W, uint32_t H, uint32_t 
         return GSB200_E_UNSUPPORTED;
     return GSB200_OK;
 }
+
+// The compositing launches of the dense and sparse entries, after each entry's own checks: n_ctas CTAs over the tiles
+// of the pixel policy pm, with the kernel's arguments before pm.
+template<class Pix, class... Args>
+int surfel_raster_fwd(int D, unsigned n_ctas, const Pix &pm, cudaStream_t st, const Args &...args)
+{
+    return with_channels(D, [&](auto C) {
+        surfel_raster_fwd_kernel<C, Pix><<<n_ctas, kSurfThreads, 0, st>>>(args..., pm);
+        return check_launch();
+    });
+}
+
+template<class Pix, class... Args>
+int surfel_raster_bwd(int D, unsigned n_ctas, const Pix &pm, cudaStream_t st, const Args &...args)
+{
+    return with_channels(D, [&](auto C) {
+        surfel_raster_bwd_kernel<C, Pix><<<n_ctas, kSurfThreads, 0, st>>>(args..., pm);
+        return check_launch();
+    });
+}
 } // namespace
 } // namespace gsb
 
@@ -861,14 +811,12 @@ extern "C" int gsb200_surfel_raster_fwd(
         return GSB200_OK;
     if(int rc = gsb::surfel_raster_limits(I, N, image_width, image_height, tile_width, tile_height))
         return rc;
-    return gsb::with_channels(D, [&](auto C) {
-        gsb::surfel_raster_fwd_kernel<C><<<(uint32_t)I * tile_width * tile_height, gsb::kSurfThreads, 0, (cudaStream_t)stream>>>(
-            (uint32_t)I, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height,
-            tile_width, tile_height, offsets, flatten_ids, n_isects, render_colors, render_alphas, render_normals,
-            render_distort, render_median, last_ids, median_ids
-        );
-        return gsb::check_launch();
-    });
+    return gsb::surfel_raster_fwd(
+        D, (uint32_t)I * tile_width * tile_height, gsb::DensePixels{}, (cudaStream_t)stream, (uint32_t)I, means2d,
+        ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height, tile_width, tile_height,
+        offsets, flatten_ids, n_isects, render_colors, render_alphas, render_normals, render_distort, render_median,
+        last_ids, median_ids
+    );
 }
 
 extern "C" int gsb200_surfel_raster_bwd(
@@ -895,14 +843,12 @@ extern "C" int gsb200_surfel_raster_bwd(
     if(int rc = gsb::surfel_raster_limits(I, N, image_width, image_height, tile_width, tile_height))
         return rc;
     const gsb::SurfGradDst dst{v_means2d, v_ray_transforms, v_colors, v_opacities, v_normals, v_densify, v_means2d_abs};
-    return gsb::with_channels(D, [&](auto C) {
-        gsb::surfel_raster_bwd_kernel<C><<<(uint32_t)I * tile_width * tile_height, gsb::kSurfThreads, 0, (cudaStream_t)stream>>>(
-            (uint32_t)I, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height,
-            tile_width, tile_height, offsets, flatten_ids, n_isects, render_colors, render_alphas, last_ids, median_ids,
-            v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst
-        );
-        return gsb::check_launch();
-    });
+    return gsb::surfel_raster_bwd(
+        D, (uint32_t)I * tile_width * tile_height, gsb::DensePixels{}, (cudaStream_t)stream, (uint32_t)I, means2d,
+        ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height, tile_width, tile_height,
+        offsets, flatten_ids, n_isects, render_colors, render_alphas, last_ids, median_ids, v_render_colors,
+        v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst
+    );
 }
 
 // ---- sparse pixels (rasterize_to_pixels_2dgs_sparse): one CTA per active tile of the layout of gsb200_sparse_layout_*,
@@ -937,14 +883,11 @@ extern "C" int gsb200_surfel_raster_sparse_fwd(
     if(int rc = surfel_rows_ok(n_rows))
         return rc;
     const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
-    return gsb::with_channels(D, [&](auto C) {
-        gsb::surfel_raster_fwd_kernel<C, gsb::SparsePixels><<<(uint32_t)n_active, gsb::kSurfThreads, 0, (cudaStream_t)stream>>>(
-            1u, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height, tile_width,
-            tile_height, tile_offsets, flatten_ids, n_isects, render_colors, render_alphas, render_normals, render_distort,
-            render_median, last_ids, median_ids, pm
-        );
-        return gsb::check_launch();
-    });
+    return gsb::surfel_raster_fwd(
+        D, (uint32_t)n_active, pm, (cudaStream_t)stream, 1u, means2d, ray_transforms, colors, opacities, normals,
+        backgrounds, masks, image_width, image_height, tile_width, tile_height, tile_offsets, flatten_ids, n_isects,
+        render_colors, render_alphas, render_normals, render_distort, render_median, last_ids, median_ids
+    );
 }
 
 extern "C" int gsb200_surfel_raster_sparse_bwd(
@@ -975,14 +918,12 @@ extern "C" int gsb200_surfel_raster_sparse_bwd(
         return rc;
     const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
     const gsb::SurfGradDst dst{v_means2d, v_ray_transforms, v_colors, v_opacities, v_normals, v_densify, v_means2d_abs};
-    return gsb::with_channels(D, [&](auto C) {
-        gsb::surfel_raster_bwd_kernel<C, gsb::SparsePixels><<<(uint32_t)n_active, gsb::kSurfThreads, 0, (cudaStream_t)stream>>>(
-            1u, means2d, ray_transforms, colors, opacities, normals, backgrounds, masks, image_width, image_height, tile_width,
-            tile_height, tile_offsets, flatten_ids, n_isects, render_colors, render_alphas, last_ids, median_ids,
-            v_render_colors, v_render_alphas, v_render_normals, v_render_distort, v_render_median, dst, pm
-        );
-        return gsb::check_launch();
-    });
+    return gsb::surfel_raster_bwd(
+        D, (uint32_t)n_active, pm, (cudaStream_t)stream, 1u, means2d, ray_transforms, colors, opacities, normals,
+        backgrounds, masks, image_width, image_height, tile_width, tile_height, tile_offsets, flatten_ids, n_isects,
+        render_colors, render_alphas, last_ids, median_ids, v_render_colors, v_render_alphas, v_render_normals,
+        v_render_distort, v_render_median, dst
+    );
 }
 
 // ---- rasterize_to_indices_in_range_2dgs: count pass (emit = 0) and emit pass (emit = 1) over one workspace (indices.cuh)
@@ -1000,17 +941,18 @@ extern "C" int gsb200_surfel_indices(
         I, N, image_width, image_height, tile_size, tile_width, tile_height, n_isects, range_start, range_end, inputs_ok, emit,
         workspace, workspace_bytes, total, gaussian_ids, pixel_ids, image_ids, st,
         [&](unsigned n_tiles, int32_t b0, int32_t b1, auto sink) {
-            gsb::surfel_indices_kernel<<<n_tiles, gsb::kSurfThreads, 0, st>>>(
-                (uint32_t)I, means2d, ray_transforms, opacities, transmittances, image_width, image_height, tile_width,
-                tile_height, offsets, flatten_ids, n_isects, b0, b1, sink
+            const gsb::SurfelModel model{(uint32_t)I, image_width, image_height, tile_width, tile_height, means2d,
+                                         ray_transforms, opacities};
+            gsb::pair_walk_kernel<<<n_tiles, gsb::kIndexBatch, 0, st>>>(
+                model, transmittances, offsets, flatten_ids, n_isects, b0, b1, sink
             );
             return gsb::check_launch();
         }
     );
 }
 
-// ---- 2DGS per-pixel contributor queries over surfel_indices_kernel (indices.cuh: run_contrib and its checks, in the
-// order and with the return codes of gsb200_contrib_*)
+// ---- 2DGS per-pixel contributor queries over the pair walk of SurfelModel (indices.cuh: run_contrib and its checks, in
+// the order and with the return codes of gsb200_contrib_*)
 namespace gsb
 {
 struct SurfelWalk : PlanarRows
@@ -1019,15 +961,16 @@ struct SurfelWalk : PlanarRows
     int launch(const ContribArgs &a, unsigned n_tiles, const Pix &pm, const Sink &sink, size_t smem, cudaStream_t st) const
     {
         return launch_walk(
-            surfel_indices_kernel<Sink, Pix>, n_tiles, smem, st, (uint32_t)a.I, means2d, rows, opacities,
-            (const float *)nullptr, a.W, a.H, a.tw, a.th, a.offsets, a.flatten_ids, a.n_isects, (int32_t)0,
-            (int32_t)0x7fffffff, sink, pm
+            pair_walk_kernel<SurfelModel, Sink, Pix>, n_tiles, smem, st,
+            SurfelModel{(uint32_t)a.I, a.W, a.H, a.tw, a.th, means2d, rows, opacities}, (const float *)nullptr, a.offsets,
+            a.flatten_ids, a.n_isects, (int32_t)0, (int32_t)0x7fffffff, sink, pm
         );
     }
     static int max_samples()
     {
         return top_max_samples({
-            (const void *)surfel_indices_kernel<TopSink, DensePixels>, (const void *)surfel_indices_kernel<TopSink, SparsePixels>
+            (const void *)pair_walk_kernel<SurfelModel, TopSink, DensePixels>,
+            (const void *)pair_walk_kernel<SurfelModel, TopSink, SparsePixels>
         });
     }
 };

@@ -439,122 +439,56 @@ __global__ void __launch_bounds__(kUtThreads, 1) eval3d_fwd_kernel(
     last_ids[pix] = cur_idx;
 }
 
-// The pair-query walk of rasterize_to_indices_in_range_eval3d and the 3DGUT contributor queries: the (pixel, gaussian)
-// pairs eval3d_fwd_kernel composites, walking only the batches [b0, b1) of each tile's list from the pixel's given
-// transmittance (null: T = 1).  The tiles, the pixel mapping, the ray (camera model, rolling-shutter pose), staging,
-// eval_hit and the stop rule are the forward's, so the alphas are its render_alphas bit for bit.  As in the forward, a
-// pixel composites only when it has an output row (live) and lies inside the W x H image with a ray; a live pixel that
-// does not composite still gets begin and end (count 0, T as given).  Every thread stages records and meets every
-// barrier.  What the walk does with a pixel's pairs is the Sink's (indices.cuh).
-template<class Sink, class Shutter, class Lens, class Pix = DensePixels>
-__global__ void __launch_bounds__(kUtThreads, 1) eval3d_indices_kernel(
-    EvalGeom geo, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
-    const float *__restrict__ opacities, const float *__restrict__ transmittances, const int32_t *__restrict__ offsets,
-    const int32_t *__restrict__ flatten_ids, int64_t n_isects, int32_t b0, int32_t b1, Sink sink, Shutter shutter,
-    Lens lens, const Pix pixmap = Pix{}
-)
+// The 3DGUT model of pair_walk_kernel (indices.cuh), the pair query and contributor queries of the _eval3d ops:
+// eval3d_fwd_kernel's staging, ray (camera model, rolling-shutter pose) and eval_hit.  As in the forward, a pixel
+// composites only when it is live, lies inside the W x H image and has a ray.
+template<class Shutter, class Lens>
+struct Eval3dModel : EvalGeom
 {
-    static_assert(kUtThreads == kIndexBatch, "one record of a batch per thread");
-    __shared__ EvalRec rec[kUtThreads];
-    const uint32_t tile  = pixmap.tile(blockIdx.x); // image * th * tw + tile row * tw + tile col
-    const uint32_t img   = tile / (geo.tw * geo.th);
-    const uint32_t tin   = tile - img * geo.tw * geo.th;
-    const uint32_t tr    = threadIdx.x;
-    const uint32_t i     = (tin / geo.tw) * kTile + tr / kTile;
-    const uint32_t j     = (tin % geo.tw) * kTile + tr % kTile;
-    const int64_t pix_in = (int64_t)i * geo.W + j;
-    bool live, inside = i < geo.H && j < geo.W;
-    int64_t pix, start, end;
-    if constexpr(Pix::kSparse)
+    const float *means, *quats, *scales, *opacities;
+    Shutter shutter;
+    Lens lens;
+    static constexpr int kMinBlocks = 1; // the forward's launch bounds
+    using Rec = EvalRec;
+    struct Pixel
     {
-        pix    = pixmap.slot(blockIdx.x, (int)tr, live);
-        inside = inside && live;
-        start  = offsets[blockIdx.x];
-        end    = offsets[blockIdx.x + 1];
-    }
-    else
+        float ro[3], rd[3];
+    };
+    __device__ __forceinline__ void stage(EvalRec &r, int32_t g) const { gsb::stage(r, g, C, N, means, quats, scales, opacities); }
+    __device__ __forceinline__ bool setup(uint32_t img, uint32_t i, uint32_t j, bool live, Pixel &p) const
     {
-        live  = inside;
-        pix   = (int64_t)img * geo.H * geo.W + pix_in;
-        start = offsets[tile];
-        end   = (tile + 1 == geo.I * geo.tw * geo.th) ? n_isects : offsets[tile + 1];
-    }
-    const int64_t b_end = min((int64_t)b1, (end - start + kUtThreads - 1) / kUtThreads);
-    float ro[3] = {0.f, 0.f, 0.f}, rd[3] = {0.f, 0.f, 1.f};
-    bool done = !inside;
-    if constexpr(Shutter::kRolling)
-    {
-        const auto cm = lens.model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
-        done          = !shutter_pixel_ray(shutter, geo.viewmats, img, inside, cm, i, j, ro, rd);
-    }
-    else if(inside)
-    {
-        const auto cm = lens.model(geo.cam_kind, geo.Ks, geo.radial, geo.tangential, geo.thin, img, geo.W, geo.H);
-        done          = !pixel_ray(geo.viewmats + (int64_t)img * 16, cm, i, j, ro, rd);
-    }
-    float T     = (live && transmittances != nullptr) ? transmittances[pix] : 1.f;
-    int32_t cnt = 0;
-    sink.begin(live, pix, pix_in, img);
-    for(int64_t b = b0; b < b_end; ++b)
-    {
-        if(__syncthreads_count(done) == kUtThreads)
-            break;
-        const int64_t batch = start + b * kUtThreads;
-        if(batch + tr < end)
-            stage(rec[tr], flatten_ids[batch + tr], geo.C, geo.N, means, quats, scales, opacities);
-        __syncthreads();
-        const int n_b = (int)min((int64_t)kUtThreads, end - batch);
-        for(int t = 0; t < n_b && !done; ++t)
+        const bool inside = i < H && j < W && live;
+        p                 = {{0.f, 0.f, 0.f}, {0.f, 0.f, 1.f}};
+        if constexpr(Shutter::kRolling)
         {
-            const EvalRec &r = rec[t];
-            const EvalHit h  = eval_hit(r, ro, rd);
-            if(!h.ok)
-                continue;
-            const float next_T = T * (1.f - h.alpha);
-            if(next_T <= kTransmittanceThreshold)
-            { // exclusive: this gaussian does not contribute
-                done = true;
-                break;
-            }
-            sink.pair(cnt, r.id, h.alpha * T);
-            ++cnt;
-            T = next_T;
+            const auto cm = lens.model(cam_kind, Ks, radial, tangential, thin, img, W, H);
+            return shutter_pixel_ray(shutter, viewmats, img, inside, cm, i, j, p.ro, p.rd);
         }
+        else if(inside)
+        {
+            const auto cm = lens.model(cam_kind, Ks, radial, tangential, thin, img, W, H);
+            return pixel_ray(viewmats + (int64_t)img * 16, cm, i, j, p.ro, p.rd);
+        }
+        return false;
     }
-    if(live)
-        sink.end(pix, cnt, T);
-}
+    __device__ __forceinline__ EvalHit hit(const EvalRec &r, const Pixel &p) const { return eval_hit(r, p.ro, p.rd); }
+};
 
 struct EvalGradDst
 {
     float *colors, *opacities, *rec; // rec: [B * N, 12] = v_mean 3 | v_M 9
-};
 
-// Butterfly-reduces gv[OFF, OFF + 32) across the warp and adds each owned slot to its gradient row; recurses over the
-// remaining 32-value chunks.
-template<int OFF, int NV>
-__device__ __forceinline__ void reduce_emit(const float *gv, unsigned lane, const EvalRec &r, const EvalGradDst &dst, int CDIM)
-{
-    constexpr int M = (NV - OFF) < 32 ? (NV - OFF) : 32;
-    float v[M];
-#pragma unroll
-    for(int k = 0; k < M; ++k)
-        v[k] = gv[OFF + k];
-    Butterfly<M, 16>::run(v, lane);
-    const int s = butterfly_slot<M>(lane);
-    if(s >= 0 && v[0] != 0.f)
+    // reduce_emit's routing (common.cuh): slot of the gradient vector of eval3d_bwd_kernel to its row
+    __device__ __forceinline__ void add(int slot, const EvalRec &r, float val, int CDIM) const
     {
-        const int slot = OFF + s;
         if(slot < CDIM)
-            atomicAdd(dst.colors + (int64_t)r.id * CDIM + slot, v[0]);
+            atomicAdd(colors + (int64_t)r.id * CDIM + slot, val);
         else if(slot == CDIM)
-            atomicAdd(dst.opacities + r.id, v[0]);
+            atomicAdd(opacities + r.id, val);
         else
-            atomicAdd(dst.rec + (int64_t)r.bn * 12 + (slot - CDIM - 1), v[0]);
+            atomicAdd(rec + (int64_t)r.bn * 12 + (slot - CDIM - 1), val);
     }
-    if constexpr(OFF + 32 < NV)
-        reduce_emit<OFF + 32, NV>(gv, lane, r, dst, CDIM);
-}
+};
 
 // Back to front over each tile's list.  Per gaussian, the warp's per-pixel gradients (colours, opacity, mean, M) are
 // butterfly-reduced and added with one atomic per value.  The tiles and the pixels that composite are the forward's
@@ -837,9 +771,59 @@ int with_policies(const float *viewmats_rs, int rolling_shutter, const gsb200_ft
     });
 }
 
-// The contributor queries' walk (indices.cuh: run_contrib): eval3d_indices_kernel over the rows and the camera of
-// gsb200_eval3d_fwd, from T = 1 through the whole lists.  Its inputs are the camera (every pixel's ray reads it) and,
-// when there are intersections, the gaussians; a sparse layout needs at least one image for its tiles to lie in.
+// The tiles and the camera of the compositing and query entries, from their parameters.
+EvalGeom eval_geom(
+    int64_t B, int64_t C, int64_t N, uint32_t W, uint32_t H, uint32_t tw, uint32_t th, int cam_kind, const float *viewmats,
+    const float *Ks, const float *radial, const float *tangential, const float *thin
+)
+{
+    return {(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, W, H, tw, th, cam_kind, viewmats, Ks, radial, tangential, thin};
+}
+
+// The compositing launches of the dense and sparse entries, after each entry's own checks: n_ctas CTAs over the tiles
+// of the pixel policy pm, with the kernel's arguments between geo and the policies.
+template<class Pix, class... Args>
+int eval3d_fwd(
+    const EvalGeom &geo, unsigned n_ctas, const Pix &pm, int D, const gsb200_ftheta_params *ft, const float *viewmats_rs,
+    int rolling_shutter, cudaStream_t st, const Args &...args
+)
+{
+    return with_policies(viewmats_rs, rolling_shutter, ft, 1, [&](auto shutter, auto lens) {
+        return with_channels(D, [&](auto CH) {
+            eval3d_fwd_kernel<CH, decltype(shutter), decltype(lens), Pix><<<n_ctas, kUtThreads, 0, st>>>(
+                geo, args..., shutter, lens, pm
+            );
+            return check_launch();
+        });
+    });
+}
+
+// composite: whether the compositing backward runs (args: its arguments between scales and dst) before the finish
+// kernel, which turns the B * N records of dst into v_means, v_quats and v_scales
+template<class Pix, class... Args>
+int eval3d_bwd(
+    const EvalGeom &geo, unsigned n_ctas, const Pix &pm, bool composite, int D, const gsb200_ftheta_params *ft,
+    const float *viewmats_rs, int rolling_shutter, cudaStream_t st, int64_t BN, const float *means, const float *quats,
+    const float *scales, const EvalGradDst &dst, float *v_means, float *v_quats, float *v_scales, const Args &...args
+)
+{
+    const int rc = !composite ? GSB200_OK : with_policies(viewmats_rs, rolling_shutter, ft, 1, [&](auto shutter, auto lens) {
+        return with_channels(D, [&](auto CH) {
+            eval3d_bwd_kernel<CH, decltype(shutter), decltype(lens), Pix><<<n_ctas, kUtThreads, 0, st>>>(
+                geo, means, quats, scales, args..., dst, shutter, lens, pm
+            );
+            return check_launch();
+        });
+    });
+    if(rc)
+        return rc;
+    eval3d_finish_kernel<<<grid_for(BN, kUtThreads), kUtThreads, 0, st>>>(BN, quats, scales, dst.rec, v_means, v_quats, v_scales);
+    return check_launch();
+}
+
+// The contributor queries' walk (indices.cuh: run_contrib): pair_walk_kernel of Eval3dModel over the rows and the
+// camera of gsb200_eval3d_fwd, from T = 1 through the whole lists.  Its inputs are the camera (every pixel's ray reads
+// it) and, when there are intersections, the gaussians; a sparse layout needs at least one image for its tiles to lie in.
 struct Eval3dWalk
 {
     EvalGeom geo;
@@ -852,14 +836,21 @@ struct Eval3dWalk
     {
         return geo.I > 0 && geo.viewmats && geo.Ks && (n_isects == 0 || (means && quats && scales && opacities));
     }
+    // runs f with the Eval3dModel of the walk's shutter and lens
+    template<class F>
+    int with_model(F &&f) const
+    {
+        return with_policies(viewmats_rs, rolling_shutter, ft, 1, [&](auto shutter, auto lens) {
+            return f(Eval3dModel<decltype(shutter), decltype(lens)>{geo, means, quats, scales, opacities, shutter, lens});
+        });
+    }
     template<class Pix, class Sink>
     int launch(const ContribArgs &a, unsigned n_tiles, const Pix &pm, const Sink &sink, size_t smem, cudaStream_t st) const
     {
-        return with_policies(viewmats_rs, rolling_shutter, ft, 1, [&](auto shutter, auto lens) {
+        return with_model([&](const auto &model) {
             return launch_walk(
-                eval3d_indices_kernel<Sink, decltype(shutter), decltype(lens), Pix>, n_tiles, smem, st, geo, means, quats,
-                scales, opacities, (const float *)nullptr, a.offsets, a.flatten_ids, a.n_isects, (int32_t)0,
-                (int32_t)0x7fffffff, sink, shutter, lens, pm
+                pair_walk_kernel<std::decay_t<decltype(model)>, Sink, Pix>, n_tiles, smem, st, model, (const float *)nullptr,
+                a.offsets, a.flatten_ids, a.n_isects, (int32_t)0, (int32_t)0x7fffffff, sink, pm
             );
         });
     }
@@ -868,32 +859,32 @@ struct Eval3dWalk
     static int max_samples()
     {
         return top_max_samples({
-            (const void *)eval3d_indices_kernel<TopSink, GlobalShutter, CamLens, DensePixels>,
-            (const void *)eval3d_indices_kernel<TopSink, GlobalShutter, FThetaLens, DensePixels>,
-            (const void *)eval3d_indices_kernel<TopSink, RollingShutter, CamLens, DensePixels>,
-            (const void *)eval3d_indices_kernel<TopSink, RollingShutter, FThetaLens, DensePixels>,
-            (const void *)eval3d_indices_kernel<TopSink, GlobalShutter, CamLens, SparsePixels>,
-            (const void *)eval3d_indices_kernel<TopSink, GlobalShutter, FThetaLens, SparsePixels>,
-            (const void *)eval3d_indices_kernel<TopSink, RollingShutter, CamLens, SparsePixels>,
-            (const void *)eval3d_indices_kernel<TopSink, RollingShutter, FThetaLens, SparsePixels>,
+            (const void *)pair_walk_kernel<Eval3dModel<GlobalShutter, CamLens>, TopSink, DensePixels>,
+            (const void *)pair_walk_kernel<Eval3dModel<GlobalShutter, FThetaLens>, TopSink, DensePixels>,
+            (const void *)pair_walk_kernel<Eval3dModel<RollingShutter, CamLens>, TopSink, DensePixels>,
+            (const void *)pair_walk_kernel<Eval3dModel<RollingShutter, FThetaLens>, TopSink, DensePixels>,
+            (const void *)pair_walk_kernel<Eval3dModel<GlobalShutter, CamLens>, TopSink, SparsePixels>,
+            (const void *)pair_walk_kernel<Eval3dModel<GlobalShutter, FThetaLens>, TopSink, SparsePixels>,
+            (const void *)pair_walk_kernel<Eval3dModel<RollingShutter, CamLens>, TopSink, SparsePixels>,
+            (const void *)pair_walk_kernel<Eval3dModel<RollingShutter, FThetaLens>, TopSink, SparsePixels>,
         });
     }
 };
 
-// The checks of every 3DGUT query entry before its own: sizes, camera, and the sparse layout when there is one.
+// The checks of every 3DGUT query entry before its own: sizes, the walk's camera, then the sparse layout if any.
 int eval3d_query_checks(
-    int64_t B, int64_t C, int64_t N, int cam_kind, const float *radial, const float *tangential, const float *thin,
-    const gsb200_ftheta_params *ft, const float *viewmats_rs, int rolling_shutter, uint32_t W, uint32_t H,
-    uint32_t tile_size, uint32_t tw, uint32_t th, int64_t n_active, const int32_t *active_tiles, const int32_t *offsets,
-    const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum, const int64_t *pixel_map
+    int64_t B, int64_t C, int64_t N, const Eval3dWalk &w, uint32_t tile_size, int64_t n_active,
+    const int32_t *active_tiles, const int32_t *offsets, const uint64_t *tile_pixel_mask, const int64_t *tile_pixel_cumsum,
+    const int64_t *pixel_map
 )
 {
-    if(int rc = eval3d_checks(B, C, N, W, H, tile_size, tw, th))
+    const EvalGeom &g = w.geo;
+    if(int rc = eval3d_checks(B, C, N, g.W, g.H, tile_size, g.tw, g.th))
         return rc;
-    if(int rc = camera_checks(cam_kind, radial, tangential, thin, ft, viewmats_rs, rolling_shutter, W, H))
+    if(int rc = camera_checks(g.cam_kind, g.radial, g.tangential, g.thin, w.ft, w.viewmats_rs, w.rolling_shutter, g.W, g.H))
         return rc;
     if(active_tiles != nullptr)
-        return sparse_args_ok(n_active, active_tiles, offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, W, H, tw, th);
+        return sparse_args_ok(n_active, active_tiles, offsets, tile_pixel_mask, tile_pixel_cumsum, pixel_map, g.W, g.H, g.tw, g.th);
     return GSB200_OK;
 }
 } // namespace
@@ -961,17 +952,13 @@ extern "C" int gsb200_eval3d_fwd(
         return GSB200_E_INVALID;
     if(n_isects > 0 && (!means || !quats || !scales || !colors || !opacities || !flatten_ids))
         return GSB200_E_INVALID;
-    const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height,
-                            camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
-    return gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
-        return gsb::with_channels(D, [&](auto CH) {
-            gsb::eval3d_fwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
-                geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
-                render_colors, render_alphas, last_ids, shutter, lens
-            );
-            return gsb::check_launch();
-        });
-    });
+    const gsb::EvalGeom geo = gsb::eval_geom(B, C, N, image_width, image_height, tile_width, tile_height, camera_model,
+                                             viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs);
+    return gsb::eval3d_fwd(
+        geo, geo.I * tile_width * tile_height, gsb::DensePixels{}, D, ftheta, viewmats_rs, rolling_shutter,
+        (cudaStream_t)stream, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
+        render_colors, render_alphas, last_ids
+    );
 }
 
 extern "C" int gsb200_eval3d_bwd(
@@ -996,31 +983,19 @@ extern "C" int gsb200_eval3d_bwd(
         return GSB200_OK;
     if(!quats || !scales || !grad_records || !v_means || !v_quats || !v_scales)
         return GSB200_E_INVALID;
-    cudaStream_t st = (cudaStream_t)stream;
-    if(n_isects > 0 && B * C > 0 && image_width > 0 && image_height > 0)
-    {
-        if(!means || !colors || !opacities || !viewmats || !Ks || !offsets || !flatten_ids || !render_alphas || !last_ids
-           || !v_render_colors || !v_colors || !v_opacities)
-            return GSB200_E_INVALID;
-        const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width,
-                                tile_height, camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
-        const gsb::EvalGradDst dst{v_colors, v_opacities, grad_records};
-        const int rc = gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
-            return gsb::with_channels(D, [&](auto CH) {
-                gsb::eval3d_bwd_kernel<CH><<<geo.I * tile_width * tile_height, gsb::kUtThreads, 0, st>>>(
-                    geo, means, quats, scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects,
-                    render_alphas, last_ids, v_render_colors, v_render_alphas, dst, shutter, lens
-                );
-                return gsb::check_launch();
-            });
-        });
-        if(rc)
-            return rc;
-    }
-    gsb::eval3d_finish_kernel<<<gsb::grid_for(B * N, gsb::kUtThreads), gsb::kUtThreads, 0, st>>>(
-        B * N, quats, scales, grad_records, v_means, v_quats, v_scales
+    const bool composite = n_isects > 0 && B * C > 0 && image_width > 0 && image_height > 0;
+    if(composite
+       && (!means || !colors || !opacities || !viewmats || !Ks || !offsets || !flatten_ids || !render_alphas || !last_ids
+           || !v_render_colors || !v_colors || !v_opacities))
+        return GSB200_E_INVALID;
+    const gsb::EvalGeom geo = gsb::eval_geom(B, C, N, image_width, image_height, tile_width, tile_height, camera_model,
+                                             viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs);
+    return gsb::eval3d_bwd(
+        geo, geo.I * tile_width * tile_height, gsb::DensePixels{}, composite, D, ftheta, viewmats_rs, rolling_shutter,
+        (cudaStream_t)stream, B * N, means, quats, scales, gsb::EvalGradDst{v_colors, v_opacities, grad_records}, v_means,
+        v_quats, v_scales, colors, opacities, backgrounds, masks, offsets, flatten_ids, n_isects, render_alphas, last_ids,
+        v_render_colors, v_render_alphas
     );
-    return gsb::check_launch();
 }
 
 // ---- sparse pixels (rasterize_to_pixels_eval3d_sparse): one CTA per active tile of the layout of gsb200_sparse_layout_*,
@@ -1053,19 +1028,13 @@ extern "C" int gsb200_eval3d_sparse_fwd(
         return GSB200_E_INVALID;
     if(n_isects > 0 && (!means || !quats || !scales || !colors || !opacities || !flatten_ids))
         return GSB200_E_INVALID;
-    const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height,
-                            camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
     const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
-    return gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
-        return gsb::with_channels(D, [&](auto CH) {
-            gsb::eval3d_fwd_kernel<CH, decltype(shutter), decltype(lens), gsb::SparsePixels>
-                <<<(uint32_t)n_active, gsb::kUtThreads, 0, (cudaStream_t)stream>>>(
-                    geo, means, quats, scales, colors, opacities, backgrounds, masks, tile_offsets, flatten_ids, n_isects,
-                    render_colors, render_alphas, last_ids, shutter, lens, pm
-                );
-            return gsb::check_launch();
-        });
-    });
+    return gsb::eval3d_fwd(
+        gsb::eval_geom(B, C, N, image_width, image_height, tile_width, tile_height, camera_model, viewmats, Ks,
+                       radial_coeffs, tangential_coeffs, thin_prism_coeffs),
+        (uint32_t)n_active, pm, D, ftheta, viewmats_rs, rolling_shutter, (cudaStream_t)stream, means, quats, scales,
+        colors, opacities, backgrounds, masks, tile_offsets, flatten_ids, n_isects, render_colors, render_alphas, last_ids
+    );
 }
 
 extern "C" int gsb200_eval3d_sparse_bwd(
@@ -1097,33 +1066,19 @@ extern "C" int gsb200_eval3d_sparse_bwd(
     // the finish kernel runs without the compositing: an unsupported channel count is refused before either
     if(gsb::with_channels(D, [](auto) { return GSB200_OK; }))
         return GSB200_E_UNSUPPORTED;
-    cudaStream_t st = (cudaStream_t)stream;
-    if(n_isects > 0 && n_active > 0)
-    {
-        if(B * C == 0 || !means || !colors || !opacities || !viewmats || !Ks || !flatten_ids || !render_alphas || !last_ids
-           || !v_render_colors || !v_colors || !v_opacities)
-            return GSB200_E_INVALID;
-        const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width,
-                                tile_height, camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
-        const gsb::EvalGradDst dst{v_colors, v_opacities, grad_records};
-        const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
-        const int rc = gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
-            return gsb::with_channels(D, [&](auto CH) {
-                gsb::eval3d_bwd_kernel<CH, decltype(shutter), decltype(lens), gsb::SparsePixels>
-                    <<<(uint32_t)n_active, gsb::kUtThreads, 0, st>>>(
-                        geo, means, quats, scales, colors, opacities, backgrounds, masks, tile_offsets, flatten_ids,
-                        n_isects, render_alphas, last_ids, v_render_colors, v_render_alphas, dst, shutter, lens, pm
-                    );
-                return gsb::check_launch();
-            });
-        });
-        if(rc)
-            return rc;
-    }
-    gsb::eval3d_finish_kernel<<<gsb::grid_for(B * N, gsb::kUtThreads), gsb::kUtThreads, 0, st>>>(
-        B * N, quats, scales, grad_records, v_means, v_quats, v_scales
+    const bool composite = n_isects > 0 && n_active > 0;
+    if(composite
+       && (B * C == 0 || !means || !colors || !opacities || !viewmats || !Ks || !flatten_ids || !render_alphas || !last_ids
+           || !v_render_colors || !v_colors || !v_opacities))
+        return GSB200_E_INVALID;
+    const gsb::SparsePixels pm{active_tiles, tile_pixel_mask, tile_pixel_cumsum, pixel_map};
+    return gsb::eval3d_bwd(
+        gsb::eval_geom(B, C, N, image_width, image_height, tile_width, tile_height, camera_model, viewmats, Ks,
+                       radial_coeffs, tangential_coeffs, thin_prism_coeffs),
+        (uint32_t)n_active, pm, composite, D, ftheta, viewmats_rs, rolling_shutter, (cudaStream_t)stream, B * N, means,
+        quats, scales, gsb::EvalGradDst{v_colors, v_opacities, grad_records}, v_means, v_quats, v_scales, colors, opacities,
+        backgrounds, masks, tile_offsets, flatten_ids, n_isects, render_alphas, last_ids, v_render_colors, v_render_alphas
     );
-    return gsb::check_launch();
 }
 
 // ---- rasterize_to_indices_in_range_eval3d: count pass (emit = 0) and emit pass (emit = 1) over one workspace
@@ -1138,22 +1093,20 @@ extern "C" int gsb200_eval3d_indices(
     int64_t *pixel_ids, int64_t *image_ids, void *stream
 )
 {
-    if(int rc = gsb::eval3d_query_checks(B, C, N, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta,
-                                         viewmats_rs, rolling_shutter, image_width, image_height, tile_size, tile_width,
-                                         tile_height, 0, nullptr, nullptr, nullptr, nullptr, nullptr))
+    const gsb::Eval3dWalk walk{gsb::eval_geom(B, C, N, image_width, image_height, tile_width, tile_height, camera_model,
+                                              viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs),
+                               means, quats, scales, opacities, ftheta, viewmats_rs, rolling_shutter};
+    if(int rc = gsb::eval3d_query_checks(B, C, N, walk, tile_size, 0, nullptr, nullptr, nullptr, nullptr, nullptr))
         return rc;
     const cudaStream_t st = (cudaStream_t)stream;
     const bool inputs_ok  = means && quats && scales && opacities && viewmats && Ks && transmittances && offsets && flatten_ids;
-    const gsb::EvalGeom geo{(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height,
-                            camera_model, viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs};
     return gsb::run_index_pass(
         B * C, N, image_width, image_height, tile_size, tile_width, tile_height, n_isects, range_start, range_end, inputs_ok,
         emit, workspace, workspace_bytes, total, gaussian_ids, pixel_ids, image_ids, st,
         [&](unsigned n_tiles, int32_t b0, int32_t b1, auto sink) {
-            return gsb::with_policies(viewmats_rs, rolling_shutter, ftheta, 1, [&](auto shutter, auto lens) {
-                gsb::eval3d_indices_kernel<<<n_tiles, gsb::kUtThreads, 0, st>>>(
-                    geo, means, quats, scales, opacities, transmittances, offsets, flatten_ids, n_isects, b0, b1, sink,
-                    shutter, lens
+            return walk.with_model([&](const auto &model) {
+                gsb::pair_walk_kernel<<<n_tiles, gsb::kIndexBatch, 0, st>>>(
+                    model, transmittances, offsets, flatten_ids, n_isects, b0, b1, sink
                 );
                 return gsb::check_launch();
             });
@@ -1161,23 +1114,8 @@ extern "C" int gsb200_eval3d_indices(
     );
 }
 
-// ---- 3DGUT per-pixel contributor queries over eval3d_indices_kernel: the size, camera and (sparse) layout checks of
+// ---- 3DGUT per-pixel contributor queries over Eval3dWalk: the size, camera and (sparse) layout checks of
 // gsb200_eval3d_sparse_fwd, then run_contrib's (indices.cuh), in the order and with the return codes of gsb200_contrib_*
-// the checks and the walk of a contributor entry, from its parameters (named as gsb200_eval3d_contrib_count's)
-#define GSB200_EVAL3D_QUERY_CHECKS                                                                                      \
-    gsb::eval3d_query_checks(                                                                                           \
-        B, C, N, camera_model, radial_coeffs, tangential_coeffs, thin_prism_coeffs, ftheta, viewmats_rs, rolling_shutter, \
-        image_width, image_height, tile_size, tile_width, tile_height, n_active, active_tiles, offsets, tile_pixel_mask,  \
-        tile_pixel_cumsum, pixel_map                                                                                    \
-    )
-#define GSB200_EVAL3D_WALK                                                                                              \
-    gsb::Eval3dWalk                                                                                                     \
-    {                                                                                                                   \
-        {(uint32_t)(B * C), (uint32_t)C, (uint32_t)N, image_width, image_height, tile_width, tile_height, camera_model,  \
-         viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs},                                            \
-            means, quats, scales, opacities, ftheta, viewmats_rs, rolling_shutter                                       \
-    }
-
 extern "C" int gsb200_eval3d_contrib_max_samples(void)
 {
     return gsb::Eval3dWalk::max_samples();
@@ -1193,9 +1131,13 @@ extern "C" int gsb200_eval3d_contrib_count(
     float *alphas, void *stream
 )
 {
-    if(int rc = GSB200_EVAL3D_QUERY_CHECKS)
+    const gsb::Eval3dWalk walk{gsb::eval_geom(B, C, N, image_width, image_height, tile_width, tile_height, camera_model,
+                                              viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs),
+                               means, quats, scales, opacities, ftheta, viewmats_rs, rolling_shutter};
+    if(int rc = gsb::eval3d_query_checks(B, C, N, walk, tile_size, n_active, active_tiles, offsets, tile_pixel_mask,
+                                         tile_pixel_cumsum, pixel_map))
         return rc;
-    return gsb::contrib_count(GSB200_EVAL3D_WALK, GSB200_CONTRIB_ARGS(B * C), counts, alphas, (cudaStream_t)stream);
+    return gsb::contrib_count(walk, GSB200_CONTRIB_ARGS(B * C), counts, alphas, (cudaStream_t)stream);
 }
 
 extern "C" int gsb200_eval3d_contrib_ids(
@@ -1208,9 +1150,13 @@ extern "C" int gsb200_eval3d_contrib_ids(
     int32_t *ids, float *weights, void *stream
 )
 {
-    if(int rc = GSB200_EVAL3D_QUERY_CHECKS)
+    const gsb::Eval3dWalk walk{gsb::eval_geom(B, C, N, image_width, image_height, tile_width, tile_height, camera_model,
+                                              viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs),
+                               means, quats, scales, opacities, ftheta, viewmats_rs, rolling_shutter};
+    if(int rc = gsb::eval3d_query_checks(B, C, N, walk, tile_size, n_active, active_tiles, offsets, tile_pixel_mask,
+                                         tile_pixel_cumsum, pixel_map))
         return rc;
-    return gsb::contrib_ids(GSB200_EVAL3D_WALK, GSB200_CONTRIB_ARGS(B * C), max_samples, ids, weights, (cudaStream_t)stream);
+    return gsb::contrib_ids(walk, GSB200_CONTRIB_ARGS(B * C), max_samples, ids, weights, (cudaStream_t)stream);
 }
 
 extern "C" int gsb200_eval3d_contrib_top(
@@ -1223,7 +1169,11 @@ extern "C" int gsb200_eval3d_contrib_top(
     int32_t *ids, float *weights, void *stream
 )
 {
-    if(int rc = GSB200_EVAL3D_QUERY_CHECKS)
+    const gsb::Eval3dWalk walk{gsb::eval_geom(B, C, N, image_width, image_height, tile_width, tile_height, camera_model,
+                                              viewmats, Ks, radial_coeffs, tangential_coeffs, thin_prism_coeffs),
+                               means, quats, scales, opacities, ftheta, viewmats_rs, rolling_shutter};
+    if(int rc = gsb::eval3d_query_checks(B, C, N, walk, tile_size, n_active, active_tiles, offsets, tile_pixel_mask,
+                                         tile_pixel_cumsum, pixel_map))
         return rc;
-    return gsb::contrib_top(GSB200_EVAL3D_WALK, GSB200_CONTRIB_ARGS(B * C), num_samples, ids, weights, (cudaStream_t)stream);
+    return gsb::contrib_top(walk, GSB200_CONTRIB_ARGS(B * C), num_samples, ids, weights, (cudaStream_t)stream);
 }

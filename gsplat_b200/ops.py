@@ -2020,7 +2020,8 @@ def rasterize_to_pixels_2dgs_sparse(
 # rasterize_to_indices_in_range(0, inf) composites from T = 1, per pixel, as counts, padded id lists or the K heaviest.
 # Every query is one walk of the pair-query kernel (csrc/raster.cu, raster_indices_kernel) with its own per-pair sink,
 # dense over every tile or sparse over the active tiles of a build_sparse_tile_layout layout.  The _2dgs forms (the
-# reference has none) are the same queries over the surfel walk (csrc/surfel.cu, surfel_indices_kernel).
+# reference has none) are the same queries over the surfel walk (csrc/indices.cuh, pair_walk_kernel with
+# csrc/surfel.cu's SurfelModel).
 
 class _ContribWalk(NamedTuple):
     """One pair-query walk of the contributor queries: its rows (tail and name) and its C entries."""
@@ -3268,9 +3269,9 @@ def rasterize_to_pixels_eval3d_sparse(
 
 # --------------------------------------------------------------------------------------------
 # 3DGUT pair query and per-pixel contributor queries (the reference has none): the pairs rasterize_to_pixels_eval3d
-# composites, from the walk of csrc/ut.cu (eval3d_indices_kernel) with the forward's rays, responses and stop rule.  The
-# contributor forms are those of the 3DGS / 2DGS queries over that walk, with the geometry and cameras of
-# rasterize_to_pixels_eval3d in place of 2-D rows.
+# composites, from the walk of csrc/indices.cuh (pair_walk_kernel with csrc/ut.cu's Eval3dModel) with the forward's
+# rays, responses and stop rule.  The contributor forms are those of the 3DGS / 2DGS queries over that walk, with the
+# geometry and cameras of rasterize_to_pixels_eval3d in place of 2-D rows.
 
 @torch.no_grad()
 def rasterize_to_indices_in_range_eval3d(

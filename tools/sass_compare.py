@@ -10,9 +10,11 @@ old self.  Names are compared demangled, with the pixel-addressing policy of the
 (``gsb::DensePixels``) removed, so that a kernel that only gained that template argument is matched with its old self,
 with ``isect_count_kernel<true / false>`` under the names the two count kernels had before they became one template,
 with the unmasked ``isect_count_kernel`` and ``isect_emit_kernel`` (``MASKED`` = false) without that template argument
-and the tile-mask parameters that came with it, and with the pair-query kernels ``raster_indices_kernel`` and
-``surfel_indices_kernel`` named by their sink without their parameter list (``<false / true>`` became the
-``CountSink`` / ``PairSink`` instantiations when each walk took a sink), and with the 3DGUT kernels
+and the tile-mask parameters that came with it, and with the pair-query kernels ``raster_indices_kernel``,
+``surfel_indices_kernel`` and ``eval3d_indices_kernel`` named by their template arguments without their parameter list
+(``<false / true>`` became the ``CountSink`` / ``PairSink`` instantiations when each walk took a sink; the 2DGS and
+3DGUT walks became ``pair_walk_kernel<SurfelModel, Sink, Pix>`` and ``pair_walk_kernel<Eval3dModel<Shutter, Lens>,
+Sink, Pix>``, named as the kernels they were, so that they are reported as changed), and with the 3DGUT kernels
 (``ut_project_kernel``, ``eval3d_fwd_kernel``, ``eval3d_bwd_kernel``) without their ``gsb::GlobalShutter`` policy, the
 template argument and the trailing empty parameter they gained with the rolling shutter, and without their
 ``gsb::CamLens`` policy, the template argument and trailing empty parameter they gained with the FTheta lens.  Instructions and their encodings must be
@@ -45,8 +47,13 @@ MASKED_KERNEL = re.compile(
 COUNT_KERNEL = re.compile(r"^void gsb::isect_count_kernel<\(bool\)([01])>\((.*), unsigned long long \*\)$")
 # raster_indices_kernel<EMIT> became raster_indices_kernel<Sink, Pix> and surfel_indices_kernel<EMIT> became
 # surfel_indices_kernel<Sink>: <false> is the CountSink walk, <true> the PairSink
-INDICES_KERNEL = re.compile(r"^void (gsb::(?:<unnamed>::)?(?:raster|surfel)_indices_kernel)<(.*)>\(.*\)$")
+INDICES_KERNEL = re.compile(r"^void (gsb::(?:<unnamed>::)?(?:raster|surfel|eval3d)_indices_kernel)<(.*)>\(.*\)$")
 INDICES_SINK = {"(bool)0": "gsb::CountSink", "(bool)1": "gsb::PairSink"}
+# surfel_indices_kernel<Sink, Pix> and eval3d_indices_kernel<Sink, Shutter, Lens, Pix> became pair_walk_kernel of the
+# SurfelModel / Eval3dModel<Shutter, Lens>: renamed as they were, before the policies are removed
+PAIR_WALK = re.compile(
+    r"^void gsb::pair_walk_kernel<gsb::<unnamed>::(?:(SurfelModel)|Eval3dModel<([^<>]*)>), (gsb::\w+), (gsb::\w+)>(\(.*\))$"
+)
 
 
 def _tree_at(rev: str, dst: str) -> None:
@@ -90,6 +97,10 @@ def kernels(obj: str):
     names = list(raw)
     out = {}
     for n, d in zip(names, _demangle(names)):
+        m = PAIR_WALK.match(d)
+        if m:  # <Sink, Pix> of the 2DGS walk, <Sink, Shutter, Lens, Pix> of the 3DGUT one
+            policies = "" if m[1] else f"{m[2]}, "
+            d = f"void gsb::<unnamed>::{'surfel' if m[1] else 'eval3d'}_indices_kernel<{m[3]}, {policies}{m[4]}>{m[5]}"
         if "DensePixels" in n or "SparsePixels" in n:
             d = POLICY_PARAM.sub(")", d).replace(", gsb::DensePixels>", ">")
         m = MASKED_KERNEL.match(d)
