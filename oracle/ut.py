@@ -45,6 +45,8 @@ RS_ITERATIONS = 10
 # FTheta
 PIXELDIST_TO_ANGLE, ANGLE_TO_PIXELDIST = 0, 1
 NEWTON_STEPS, NEWTON_TOL = 3, 1e-6
+# pinhole validity: the radial factor above 0.8, compared at float32(0.8) as the kernels do
+ICD_MIN = float(torch.tensor(0.8, dtype=torch.float32))
 
 
 class Camera:
@@ -101,7 +103,7 @@ class Camera:
                 dx = p[0] * a1 + p[1] * (r2 + 2 * xn * xn) + r2 * (s[0] + r2 * s[1])
                 dy = p[0] * (r2 + 2 * yn * yn) + p[1] * a1 + r2 * (s[2] + r2 * s[3])
                 xn, yn = icd * xn + dx, icd * yn + dy
-                ok = icd > 0.8
+                ok = icd > ICD_MIN
             u, v = xn * self.fx + self.cx, yn * self.fy + self.cy
         else:
             rxy = torch.sqrt(x * x + y * y).clamp_min(torch.finfo(torch.float32).eps)
