@@ -315,7 +315,9 @@ __device__ __forceinline__ EvalHit eval_hit(const EvalRec &r, const float *ro, c
     const float dist = h.c[0] * h.c[0] + h.c[1] * h.c[1] + h.c[2] * h.c[2];
     h.resp  = fast_exp(-0.5f * dist);
     h.alpha = fminf(kMaxAlpha, r.o * h.resp);
-    h.ok    = !(hit_t < 0.f) && !(h.alpha < kAlphaThreshold) && l2 > 0.f;
+    // Ordered comparisons: a NaN hit_t or response (a zero, sub-1/FLT_MAX or infinite scale, a non-finite mean) makes
+    // no contribution.  fminf would turn a NaN response into alpha 0.99.
+    h.ok    = hit_t >= 0.f && r.o * h.resp >= kAlphaThreshold && l2 > 0.f;
     return h;
 }
 
@@ -673,6 +675,10 @@ __global__ void __launch_bounds__(kUtThreads) eval3d_finish_kernel(
         v_means[g * 3 + k] = rg[k];
     const float q[4] = {quats[g * 4], quats[g * 4 + 1], quats[g * 4 + 2], quats[g * 4 + 3]};
     const M3 R       = quat_to_rotmat(q);
+    // a gaussian with no v_M gets zero v_scales and v_quats, also when its scale or quaternion makes M non-finite (such
+    // a gaussian never contributes)
+    const bool any_vm = rg[3] != 0.f || rg[4] != 0.f || rg[5] != 0.f || rg[6] != 0.f || rg[7] != 0.f || rg[8] != 0.f
+                        || rg[9] != 0.f || rg[10] != 0.f || rg[11] != 0.f;
     M3 vR;
 #pragma unroll
     for(int i = 0; i < 3; ++i)
@@ -687,11 +693,10 @@ __global__ void __launch_bounds__(kUtThreads) eval3d_finish_kernel(
             vR.m[j * 3 + i]    = vm * inv;
             acc               += vm * R.m[j * 3 + i];
         }
-        v_scales[g * 3 + i] = -acc * inv * inv;
+        v_scales[g * 3 + i] = any_vm ? -acc * inv * inv : 0.f;
     }
     float vq[4] = {0.f, 0.f, 0.f, 0.f};
-    if(rg[3] != 0.f || rg[4] != 0.f || rg[5] != 0.f || rg[6] != 0.f || rg[7] != 0.f || rg[8] != 0.f || rg[9] != 0.f
-       || rg[10] != 0.f || rg[11] != 0.f)
+    if(any_vm)
         quat_to_rotmat_vjp(q, vR, vq);
 #pragma unroll
     for(int k = 0; k < 4; ++k)

@@ -118,10 +118,16 @@ class Camera:
         uv = torch.stack([torch.where(front, u, torch.zeros_like(u)), torch.where(front, v, torch.zeros_like(v))], -1)
         return uv, front & ok & inb
 
-    def unproject(self, u, v):
-        """image points -> (unit camera rays [..., 3], valid), the distortion inverted by Newton iteration."""
+    def unproject(self, u, v, rule="converged"):
+        """image points -> (unit camera rays [..., 3], valid), the distortion inverted by Newton iteration.  rule
+        "converged": iterate float64 to convergence.  rule "reference": replay the kernels' rule in float64 (pinhole:
+        at most 5 steps, giving up at icD <= 0 or |det| < 1e-6, converged once both steps are below 1e-6; fisheye: at
+        most 20 steps, converged once the step is below 1e-6, invalid at t < 0 or t >= max_angle) and keep in
+        ``self.trace`` what each decision compared, per step [steps, ...] (NaN once a point has stopped)."""
         u, v = torch.as_tensor(u, dtype=F64), torch.as_tensor(v, dtype=F64)
         x0, y0 = (u - self.cx) / self.fx, (v - self.cy) / self.fy
+        if rule == "reference":
+            return self._unproject_reference(x0, y0)
         if self.kind == "pinhole":
             x, y, ok = x0.clone(), y0.clone(), torch.ones_like(x0, dtype=torch.bool)
             if self.distorted:
@@ -154,6 +160,63 @@ class Camera:
         sc = torch.where(delta >= 1e-6, torch.sin(t) / delta.clamp_min(1e-300), torch.zeros_like(t))
         d = torch.stack([sc * x0, sc * y0, torch.where(delta >= 1e-6, torch.cos(t), torch.ones_like(t))], -1)
         return d, ok
+
+    def _unproject_reference(self, x0, y0):
+        nan = torch.full_like(x0, math.nan)
+        trace = {}
+
+        def rec(key, live, val):
+            trace.setdefault(key, []).append(torch.where(live, val, nan))
+
+        if self.kind == "pinhole":
+            x, y = x0.clone(), y0.clone()
+            ok = torch.full_like(x0, not self.distorted, dtype=torch.bool)
+            live = torch.full_like(ok, self.distorted)
+            k, p, s = self.k, self.p, self.s
+            for _ in range(5 if self.distorted else 0):
+                r2 = x * x + y * y
+                num = 1 + r2 * (k[0] + r2 * (k[1] + r2 * k[2]))
+                den = 1 + r2 * (k[3] + r2 * (k[4] + r2 * k[5]))
+                icd = num / den
+                rec("icd", live, icd)
+                live = live & (icd > 0)
+                dicd = ((k[0] + r2 * (2 * k[1] + 3 * r2 * k[2])) - icd * (k[3] + r2 * (2 * k[4] + 3 * r2 * k[5]))) / den
+                gx, gy = s[0] + 2 * s[1] * r2, s[2] + 2 * s[3] * r2
+                Dx = icd * x + p[0] * 2 * x * y + p[1] * (r2 + 2 * x * x) + r2 * (s[0] + r2 * s[1])
+                Dy = icd * y + p[0] * (r2 + 2 * y * y) + p[1] * 2 * x * y + r2 * (s[2] + r2 * s[3])
+                J0 = icd + 2 * x * x * dicd + 2 * p[0] * y + 6 * p[1] * x + 2 * x * gx
+                J1 = 2 * x * y * dicd + 2 * p[0] * x + 2 * p[1] * y + 2 * y * gx
+                J2 = 2 * x * y * dicd + 2 * p[0] * x + 2 * p[1] * y + 2 * x * gy
+                J3 = icd + 2 * y * y * dicd + 6 * p[0] * y + 2 * p[1] * x + 2 * y * gy
+                det = J0 * J3 - J1 * J2
+                rec("det", live, det)
+                rec("jinv", live, torch.maximum(J3.abs() + J1.abs(), J0.abs() + J2.abs()) / det.abs())  # |J^-1|_inf
+                live = live & (det.abs() >= 1e-6)
+                ex, ey = x0 - Dx, y0 - Dy
+                sx, sy = (J3 * ex - J1 * ey) / det, (J0 * ey - J2 * ex) / det
+                x, y = torch.where(live, x + sx, x), torch.where(live, y + sy, y)
+                step = torch.maximum(sx.abs(), sy.abs())
+                rec("step", live, step)
+                conv = live & (step < 1e-6)
+                ok, live = ok | conv, live & ~conv
+            self.trace = {key: torch.stack(v) for key, v in trace.items()}
+            d = torch.stack([x, y, torch.ones_like(x)], -1)
+            return d / d.norm(dim=-1, keepdim=True), ok
+        delta = torch.sqrt(x0 * x0 + y0 * y0)
+        t = self.inv_slope * delta
+        live = torch.ones_like(delta, dtype=torch.bool)
+        for _ in range(20):
+            dx = (self._fe(t) - delta) / self._dfe(t)
+            t = torch.where(live, t - dx, t)
+            rec("step", live, dx.abs())
+            live = live & ~(dx.abs() < 1e-6)
+        self.trace = {key: torch.stack(v) for key, v in trace.items()}
+        self.trace["t"] = t
+        ok = ~live & (t >= 0) & (t < self.max_angle)
+        big = delta >= 1e-6
+        sc = torch.where(big, torch.sin(t) / torch.where(big, delta, torch.ones_like(delta)), torch.zeros_like(t))
+        d = torch.stack([sc * x0, sc * y0, torch.where(big, torch.cos(t), torch.ones_like(t))], -1)
+        return torch.where(ok[..., None], d, torch.tensor([0.0, 0.0, 1.0], dtype=F64)), ok
 
 
 def quat_to_rotmat(q):
